@@ -8,6 +8,7 @@ object / background points) per candidate, plus one NUNOCS forward (8192 points)
 `config`), `value` = candidates scored / second over all ranks.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config K1|K2|K3|K4|K5]
+                    [--dump-outputs DIR]
 
 Default configuration by GPU count (BASELINE.json `configs`):
     --gpus 1 -> K2  nut clutter pile, 20 000-pt scene, 4 096 candidates                       (weak when forced at N > 1)
@@ -17,6 +18,10 @@ Default configuration by GPU count (BASELINE.json `configs`):
                     (adjust_collision_pose off) -> grasp-Q on the survivors; ~1 M candidates over all ranks
 N > 1 is launched by torchrun (one rank per GPU); no data-path collective, one NCCL all-gather of the 48-byte result
 records per pass.  Prints ONE JSON line (rank 0).
+
+--dump-outputs DIR writes what the timed path computed in its last step (rank 0) as DIR/<name>.npy (float32), at most
+64 MB in all.  The inputs are synthetic and seeded, so two builds run with the same arguments can be compared output
+for output.
 """
 import argparse
 import json
@@ -38,9 +43,10 @@ FLOP_PER_CAND = {1024: 880045568, 2048: 1754052096}     # SURVEY.md 8(d), exact 
 TRUNK_MAC_PER_PT = [6 * 64 + 64 * 128 + 128 * 1024,            # STN3d trunk
                     6 * 64 + 64 * 64 + 64 * 128 + 128 * 1024,  # conv1 + STNkd trunk
                     6 * 64 + 64 * 64 + 64 * 128 + 128 * 1024]  # conv1 + @T64 + conv2 + conv3
-ENGINE_NAMES = ["fp32-simt", "tcgen05-bf16x3", "tcgen05-f16x2", "tcgen05-f16x1-persistent"]
-ENGINE_DTYPES = ["f32", "f32 (bf16 hi/lo x3 on tcgen05, f32 accumulate)", "f32 (f16 hi/lo x2 on tcgen05, f32 accumulate)",
-                 "f32 (128->1024 layer f16 x f16 single pass on tcgen05, f32 accumulate; other layers bf16 hi/lo x3)"]
+ENGINE_NAMES = ["fp32-simt", "wgmma-bf16x3", "wgmma-f16x2", "wgmma-f16x1"]
+ENGINE_DTYPES = ["f32", "f32 (bf16 hi/lo x3 on wgmma, f32 accumulate)", "f32 (f16 hi/lo x2 on wgmma, f32 accumulate)",
+                 "f32 (128->1024 layer f16 x f16 single pass on wgmma, f32 accumulate; other layers bf16 hi/lo x3)"]
+DUMP_LIMIT_BYTES = 64 << 20
 CONFIGS = {
     "K1": dict(name="K1 nut: single-object 1024-pt crop, 64 candidates", scenes=1, scene_pts=1024, total=64, objects=1),
     "K2": dict(name="K2 nut clutter pile: 20000-pt scene, 4096 candidates", scenes=1, scene_pts=20000, total=4096, objects=12),
@@ -62,12 +68,14 @@ def parse_args():
     ap.add_argument("--config", default=None, choices=sorted(CONFIGS), help="default: K2 / K3 / K4 for 1 / 2 / >=4 GPUs")
     ap.add_argument("--n-pts", type=int, default=1024, help="points per candidate (config_grasp.yml n_pts)")
     ap.add_argument("--nunocs-pts", type=int, default=8192)
-    ap.add_argument("--engine", type=int, default=None, help="0 fp32 SIMT, 1 tcgen05 3-pass bf16, 2 tcgen05 2-pass fp16, "
-                    "3 persistent tcgen05 1-pass fp16 (default: library default = 3)")
+    ap.add_argument("--engine", type=int, default=None, help="0 fp32 SIMT, 1 wgmma 3-pass bf16, 2 wgmma 2-pass fp16, "
+                    "3 wgmma 1-pass fp16 (default: library default = 3)")
     ap.add_argument("--passes-per-step", type=int, default=0, help="0 = calibrate so that the timed region is ~1.2 s")
     ap.add_argument("--cpu-sample", type=int, default=192, help="candidates in the CPU-baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-api-leg", action="store_true", help="skip the e2e_api leg (GraspPredicter.predict_batch wall clock)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     if args.config is None:
         args.config = "K2" if args.gpus == 1 else ("K3" if args.gpus == 2 else "K4")
@@ -80,11 +88,29 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- a bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: array} as out_dir/<name>.npy in float32.  Should the total exceed DUMP_LIMIT_BYTES, every array keeps
+    the same fixed, seeded sample of its leading-axis rows (written as row_sample.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float32) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        frac = DUMP_LIMIT_BYTES / (2.0 * total)
+        for k, a in list(arrays.items()):
+            keep = max(1, int(a.shape[0] * frac))
+            rows = np.sort(np.random.RandomState(0).choice(a.shape[0], keep, replace=False))
+            arrays[k] = a[rows]
+            arrays[k + "__row_sample"] = rows.astype(np.float32)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index = index
@@ -349,8 +375,7 @@ def api_leg(dev_index, n_pts):
         out["nunocs_predict_nocs_ms"] = 1e3 * (time.perf_counter() - t0) / 5
     out["note"] = ("wall clock through catgrasp_b200.predicter (draw, H2D, forward, D2H, result list); 'host' = the reference's "
                    "numpy draw bit for bit (C continuation of MT19937, pipelined with the GPU), 'device' = counter-based "
-                   "draw on the GPU (same distribution, not the reference's random stream); round 1 (numpy loop): 3.2k cand/s "
-                   "at 20000 pts, 17.8k at 3000 pts")
+                   "draw on the GPU (same distribution, not the reference's random stream)")
     return out
 
 
@@ -364,7 +389,7 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
-    assert torch.cuda.is_available(), "bench.py needs a B200; there is no CPU fallback"
+    assert torch.cuda.is_available(), "bench.py needs an H100; there is no CPU fallback"
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -407,20 +432,23 @@ def main():
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
     def one_pass():
-        recs, coords = [], None
+        recs, outs = [], []
         for j in jobs:
             d = j["d"]
-            coords, conf, _ = seg.nunocs_dev(d["nun"], 100)
+            coords, conf, bins = seg.nunocs_dev(d["nun"], 100)
+            o = {"nunocs_coords": coords, "nunocs_conf_z": conf, "nunocs_bins": bins}
+            outs.append(o)
             if j["B"] == 0:
                 continue
             probs, label = cls.graspq_dev(d["xyz"], d["nrm"], d["pose"], d["ids"], d_mean, d_std)
             st, off, poses = my_cpp.filter_grasp_pose_raw(d["pose32"], eye[None], eye, eye, g["gripper_in_grasp"], True, True,
                                                           so, d["open"], se, d["bg"])
+            o.update(graspq_probs=probs, graspq_label=label, collision_status=st, collision_offset=off, collision_poses=poses)
             recs.append(pack_records(probs, st, off))
         rec = torch.cat(recs) if len(recs) > 1 else (recs[0] if recs else torch.zeros((0, 12), device=dev))
         if world > 1:
             rec = all_gather_records(rec, per_rank_max * world)     # one ncclAllGather per pass, no host sync before it
-        return rec, coords
+        return rec, outs
 
     def barrier():
         if world > 1:
@@ -445,11 +473,11 @@ def main():
     passes = args.passes_per_step or int(min(128, max(1, round(1200.0 / (float(pass_ms.item()) * max(args.steps, 1))))))
 
     def step_device():
-        rec = coords = None
+        rec = outs = None
         for _ in range(passes):
             flush.fill_(1)                  # evict L2 between timed passes
-            rec, coords = one_pass()
-        return rec, coords
+            rec, outs = one_pass()
+        return rec, outs
 
     for _ in range(max(args.warmup, 3)):
         step_device()
@@ -464,7 +492,7 @@ def main():
     barrier()
     ev0.record()
     for _ in range(args.steps):
-        rec, coords = step_device()
+        rec, outs = step_device()
     ev1.record()
     barrier()
     ms = ev0.elapsed_time(ev1)
@@ -480,6 +508,10 @@ def main():
     checksum = float(rec[:, :10].sum().item())
     main_engine = ctx.get_engine()
     overflow = ctx.fp16_overflow()
+    if args.dump_outputs and rank == 0:    # outputs of the last timed pass, concatenated over this rank's scenes
+        names = dict.fromkeys(k for o in outs for k in o)
+        dump_outputs(args.dump_outputs, {k: torch.cat([o[k].reshape(o[k].shape[0], -1) for o in outs if k in o]).float().cpu().numpy()
+                                         for k in names})
 
     # ---------------- same workload on the 3-pass (near-fp32) tensor-core engine, for the record
     alt = None
@@ -705,11 +737,11 @@ def run_k5(args, rank, world, local, dev):
                                                     None, none_bg)
         keep = torch.nonzero(st == 0).flatten()
         n_keep = int(keep.numel())
-        probs = None
+        outs = {"collision_status": st, "survivor_index": keep}
         if n_keep:
             ids = cls.draw_ids_dev(pts.shape[0], args.n_pts, n_keep, seed=1234, first_candidate=0)
-            probs, _ = cls.graspq_dev(d_xyz, d_nrm, p64[keep].contiguous(), ids)
-        return n_keep, probs
+            outs["graspq_probs"], outs["graspq_label"] = cls.graspq_dev(d_xyz, d_nrm, p64[keep].contiguous(), ids)
+        return n_keep, outs
 
     def barrier():
         if world > 1:
@@ -717,13 +749,13 @@ def run_k5(args, rank, world, local, dev):
         torch.cuda.synchronize()
 
     for _ in range(max(min(args.warmup, 3), 1)):
-        n_keep, probs = one_pass()
+        n_keep, outs = one_pass()
     barrier()
-    steps = max(1, min(args.steps, 5))
+    steps = args.steps
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     for _ in range(steps):
-        n_keep, probs = one_pass()
+        n_keep, outs = one_pass()
     ev1.record()
     barrier()
     t = torch.tensor([ev0.elapsed_time(ev1)], dtype=torch.float64, device=dev)
@@ -732,6 +764,8 @@ def run_k5(args, rank, world, local, dev):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         dist.all_reduce(k)
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {k: v.reshape(v.shape[0], -1).float().cpu().numpy() for k, v in outs.items()})
         ms = float(t.item())
         line = {"metric": "candidate grasps scored/sec", "value": total * steps / (ms * 1e-3), "unit": "candidates/s",
                 "n_gpus": world, "steps": steps, "warmup": max(min(args.warmup, 3), 1), "ms_per_step": ms / steps,

@@ -1,8 +1,8 @@
 """ctypes binding of libcatgrasp_b200.so (the C ABI declared in include/catgrasp_b200.h).
 
 The product path has NO CPU fallback: if the shared library is missing or no
-B200 is present, every entry point raises.  Build the library with
-``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_100a).
+H100 is present, every entry point raises.  Build the library with
+``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_90a).
 """
 import ctypes as C
 import os
@@ -49,7 +49,6 @@ SIGNATURES = {
     "cg_ctx_set_engine": (_i, [_vp, _i]),
     "cg_ctx_get_engine": (_i, [_vp]),
     "cg_ctx_fp16_overflow": (_i, [_vp, C.POINTER(_i)]),
-    "cg_tmem_layout_selftest": (_i, [_vp, _vp]),
     "cg_ctx_profile": (_i, [_vp, _i]),
     "cg_ctx_profile_read": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "cg_net_create": (_i, [_vp, _i, _i, _vp, _sz, C.POINTER(_vp)]),
@@ -134,7 +133,7 @@ class Context:
         rc = lib.cg_ctx_create(self.device, C.byref(h))
         if rc != CG_OK:
             raise CgError(f"cg_ctx_create(device={device}) failed with {rc}: "
-                          "a B200 (sm_100) GPU is required; there is no CPU fallback")
+                          "an H100 (sm_90) GPU is required; there is no CPU fallback")
         self.h = h
 
     @classmethod

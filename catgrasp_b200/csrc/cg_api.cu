@@ -2,7 +2,7 @@
 #include "cg_common.cuh"
 #include <stdlib.h>
 
-extern "C" const char *cg_version(void) { return "catgrasp_b200 0.1 (sm_100a)"; }
+extern "C" const char *cg_version(void) { return "catgrasp_b200 0.1 (sm_90a)"; }
 
 extern "C" int cg_ctx_create(int device, cg_ctx **out) {
   if (!out) return CG_EINVAL;
@@ -10,9 +10,9 @@ extern "C" int cg_ctx_create(int device, cg_ctx **out) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || device < 0 || device >= n) return CG_ECUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return CG_ECUDA;
-  if (prop.major != 10) {
-    // no multi-backend dispatch: this library only carries sm_100a code
-    fprintf(stderr, "catgrasp_b200: device %d is sm_%d%d, this library is sm_100a-only\n", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    // no multi-backend dispatch: this library only carries sm_90a code
+    fprintf(stderr, "catgrasp_b200: device %d is sm_%d%d, this library is sm_90a-only\n", device, prop.major,
             prop.minor);
     return CG_EUNSUPPORTED;
   }
@@ -102,7 +102,7 @@ extern "C" void cg_ctx_reset_launch_count(cg_ctx *ctx) { if (ctx) ctx->launches 
 extern "C" int cg_ctx_set_engine(cg_ctx *ctx, int engine) {
   if (!ctx) return CG_EINVAL;
   CG_REQUIRE(ctx, engine >= 0 && engine <= 3,
-             "engine must be 0 (fp32 SIMT), 1 (tcgen05 3-pass), 2 (tcgen05 2-pass) or 3 (persistent tcgen05 1-pass)");
+             "engine must be 0 (fp32 SIMT), 1 (wgmma 3-pass), 2 (wgmma 2-pass) or 3 (wgmma 1-pass)");
   ctx->engine = engine;
   return CG_OK;
 }

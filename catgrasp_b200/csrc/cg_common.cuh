@@ -1,4 +1,4 @@
-// cg_common.cuh -- shared internals of libcatgrasp_b200 (sm_100a only).
+// cg_common.cuh -- shared internals of libcatgrasp_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,8 +9,8 @@
 #include <vector>
 #include "../../include/catgrasp_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libcatgrasp_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libcatgrasp_b200 is written for sm_90a (H100) only"
 #endif
 
 constexpr int CG_MAX_DEVICES = 64;   // per-device one-time kernel attributes are tracked in arrays of this size
@@ -21,11 +21,11 @@ struct cg_ctx {
   cudaStream_t stream = nullptr;
   std::string err;
   int64_t launches = 0;
-  // 0 = fp32 SIMT, 1 = tcgen05 bf16 3-pass, 2 = tcgen05 fp16 2-pass, 3 = persistent tcgen05, single fp16 pass (default)
+  // 0 = fp32 SIMT, 1 = wgmma bf16 3-pass, 2 = wgmma fp16 2-pass, 3 = wgmma single fp16 pass (default)
   int engine = 3;
   cudaEvent_t switch_event = nullptr;   // orders a newly selected stream behind the previous one (shared workspaces)
   uint32_t *ovf_flag = nullptr;   // device word: engine 3 saw a 128->1024 input above the fp16 range (clamped)
-  int num_sms = 148;
+  int num_sms = 132;
   // optional event-pair timing of trunk launches (bench roofline)
   bool prof = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;

@@ -1,256 +1,119 @@
-// cg_linear_tc.cu -- fully-connected layers on tcgen05 (bf16 hi/lo x3, fp32 accumulate in TMEM).
+// cg_linear_tc.cu -- fully-connected layers on wgmma (bf16 hi/lo x3, fp32 accumulate in registers).
 //
 //   Y[M][N] = act( X[M][K] @ Wt[K][N] + bias[row / bias_row_div][N] )      K % 64 == 0
 //
 // replaces nn.Linear / Conv1d(k=1) + folded BN (+ReLU) of the PointNet heads (pointnet2.py:176-183, :214-221,
-// :295-298, :323-327) for M >= 64 rows.  One CTA = 128 rows x 128 output columns; K runs through a 3-stage ring of
-// 64-wide K-blocks: the weight block arrives as a bulk copy of the host-prepared UMMA image, the activation block is
-// read as fp32 (or as the trunk's order-preserving keys), split into bf16 hi/lo and written in the canonical K-major
-// SWIZZLE_128B layout by four converter warps that double as the epilogue (TMEM -> bias/ReLU -> fp32 rows).
-#include <cuda_bf16.h>
-
+// :295-298, :323-327) for M >= 64 rows.  One CTA = 128 rows x 128 output columns, one warpgroup per 64 rows; K runs
+// through a 3-stage ring of 64-wide K-blocks: the weight block arrives as a bulk copy of the host-prepared swizzled
+// image (B operand), the activations are read as fp32 (or as the trunk's order-preserving keys) straight into the
+// A-operand register fragments, split into bf16 hi/lo on the way.
 #include <unordered_map>
 
 #include "cg_net.cuh"
+#include "cg_tc_ptx.cuh"
 
 namespace {
+using namespace cg_ptx;
 
 constexpr uint32_t PIECE = 16384;             // [128 rows x 64 bf16]
 constexpr int STAGES = 3;
-constexpr uint32_t STAGE_BYTES = 4 * PIECE;   // A hi, A lo, B hi, B lo
-constexpr int NCONV = 4;                      // converter / epilogue warps (thread = row)
-constexpr int LT = (NCONV + 2) * 32;          // + producer warp + MMA warp = 192 threads
+constexpr uint32_t STAGE_BYTES = 2 * PIECE;   // B hi, B lo of one 64-wide K-block
+constexpr int LT = 256;                       // two consumer warpgroups: rows 0-63 / 64-127 of the tile
 
 struct Bars {
-  unsigned long long a_full[STAGES], b_full[STAGES], empty[STAGES], done;
-  uint32_t tmem_base;
+  unsigned long long full[STAGES], empty[STAGES];
 };
-constexpr size_t LSMEM = STAGES * STAGE_BYTES + sizeof(Bars) + 1024;
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-__host__ __device__ __forceinline__ uint32_t row_chunk_off(int row, int c16) {
-  return (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u + (uint32_t)((c16 ^ (row & 7)) << 4);
-}
+constexpr size_t LSMEM = STAGES * STAGE_BYTES + sizeof(Bars);
 
 __global__ void __launch_bounds__(LT, 1) linear_tc_kernel(const float *__restrict__ X, int M, int K,
                                                           const unsigned char *__restrict__ wimg,
                                                           const float *__restrict__ bias, int N, int relu,
                                                           int bias_row_div, int x_is_keys, float *__restrict__ Y) {
-  // no static shared memory in this kernel: the dynamic window starts 1024-byte aligned (checked); using the array
-  // directly keeps the accesses in the shared address space (LDS / STS / ATOMS, not generic LD / ST / ATOM)
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  unsigned char *smem = smem_dyn;
-  if ((static_cast<uint32_t>(__cvta_generic_to_shared(smem)) & 1023u) != 0u) __trap();
+  // no static shared memory in this kernel: the dynamic window starts 1024-byte aligned (checked)
+  extern __shared__ __align__(1024) unsigned char smem[];
+  if ((smem_u32(smem) & 1023u) != 0u) __trap();
   Bars &S = *reinterpret_cast<Bars *>(smem + STAGES * STAGE_BYTES);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+  const int g = lane >> 2, q = lane & 3;
   const int n0 = blockIdx.x * 128, m0 = blockIdx.y * 128;
   const int nkb = K >> 6;
+  const uint32_t smem_s = smem_u32(smem);
+  const unsigned char *src = wimg + (size_t)blockIdx.x * nkb * STAGE_BYTES;   // this column tile's K-blocks
   if (tid == 0) {
     for (int s = 0; s < STAGES; s++) {
-      mbar_init(smem_u32(&S.a_full[s]), NCONV);
-      mbar_init(smem_u32(&S.b_full[s]), 1);
-      mbar_init(smem_u32(&S.empty[s]), 1);
+      mbar_init(smem_u32(&S.full[s]), 1);
+      mbar_init(smem_u32(&S.empty[s]), LT / 32);
     }
-    mbar_init(smem_u32(&S.done), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(128u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = S.tmem_base;
-  const uint32_t smem_s = smem_u32(smem);
-
-  if (warp == NCONV) {
-    // ---------------- producer: weight K-blocks [hi 16 KB | lo 16 KB] of this column tile ----------------
-    const unsigned char *src = wimg + (size_t)blockIdx.x * nkb * 2 * PIECE;
-    for (int kb = 0; kb < nkb; kb++) {
-      const int s = kb % STAGES;
-      mbar_wait(smem_u32(&S.empty[s]), (((uint32_t)(kb / STAGES)) & 1u) ^ 1u);
-      if (elect_one()) {
-        const uint32_t fb = smem_u32(&S.b_full[s]);
-        mbar_expect_tx(fb, 2 * PIECE);
-        bulk_g2s(smem_s + (uint32_t)s * STAGE_BYTES + 2 * PIECE, src + (size_t)kb * 2 * PIECE, 2 * PIECE, fb);
-      }
-      __syncwarp();
+    mbar_init_fence();
+    for (int kb = 0; kb < nkb && kb < STAGES; kb++) {
+      mbar_expect_tx(smem_u32(&S.full[kb]), STAGE_BYTES);
+      bulk_g2s(smem_s + (uint32_t)kb * STAGE_BYTES, src + (size_t)kb * STAGE_BYTES, STAGE_BYTES, smem_u32(&S.full[kb]));
     }
-  } else if (warp == NCONV + 1) {
-    // ---------------- UMMA issuer ----------------
-    for (int kb = 0; kb < nkb; kb++) {
-      const int s = kb % STAGES;
-      const uint32_t par = ((uint32_t)(kb / STAGES)) & 1u;
-      mbar_wait(smem_u32(&S.a_full[s]), par);
-      mbar_wait(smem_u32(&S.b_full[s]), par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_s = smem_s + (uint32_t)s * STAGE_BYTES, b_s = a_s + 2 * PIECE;
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < 4; ks++) {
-          const uint32_t koff = (uint32_t)ks * 32u;
-          const uint64_t a_hi = umma_desc(a_s + koff), a_lo = umma_desc(a_s + PIECE + koff);
-          const uint64_t b_hi = umma_desc(b_s + koff), b_lo = umma_desc(b_s + PIECE + koff);
-          umma(tmem_base, a_lo, b_hi, (kb | ks) ? 1u : 0u);
-          umma(tmem_base, a_hi, b_lo, 1u);
-          umma(tmem_base, a_hi, b_hi, 1u);
-        }
-        umma_commit(smem_u32(&S.empty[s]));
-        if (kb == nkb - 1) umma_commit(smem_u32(&S.done));
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------- converter warps: thread = row ----------------
-    const int row = tid;                       // 0..127
-    const int m = m0 + row;
-    const bool live = m < M;
-    const float *xr = X + (size_t)(live ? m : 0) * K;
-    float4 nxt[16];
-    auto gload = [&](int kb) {
-#pragma unroll
-      for (int q = 0; q < 16; q++)
-        nxt[q] = live ? *reinterpret_cast<const float4 *>(xr + kb * 64 + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-    };
-    gload(0);
-    for (int kb = 0; kb < nkb; kb++) {
-      const int s = kb % STAGES;
-      float v[64];
-#pragma unroll
-      for (int q = 0; q < 16; q++) {
-        v[4 * q] = nxt[q].x; v[4 * q + 1] = nxt[q].y; v[4 * q + 2] = nxt[q].z; v[4 * q + 3] = nxt[q].w;
-      }
-      if (kb + 1 < nkb) gload(kb + 1);         // next block's loads fly while this one is converted
-      if (x_is_keys) {
-#pragma unroll
-        for (int j = 0; j < 64; j++) v[j] = live ? cg_key2f(__float_as_uint(v[j])) : 0.f;
-      }
-      mbar_wait(smem_u32(&S.empty[s]), (((uint32_t)(kb / STAGES)) & 1u) ^ 1u);
-      unsigned char *a_hi = smem + (size_t)s * STAGE_BYTES, *a_lo = a_hi + PIECE;
-#pragma unroll
-      for (int c16 = 0; c16 < 8; c16++) {
-        uint32_t h[4], l[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const float x0 = v[c16 * 8 + 2 * j], x1 = v[c16 * 8 + 2 * j + 1];
-          const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-          const __nv_bfloat16 l0 = __float2bfloat16_rn(x0 - __bfloat162float(h0));
-          const __nv_bfloat16 l1 = __float2bfloat16_rn(x1 - __bfloat162float(h1));
-          h[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-          l[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-        }
-        const uint32_t off = row_chunk_off(row, c16);
-        *reinterpret_cast<uint4 *>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4 *>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&S.a_full[s]));
-    }
-    // ---------------- epilogue: D[row][col] -> + bias, ReLU -> Y ----------------
-    mbar_wait(smem_u32(&S.done), 0u);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    const float *brow = bias ? (bias + (size_t)(bias_row_div > 0 ? ((live ? m : 0) / bias_row_div) : 0) * N) : nullptr;
-#pragma unroll 1
-    for (int j32 = 0; j32 < 4; j32++) {
-      float v[32];
-      tmem_ld32(tmem_base + lane_sel + (uint32_t)j32 * 32u, v);
-      if (live) {
-        const int nb = n0 + j32 * 32;
-        if (nb + 32 <= N && (N & 3) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 o;
-            o.x = v[j] + (brow ? brow[nb + j] : 0.f); o.y = v[j + 1] + (brow ? brow[nb + j + 1] : 0.f);
-            o.z = v[j + 2] + (brow ? brow[nb + j + 2] : 0.f); o.w = v[j + 3] + (brow ? brow[nb + j + 3] : 0.f);
-            if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-            *reinterpret_cast<float4 *>(Y + (size_t)m * N + nb + j) = o;
-          }
-        } else {
-          for (int j = 0; j < 32; j++) {
-            const int n = nb + j;
-            if (n < N) {
-              float o = v[j] + (brow ? brow[n] : 0.f);
-              if (relu) o = fmaxf(o, 0.f);
-              Y[(size_t)m * N + n] = o;
-            }
-          }
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   }
   __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128u) : "memory");
+  // this thread's rows of the A fragments: m0 + 16 * warp + g and + 8
+  const int ma = m0 + 16 * warp + g, mb = ma + 8;
+  const bool la = ma < M, lb = mb < M;
+  const float *xa = X + (size_t)(la ? ma : 0) * K + 2 * q, *xb = X + (size_t)(lb ? mb : 0) * K + 2 * q;
+  auto ld2 = [&](const float *p, bool live) {
+    if (!live) return make_float2(0.f, 0.f);
+    float2 v = *reinterpret_cast<const float2 *>(p);
+    if (x_is_keys) v = make_float2(cg_key2f(__float_as_uint(v.x)), cg_key2f(__float_as_uint(v.y)));
+    return v;
+  };
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; i++) acc[i] = 0.f;
+  for (int kb = 0; kb < nkb; kb++) {
+    const int s = kb % STAGES;
+    // A fragments of the 4 k-steps of this K-block, straight from the fp32 rows (split into bf16 hi / lo)
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      const int k = kb * 64 + ks * 16;
+      const float2 v0 = ld2(xa + k, la), v1 = ld2(xb + k, lb), v2 = ld2(xa + k + 8, la), v3 = ld2(xb + k + 8, lb);
+      split_bf16x2(v0.x, v0.y, ah[ks][0], al[ks][0]);
+      split_bf16x2(v1.x, v1.y, ah[ks][1], al[ks][1]);
+      split_bf16x2(v2.x, v2.y, ah[ks][2], al[ks][2]);
+      split_bf16x2(v3.x, v3.y, ah[ks][3], al[ks][3]);
+    }
+    mbar_wait(smem_u32(&S.full[s]), ((uint32_t)(kb / STAGES)) & 1u);
+    const uint32_t b_s = smem_s + (uint32_t)s * STAGE_BYTES;
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      const uint64_t bh = wg_desc(b_s + 32u * ks), bl = wg_desc(b_s + PIECE + 32u * ks);
+      wg_m64n128<false>(acc, al[ks], bh, 1u);
+      wg_m64n128<false>(acc, ah[ks], bl, 1u);
+      wg_m64n128<false>(acc, ah[ks], bh, 1u);
+    }
+    wg_commit();
+    wg_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&S.empty[s]));
+    if (tid == 0 && kb + STAGES < nkb) {   // refill the stage once all eight warps have read it
+      mbar_wait(smem_u32(&S.empty[s]), ((uint32_t)(kb / STAGES)) & 1u);
+      mbar_expect_tx(smem_u32(&S.full[s]), STAGE_BYTES);
+      bulk_g2s(b_s, src + (size_t)(kb + STAGES) * STAGE_BYTES, STAGE_BYTES, smem_u32(&S.full[s]));
+    }
+  }
+  // ---------------- epilogue: D[row][col] -> + bias, ReLU -> Y ----------------
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+    const int m = r ? mb : ma;
+    if (!(r ? lb : la)) continue;
+    const float *brow = bias ? (bias + (size_t)(bias_row_div > 0 ? m / bias_row_div : 0) * N) : nullptr;
+#pragma unroll
+    for (int i = 0; i < 16; i++)
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const int n = n0 + 8 * i + 2 * q + e;
+        if (n < N) {
+          float o = acc[4 * i + 2 * r + e] + (brow ? brow[n] : 0.f);
+          if (relu) o = fmaxf(o, 0.f);
+          Y[(size_t)m * N + n] = o;
+        }
+      }
   }
 }
 
@@ -268,7 +131,7 @@ float bf16_to_f(unsigned short h) {
   return f;
 }
 
-std::unordered_map<const float *, void *> g_images;   // device Wt pointer -> device UMMA image
+std::unordered_map<const float *, void *> g_images;   // device Wt pointer -> device operand image
 
 }  // namespace
 

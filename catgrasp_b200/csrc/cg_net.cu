@@ -111,9 +111,7 @@ int trunk_launch(cg_ctx *ctx, const cg_trunk_args &a) {
     CG_CUDA(ctx, cudaEventRecord(e0, ctx->stream));
   }
   int rc;
-  if (ctx->engine == 3 && a.tc_f16_ok) rc = cg_trunk_launch_p(ctx, a);   // persistent, single fp16 pass
-  else if (ctx->engine >= 1) rc = cg_trunk_launch_tc(ctx, a);            // 3-pass bf16 / 2-pass fp16 (also the
-                                                                          // fallback when W3 exceeds the fp16 range)
+  if (ctx->engine >= 1) rc = cg_trunk_launch_tc(ctx, a);   // 3-pass bf16 / 2-pass fp16 / 1-pass fp16 on wgmma
   else rc = cg_trunk_launch_simt(ctx, a);
   if (ctx->prof) {
     CG_CUDA(ctx, cudaEventRecord(e1, ctx->stream));
@@ -151,7 +149,7 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   const cg_layer *L = net->L;
   int rc;
   cg_trunk_args a;
-  a.in = in; a.B = B; a.N = N; a.dbg = nullptr; a.exp_flags = 0; a.ovf_flag = ctx->ovf_flag;
+  a.in = in; a.B = B; a.N = N; a.ovf_flag = ctx->ovf_flag;
   // --- trunk A: STN3d convs + max (pointnet2.py:170-175)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.T3 = nullptr; a.l0 = L[L_S3_C1]; a.stage1_mode = 0; a.l1 = cg_layer{nullptr, nullptr, 0, 0}; a.T64 = nullptr;

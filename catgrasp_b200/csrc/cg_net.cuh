@@ -25,7 +25,7 @@ struct cg_net {
   float *blob_dev;
   size_t blob_floats;
   cg_layer L[L_COUNT];
-  // engine-1 (tcgen05) bf16 hi/lo operand images of each trunk's 128->1024, 64->128 and (STNkd) 64->64
+  // tensor-core (wgmma) bf16 hi/lo + fp16 operand images of each trunk's 128->1024, 64->128 and (STNkd) 64->64
   // layers, built at create time: [W3 | W2 | W1]; indices 0 = STN3d, 1 = STNkd, 2 = encoder
   void *tc_img[3];
   int tc_f16_ok[3];   // 128->1024 weights fit fp16 (|w| < 65504): the 2-pass engine may be used for this trunk
@@ -53,20 +53,16 @@ struct cg_trunk_args {
   const float *T64;  // (B,64,64) when stage1_mode == 2
   cg_layer l2;       // 64 -> 128 (+ReLU)
   cg_layer l3;       // 128 -> 1024
-  const void *tc_img; // tcgen05 operand images [W3 | W2 | W1 | W3 fp16] of l3 / l2 / l1 (engines 1, 2)
+  const void *tc_img; // wgmma operand images [W3 | W2 | W1 | W3 fp16] of l3 / l2 / l1 (engines 1-3)
   int tc_f16_ok;      // engine 2 allowed for this trunk (else it runs the 3-pass kernel)
   int relu3;
   uint32_t *gmax_keys;  // (B,1024) order-preserving keys, zero-initialised by the launcher
   float *pf_out;        // (B,N,64) stage-1 output (PointNetSeg point feature) or nullptr
-  unsigned long long *dbg;  // optional per-CTA cycle counters (CG_TRUNK_DEBUG=1), else nullptr
   uint32_t *ovf_flag;       // engine 3: set to 1 when an activation had to be clamped to the fp16 range (or nullptr)
-  int exp_flags;            // timing experiments only (CG_TRUNK_EXP bitmask, results become wrong): 1 = no W3 copies,
-                            // 2 = max warps skip the TMEM reads, 4 = front warps skip their math
 };
 
 int cg_trunk_launch_simt(cg_ctx *ctx, const cg_trunk_args &a);
-int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a);
-int cg_trunk_launch_p(cg_ctx *ctx, const cg_trunk_args &a);   // persistent single-pass kernel (engine 3)
+int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a);   // engines 1-3 (wgmma)
 size_t cg_tc_image_bytes();
 // Wt3 [128][1024], Wt2 [64][128], Wt1 [64][64] or nullptr (folded fp32, k-major rows, host)
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok);

@@ -329,9 +329,9 @@ extern "C" int cg_fps_dev(cg_ctx *ctx, const float *xyz, int B, int N, int npoin
     cudaGetLastError();
     csize_dev[ctx->device] = cs;
   }
-  // Cluster size: measured per-round cost ~ base(csize) + 0.025 us x points per thread, base = 0.70 / 0.83 / 1.0 / 1.45 us
-  // for 2 / 4 / 8 / 16 CTAs (the cross-CTA exchange is the floor: remote store + remote mbarrier arrive + acquire wait);
-  // pick the cheapest size whose points fit the 32-registers-per-thread budget.
+  // Cluster size: cost model per round ~ base(csize) + 0.025 x points per thread, base = 0.70 / 0.83 / 1.0 / 1.45
+  // for 2 / 4 / 8 / 16 CTAs (the cross-CTA exchange is the floor: remote store + remote mbarrier arrive + acquire wait,
+  // and it grows with the cluster); pick the cheapest size whose points fit the 32-registers-per-thread budget.
   int csize = csize_dev[ctx->device];
   {
     const int sizes[4] = {2, 4, 8, 16};

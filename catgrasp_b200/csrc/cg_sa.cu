@@ -8,7 +8,7 @@
 //   SA:  sample_and_group -> (B,S,K,3+D) -> [1x1 conv + BN + ReLU] x L over all B*S*K rows -> max over K -> (B,S,C_L)
 //   FP:  3 nearest neighbours of every dense point among the S sparse points (expanded-form square_distance, :14-33),
 //        weights (1/(d+1e-8)) / sum, weighted sum of their features -> concat skip features -> [conv + BN + ReLU] x L
-// A layer whose K is a multiple of 64 and that has >= 64 rows runs on tcgen05 (linear_tc_kernel, bf16 hi/lo x3, fp32
+// A layer whose K is a multiple of 64 and that has >= 64 rows runs on wgmma (linear_tc_kernel, bf16 hi/lo x3, fp32
 // accumulate); the first layer of an SA stack (K = 3 + D, typically 6) is an FMA kernel -- it is not a tensor-core shape.
 #include <float.h>
 

@@ -1,5 +1,5 @@
 // cg_trunk_common.cuh -- device helpers shared by the fp32-SIMT trunk (engine 0) and the
-// tcgen05 trunk (engine 1): register-tiled fp32 layers over k-major shared-memory tiles, the
+// tensor-core trunk (engines 1-3): register-tiled fp32 layers over k-major shared-memory tiles, the
 // float64 pose inverse and cp.async wrappers.
 #pragma once
 #include "cg_net.cuh"

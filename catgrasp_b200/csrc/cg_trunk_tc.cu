@@ -1,73 +1,56 @@
-// cg_trunk_tc.cu -- tcgen05 "trunk" kernel (engine 1): the fused per-point shared-MLP chain + max of
-// cg_trunk_simt.cu with every layer that is a genuine dense contraction on the 5th-gen tensor cores.
+// cg_trunk_tc.cu -- tensor-core "trunk" kernel (engines 1, 2, 3): the fused per-point shared-MLP chain + max of
+// cg_trunk_simt.cu with every layer that is a genuine dense contraction on Hopper's wgmma.
 //
-//   layer            UMMA (cta_group::1, kind::f16, bf16 x bf16 -> fp32 in TMEM)         epilogue
-//   6 -> 64          fp32 FMA (K = 6 is not a tensor-core shape; thread = point)          -> X1 | X2 tile
-//   64 -> 64 (L1)    D1[pt][ch]   = X1[pt][k]  . W1[ch][k]    M=128 N=64  K=64          bias/ReLU -> X2 tile
-//   64 -> 128 (L2)   D2[pt][ch]   = X2[pt][k]  . W2[ch][k]    M=128 N=128 K=64          bias/ReLU -> X3 tile
-//   128 -> 1024 (L3) D3[ch][pt]   = W3c[ch][k] . X3[pt][k]    M=128 N=128 K=128, x8 chunks  bias/ReLU/max over points
+//   layer            wgmma (m64nNk16, fp32 accumulators in registers)                          epilogue
+//   6 -> 64          fp32 FMA (K = 6 is not a tensor-core shape), computed in the A-fragment layout -> X1
+//   64 -> 64 (L1)    D1[pt][ch] = X1[pt][k] (registers) . W1[ch][k] (smem)   bf16 hi/lo x3, N = 64    bias/ReLU -> X2
+//   64 -> 128 (L2)   D2[pt][ch] = X2[pt][k] (registers) . W2[ch][k] (smem)   bf16 hi/lo x3, N = 128   bias/ReLU -> X3
+//   128 -> 1024 (L3) D3[pt][ch] = X3[pt][k] (registers) . W3[ch][k] (smem ring), 8 chunks of 128   max over points
 //
-// L1/L2 put points on TMEM lanes, so a thread owns one point's channel row and writes it straight into the
-// next layer's K-major operand tile with 16-byte stores; L3 puts channels on lanes, so the max over the
-// tile's points is a per-thread reduction over TMEM columns and the N x 1024 activation never leaves the SM.
+// The accumulator fragment of one layer is the A-operand fragment of the next (cg_tc_ptx.cuh), so the activations of a
+// tile never touch shared memory: shared memory holds only the resident W1 / W2 and a ring through which a producer
+// warp streams W3 with cp.async.bulk, completion counted on mbarriers.
 //
-// Precision (SURVEY.md 7.3 #1): scores must stay within 1e-4 of the fp32 reference, which rules out a single
-// bf16 pass.  Every operand is split x = hi + lo (hi = bf16(x), lo = bf16(x - hi)) and each product is
-// accumulated as lo*hi + hi*lo + hi*hi in the fp32 accumulator (three UMMAs per K-step, lo*lo ~ 2^-16 dropped).
+// Precision of L3 (PASSES, the template parameter; L1 / L2 are always near-fp32):
+//   3 (engine 1)  W3 and X3 split x = hi + lo in bf16, products lo*hi + hi*lo + hi*hi (lo*lo ~ 2^-16 dropped): near-fp32
+//   2 (engine 2)  W3 one fp16 term, X3 fp16 hi + lo
+//   1 (engine 3)  W3 and X3 one fp16 term each.  X3 values above the fp16 range are clamped to 65504 AND reported
+//                 through cg_trunk_args::ovf_flag so that the host can re-run on engine 1.
 //
-// Operand tiles use the canonical UMMA K-major SWIZZLE_128B layout (64 bf16 = one 128-byte row per M/N index,
-// 8-row / 1024-byte swizzle atoms, 16-byte chunk index XOR (row & 7)).  Weights are pre-arranged in that image
-// on the host, so they arrive with plain 1-D bulk copies (cp.async.bulk -> UBLKCP) completing on mbarriers:
-// W1/W2 once per CTA, W3 as a stream of 16 KB pieces through a 4-slot ring filled by a dedicated producer warp.
-//
-// Warp roles (448 threads, 1 CTA / SM):  warps 0-7 "front" (6->64 FMA layer, L1/L2 epilogues, thread = point),
-// warps 8-11 "max" (L3 epilogue, thread = channel), warp 12 W3 producer, warp 13 UMMA issuer.  All hand-overs
-// are mbarriers, so the front layers of tile t+1 (FMA + L1 + L2 UMMAs) run in the shadow of tile t's L3 stream;
-// only the L2 epilogue (TMEM -> X3) has to wait for the previous tile's last UMMA.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
+// CTA = 288 threads, 1 per SM: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the
+// whole layer chain for its points) and one producer warp.  The two warpgroups are independent except for the shared
+// W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core work.
 #include <stdlib.h>
 
+#include "cg_tc_ptx.cuh"
 #include "cg_trunk_common.cuh"
 
 namespace {
 using namespace cg_trunk;
+using namespace cg_ptx;
 
-constexpr int NFRONT = 8;                  // front warps 0..7  : thread = (point, channel half); L0 + L1/L2 epilogues
-constexpr int NMAXW = 4;                   // max warps   8..11 : thread = channel; L3 max-epilogue
-constexpr int PROD_WARP = NFRONT + NMAXW;  // warp 12: W3 ring producer
-constexpr int MMA_WARP = PROD_WARP + 1;    // warp 13: UMMA issuer
-constexpr int NTC = (MMA_WARP + 1) * 32;   // 448 threads
-constexpr int NFT = NFRONT * 32;           // 256 front threads
-constexpr uint32_t PIECE = 16384;          // [128 rows x 64 bf16] one swizzled K-block
-// Shared-memory map (multiples of the 16 KB piece).  TS = false: the L3 input tile X3 lives in shared memory
-// (SS-mode UMMA) and the W3 ring has 4 slots.  TS = true: X3 lives in TMEM as the A operand (TS-mode UMMA), which
-// halves the L3 operand traffic on the shared-memory port and frees 64 KB for an 8-slot ring.
-constexpr uint32_t XA_OFF = 0;             // [hi|lo] 32 KB: X1 (L1 input), then X2 (L2 input) of the same tile
-constexpr uint32_t W1_OFF = 2 * PIECE;     // [hi|lo][64 rows x 128 B] 16 KB
-constexpr uint32_t W2_OFF = 3 * PIECE;     // [hi|lo][128 rows x 128 B] 32 KB
-constexpr uint32_t X3_OFF = 5 * PIECE;     // SS only: [hi|lo][kb0|kb1] 64 KB
-template <bool TS> struct Lay {
-  static constexpr int NSLOT = TS ? 8 : 4;
-  static constexpr int SLOT_SHIFT = TS ? 3 : 2;
-  static constexpr uint32_t RING_OFF = TS ? 5 * PIECE : 9 * PIECE;
-  static constexpr uint32_t MISC_OFF = 13 * PIECE;          // 208 KB in both variants
-  // TMEM columns: D3 x2 at 0 / 128;  SS: D1 256, D2 320;  TS: D2 256 (D1 aliases it), X3 hi 384, X3 lo 448
-  // SS: D1 256, D2 320.  TS: two 128-column activation buffers XB(it) = 256 + (it & 1) * 128; D1 and D2 of tile `it`
-  // land in XB(it) and the L2 epilogue converts D2 in place into X3 hi (64 cols) | X3 lo (64 cols), so the L3 input
-  // tile is double-buffered without extra columns and tile t+1's front layers never wait for tile t's L3 stream.
-  static constexpr uint32_t D1_COL = 256, D2_COL = TS ? 256 : 320;
-  static __host__ __device__ constexpr uint32_t xb(int it) { return TS ? 256u + (uint32_t)(it & 1) * 128u : 0u; }
-};
+constexpr int NCW = 8;                      // consumer warps (two warpgroups)
+constexpr int PROD_WARP = NCW;              // warp 8: W1 / W2 / W3 producer
+constexpr int NTC = (NCW + 1) * 32;         // 288 threads
+constexpr int NCHUNK = 8;                   // 1024 output channels / 128
+constexpr uint32_t PIECE = 16384;           // [128 rows x 64 x 16-bit] one swizzled K-block
+// shared-memory map
+constexpr uint32_t W1_OFF = 0;              // [hi 8 KB | lo 8 KB]: shared W1, or the per-candidate T64 operand
+constexpr uint32_t W2_OFF = PIECE;          // [hi 16 KB | lo 16 KB]
+constexpr uint32_t RING_OFF = 3 * PIECE;    // 128 KB of W3 slots (one slot = one 64-wide K-block of a 128-channel chunk)
+constexpr uint32_t RING_BYTES = 8 * PIECE;
+constexpr uint32_t SACC_OFF = RING_OFF + RING_BYTES;   // running max: float2 per (warpgroup, half-chunk, warp, lane)
+constexpr uint32_t SACC_BYTES = 2 * 2 * NCHUNK * 4 * 32 * 8;
+constexpr uint32_t MISC_OFF = SACC_OFF + SACC_BYTES;
 constexpr int NSLOT_MAX = 8;
-constexpr int NCHUNK = 8;                  // 1024 output channels / 128
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t W3_IMG = NCHUNK * 4 * PIECE, W2_IMG = 2 * PIECE, W1_IMG = PIECE;
-constexpr uint32_t W3H_OFF = W3_IMG + W2_IMG + W1_IMG;   // fp16 single-term image of W3 (2-pass engine)
-constexpr uint32_t W3H_IMG = NCHUNK * 2 * PIECE;
+// operand image built by cg_tc_prepare
+constexpr uint32_t IMG_W3B = NCHUNK * 2 * 2 * PIECE;   // bf16: [chunk][kb][hi 16 KB | lo 16 KB]
+constexpr uint32_t IMG_W2 = 2 * PIECE, IMG_W1 = PIECE;
+constexpr uint32_t IMG_W2_OFF = IMG_W3B, IMG_W1_OFF = IMG_W3B + IMG_W2;
+constexpr uint32_t IMG_W3H_OFF = IMG_W1_OFF + IMG_W1;  // fp16: [chunk][kb] 16 KB
+constexpr uint32_t IMG_W3H = NCHUNK * 2 * PIECE;
 
 struct Misc {
-  uint32_t gmax_s[1024];   // TS variant: running max per channel (order-preserving keys)
   float w0[6 * 64];
   float bias0[64];
   float bias1[64];
@@ -76,223 +59,28 @@ struct Misc {
   double mean[6];
   double sden[6];
   float T3[12];
-  unsigned long long full_bar[NSLOT_MAX]; // producer -> MMA : W3 piece landed in ring slot
-  unsigned long long free_bar[NSLOT_MAX];     // MMA -> producer : UMMAs reading the slot have completed
-  unsigned long long acc_bar[2];          // MMA -> max      : chunk accumulated into D3[buf]
-  unsigned long long accfree_bar[2];      // max -> MMA      : D3[buf] drained (one arrival per max warp)
-  unsigned long long x1_bar, x2_bar, x3_bar;   // front -> MMA : XA holds X1 / XA holds X2 / X3 written
-  unsigned long long l1_bar, l2_bar;      // MMA -> front    : D1 / D2 complete
-  unsigned long long tile_bar;            // MMA -> front    : every L3 UMMA of the tile completed (X3 reusable)
-  unsigned long long w_bar;               // resident W1/W2 images landed
-  uint32_t tmem_base;
+  unsigned long long full_bar[NSLOT_MAX];    // producer -> consumers: W3 slot landed
+  unsigned long long empty_bar[NSLOT_MAX];   // consumers -> producer: every consumer warp is done reading the slot
+  unsigned long long w_bar;                  // resident W1 / W2 landed
 };
 
-constexpr size_t SMEM_BYTES = 13 * PIECE + sizeof(Misc) + 1024;  // + slack for manual 1024-byte alignment
-static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_100");
+constexpr size_t SMEM_BYTES = MISC_OFF + sizeof(Misc);
+static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_90");
 
-// ------------------------------------------------------------------ PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void bar_front() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
+__device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B: start address (>>4), LBO = 1 (ignored for swizzled
-// K-major), SBO = 1024 B between 8-row groups, version = 1 (Blackwell), layout type 2 = SWIZZLE_128B.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor: D = f32 (bit 4), A = B = bf16 (bits 7, 10), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-constexpr uint32_t idesc(uint32_t M, uint32_t N, uint32_t a_fmt = 1u, uint32_t b_fmt = 1u) {   // fmt: 0 = f16, 1 = bf16
-  return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t id, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(id), "r"(accumulate)
-      : "memory");
-}
-// true in exactly one (converged-warp) lane; the compiler treats the guarded region as single-threaded, so
-// warp-uniform operands stay in uniform registers instead of going through per-lane R2UR broadcast loops
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-// TS mode: A operand read from TMEM (lane = M row, 32-bit column = two consecutive K elements), B from shared memory
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t id, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(id), "r"(accumulate)
-      : "memory");
-}
-// 32 registers per thread -> 32 lanes x 32 consecutive 32-bit TMEM columns (thread t <-> lane base + t)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t *r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Column-wise max over the 32 lanes of a warp for 32 columns: one warp-wide fp32 max reduction per column
-// (redux.sync.max.f32 -> CREDUX.MAX.F32 into a uniform register); thread t keeps the result of column t.
-__device__ __forceinline__ float warp_colmax32(const float *v, int lane) {
-  float mine = 0.f;
-#pragma unroll
-  for (int i = 0; i < 32; i++) {
-    float r;
-    asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v[i]));
-    mine = (lane == i) ? r : mine;
-  }
-  return mine;
-}
-
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns of TMEM -> 32 registers per thread (thread t <-> lane base + t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-
-// byte offset of the 16-byte chunk `c16` (8 bf16) of row `row` inside one swizzled [rows x 64] K-block
-__host__ __device__ __forceinline__ uint32_t row_chunk_off(int row, int c16) {
-  return (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u + (uint32_t)((c16 ^ (row & 7)) << 4);
-}
-
-// pack 8 fp32 values into 4+4 words of bf16 (or fp16) hi / lo pairs, two values per conversion instruction
-template <bool FP16>
-__device__ __forceinline__ void pack_hilo8(const float *v, uint32_t *h, uint32_t *l) {
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    if (FP16) {
-      const float a0 = fminf(v[2 * j], 65504.f), a1 = fminf(v[2 * j + 1], 65504.f);   // inputs are post-ReLU (>= 0)
-      const __half2 hh = __floats2half2_rn(a0, a1);
-      const float2 hf = __half22float2(hh);
-      const __half2 ll = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-      h[j] = *reinterpret_cast<const uint32_t *>(&hh);
-      l[j] = *reinterpret_cast<const uint32_t *>(&ll);
-    } else {
-      const __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-      const uint32_t hb = *reinterpret_cast<const uint32_t *>(&hh);
-      const float h0 = __uint_as_float(hb << 16), h1 = __uint_as_float(hb & 0xffff0000u);
-      const __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * j] - h0, v[2 * j + 1] - h1);
-      h[j] = hb;
-      l[j] = *reinterpret_cast<const uint32_t *>(&ll);
-    }
-  }
-}
-
-// fp16 flavour (2-pass engine: tcgen05 kind::f16 needs A and B in the same 16-bit format; mixing f16 x bf16 traps).
-// hi is clamped to the fp16 range so that an outlier saturates instead of turning into inf.
-__device__ __forceinline__ void store_hilo8_f16(unsigned char *hi_dst, unsigned char *lo_dst, const float *v) {
-  uint32_t h[4], l[4];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    const float a0 = fminf(v[2 * j], 65504.f), a1 = fminf(v[2 * j + 1], 65504.f);   // inputs are post-ReLU (>= 0)
-    const __half h0 = __float2half_rn(a0), h1 = __float2half_rn(a1);
-    const __half l0 = __float2half_rn(a0 - __half2float(h0)), l1 = __float2half_rn(a1 - __half2float(h1));
-    h[j] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-    l[j] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-  }
-  *reinterpret_cast<uint4 *>(hi_dst) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4 *>(lo_dst) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-// split 8 fp32 values into bf16 hi / lo and store them as the two 16-byte chunks of an operand row
-__device__ __forceinline__ void store_hilo8(unsigned char *hi_dst, unsigned char *lo_dst, const float *v) {
-  uint32_t h[4], l[4];
-  pack_hilo8<false>(v, h, l);
-  *reinterpret_cast<uint4 *>(hi_dst) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4 *>(lo_dst) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-// K = 64 layer: 4 K-steps x (x_lo*w_hi + x_hi*w_lo + x_hi*w_hi);  A = activations (M = 128 points), B = weights
-__device__ __forceinline__ void issue_k64(uint32_t d, uint32_t x_s, uint32_t x_part, uint32_t w_s, uint32_t w_part,
-                                          uint32_t id) {
-  uint32_t acc = 0u;
-#pragma unroll
-  for (int ks = 0; ks < 4; ks++) {
-    const uint32_t koff = (uint32_t)ks * 32u;
-    const uint64_t a_hi = umma_desc(x_s + koff), a_lo = umma_desc(x_s + x_part + koff);
-    const uint64_t b_hi = umma_desc(w_s + koff), b_lo = umma_desc(w_s + w_part + koff);
-    umma(d, a_lo, b_hi, id, acc);
-    umma(d, a_hi, b_lo, id, 1u);
-    umma(d, a_hi, b_hi, id, 1u);
-    acc = 1u;
-  }
-}
-
-// PASSES = 3: W3 = bf16 hi + lo, products lo*hi + hi*lo + hi*hi (near-fp32).
-// PASSES = 2: W3 = one fp16 term (11-bit mantissa, rounding error 2^-12 per weight), X3 = fp16 hi + lo.
-template <int PASSES, bool TS>
+template <int PASSES>
 __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a, int tiles_per_cta) {
-  constexpr int PPC = (PASSES == 3) ? 4 : 2;   // W3 ring pieces per 128-channel chunk
-  using L = Lay<TS>;
-  constexpr int NSLOT = L::NSLOT;
-  constexpr uint32_t D1_COL = L::D1_COL, D2_COL = L::D2_COL;
-  // no static shared memory in this kernel: the dynamic window starts 1024-byte aligned (checked); using the array
-  // directly keeps the accesses in the shared address space (LDS / STS / ATOMS, not generic LD / ST / ATOM)
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  unsigned char *smem = smem_dyn;
-  if ((static_cast<uint32_t>(__cvta_generic_to_shared(smem)) & 1023u) != 0u) __trap();
-  unsigned char *x3 = smem + X3_OFF, *xa = smem + XA_OFF, *w1 = smem + W1_OFF;
-  Misc &S = *reinterpret_cast<Misc *>(smem + L::MISC_OFF);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr int NSLOT = PASSES == 3 ? 4 : 8;
+  constexpr uint32_t SLOT_BYTES = PASSES == 3 ? 2 * PIECE : PIECE;
+  constexpr bool F16 = PASSES < 3;
+  // the operand tiles need 1024-byte alignment (SWIZZLE_128B atoms); the kernel has no static shared memory
+  extern __shared__ __align__(1024) unsigned char smem[];
+  if ((smem_u32(smem) & 1023u) != 0u) __trap();
+  Misc &S = *reinterpret_cast<Misc *>(smem + MISC_OFF);
+  float2 *sacc = reinterpret_cast<float2 *>(smem + SACC_OFF);
+  // warp index through a shuffle: the compiler then knows it is warp-uniform and the role branches are not divergent
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int b = blockIdx.y;
   const int N = a.N;
   const int ntiles = (N + TP - 1) / TP;
@@ -302,9 +90,13 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   const int my_tiles = tile_end - tile_begin;
   const unsigned char *img = static_cast<const unsigned char *>(a.tc_img);
   const bool has_l1 = a.stage1_mode != 0;
+  const uint32_t smem_s = smem_u32(smem);
+  const uint32_t w1_s = smem_s + W1_OFF, w2_s = smem_s + W2_OFF, ring_s = smem_s + RING_OFF;
+  const uint32_t misc_s = smem_s + MISC_OFF;
+  const uint32_t full_s = misc_s + (uint32_t)offsetof(Misc, full_bar), empty_s = misc_s + (uint32_t)offsetof(Misc, empty_bar);
+  const uint32_t wbar_s = misc_s + (uint32_t)offsetof(Misc, w_bar);
 
-  // ---- one-time setup: constants, mbarriers, TMEM, per-candidate T64 operand ---------------------------
-  for (int i = tid; i < 1024; i += NTC) S.gmax_s[i] = 0u;
+  // ---- one-time setup --------------------------------------------------------------------------------------
   for (int i = tid; i < 6 * 64; i += NTC) S.w0[i] = a.l0.Wt[i];
   if (tid < 64) {
     S.bias0[tid] = a.l0.b[tid];
@@ -319,12 +111,14 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
       S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: the hot loop multiplies
     }
   }
+  for (int i = tid; i < (int)(SACC_BYTES / 8); i += NTC) sacc[i] = make_float2(-INFINITY, -INFINITY);
   if (a.stage1_mode == 2) {
     // per-candidate feature transform as the B operand of L1:  B[j][k] = T64[k][j]   (pointnet2.py:257)
     const float *T = a.T64 + (size_t)b * 4096;
+    unsigned char *w1 = smem + W1_OFF;
     for (int idx = tid; idx < 4096; idx += NTC) {
       const int k = idx >> 6, j = idx & 63;
-      const float v = T[idx];
+      const float v = __ldg(T + idx);
       const __nv_bfloat16 h = __float2bfloat16_rn(v);
       const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
       const uint32_t off = row_chunk_off(j, k >> 3) + (uint32_t)(k & 7) * 2u;
@@ -335,410 +129,254 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   }
   if (tid == 0) {
     for (int i = 0; i < NSLOT; i++) {
-      mbar_init(smem_u32(&S.full_bar[i]), 1);
-      mbar_init(smem_u32(&S.free_bar[i]), 1);
+      mbar_init(full_s + 8u * i, 1);
+      mbar_init(empty_s + 8u * i, NCW);
     }
-    for (int i = 0; i < 2; i++) {
-      mbar_init(smem_u32(&S.acc_bar[i]), 1);
-      mbar_init(smem_u32(&S.accfree_bar[i]), NMAXW);
-    }
-    mbar_init(smem_u32(&S.x1_bar), 1);
-    mbar_init(smem_u32(&S.x2_bar), 1);
-    mbar_init(smem_u32(&S.x3_bar), 1);
-    mbar_init(smem_u32(&S.l1_bar), 1);
-    mbar_init(smem_u32(&S.l2_bar), 1);
-    mbar_init(smem_u32(&S.tile_bar), 1);
-    mbar_init(smem_u32(&S.w_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(wbar_s, 1);
+    mbar_init_fence();
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)),
-                 "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S.tmem_base;
-  const uint32_t x3_s = smem_u32(x3), xa_s = smem_u32(xa), w1_s = smem_u32(w1), w2_s = smem_u32(smem + W2_OFF);
-  const uint32_t ring_s = smem_u32(smem + L::RING_OFF);
 
   if (warp == PROD_WARP) {
-    // ======================= producer: stream W3 pieces through the ring =======================
-    // pieces travel in pairs (32 KB, adjacent in the image and in the ring): one mbarrier round trip per pair
-    constexpr int NPAIR = NSLOT / 2, PAIR_SHIFT = L::SLOT_SHIFT - 1;
-    const int total = my_tiles * NCHUNK * PPC / 2;
-    const unsigned char *w3src = img + (PASSES == 3 ? 0u : W3H_OFF);
-    for (int gp = 0; gp < total; gp++) {
-      const int d = gp & (NPAIR - 1);
-      mbar_wait(smem_u32(&S.free_bar[d]), (((uint32_t)gp >> PAIR_SHIFT) & 1u) ^ 1u);   // first round passes immediately
-      if (elect_one()) {
-        const uint32_t fb = smem_u32(&S.full_bar[d]);
-        if ((a.exp_flags & 1) && gp >= NPAIR) { mbar_arrive(fb); }
-        else {
-          mbar_expect_tx(fb, 2 * PIECE);
-          bulk_g2s(ring_s + (uint32_t)d * 2 * PIECE, w3src + (size_t)(gp & (NCHUNK * PPC / 2 - 1)) * 2 * PIECE, 2 * PIECE, fb);
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp == MMA_WARP) {
-    // ======================= UMMA issuer: the warp stays converged, one elected lane issues =======================
-    const uint32_t wb = smem_u32(&S.w_bar);   // resident weights: W2 (and the shared W1 of the STNkd trunk)
-    if (elect_one()) {
-      mbar_expect_tx(wb, W2_IMG + (a.stage1_mode == 1 ? W1_IMG : 0u));
-      bulk_g2s(w2_s, img + W3_IMG, PIECE, wb);
-      bulk_g2s(w2_s + PIECE, img + W3_IMG + PIECE, PIECE, wb);
-      if (a.stage1_mode == 1) bulk_g2s(w1_s, img + W3_IMG + W2_IMG, W1_IMG, wb);
-    }
-    __syncwarp();
-    mbar_wait(wb, 0u);
-    uint32_t g = 0;                       // consumed W3 pieces
-    uint32_t ph_x1 = 0u, ph_x2 = 0u;      // parities of the next x1 / x2 hand-over
-    long long t_all = clock64(), t_x3 = 0, t_full = 0, t_accf = 0, t_x12 = 0, tw;
-    const uint32_t l1b = smem_u32(&S.l1_bar), l2b = smem_u32(&S.l2_bar);
-    // front layers of the first tile
-    if (has_l1) {
-      mbar_wait(smem_u32(&S.x1_bar), ph_x1); ph_x1 ^= 1u;
-      tc_fence_after();
-      if (elect_one()) {
-        issue_k64(tmem_base + (TS ? L::xb(0) : D1_COL), xa_s, PIECE, w1_s, 8192u, idesc(128, 64));
-        umma_commit(l1b);
-      }
-      __syncwarp();
-    }
-    mbar_wait(smem_u32(&S.x2_bar), ph_x2); ph_x2 ^= 1u;
-    tc_fence_after();
-    if (elect_one()) {
-      issue_k64(tmem_base + (TS ? L::xb(0) : D2_COL), xa_s, PIECE, w2_s, PIECE, idesc(128, 128));
-      umma_commit(l2b);
-    }
-    __syncwarp();
-    for (int it = 0; it < my_tiles; it++) {
-      tw = clock64();
-      mbar_wait(smem_u32(&S.x3_bar), (uint32_t)it & 1u);
-      t_x3 += clock64() - tw;
-      const bool has_next = it + 1 < my_tiles;
-      for (int c = 0; c < NCHUNK; c++) {
-        const int buf = c & 1;
-        const uint32_t use = (uint32_t)it * 4u + (uint32_t)(c >> 1);   // earlier uses of this accumulator
-        tw = clock64();
-        if (use >= 1u) mbar_wait(smem_u32(&S.accfree_bar[buf]), (use - 1u) & 1u);
-        t_accf += clock64() - tw;
-        tc_fence_after();
-        const uint32_t d = tmem_base + (uint32_t)buf * 128u;
-        constexpr uint32_t id = (PASSES == 3) ? idesc(128, 128) : idesc(128, 128, 0u, 0u);   // bf16 x bf16 | f16 x f16
-#pragma unroll
-        for (int i = 0; i < PPC; i++) {    // 3-pass pieces: W3 hi kb0, hi kb1, lo kb0, lo kb1;  2-pass: W3 kb0, kb1
-          const int slot = g & (NSLOT - 1);
-          if ((i & 1) == 0) {   // pieces arrive in pairs
-            tw = clock64();
-            mbar_wait(smem_u32(&S.full_bar[slot >> 1]), (g >> L::SLOT_SHIFT) & 1u);
-            t_full += clock64() - tw;
-            tc_fence_after();
-          }
-          const uint32_t a_s = ring_s + (uint32_t)slot * PIECE;
-          const uint32_t kb = (uint32_t)(i & 1) * PIECE;
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < 4; ks++) {
-              const uint32_t koff = (uint32_t)ks * 32u;
-              const uint64_t wd = umma_desc(a_s + koff);     // W3 piece rows = 128 channels
-              const uint32_t first = (i | ks) ? 1u : 0u;
-              if (TS) {
-                // D3[pt][ch] = X3[pt][k] (TMEM) . W3[ch][k] (smem): K-step ks of K-block (i & 1) = 8 packed columns
-                const uint32_t xcol = (uint32_t)(i & 1) * 32u + (uint32_t)ks * 8u;
-                if (PASSES == 2 || i < 2) {
-                  umma_ts(d, tmem_base + L::xb(it) + 64u + xcol, wd, id, first);   // x_lo * w(_hi)
-                  umma_ts(d, tmem_base + L::xb(it) + xcol, wd, id, 1u);            // x_hi * w(_hi)
-                } else {
-                  umma_ts(d, tmem_base + L::xb(it) + xcol, wd, id, 1u);            // x_hi * w_lo
-                }
-              } else if (PASSES == 2 || i < 2) {
-                umma(d, wd, umma_desc(x3_s + 2 * PIECE + kb + koff), id, first);   // w(_hi) * x_lo
-                umma(d, wd, umma_desc(x3_s + kb + koff), id, 1u);                  // w(_hi) * x_hi
-              } else {
-                umma(d, wd, umma_desc(x3_s + kb + koff), id, 1u);                  // w_lo * x_hi
-              }
-            }
-            if (i & 1) umma_commit(smem_u32(&S.free_bar[slot >> 1]));
-            if (i == PPC - 1) {
-              umma_commit(smem_u32(&S.acc_bar[buf]));
-              if (c == NCHUNK - 1) umma_commit(smem_u32(&S.tile_bar));
-            }
-          }
-          __syncwarp();
-          g++;
-        }
-        // front layers of the NEXT tile run in the shadow of this tile's L3 stream
-        if (has_next && c == 1 && has_l1) {
-          tw = clock64();
-          mbar_wait(smem_u32(&S.x1_bar), ph_x1); ph_x1 ^= 1u;
-          t_x12 += clock64() - tw;
-          tc_fence_after();
-          if (elect_one()) {
-            issue_k64(tmem_base + (TS ? L::xb(it + 1) : D1_COL), xa_s, PIECE, w1_s, 8192u, idesc(128, 64));
-            umma_commit(l1b);
-          }
-          __syncwarp();
-        }
-        if (has_next && c == (has_l1 ? 3 : 1)) {
-          tw = clock64();
-          mbar_wait(smem_u32(&S.x2_bar), ph_x2); ph_x2 ^= 1u;
-          t_x12 += clock64() - tw;
-          tc_fence_after();
-          if (elect_one()) {
-            issue_k64(tmem_base + (TS ? L::xb(it + 1) : D2_COL), xa_s, PIECE, w2_s, PIECE, idesc(128, 128));
-            umma_commit(l2b);
-          }
-          __syncwarp();
-        }
+    // ======================= producer: resident W2 (+ shared W1), then W3 slot by slot =======================
+    if (lane == 0) {
+      mbar_expect_tx(wbar_s, IMG_W2 + (a.stage1_mode == 1 ? IMG_W1 : 0u));
+      bulk_g2s(w2_s, img + IMG_W2_OFF, IMG_W2, wbar_s);
+      if (a.stage1_mode == 1) bulk_g2s(w1_s, img + IMG_W1_OFF, IMG_W1, wbar_s);
+      const unsigned char *w3src = img + (PASSES == 3 ? 0u : IMG_W3H_OFF);
+      const int total = my_tiles * NCHUNK * 2;
+      for (int gs = 0; gs < total; gs++) {
+        const int s = gs % NSLOT;
+        mbar_wait(empty_s + 8u * s, (((uint32_t)(gs / NSLOT)) & 1u) ^ 1u);   // the first round passes immediately
+        mbar_expect_tx(full_s + 8u * s, SLOT_BYTES);
+        bulk_g2s(ring_s + (uint32_t)s * SLOT_BYTES, w3src + (size_t)(gs % (NCHUNK * 2)) * SLOT_BYTES, SLOT_BYTES,
+                 full_s + 8u * s);
       }
     }
-    if (a.dbg && lane == 0) {
-      unsigned long long *dd = a.dbg + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 8;
-      dd[0] = clock64() - t_all; dd[1] = t_x3; dd[2] = t_full; dd[3] = t_accf; dd[4] = t_x12; dd[5] = my_tiles;
-    }
-  } else if (warp >= NFRONT) {
-    // ======================= max warps: L3 epilogue =======================
-    const int q = warp & 3;
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    if (TS) {
-      // D3[pt][ch]: lanes = points.  Each warp folds its 32 points per channel with the exchange network, the four
-      // warps meet in the shared running max.
-      for (int it = 0; it < my_tiles; it++) {
-#pragma unroll 1
-        for (int c = 0; c < NCHUNK; c++) {
-          const int buf = c & 1;
-          const uint32_t use = (uint32_t)it * 4u + (uint32_t)(c >> 1);
-          mbar_wait(smem_u32(&S.acc_bar[buf]), use & 1u);
-          tc_fence_after();
-          const uint32_t taddr = tmem_base + lane_sel + (uint32_t)buf * 128u;
-          float r4[4] = {0.f, 0.f, 0.f, 0.f};
-          if (!(a.exp_flags & 2)) {
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            float v[32];
-            tmem_ld32(taddr + (uint32_t)j * 32u, v);
-            r4[j] = warp_colmax32(v, lane);
-          }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&S.accfree_bar[buf]));
-#pragma unroll
-          for (int j = 0; j < 4; j++) atomicMax(&S.gmax_s[c * 128 + j * 32 + lane], cg_f2key(r4[j]));
-        }
-      }
-      asm volatile("bar.sync 2, 128;" ::: "memory");   // all four max warps have folded their last chunk
-      for (int ch = tid - NFT; ch < 1024; ch += NMAXW * 32) {
-        float m = cg_key2f(S.gmax_s[ch]) + __ldg(&a.l3.b[ch]);   // bias is constant over points: add after the max
-        if (a.relu3) m = fmaxf(m, 0.f);
-        atomicMax(&a.gmax_keys[(size_t)b * 1024 + ch], cg_f2key(m));
-      }
-    } else {
-    // D3[ch][pt]: thread = output channel, the max over the tile's points is a per-thread reduction over columns
-    float run[NCHUNK];
-#pragma unroll
-    for (int c = 0; c < NCHUNK; c++) run[c] = -INFINITY;
-    for (int it = 0; it < my_tiles; it++) {
-#pragma unroll
-      for (int c = 0; c < NCHUNK; c++) {
-        const int buf = c & 1;
-        const uint32_t use = (uint32_t)it * 4u + (uint32_t)(c >> 1);
-        mbar_wait(smem_u32(&S.acc_bar[buf]), use & 1u);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + lane_sel + (uint32_t)buf * 128u;
-        float m = run[c];
-#pragma unroll
-        for (int j = 0; j < ((a.exp_flags & 2) ? 0 : 4); j++) {
-          float v[32];
-          tmem_ld32(taddr + (uint32_t)j * 32u, v);
-#pragma unroll
-          for (int i = 0; i < 32; i++) m = fmaxf(m, v[i]);
-        }
-        run[c] = m;
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&S.accfree_bar[buf]));
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < NCHUNK; c++) {
-      const int ch = c * 128 + q * 32 + lane;
-      float m = run[c] + __ldg(&a.l3.b[ch]);   // bias is constant over points: add after the max
-      if (a.relu3) m = fmaxf(m, 0.f);
-      atomicMax(&a.gmax_keys[(size_t)b * 1024 + ch], cg_f2key(m));
-    }
-    }
-  } else {
-    // ======================= front warps: thread = (point, channel half) =======================
-    const int p = tid & 127, half = tid >> 7;
-    const int q = warp & 3;                         // TMEM lane quadrant of this warp
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    // raw input row of this thread's point for the tile being prepared (prefetched one tile ahead so that the
-    // dependent global loads ids -> cloud row are off the critical path between two tiles)
-    double rx[6];
-    float rv[6];
-    auto prefetch = [&](int tile) {
-      int n = tile * TP + p;
-      if (n >= N) n = N - 1;   // duplicate a valid point: cannot change a max
-      if (a.in.x_direct) {
-        const float *xr = a.in.x_direct + ((size_t)b * N + n) * 6;
-#pragma unroll
-        for (int k = 0; k < 6; k++) rv[k] = xr[k];
-      } else {
-        const int id = a.in.ids ? a.in.ids[(size_t)b * N + n] : n;
-        const double *px = a.in.cloud_xyz + (size_t)id * 3;
-        const double *pn = a.in.cloud_nrm + (size_t)id * 3;
-        rx[0] = px[0]; rx[1] = px[1]; rx[2] = px[2]; rx[3] = pn[0]; rx[4] = pn[1]; rx[5] = pn[2];
-      }
-    };
-    // 6 -> 64 (+bias, ReLU) of the prefetched row -> this thread's 32-channel slice of the XA tile
-    auto layer0 = [&]() {
-      if (a.exp_flags & 4) { fence_proxy_async(); bar_front(); return; }
-      float v[6];
-      if (a.in.x_direct) {
-#pragma unroll
-        for (int k = 0; k < 6; k++) v[k] = rv[k];
-      } else {
-        const double x = rx[0], y = rx[1], z = rx[2];
-        const double nx = rx[3], ny = rx[4], nz = rx[5];
-        const double *R = S.pinv;
-        double w[6];
-        w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
-        w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
-        w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
-        w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
-        w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
-        w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
-#pragma unroll
-        for (int k = 0; k < 6; k++) v[k] = (float)((w[k] - S.mean[k]) * S.sden[k]);
-      }
-      if (a.T3) {  // xyz @ T3 (pointnet2.py:248), normals pass through (:245-250)
-        const float x = v[0], y = v[1], z = v[2];
-        v[0] = fmaf(z, S.T3[6], fmaf(y, S.T3[3], x * S.T3[0]));
-        v[1] = fmaf(z, S.T3[7], fmaf(y, S.T3[4], x * S.T3[1]));
-        v[2] = fmaf(z, S.T3[8], fmaf(y, S.T3[5], x * S.T3[2]));
-      }
-#pragma unroll
-      for (int cc = 0; cc < 4; cc++) {
-        const int c0 = half * 32 + cc * 8;
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) o[j] = 0.f;
-#pragma unroll
-        for (int k = 0; k < 6; k++) {
-          const float4 wa = *reinterpret_cast<const float4 *>(&S.w0[k * 64 + c0]);
-          const float4 wb = *reinterpret_cast<const float4 *>(&S.w0[k * 64 + c0 + 4]);
-          o[0] = fmaf(v[k], wa.x, o[0]); o[1] = fmaf(v[k], wa.y, o[1]); o[2] = fmaf(v[k], wa.z, o[2]); o[3] = fmaf(v[k], wa.w, o[3]);
-          o[4] = fmaf(v[k], wb.x, o[4]); o[5] = fmaf(v[k], wb.y, o[5]); o[6] = fmaf(v[k], wb.z, o[6]); o[7] = fmaf(v[k], wb.w, o[7]);
-        }
-#pragma unroll
-        for (int j = 0; j < 8; j++) o[j] = fmaxf(o[j] + S.bias0[c0 + j], 0.f);
-        const uint32_t off = row_chunk_off(p, c0 >> 3);
-        store_hilo8(xa + off, xa + PIECE + off, o);
-      }
-      fence_proxy_async();   // generic-proxy tile writes -> visible to the async proxy (UMMA operand reads)
-      bar_front();
-    };
-    // L1 epilogue of tile `tile` (local index it): D1 -> (bias, ReLU | nothing) -> XA as the L2 input
-    auto l1_epilogue = [&](int tile, int it) {
-      mbar_wait(smem_u32(&S.l1_bar), (uint32_t)it & 1u);
-      tc_fence_after();
-      if (a.exp_flags & 4) { tc_fence_before(); bar_front(); if (tid == 0) mbar_arrive(smem_u32(&S.x2_bar)); return; }
-      float v[32];
-      tmem_ld32(tmem_base + lane_sel + (TS ? L::xb(it) : D1_COL) + (uint32_t)half * 32u, v);
-      if (a.stage1_mode == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j] + S.bias1[half * 32 + j], 0.f);
-      }
-      if (a.pf_out) {   // PointNetSeg point feature (pointnet2.py:261)
-        const int n = tile * TP + p;
-        if (n < N) {
-          float4 *dstg = reinterpret_cast<float4 *>(a.pf_out + ((size_t)b * N + n) * 64 + half * 32);
-#pragma unroll
-          for (int j = 0; j < 8; j++) dstg[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-      }
-#pragma unroll
-      for (int cc = 0; cc < 4; cc++) {
-        const uint32_t off = row_chunk_off(p, half * 4 + cc);
-        store_hilo8(xa + off, xa + PIECE + off, v + cc * 8);
-      }
-      tc_fence_before();
-      fence_proxy_async();
-      bar_front();
-      if (tid == 0) mbar_arrive(smem_u32(&S.x2_bar));
-    };
-
-    // ---- prologue: front layers of the first tile ----
-    prefetch(tile_begin);
-    layer0();
-    if (tid == 0) mbar_arrive(smem_u32(has_l1 ? &S.x1_bar : &S.x2_bar));
-    if (my_tiles > 1) prefetch(tile_begin + 1);
-    if (has_l1) l1_epilogue(tile_begin, 0);
-
-    for (int it = 0; it < my_tiles; it++) {
-      const int tile = tile_begin + it;
-      const bool has_next = it + 1 < my_tiles;
-      // A. D2(tile) complete; its UMMAs no longer read XA
-      mbar_wait(smem_u32(&S.l2_bar), (uint32_t)it & 1u);
-      tc_fence_after();
-      // C. L2 epilogue: D2 -> bias, ReLU -> packed hi/lo in registers; the X3 stores wait until the previous tile's
-      //    L3 has let go of X3, so only 16 x st.shared.v4 sit between two tiles' L3 streams
-      uint32_t ph[2][4][4], pl[2][4][4];
-#pragma unroll
-      for (int j32 = 0; j32 < ((a.exp_flags & 4) ? 0 : 2); j32++) {
-        float v[32];
-        tmem_ld32(tmem_base + lane_sel + (TS ? L::xb(it) : D2_COL) + (uint32_t)half * 64u + (uint32_t)j32 * 32u, v);
-#pragma unroll
-        for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j] + S.bias2[half * 64 + j32 * 32 + j], 0.f);
-#pragma unroll
-        for (int cc = 0; cc < 4; cc++) pack_hilo8<PASSES == 2>(v + cc * 8, ph[j32][cc], pl[j32][cc]);
-      }
-      if (!TS && it >= 1) mbar_wait(smem_u32(&S.tile_bar), (uint32_t)(it - 1) & 1u);
-      if (a.exp_flags & 4) {
-      } else if (TS) {
-        // word j of this thread = channels (half*64 + 2j, +1) of its point = packed K column half*32 + j
-        // in-place conversion of XB(it): every front thread must have pulled its fp32 half-row out of D2 first
-        tc_fence_before();
-        bar_front();
-        tc_fence_after();
-        tmem_st32(tmem_base + lane_sel + L::xb(it) + (uint32_t)half * 32u, &ph[0][0][0]);
-        tmem_st32(tmem_base + lane_sel + L::xb(it) + 64u + (uint32_t)half * 32u, &pl[0][0][0]);
-        tmem_st_wait();
-      } else {
-#pragma unroll
-        for (int j32 = 0; j32 < 2; j32++)
-#pragma unroll
-          for (int cc = 0; cc < 4; cc++) {
-            // channel = half*64 + j32*32 + cc*8 ..  ->  K-block `half`, 16-byte chunk j32*4 + cc
-            const uint32_t off = (uint32_t)half * PIECE + row_chunk_off(p, j32 * 4 + cc);
-            *reinterpret_cast<uint4 *>(x3 + off) = make_uint4(ph[j32][cc][0], ph[j32][cc][1], ph[j32][cc][2], ph[j32][cc][3]);
-            *reinterpret_cast<uint4 *>(x3 + 2 * PIECE + off) = make_uint4(pl[j32][cc][0], pl[j32][cc][1], pl[j32][cc][2], pl[j32][cc][3]);
-          }
-        fence_proxy_async();
-      }
-      tc_fence_before();
-      bar_front();
-      if (tid == 0) mbar_arrive(smem_u32(&S.x3_bar));
-      // B. 6 -> 64 of the NEXT tile (inputs were prefetched a tile ago)
-      if (has_next) {
-        layer0();
-        if (tid == 0) mbar_arrive(smem_u32(has_l1 ? &S.x1_bar : &S.x2_bar));
-        if (it + 2 < my_tiles) prefetch(tile + 2);   // loads stay in flight across the waits below
-      }
-      // D. L1 epilogue of the next tile
-      if (has_next && has_l1) l1_epilogue(tile + 1, it + 1);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+  // ======================= consumer warpgroups =======================
+  const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, q = lane & 3;
+  float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU): reported if beyond the fp16 range
+  mbar_wait(wbar_s, 0u);
+
+  // input row (6 floats after pose transform / normalisation / T3) of point n of candidate b
+  auto load_row = [&](int n, float *v) {
+    if (n >= N) n = N - 1;   // duplicate a valid point: cannot change a max
+    if (a.in.x_direct) {
+      const float *xr = a.in.x_direct + ((size_t)b * N + n) * 6;
+#pragma unroll
+      for (int k = 0; k < 6; k++) v[k] = __ldg(xr + k);
+    } else {
+      const int id = a.in.ids ? __ldg(a.in.ids + (size_t)b * N + n) : n;
+      const double *px = a.in.cloud_xyz + (size_t)id * 3;
+      const double *pn = a.in.cloud_nrm + (size_t)id * 3;
+      const double x = __ldg(px), y = __ldg(px + 1), z = __ldg(px + 2);
+      const double nx = __ldg(pn), ny = __ldg(pn + 1), nz = __ldg(pn + 2);
+      const double *R = S.pinv;
+      double w[6];
+      w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
+      w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
+      w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
+      w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
+      w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
+      w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
+#pragma unroll
+      for (int k = 0; k < 6; k++) v[k] = (float)((w[k] - S.mean[k]) * S.sden[k]);
+    }
+    if (a.T3) {  // xyz @ T3 (pointnet2.py:248), normals pass through (:245-250)
+      const float x = v[0], y = v[1], z = v[2];
+      v[0] = fmaf(z, S.T3[6], fmaf(y, S.T3[3], x * S.T3[0]));
+      v[1] = fmaf(z, S.T3[7], fmaf(y, S.T3[4], x * S.T3[1]));
+      v[2] = fmaf(z, S.T3[8], fmaf(y, S.T3[5], x * S.T3[2]));
+    }
+  };
+
+  uint32_t gslot = 0;   // W3 slots consumed so far
+  for (int it = 0; it < my_tiles; it++) {
+    const int tile = tile_begin + it;
+    const int p0 = tile * TP + wg * 64 + w4 * 16 + g;   // this thread's rows: points p0 and p0 + 8
+    // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
+    float d64[32];
+    {
+      float v0[6], v1[6];
+      load_row(p0, v0);
+      load_row(p0 + 8, v1);
+#pragma unroll
+      for (int m = 0; m < 8; m++)
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const int c = 8 * m + 2 * q + e;
+          float o0 = S.bias0[c], o1 = o0;
+#pragma unroll
+          for (int k = 0; k < 6; k++) {
+            const float w = S.w0[k * 64 + c];
+            o0 = fmaf(v0[k], w, o0);
+            o1 = fmaf(v1[k], w, o1);
+          }
+          d64[4 * m + e] = fmaxf(o0, 0.f);
+          d64[4 * m + 2 + e] = fmaxf(o1, 0.f);
+        }
+    }
+    uint32_t xh[8][4], xl[8][4];   // A fragments of the current layer input (up to K = 128), bf16 / fp16 hi + lo
+    // ---- L1: 64 -> 64 (STNkd shared conv, or the per-candidate T64 feature transform) ----
+    if (has_l1) {
+      d_to_a<4, false>(d64, xh, xl);
+      wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ks++) {
+        const uint64_t bh = wg_desc(w1_s + 32u * ks), bl = wg_desc(w1_s + 8192u + 32u * ks);
+        wg_m64n64<false>(d64, xl[ks], bh, ks > 0 ? 1u : 0u);
+        wg_m64n64<false>(d64, xh[ks], bl, 1u);
+        wg_m64n64<false>(d64, xh[ks], bh, 1u);
+      }
+      wg_commit();
+      wg_wait<0>();
+#pragma unroll
+      for (int i = 0; i < 32; i++) {
+        if (a.stage1_mode == 1) d64[i] = fmaxf(d64[i] + S.bias1[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
+      }
+      if (a.pf_out) {   // PointNetSeg point feature (pointnet2.py:261)
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+          const int n = p0 + 8 * r;
+          if (n < N) {
+            float *dst = a.pf_out + ((size_t)b * N + n) * 64 + 2 * q;
+#pragma unroll
+            for (int m = 0; m < 8; m++)
+              *reinterpret_cast<float2 *>(dst + 8 * m) = make_float2(d64[4 * m + 2 * r], d64[4 * m + 2 * r + 1]);
+          }
+        }
+      }
+    }
+    // ---- L2: 64 -> 128 ----
+    float acc[64];
+    d_to_a<4, false>(d64, xh, xl);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ks++) {
+      const uint64_t bh = wg_desc(w2_s + 32u * ks), bl = wg_desc(w2_s + PIECE + 32u * ks);
+      wg_m64n128<false>(acc, xl[ks], bh, ks > 0 ? 1u : 0u);
+      wg_m64n128<false>(acc, xh[ks], bl, 1u);
+      wg_m64n128<false>(acc, xh[ks], bh, 1u);
+    }
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = fmaxf(acc[i] + S.bias2[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
+    if (PASSES == 1) {
+#pragma unroll
+      for (int j = 0; j < 8; j++)
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+          const float x0 = acc[8 * j + 2 * r], x1 = acc[8 * j + 2 * r + 1];
+          vmax = fmaxf(vmax, fmaxf(x0, x1));
+          // values beyond the fp16 range saturate to 65504 instead of becoming inf (x0 -> low half)
+          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(xh[j][r]) : "f"(x1), "f"(x0));
+        }
+    } else {
+      d_to_a<8, F16>(acc, xh, xl);
+    }
+    // ---- L3: 128 -> 1024 in 16 half-chunks of 64 channels; max over the tile's points ----
+    // Two 32-register accumulators: half-chunk h + 1 is issued before half-chunk h is reduced, so the reduction
+    // overlaps the tensor cores.  Half-chunk h = channels 64h .. 64h+63 = rows 64 (h & 1) .. of chunk h / 2's W3 slots.
+    auto issue = [&](int h, float *d) {
+      const int c = h >> 1;
+      wg_fence();
+#pragma unroll
+      for (int kb = 0; kb < 2; kb++) {
+        const uint32_t gs = gslot + 2u * c + kb;
+        const uint32_t s = gs % NSLOT;
+        if ((h & 1) == 0) mbar_wait(full_s + 8u * s, (gs / NSLOT) & 1u);
+        const uint32_t ws = ring_s + s * SLOT_BYTES + (uint32_t)(h & 1) * (PIECE / 2);
+#pragma unroll
+        for (int ks = 0; ks < 4; ks++) {
+          const int j = kb * 4 + ks;
+          const uint32_t first = (kb | ks) ? 1u : 0u;
+          const uint64_t bw = wg_desc(ws + 32u * ks);
+          if (PASSES == 3) {
+            const uint64_t bl = wg_desc(ws + PIECE + 32u * ks);
+            wg_m64n64<false>(d, xl[j], bw, first);   // x_lo * w_hi
+            wg_m64n64<false>(d, xh[j], bl, 1u);      // x_hi * w_lo
+            wg_m64n64<false>(d, xh[j], bw, 1u);      // x_hi * w_hi
+          } else if (PASSES == 2) {
+            wg_m64n64<true>(d, xl[j], bw, first);
+            wg_m64n64<true>(d, xh[j], bw, 1u);
+          } else {
+            wg_m64n64<true>(d, xh[j], bw, first);
+          }
+        }
+      }
+      wg_commit();
+    };
+    // half-chunk h is complete in this warp: fold its column max into the running max; after the second half of a
+    // chunk hand the chunk's two W3 slots back
+    auto reduce = [&](int h, const float *d) {
+      const int c = h >> 1;
+      if (h & 1) {
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(empty_s + 8u * ((gslot + 2u * c) % NSLOT));
+          mbar_arrive(empty_s + 8u * ((gslot + 2u * c + 1u) % NSLOT));
+        }
+      }
+      // column max over this warp's 16 rows: own two rows, then a transposing butterfly over lane bits 4, 3, 2
+      // (each step halves the columns a thread is responsible for).  Afterwards thread (g, q) holds the columns
+      // 8g + 2q + {0, 1} of the half-chunk.
+      float x[16];
+#pragma unroll
+      for (int i = 0; i < 8; i++) {
+        x[2 * i] = fmaxf(d[4 * i], d[4 * i + 2]);
+        x[2 * i + 1] = fmaxf(d[4 * i + 1], d[4 * i + 3]);
+      }
+#pragma unroll
+      for (int step = 16; step >= 4; step >>= 1) {
+        const bool up = (lane & step) != 0;
+#pragma unroll
+        for (int k = 0; k < step / 2; k++) {
+          const float send = up ? x[k] : x[k + step / 2];
+          const float keep = up ? x[k + step / 2] : x[k];
+          x[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, step));
+        }
+      }
+      float2 &slot = sacc[((wg * 2 * NCHUNK + h) * 4 + w4) * 32 + lane];   // private to this thread
+      const float2 old = slot;
+      slot = make_float2(fmaxf(old.x, x[0]), fmaxf(old.y, x[1]));
+    };
+    float da[32], db[32];   // even / odd half-chunks
+    issue(0, da);
+#pragma unroll 1
+    for (int h = 0; h < 2 * NCHUNK; h += 2) {
+      issue(h + 1, db);
+      wg_wait<1>();
+      reduce(h, da);
+      if (h + 2 < 2 * NCHUNK) {
+        issue(h + 2, da);
+        wg_wait<1>();
+      } else {
+        wg_wait<0>();
+      }
+      reduce(h + 1, db);
+    }
+    gslot += 2u * NCHUNK;
+  }
+  if (PASSES == 1 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
+
+  // ---- fold the eight warps' running maxima of every channel into the global feature ----
+  bar_consumers();
+  for (int ch = tid; ch < 1024; ch += NCW * 32) {
+    const int h = ch >> 6, col = ch & 63;
+    const int ln = 4 * (col >> 3) + ((col & 7) >> 1), k = col & 1;
+    float m = -INFINITY;
+#pragma unroll
+    for (int w = 0; w < 8; w++) {
+      const float *sv = reinterpret_cast<const float *>(&sacc[(((w >> 2) * 2 * NCHUNK + h) * 4 + (w & 3)) * 32 + ln]);
+      m = fmaxf(m, sv[k]);
+    }
+    m += __ldg(&a.l3.b[ch]);   // bias is constant over points: add after the max
+    if (a.relu3) m = fmaxf(m, 0.f);
+    atomicMax(&a.gmax_keys[(size_t)b * 1024 + ch], cg_f2key(m));
   }
 }
 
@@ -756,42 +394,43 @@ float bf16_to_f(unsigned short h) {
   return f;
 }
 
-// B-operand / A-operand image of a folded layer: rows = output channels [c0, c0+rows), K-major, nkb K-blocks of 64,
-// layout [hi|lo][kb][rows x 128 B swizzled].  Wt is [K][C] (k-major rows, as in the weight blob).
-void pack_image(const float *Wt, int C, int c0, int rows, int nkb, unsigned char *dst) {
-  const size_t kb_bytes = (size_t)rows * 128, part_bytes = kb_bytes * nkb;
+// One [rows x 64] K-block (k0 .. k0+63) of a folded layer as bf16 hi / lo swizzled images; rows = output channels
+// c0 .. c0+rows-1.  Wt is [K][C] (k-major rows, as in the weight blob).
+void pack_block(const float *Wt, int C, int c0, int rows, int k0, unsigned char *hi, unsigned char *lo) {
   for (int r = 0; r < rows; r++)
-    for (int k = 0; k < nkb * 64; k++) {
-      const float w = Wt[(size_t)k * C + c0 + r];
-      const unsigned short hi = bf16_rne(w);
-      const unsigned short lo = bf16_rne(w - bf16_to_f(hi));
-      const size_t off = (size_t)(k >> 6) * kb_bytes + row_chunk_off(r, (k & 63) >> 3) + (size_t)(k & 7) * 2;
-      memcpy(dst + off, &hi, 2);
-      memcpy(dst + part_bytes + off, &lo, 2);
+    for (int kk = 0; kk < 64; kk++) {
+      const float w = Wt[(size_t)(k0 + kk) * C + c0 + r];
+      const unsigned short h = bf16_rne(w), l = bf16_rne(w - bf16_to_f(h));
+      const size_t off = row_chunk_off(r, kk >> 3) + (size_t)(kk & 7) * 2;
+      memcpy(hi + off, &h, 2);
+      memcpy(lo + off, &l, 2);
     }
 }
 
 }  // namespace
 
-size_t cg_tc_image_bytes() { return (size_t)W3_IMG + W2_IMG + W1_IMG + W3H_IMG; }
+size_t cg_tc_image_bytes() { return (size_t)IMG_W3H_OFF + IMG_W3H; }
 
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok) {
   float wmax = 0.f;
   for (size_t i = 0; i < (size_t)128 * 1024; i++) wmax = fmaxf(wmax, fabsf(Wt3[i]));
   *f16_ok = (wmax < 65504.f) ? 1 : 0;   // otherwise the fp16 image would hold infinities
   std::vector<unsigned char> img(cg_tc_image_bytes(), 0);
-  // W3: per 128-channel chunk one 64 KB tile whose four 16 KB pieces are [hi kb0][hi kb1][lo kb0][lo kb1]
-  for (int ch = 0; ch < NCHUNK; ch++) pack_image(Wt3, 1024, ch * 128, 128, 2, img.data() + (size_t)ch * 4 * PIECE);
-  pack_image(Wt2, 128, 0, 128, 1, img.data() + W3_IMG);            // [hi 16 KB][lo 16 KB]
-  if (Wt1) pack_image(Wt1, 64, 0, 64, 1, img.data() + W3_IMG + W2_IMG);   // [hi 8 KB][lo 8 KB]
-  // fp16 single-term W3 for the 2-pass engine: per chunk [kb0 16 KB][kb1 16 KB]
+  for (int ch = 0; ch < NCHUNK; ch++)
+    for (int kb = 0; kb < 2; kb++) {
+      unsigned char *hi = img.data() + (size_t)(ch * 2 + kb) * 2 * PIECE;
+      pack_block(Wt3, 1024, ch * 128, 128, kb * 64, hi, hi + PIECE);
+    }
+  pack_block(Wt2, 128, 0, 128, 0, img.data() + IMG_W2_OFF, img.data() + IMG_W2_OFF + PIECE);
+  if (Wt1) pack_block(Wt1, 64, 0, 64, 0, img.data() + IMG_W1_OFF, img.data() + IMG_W1_OFF + 8192);
+  // fp16 single-term W3 for the fp16 engines: [chunk][kb] 16 KB
   for (int ch = 0; ch < NCHUNK; ch++)
     for (int r = 0; r < 128; r++)
       for (int k = 0; k < 128; k++) {
         const __half h = __float2half_rn(Wt3[(size_t)k * 1024 + ch * 128 + r]);
         unsigned short bits;
         memcpy(&bits, &h, 2);
-        const size_t off = (size_t)W3H_OFF + (size_t)ch * 2 * PIECE + (size_t)(k >> 6) * PIECE + row_chunk_off(r, (k & 63) >> 3) +
+        const size_t off = (size_t)IMG_W3H_OFF + (size_t)(ch * 2 + (k >> 6)) * PIECE + row_chunk_off(r, (k & 63) >> 3) +
                            (size_t)(k & 7) * 2;
         memcpy(img.data() + off, &bits, 2);
       }
@@ -806,60 +445,22 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
   CG_REQUIRE(ctx, a.tc_img != nullptr, "trunk: tensor-core weight image missing");
   static bool attr_set[CG_MAX_DEVICES] = {};   // the attribute is per device
   if (!attr_set[ctx->device]) {
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
     attr_set[ctx->device] = true;
   }
+  // split a candidate's tiles over CTAs only while there are fewer than ~4 CTAs per SM
   const int ntiles = (a.N + TP - 1) / TP;
   int splits = 1;
   while ((long)a.B * splits < 4L * ctx->num_sms && splits < ntiles) splits *= 2;
   const int tiles_per_cta = (ntiles + splits - 1) / splits;
   dim3 grid((ntiles + tiles_per_cta - 1) / tiles_per_cta, a.B);
-  const bool two_pass = ctx->engine >= 2 && a.tc_f16_ok;
-#ifdef CG_EXPERIMENTS   // timing experiments (results become wrong): never read from the environment in a release build
-  static const bool ts_mode = getenv("CG_TRUNK_SS") == nullptr;   // A operand of L3 from TMEM unless CG_TRUNK_SS is set
-  static const int exp_flags = getenv("CG_TRUNK_EXP") ? atoi(getenv("CG_TRUNK_EXP")) : 0;
-  static const bool debug = getenv("CG_TRUNK_DEBUG") != nullptr;
-#else
-  constexpr bool ts_mode = true;
-  constexpr int exp_flags = 0;
-  constexpr bool debug = false;
-#endif
-  auto launch = [&](const cg_trunk_args &a0) {
-    cg_trunk_args aa = a0;
-    aa.exp_flags = exp_flags;
-    if (two_pass) {
-      if (ts_mode) trunk_tc_kernel<2, true><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(aa, tiles_per_cta);
-      else trunk_tc_kernel<2, false><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(aa, tiles_per_cta);
-    } else {
-      if (ts_mode) trunk_tc_kernel<3, true><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(aa, tiles_per_cta);
-      else trunk_tc_kernel<3, false><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(aa, tiles_per_cta);
-    }
-  };
-  if (debug) {
-    cg_trunk_args ad = a;
-    const size_t n = (size_t)grid.x * grid.y;
-    unsigned long long *d_dbg = nullptr;
-    CG_CUDA(ctx, cudaMalloc(&d_dbg, n * 64));
-    CG_CUDA(ctx, cudaMemsetAsync(d_dbg, 0, n * 64, ctx->stream));
-    ad.dbg = d_dbg;
-    launch(ad);
-    CG_LAUNCH_CHECK(ctx);
-    std::vector<unsigned long long> h(n * 8);
-    CG_CUDA(ctx, cudaMemcpyAsync(h.data(), d_dbg, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
-    CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(d_dbg);
-    double s[6] = {0, 0, 0, 0, 0, 0};
-    for (size_t i = 0; i < n; i++)
-      for (int k = 0; k < 6; k++) s[k] += (double)h[i * 8 + k];
-    const double tiles = s[5] > 0 ? s[5] : 1;
-    fprintf(stderr, "[trunk_tc dbg] CTAs=%zu tiles=%.0f  MMA thread per tile: total %.0f  x3-wait %.0f  x1/x2-wait %.0f  full-wait %.0f  accfree-wait %.0f cycles\n",
-            n, tiles, s[0] / tiles, s[1] / tiles, s[4] / tiles, s[2] / tiles, s[3] / tiles);
-    return CG_OK;
-  }
-  launch(a);
+  // W3 beyond the fp16 range: the fp16 engines fall back to the 3-pass bf16 kernel
+  const int passes = !a.tc_f16_ok || ctx->engine == 1 ? 3 : (ctx->engine == 2 ? 2 : 1);
+  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
+  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
+  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
 }

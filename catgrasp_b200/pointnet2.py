@@ -1,6 +1,6 @@
 """PointNet++ sampling/grouping primitives and the PointNet models, with the
 names and call signatures of the reference's ``pointnet2.py`` (file:line cited
-per function), executing on B200 through libcatgrasp_b200.so.
+per function), executing on H100 through libcatgrasp_b200.so.
 
 All tensors are CUDA tensors; indices are returned as int64 like the reference.
 """

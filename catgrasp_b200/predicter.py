@@ -113,7 +113,7 @@ class GraspPredicter:
         self.class_name = class_name
         self.cfg = _load_artifacts(artifact_dir, "config_grasp.yml")
         n_out = len(self.cfg["classes"]) - 1
-        assert self.cfg["input_channel"] == 6, "the B200 path implements the shipped 6-channel input"
+        assert self.cfg["input_channel"] == 6, "the H100 path implements the shipped 6-channel input"
         sd = load_checkpoint(f"{artifact_dir}/best_val.pth.tar")
         print("Load ckpt from {}/best_val.pth.tar".format(artifact_dir))
         self.model = PointNetCls(sd, device=device)
@@ -267,7 +267,7 @@ class GraspPredicter:
             probs = None if shard is not None else d_probs.cpu().numpy()
             if net.ctx.get_engine() >= 2 and net.ctx.fp16_overflow():
                 # the fast engines clamp the 128->1024 layer's inputs to the fp16 range: redo on the near-fp32 engine
-                print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (tcgen05 bf16 hi/lo x3)")
+                print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (wgmma bf16 hi/lo x3)")
                 eng = net.ctx.get_engine()
                 net.ctx.set_engine(1)
                 try:

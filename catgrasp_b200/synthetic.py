@@ -103,7 +103,7 @@ _LATTICE_HINGES = LATTICE_LEVELS + 2
 def make_lattice_seg_state_dict(seed=0, mean=None, std=None, bins=100, beta=10.0, module_prefix=True, as_torch=True):
     """A PointNetSeg state_dict that *reads the NUNOCS bins off the input*: for a cloud whose min/max-normalised
     coordinates (augmentations.py:70-75) sit on the lattice {0, 0.04, ..., 1.0}, bin min(4*g, 99) wins with a logit gap of
-    ``beta``, so every implementation (fp32 CPU, tcgen05 split precision) yields the same NOCS cloud and the full
+    ``beta``, so every implementation (fp32 CPU, tensor-core split precision) yields the same NOCS cloud and the full
     ``NunocsPredicter.predict`` success path (predicter.py:135-203) can be compared end to end.
 
     All other weights and every BatchNorm statistic stay as random as in :func:`make_state_dict`; the hand-set

@@ -1,5 +1,5 @@
 /*
- * catgrasp_b200.h -- C ABI of libcatgrasp_b200.so (sm_100a).
+ * catgrasp_b200.h -- C ABI of libcatgrasp_b200.so (sm_90a, H100).
  *
  * This is the drop-in boundary for CaTGrasp's per-scene grasp-scoring hot
  * path.  Every entry point is `extern "C"`, takes plain pointers and sizes,
@@ -54,11 +54,12 @@ int64_t     cg_ctx_launch_count(cg_ctx *ctx);
 void        cg_ctx_reset_launch_count(cg_ctx *ctx);
 /* GEMM engine of the fused shared-MLP "trunk":
  *   0 = fp32 SIMT (exact-order reference engine)
- *   1 = tcgen05, bf16 hi/lo x hi/lo, 3 passes (near-fp32: |dprob| ~ 1e-7)
- *   2 = tcgen05, 128->1024 layer with fp16 hi/lo activations x one fp16 weight
- *       term, 2 passes (|dprob| ~ 2e-6 vs the 1e-4 tolerance)
- *   3 = persistent tcgen05 kernel (one CTA per SM looping over candidates), the
- *       128->1024 layer as ONE fp16 x fp16 pass (|dprob| ~ 4e-6)            [default]
+ *   1 = wgmma, bf16 hi/lo x hi/lo, 3 passes (near-fp32)
+ *   2 = wgmma, 128->1024 layer with fp16 hi/lo activations x one fp16 weight
+ *       term, 2 passes
+ *   3 = wgmma, the 128->1024 layer as ONE fp16 x fp16 pass               [default]
+ *   Every engine keeps grasp scores within the 1e-4 tolerance of the fp32
+ *   reference (tests/test_gpu_parity.py).
  *   (2 and 3 fall back to 1 for a net whose folded weights exceed the fp16 range) */
 int         cg_ctx_set_engine(cg_ctx *ctx, int engine);
 int         cg_ctx_get_engine(cg_ctx *ctx);
@@ -67,9 +68,6 @@ int         cg_ctx_get_engine(cg_ctx *ctx);
  * flag is cleared); the caller should then re-run on engine 1.  Synchronises
  * the context's stream.                                                      */
 int         cg_ctx_fp16_overflow(cg_ctx *ctx, int *out);
-/* Diagnostic: exercises the TMEM fragment layout the engine-3 max epilogue
- * relies on; out_host receives 768 floats (see tests/test_gpu_parity.py).    */
-int         cg_tmem_layout_selftest(cg_ctx *ctx, float *out_host);
 /* Optional in-stream timing of the dominant kernel (the fused shared-MLP+max
  * "trunk"): when enabled every trunk launch is bracketed by a CUDA event pair
  * on the launching stream; cg_ctx_profile_read() synchronises those events and
@@ -323,7 +321,7 @@ int cg_group_points_dev(cg_ctx *ctx, const float *xyz, const float *points,
  *
  * cg_mlp: a stack of nlayers shared (1x1 conv + BatchNorm + ReLU) layers, BN folded by the host:
  *   dims[nlayers+1] channel counts, Wt_host[i] = [dims[i]][dims[i+1]] k-major fp32, b_host[i] = [dims[i+1]].
- * Layers whose input width is a multiple of 64 run on tcgen05 (bf16 hi/lo x3, fp32 accumulate) when
+ * Layers whose input width is a multiple of 64 run on wgmma (bf16 hi/lo x3, fp32 accumulate) when
  * there are >= 64 rows; narrower ones (the 3+D input layer) on the FMA kernels.                        */
 typedef struct cg_mlp cg_mlp;
 int  cg_mlp_create(cg_ctx *ctx, int nlayers, const int *dims, const float *const *Wt_host,

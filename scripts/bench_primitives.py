@@ -1,4 +1,4 @@
-"""Timing of the per-scene kernels (FPS, ball query, grouping, occupancy grid, RANSAC, filter) on one B200."""
+"""Timing of the per-scene kernels (FPS, ball query, grouping, occupancy grid, RANSAC, filter) on one H100."""
 import os, sys, time, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

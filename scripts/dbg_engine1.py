@@ -1,4 +1,4 @@
-"""Debug helper: compare engine 1 (tcgen05) against engine 0 (fp32 SIMT) and the oracle."""
+"""Debug helper: compare engine 1 (wgmma, bf16 hi/lo x3) against engine 0 (fp32 SIMT) and the oracle."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

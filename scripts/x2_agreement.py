@@ -5,7 +5,7 @@ FCL / octomap are not available (not in /root/reference, not installed, versions
 float64 restatement of the SEMANTIC in oracle/fcl_semantic_ref.py (0.5 mm cubes at octomap keys vs posed triangles, 13-axis
 SAT).  CPU only; run in the authoring container:
 
-    python scripts/x2_agreement.py [--n 4096] [--procs 8]          -> profiles/r2_x2_agreement.json
+    python scripts/x2_agreement.py [--n 4096] [--procs 8]          -> JSON on stdout
 """
 import argparse
 import json
@@ -72,7 +72,6 @@ def main():
         res[name] = {"agreement": float((v == sem).mean()), "predicate_only_hits": int((v & ~sem).sum()),
                      "semantic_only_hits": int((~v & sem).sum()), "hits": int(v.sum())}
     print(json.dumps(res, indent=1))
-    json.dump(res, open(os.path.join(ROOT, "profiles", "r2_x2_agreement.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -102,5 +102,43 @@ def main():
     print("direction cases", len(d))
 
 
+def reference_runs():
+    """What the compiled reference itself returns on the oracle-facing cases: its verbose rejection counters and
+    survivor count per filter case (poses pushed sideways by 0 / 2 cm on every third candidate), and the ikfast
+    solution count of every oracle survivor of the IK cases.  The tests compare the oracle against these values."""
+    from oracle import filter_ref
+    from catgrasp_b200.my_cpp import _mm4_f32, grasp_in_cam_unshifted
+    out = {}
+    for k, (S, scale, mode, adjust, fdir) in enumerate(FILTER_CASES):
+        for j, sideways in enumerate(SIDEWAYS):
+            (p1, p2, poses, sym, nocs_pose, c2n, g), _ = filter_inputs(S, scale)
+            poses = shift_sideways(poses, sideways)
+            ref, cnt = mycpp_ref.filterGraspPose(poses, sym, nocs_pose, c2n, g["gripper_in_grasp"], fdir, adjust, mode,
+                                                 g["open"], p1, g["enclosed"], p2, counters=True)
+            out[f"counters_{k}_{j}"] = np.array([cnt["approach"], cnt["ik"], cnt["open"], cnt["close"], len(ref)], np.int64)
+    cam, ee = ik_frames()
+    f = lambda m: np.asarray(m, np.float64).astype(np.float32)      # noqa: E731
+    for k, (S, scale, mode, adjust, fdir) in enumerate(IK_CASES):
+        (p1, p2, poses, sym, nocs_pose, c2n, g), _ = filter_inputs(S, scale)
+        st, _, _ = filter_ref.filter_ref(poses, sym, nocs_pose, c2n, g["gripper_in_grasp"], fdir, adjust, mode, g["open"], p1,
+                                         g["enclosed"], p2)
+        u = grasp_in_cam_unshifted(poses, sym, nocs_pose, c2n)
+        out[f"ik_counts_{k}"] = np.array([mycpp_ref.ik_solution_count(_mm4_f32(_mm4_f32(f(cam), u[q]), f(ee)), IK_UPPER, IK_LOWER)
+                                          for q in np.nonzero(st == 0)[0]], np.int64)
+    np.savez_compressed(os.path.join(HERE, "mycpp_ref_runs.npz"), **out)
+    print("reference runs", len(out))
+
+
+SIDEWAYS = [0.0, 0.02]
+
+
+def shift_sideways(poses, sideways):
+    """every third candidate moved `sideways` metres along its gripper x axis (cases where the open gripper collides)"""
+    poses = poses.copy()
+    poses[::3, :3, 3] += poses[::3, :3, 0] * sideways
+    return poses
+
+
 if __name__ == "__main__":
     main()
+    reference_runs()

@@ -19,7 +19,7 @@ LOGIT_TOL = 5e-4
 @pytest.fixture(scope="module")
 def cuda():
     if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a B200; there is no CPU fallback")
+        pytest.fail("GPU tests need an H100; there is no CPU fallback")
     torch.cuda.set_device(0)
     return torch.device("cuda", 0)
 
@@ -62,29 +62,6 @@ def _oracle_probs(sd, xyz, nrm, poses, ids, mean=None, std=None):
 
 
 # ------------------------------------------------------------------ networks
-def test_tmem_fragment_layout(cuda):
-    """The engine-3 max epilogue reads accumulators with tcgen05.ld.16x256b and reduces columns with FMNMX3 +
-    a 3-step lane exchange.  TMEM is filled with lane*1000 + column; the column max over a warp's 32 lanes must be
-    (32*warp + 31)*1000 + column, with thread t ending up with columns 2t and 2t+1."""
-    import ctypes as C
-    from catgrasp_b200 import _lib
-    ctx = _lib.Context.get(0)
-    out = np.zeros(768, np.float32)
-    ctx.check(ctx.lib.cg_tmem_layout_selftest(ctx.h, C.c_void_p(out.ctypes.data)))
-    red = out[:256].reshape(4, 32, 2)
-    for w in range(4):
-        for t in range(32):
-            for k in range(2):
-                assert red[w, t, k] == (32 * w + 31) * 1000 + 2 * t + k, (w, t, k, red[w, t, k])
-    frag = out[256:].reshape(4, 32, 4)
-    for w in range(4):
-        for t in range(32):
-            lane = 32 * w + t // 4
-            exp = [lane * 1000 + 2 * (t % 4), lane * 1000 + 2 * (t % 4) + 1,
-                   (lane + 8) * 1000 + 2 * (t % 4), (lane + 8) * 1000 + 2 * (t % 4) + 1]
-            assert list(frag[w, t]) == exp, (w, t, frag[w, t], exp)
-
-
 @pytest.mark.parametrize("engine", _engines())
 def test_cls_vs_reference_golden(cls_net, golden_dir, engine):
     net, _ = cls_net
