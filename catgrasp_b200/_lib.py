@@ -67,6 +67,7 @@ SIGNATURES = {
     "cg_three_interp_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cg_cls_forward_dev": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "cg_seg_forward_dev": (_i, [_vp, _vp, _i, _i, _vp]),
+    "cg_encoder_probe_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "cg_nunocs_forward_host": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "cg_nunocs_forward_dev": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "cg_sdf_create": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_f), _f, C.POINTER(_vp)]),

@@ -36,7 +36,7 @@ extern "C" int cg_ctx_create(int device, cg_ctx **out) {
   return CG_OK;
 }
 
-// engine 3 clamps 128->1024 inputs to the fp16 range; *out = 1 if that happened since the last call (clears the flag)
+// engines 2 and 3 clamp 128->1024 inputs to the fp16 range; *out = 1 if that happened since the last call (clears the flag)
 extern "C" int cg_ctx_fp16_overflow(cg_ctx *ctx, int *out) {
   if (!ctx || !out) return CG_EINVAL;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));

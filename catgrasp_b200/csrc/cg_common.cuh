@@ -24,7 +24,7 @@ struct cg_ctx {
   // 0 = fp32 SIMT, 1 = wgmma bf16 3-pass, 2 = wgmma fp16 2-pass, 3 = wgmma single fp16 pass (default)
   int engine = 3;
   cudaEvent_t switch_event = nullptr;   // orders a newly selected stream behind the previous one (shared workspaces)
-  uint32_t *ovf_flag = nullptr;   // device word: engine 3 saw a 128->1024 input above the fp16 range (clamped)
+  uint32_t *ovf_flag = nullptr;   // device word: engine 2 or 3 saw a 128->1024 input above the fp16 range (clamped)
   int num_sms = 132;
   // optional event-pair timing of trunk launches (bench roofline)
   bool prof = false;

@@ -144,17 +144,21 @@ void encoder_ws_carve(cg_arena &ar, int B, EncoderWs &w) {
 
 // Runs the PointNetEncoder (pointnet2.py:241-271) for B clouds; on return w.gmax holds the
 // (B,1024) global feature as order-preserving keys; pf_out (optional) the 64-ch point feature.
-int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs &w, float *pf_out) {
+// keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.
+int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs &w, float *pf_out,
+                    uint32_t *keys_out = nullptr) {
   cg_ctx *ctx = net->ctx;
   const cg_layer *L = net->L;
   int rc;
   cg_trunk_args a;
   a.in = in; a.B = B; a.N = N; a.ovf_flag = ctx->ovf_flag;
+  const size_t kb = (size_t)B * 1024 * 4;
   // --- trunk A: STN3d convs + max (pointnet2.py:170-175)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.T3 = nullptr; a.l0 = L[L_S3_C1]; a.stage1_mode = 0; a.l1 = cg_layer{nullptr, nullptr, 0, 0}; a.T64 = nullptr;
   a.l2 = L[L_S3_C2]; a.l3 = L[L_S3_C3]; a.tc_img = net->tc_img[0]; a.tc_f16_ok = net->tc_f16_ok[0]; a.relu3 = 1; a.gmax_keys = w.gmax; a.pf_out = nullptr;
   if ((rc = trunk_launch(ctx, a))) return rc;
+  if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
   if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_S3_F1].Wt, L[L_S3_F1].b, 512, 1, 0, 1, w.f1))) return rc;
   if ((rc = cg_linear_launch(ctx, w.f1, B, 512, L[L_S3_F2].Wt, L[L_S3_F2].b, 256, 1, 0, 0, w.f2))) return rc;
   if ((rc = cg_linear_launch(ctx, w.f2, B, 256, L[L_S3_F3].Wt, L[L_S3_F3].b, 9, 0, 0, 0, w.T3))) return rc;
@@ -163,6 +167,7 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   a.T3 = w.T3; a.l0 = L[L_E_C1]; a.stage1_mode = 1; a.l1 = L[L_SK_C1];
   a.l2 = L[L_SK_C2]; a.l3 = L[L_SK_C3]; a.tc_img = net->tc_img[1]; a.tc_f16_ok = net->tc_f16_ok[1]; a.relu3 = 1;
   if ((rc = trunk_launch(ctx, a))) return rc;
+  if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out + (size_t)B * 1024, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
   if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_SK_F1].Wt, L[L_SK_F1].b, 512, 1, 0, 1, w.f1))) return rc;
   if ((rc = cg_linear_launch(ctx, w.f1, B, 512, L[L_SK_F2].Wt, L[L_SK_F2].b, 256, 1, 0, 0, w.f2))) return rc;
   if ((rc = cg_linear_launch(ctx, w.f2, B, 256, L[L_SK_F3].Wt, L[L_SK_F3].b, 4096, 0, 0, 0, w.T64))) return rc;
@@ -171,6 +176,7 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   a.stage1_mode = 2; a.T64 = w.T64; a.l1 = cg_layer{nullptr, nullptr, 64, 64};
   a.l2 = L[L_E_C2]; a.l3 = L[L_E_C3]; a.tc_img = net->tc_img[2]; a.tc_f16_ok = net->tc_f16_ok[2]; a.relu3 = 0; a.pf_out = pf_out;
   if ((rc = trunk_launch(ctx, a))) return rc;
+  if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out + (size_t)2 * B * 1024, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
   return CG_OK;
 }
 
@@ -334,6 +340,37 @@ extern "C" int cg_seg_forward_dev(cg_net *net, const float *x, int B, int N, flo
   if (!net) return CG_EINVAL;
   CG_REQUIRE(net->ctx, out_logits != nullptr, "seg: null output");
   return seg_forward_impl(net, x, B, N, out_logits, 0, nullptr, nullptr, nullptr);
+}
+
+extern "C" int cg_encoder_probe_dev(cg_net *net, const float *x, const double *cloud_xyz, const double *cloud_nrm,
+                                    int M, const double *poses, const int32_t *ids, const double *mean,
+                                    const double *stdv, int B, int N, uint32_t *out_keys, float *out_T3,
+                                    float *out_T64, float *out_pf) {
+  if (!net) return CG_EINVAL;
+  cg_ctx *ctx = net->ctx;
+  CG_REQUIRE(ctx, B > 0 && B <= CHUNK_B && N > 0, "encoder_probe: 0 < B <= 16384, N > 0");
+  CG_REQUIRE(ctx, out_keys && out_T3 && out_T64, "encoder_probe: null output");
+  cg_input_src in;
+  memset(&in, 0, sizeof(in));
+  if (x) {
+    in.x_direct = x;
+  } else {
+    CG_REQUIRE(ctx, cloud_xyz && cloud_nrm && poses && M > 0, "encoder_probe: null cloud/poses");
+    CG_REQUIRE(ctx, ids != nullptr || N <= M, "encoder_probe: ids required when N > M");
+    CG_REQUIRE(ctx, (mean == nullptr) == (stdv == nullptr), "encoder_probe: mean/std must come together");
+    in.cloud_xyz = cloud_xyz; in.cloud_nrm = cloud_nrm; in.poses = poses; in.ids = ids;
+    in.mean = mean; in.stdv = stdv; in.M = M;
+  }
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  int rc = cg_ws_reserve(ctx, encoder_ws_bytes(B) + 1024);
+  if (rc) return rc;
+  cg_arena ar(ctx->ws);
+  EncoderWs w;
+  encoder_ws_carve(ar, B, w);
+  if ((rc = encoder_forward(net, in, B, N, w, out_pf, out_keys))) return rc;
+  CG_CUDA(ctx, cudaMemcpyAsync(out_T3, w.T3, (size_t)B * 9 * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  CG_CUDA(ctx, cudaMemcpyAsync(out_T64, w.T64, (size_t)B * 4096 * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  return CG_OK;
 }
 
 extern "C" int cg_nunocs_forward_dev(cg_net *net, const float *x, int N, int bins, float *out_coords,

@@ -58,7 +58,7 @@ struct cg_trunk_args {
   int relu3;
   uint32_t *gmax_keys;  // (B,1024) order-preserving keys, zero-initialised by the launcher
   float *pf_out;        // (B,N,64) stage-1 output (PointNetSeg point feature) or nullptr
-  uint32_t *ovf_flag;       // engine 3: set to 1 when an activation had to be clamped to the fp16 range (or nullptr)
+  uint32_t *ovf_flag;       // engines 2, 3: set to 1 when an activation had to be clamped to the fp16 range (or nullptr)
 };
 
 int cg_trunk_launch_simt(cg_ctx *ctx, const cg_trunk_args &a);

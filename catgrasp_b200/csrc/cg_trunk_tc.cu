@@ -14,8 +14,9 @@
 // Precision of L3 (PASSES, the template parameter; L1 / L2 are always near-fp32):
 //   3 (engine 1)  W3 and X3 split x = hi + lo in bf16, products lo*hi + hi*lo + hi*hi (lo*lo ~ 2^-16 dropped): near-fp32
 //   2 (engine 2)  W3 one fp16 term, X3 fp16 hi + lo
-//   1 (engine 3)  W3 and X3 one fp16 term each.  X3 values above the fp16 range are clamped to 65504 AND reported
-//                 through cg_trunk_args::ovf_flag so that the host can re-run on engine 1.
+//   1 (engine 3)  W3 and X3 one fp16 term each.
+// On both fp16 engines X3 values above the fp16 range are clamped to 65504 AND reported through
+// cg_trunk_args::ovf_flag so that the host can re-run on engine 1.
 //
 // CTA = 288 threads, 1 per SM: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the
 // whole layer chain for its points) and one producer warp.  The two warpgroups are independent except for the shared
@@ -158,7 +159,7 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
 
   // ======================= consumer warpgroups =======================
   const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, q = lane & 3;
-  float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU): reported if beyond the fp16 range
+  float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU, fp16 engines): reported if beyond the fp16 range
   mbar_wait(wbar_s, 0u);
 
   // input row (6 floats after pose transform / normalisation / T3) of point n of candidate b
@@ -276,6 +277,10 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
           asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(xh[j][r]) : "f"(x1), "f"(x0));
         }
     } else {
+      if (PASSES == 2) {   // split_f16x2 clamps to the fp16 range: record what it clamps
+#pragma unroll
+        for (int i = 0; i < 64; i++) vmax = fmaxf(vmax, acc[i]);
+      }
       d_to_a<8, F16>(acc, xh, xl);
     }
     // ---- L3: 128 -> 1024 in 16 half-chunks of 64 channels; max over the tile's points ----
@@ -361,7 +366,7 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     }
     gslot += 2u * NCHUNK;
   }
-  if (PASSES == 1 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
+  if (F16 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
 
   // ---- fold the eight warps' running maxima of every channel into the global feature ----
   bar_consumers();

@@ -63,7 +63,7 @@ void        cg_ctx_reset_launch_count(cg_ctx *ctx);
  *   (2 and 3 fall back to 1 for a net whose folded weights exceed the fp16 range) */
 int         cg_ctx_set_engine(cg_ctx *ctx, int engine);
 int         cg_ctx_get_engine(cg_ctx *ctx);
-/* Engines 2/3 clamp the 128->1024 layer's inputs to the fp16 range (65504).
+/* Engines 2 and 3 clamp the 128->1024 layer's inputs to the fp16 range (65504).
  * *out = 1 if a clamp happened on this context since the previous call (the
  * flag is cleared); the caller should then re-run on engine 1.  Synchronises
  * the context's stream.                                                      */
@@ -152,6 +152,22 @@ int cg_cls_forward_dev(cg_net *net, const float *x, int B, int N,
                        float *out_logits, float *out_probs);
 int cg_seg_forward_dev(cg_net *net, const float *x, int B, int N,
                        float *out_logits);
+/* Encoder intermediates -- a test hook (device pointers, enqueued on the
+ * context stream).  Runs the PointNet encoder of either net kind on B <= 16384
+ * candidates exactly as the forward entries do and copies out, per stage:
+ *   out_keys (3,B,1024) uint32: the max-pool outputs of the STN3d, STNkd and
+ *            encoder trunks as order-preserving keys (the fp32 bits b map to
+ *            b | 0x80000000 when b's sign bit is clear, else to ~b)
+ *   out_T3 (B,9), out_T64 (B,4096) float32: the two feature transforms
+ *   out_pf (B,N,64) float32: the point feature after T64, or NULL
+ * Input: x (B,N,6) float32, or x == NULL and the fused grasp-Q form of
+ * cg_graspq_forward_dev (ids may be NULL when N <= M; mean/std both or neither). */
+int cg_encoder_probe_dev(cg_net *net, const float *x,
+                         const double *cloud_xyz, const double *cloud_nrm, int M,
+                         const double *poses, const int32_t *ids,
+                         const double *mean, const double *std, int B, int N,
+                         uint32_t *out_keys, float *out_T3, float *out_T64,
+                         float *out_pf);
 /* NUNOCS post-processing, predicter.py:144-150: logits (P, 3*bins) ->
  * coords (P,3) = argmax*(1/bins) - 0.5 and conf_z (P,) = softmax prob of the
  * z-axis argmax bin.  Fused variant of cg_seg_forward for B=1.              */
