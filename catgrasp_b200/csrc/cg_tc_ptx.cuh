@@ -58,6 +58,22 @@ template <int N>
 __device__ __forceinline__ void wg_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Operand fences: an empty asm that reads and writes each of n registers.  The "memory" clobber of the fence / commit /
+// wait wrappers above does not order register accesses, so without these the compiler may move a read of an
+// accumulator above the wait that completes it, or the write of an A fragment below the fence before its wgmma; ptxas
+// then repairs the order by injecting a full warpgroup.wait / warpgroup.arrive (C7517 / C7519) and the pipeline is lost.
+// Fence the accumulators before the wgmma.fence of a group and after the wait that completes it, and the A fragments
+// after they are written and after the last wgmma that reads them is complete.
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(float *r) {
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(uint32_t *r) {
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile("" : "+r"(r[i])::"memory");
+}
 
 #define CG_WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
                     "+f"(d[i + 6]), "+f"(d[i + 7])

@@ -20,7 +20,8 @@
 //
 // CTA = 288 threads, 1 per SM: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the
 // whole layer chain for its points) and one producer warp.  The two warpgroups are independent except for the shared
-// W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core work.
+// W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core work; warpgroup 1
+// starts one front (input + FMA + L1 + L2) behind warpgroup 0 so that their fronts do not coincide.
 #include <stdlib.h>
 
 #include "cg_tc_ptx.cuh"
@@ -70,8 +71,36 @@ static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of
 
 __device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+// One step of the transposing column-max butterfly of the L3 reduction: the lanes with bit STEP set keep the upper
+// half of their STEP columns, the others the lower half, and each takes the max with its partner's copy.  STEP is a
+// template parameter so that every index into x is a constant and x stays in registers.
+template <int STEP>
+__device__ __forceinline__ void max_butterfly_step(float *x, int lane) {
+  const bool up = (lane & STEP) != 0;
+#pragma unroll
+  for (int k = 0; k < STEP / 2; k++) {
+    const float send = up ? x[k] : x[k + STEP / 2];
+    const float keep = up ? x[k + STEP / 2] : x[k];
+    x[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, STEP));
+  }
+}
+
+#ifdef CG_EXPERIMENTS
+// Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer warp of TL_CTAS sampled CTAs (blockIdx.x 0,
+// candidates spread over the batch) sums clock64() cycles per phase over its tiles and writes one record of
+// TL_REC words: the TL_NPHASE sums, its tile count and its total cycles.  TL_L3_WAIT and TL_RING lie inside TL_L3.
+enum { TL_START, TL_INPUT, TL_FRONT, TL_L3, TL_L3_WAIT, TL_RING, TL_NPHASE };
+constexpr int TL_CTAS = 8, TL_REC = 8;
+__host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / TL_CTAS : 1; }
+#define TL_PARAM , unsigned long long *tl
+#define TL_ARG(p) , p
+#else
+#define TL_PARAM
+#define TL_ARG(p)
+#endif
+
 template <int PASSES>
-__global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a, int tiles_per_cta) {
+__global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a, int tiles_per_cta TL_PARAM) {
   constexpr int NSLOT = PASSES == 3 ? 4 : 8;
   constexpr uint32_t SLOT_BYTES = PASSES == 3 ? 2 * PIECE : PIECE;
   constexpr bool F16 = PASSES < 3;
@@ -160,21 +189,56 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   // ======================= consumer warpgroups =======================
   const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, q = lane & 3;
   float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU, fp16 engines): reported if beyond the fp16 range
+#ifdef CG_EXPERIMENTS
+  // phase timeline of the sampled CTAs (scripts/trunk_timeline.py): cycles per phase summed over this warp's tiles
+  const bool tl_on = tl != nullptr && blockIdx.x == 0 && blockIdx.y % TL_STRIDE(a.B) == TL_STRIDE(a.B) / 2 &&
+                     (int)(blockIdx.y / TL_STRIDE(a.B)) < TL_CTAS;
+  unsigned long long tl_sum[TL_NPHASE] = {}, tl_t0 = clock64(), tl_t = tl_t0, tl_s;
+#define TL_MARK(phase)                   \
+  do {                                   \
+    const unsigned long long _t = clock64(); \
+    tl_sum[phase] += _t - tl_t;          \
+    tl_t = _t;                           \
+  } while (0)
+#define TL_SPAN_BEGIN() (tl_s = clock64())
+#define TL_SPAN_END(phase) (tl_sum[phase] += clock64() - tl_s)
+#else
+#define TL_MARK(phase) ((void)0)
+#define TL_SPAN_BEGIN() ((void)0)
+#define TL_SPAN_END(phase) ((void)0)
+#endif
   mbar_wait(wbar_s, 0u);
 
-  // input row (6 floats after pose transform / normalisation / T3) of point n of candidate b
-  auto load_row = [&](int n, float *v) {
-    if (n >= N) n = N - 1;   // duplicate a valid point: cannot change a max
+  // The input of a point row is fetched one tile ahead (fetch_id / fetch_row during the previous tile's L3) and
+  // finished (finish_row) when its tile starts, so the dependent id -> cloud-row loads are off the critical path.
+  // Row n >= N duplicates a valid point: it cannot change a max.  x_direct rows travel as exact float -> double.
+  auto fetch_id = [&](int n) -> int {
+    if (n >= N) n = N - 1;
+    return (a.in.x_direct == nullptr && a.in.ids) ? __ldg(a.in.ids + (size_t)b * N + n) : n;
+  };
+  auto fetch_row = [&](int id, double *r) {
     if (a.in.x_direct) {
-      const float *xr = a.in.x_direct + ((size_t)b * N + n) * 6;
+      const float *xr = a.in.x_direct + ((size_t)b * N + id) * 6;
 #pragma unroll
-      for (int k = 0; k < 6; k++) v[k] = __ldg(xr + k);
+      for (int k = 0; k < 6; k++) r[k] = __ldg(xr + k);
     } else {
-      const int id = a.in.ids ? __ldg(a.in.ids + (size_t)b * N + n) : n;
       const double *px = a.in.cloud_xyz + (size_t)id * 3;
       const double *pn = a.in.cloud_nrm + (size_t)id * 3;
-      const double x = __ldg(px), y = __ldg(px + 1), z = __ldg(px + 2);
-      const double nx = __ldg(pn), ny = __ldg(pn + 1), nz = __ldg(pn + 2);
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        r[k] = __ldg(px + k);
+        r[3 + k] = __ldg(pn + k);
+      }
+    }
+  };
+  // input row (6 floats after pose transform / normalisation / T3)
+  auto finish_row = [&](const double *r, float *v) {
+    if (a.in.x_direct) {
+#pragma unroll
+      for (int k = 0; k < 6; k++) v[k] = (float)r[k];
+    } else {
+      const double x = r[0], y = r[1], z = r[2];
+      const double nx = r[3], ny = r[4], nz = r[5];
       const double *R = S.pinv;
       double w[6];
       w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
@@ -194,16 +258,39 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     }
   };
 
-  uint32_t gslot = 0;   // W3 slots consumed so far
+  // W3 ring slot and mbarrier phase of K-block kb of chunk c of the current tile
+  uint32_t gslot = 0;   // W3 slots consumed before the current tile
+  auto slot_of = [&](int c, int kb) { return (gslot + 2u * c + kb) % NSLOT; };
+  auto phase_of = [&](int c, int kb) { return ((gslot + 2u * c + kb) / NSLOT) & 1u; };
+
+  const int prow = wg * 64 + w4 * 16 + g;   // this thread's rows of a tile: prow and prow + 8
+  // Half-chunks per unrolled L3 group (below), and whether the whole input rows of the next tile are prefetched during
+  // L3 or only their ids: the 24 registers of two float64 rows fit beside the L3 pipeline of engine 3 only.
+  constexpr int L3_GROUP = PASSES == 1 ? 8 : 4;
+  constexpr bool ROW_PREFETCH = PASSES == 1;
+  double r0[6], r1[6];   // raw input rows of the next tile
+  int id0 = fetch_id(tile_begin * TP + prow), id1 = fetch_id(tile_begin * TP + prow + 8);
+  if (ROW_PREFETCH) {
+    fetch_row(id0, r0);
+    fetch_row(id1, r1);
+  }
+  // Warpgroup 1 starts its first tile when warpgroup 0 has finished the front layers of its own (named barrier 2), so
+  // that one warpgroup's front runs under the other's L3 instead of leaving the tensor pipe idle for both.
+  if (wg == 1) asm volatile("bar.sync 2, 256;" ::: "memory");
+  TL_MARK(TL_START);
   for (int it = 0; it < my_tiles; it++) {
-    const int tile = tile_begin + it;
-    const int p0 = tile * TP + wg * 64 + w4 * 16 + g;   // this thread's rows: points p0 and p0 + 8
+    const int p0 = (tile_begin + it) * TP + prow;   // this thread's rows: points p0 and p0 + 8
     // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
     float d64[32];
     {
       float v0[6], v1[6];
-      load_row(p0, v0);
-      load_row(p0 + 8, v1);
+      if (!ROW_PREFETCH) {
+        fetch_row(id0, r0);
+        fetch_row(id1, r1);
+      }
+      finish_row(r0, v0);
+      finish_row(r1, v1);
+      TL_MARK(TL_INPUT);
 #pragma unroll
       for (int m = 0; m < 8; m++)
 #pragma unroll
@@ -224,6 +311,9 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     // ---- L1: 64 -> 64 (STNkd shared conv, or the per-candidate T64 feature transform) ----
     if (has_l1) {
       d_to_a<4, false>(d64, xh, xl);
+      wg_fence_regs<16>(xh[0]);
+      wg_fence_regs<16>(xl[0]);
+      wg_fence_regs<32>(d64);
       wg_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ks++) {
@@ -234,6 +324,9 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
       }
       wg_commit();
       wg_wait<0>();
+      wg_fence_regs<32>(d64);
+      wg_fence_regs<16>(xh[0]);
+      wg_fence_regs<16>(xl[0]);
 #pragma unroll
       for (int i = 0; i < 32; i++) {
         if (a.stage1_mode == 1) d64[i] = fmaxf(d64[i] + S.bias1[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
@@ -254,6 +347,9 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     // ---- L2: 64 -> 128 ----
     float acc[64];
     d_to_a<4, false>(d64, xh, xl);
+    wg_fence_regs<16>(xh[0]);
+    wg_fence_regs<16>(xl[0]);
+    wg_fence_regs<64>(acc);
     wg_fence();
 #pragma unroll
     for (int ks = 0; ks < 4; ks++) {
@@ -264,6 +360,12 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     }
     wg_commit();
     wg_wait<0>();
+    wg_fence_regs<64>(acc);
+    wg_fence_regs<16>(xh[0]);
+    wg_fence_regs<16>(xl[0]);
+    // warpgroup 0's front of the first tile is done: release warpgroup 1 (see above)
+    if (it == 0 && wg == 0) asm volatile("bar.arrive 2, 256;" ::: "memory");
+    TL_MARK(TL_FRONT);
 #pragma unroll
     for (int i = 0; i < 64; i++) acc[i] = fmaxf(acc[i] + S.bias2[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
     if (PASSES == 1) {
@@ -283,18 +385,26 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
       }
       d_to_a<8, F16>(acc, xh, xl);
     }
+    wg_fence_regs<32>(xh[0]);
+    if (PASSES != 1) wg_fence_regs<32>(xl[0]);
     // ---- L3: 128 -> 1024 in 16 half-chunks of 64 channels; max over the tile's points ----
     // Two 32-register accumulators: half-chunk h + 1 is issued before half-chunk h is reduced, so the reduction
     // overlaps the tensor cores.  Half-chunk h = channels 64h .. 64h+63 = rows 64 (h & 1) .. of chunk h / 2's W3 slots.
+    // The 16 half-chunks are unrolled so that both accumulators are fixed registers: with operand fences around every
+    // issue and wait ptxas then keeps exactly one wgmma group in flight during each reduction.
     auto issue = [&](int h, float *d) {
       const int c = h >> 1;
+      if ((h & 1) == 0) {
+        TL_SPAN_BEGIN();
+        mbar_wait(full_s + 8u * slot_of(c, 0), phase_of(c, 0));
+        mbar_wait(full_s + 8u * slot_of(c, 1), phase_of(c, 1));
+        TL_SPAN_END(TL_RING);
+      }
+      wg_fence_regs<32>(d);
       wg_fence();
 #pragma unroll
       for (int kb = 0; kb < 2; kb++) {
-        const uint32_t gs = gslot + 2u * c + kb;
-        const uint32_t s = gs % NSLOT;
-        if ((h & 1) == 0) mbar_wait(full_s + 8u * s, (gs / NSLOT) & 1u);
-        const uint32_t ws = ring_s + s * SLOT_BYTES + (uint32_t)(h & 1) * (PIECE / 2);
+        const uint32_t ws = ring_s + slot_of(c, kb) * SLOT_BYTES + (uint32_t)(h & 1) * (PIECE / 2);
 #pragma unroll
         for (int ks = 0; ks < 4; ks++) {
           const int j = kb * 4 + ks;
@@ -314,6 +424,7 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
         }
       }
       wg_commit();
+      wg_fence_regs<32>(d);
     };
     // half-chunk h is complete in this warp: fold its column max into the running max; after the second half of a
     // chunk hand the chunk's two W3 slots back
@@ -322,8 +433,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
       if (h & 1) {
         __syncwarp();
         if (lane == 0) {
-          mbar_arrive(empty_s + 8u * ((gslot + 2u * c) % NSLOT));
-          mbar_arrive(empty_s + 8u * ((gslot + 2u * c + 1u) % NSLOT));
+          mbar_arrive(empty_s + 8u * slot_of(c, 0));
+          mbar_arrive(empty_s + 8u * slot_of(c, 1));
         }
       }
       // column max over this warp's 16 rows: own two rows, then a transposing butterfly over lane bits 4, 3, 2
@@ -335,38 +446,61 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
         x[2 * i] = fmaxf(d[4 * i], d[4 * i + 2]);
         x[2 * i + 1] = fmaxf(d[4 * i + 1], d[4 * i + 3]);
       }
-#pragma unroll
-      for (int step = 16; step >= 4; step >>= 1) {
-        const bool up = (lane & step) != 0;
-#pragma unroll
-        for (int k = 0; k < step / 2; k++) {
-          const float send = up ? x[k] : x[k + step / 2];
-          const float keep = up ? x[k + step / 2] : x[k];
-          x[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, step));
-        }
-      }
+      max_butterfly_step<16>(x, lane);
+      max_butterfly_step<8>(x, lane);
+      max_butterfly_step<4>(x, lane);
       float2 &slot = sacc[((wg * 2 * NCHUNK + h) * 4 + w4) * 32 + lane];   // private to this thread
       const float2 old = slot;
       slot = make_float2(fmaxf(old.x, x[0]), fmaxf(old.y, x[1]));
     };
-    float da[32], db[32];   // even / odd half-chunks
-    issue(0, da);
+    // The half-chunks run in groups of L3_GROUP, unrolled so that the two accumulators are fixed registers.  Inside a
+    // group one wgmma group is in flight during each reduction; a group ends with a full wait, so that no wgmma is in
+    // flight across the loop's back edge (ptxas would otherwise serialise the loop).  A fully unrolled L3 does not fit
+    // the 168-register budget of a 288-thread CTA (registers are allocated per
+    // warpgroup: 288 threads count as 384).
+    // The next tile's input is fetched where nothing is in flight: the ids before the first group, the dependent
+    // rows before the second (a last tile re-reads its own rows, clamped to the candidate's points).
+    const int pn = p0 + (it + 1 < my_tiles ? TP : 0);
+    id0 = fetch_id(pn);
+    id1 = fetch_id(pn + 8);
 #pragma unroll 1
-    for (int h = 0; h < 2 * NCHUNK; h += 2) {
-      issue(h + 1, db);
-      wg_wait<1>();
-      reduce(h, da);
-      if (h + 2 < 2 * NCHUNK) {
-        issue(h + 2, da);
-        wg_wait<1>();
-      } else {
-        wg_wait<0>();
+    for (int h0 = 0; h0 < 2 * NCHUNK; h0 += L3_GROUP) {
+      if (ROW_PREFETCH && h0 == L3_GROUP) {
+        fetch_row(id0, r0);
+        fetch_row(id1, r1);
       }
-      reduce(h + 1, db);
+      float acc3[2][32];   // even / odd half-chunks
+      issue(h0, acc3[0]);
+#pragma unroll
+      for (int j = 0; j < L3_GROUP; j++) {
+        if (j + 1 < L3_GROUP) issue(h0 + j + 1, acc3[(j + 1) & 1]);
+        TL_SPAN_BEGIN();
+        if (j + 1 < L3_GROUP) wg_wait<1>();
+        else wg_wait<0>();
+        TL_SPAN_END(TL_L3_WAIT);
+        wg_fence_regs<32>(acc3[j & 1]);
+        reduce(h0 + j, acc3[j & 1]);
+      }
     }
+    // the last wgmma that read the A fragments is complete: the next tile's front may overwrite them
+    wg_fence_regs<32>(xh[0]);
+    if (PASSES != 1) wg_fence_regs<32>(xl[0]);
     gslot += 2u * NCHUNK;
+    TL_MARK(TL_L3);
   }
   if (F16 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
+#ifdef CG_EXPERIMENTS
+  if (tl_on && lane == 0) {
+    unsigned long long *o = tl + ((size_t)(blockIdx.y / TL_STRIDE(a.B)) * NCW + warp) * TL_REC;
+#pragma unroll
+    for (int p = 0; p < TL_NPHASE; p++) o[p] = tl_sum[p];
+    o[TL_NPHASE] = (unsigned long long)my_tiles;
+    o[TL_NPHASE + 1] = clock64() - tl_t0;
+  }
+#endif
+#undef TL_MARK
+#undef TL_SPAN_BEGIN
+#undef TL_SPAN_END
 
   // ---- fold the eight warps' running maxima of every channel into the global feature ----
   bar_consumers();
@@ -463,9 +597,50 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
   dim3 grid((ntiles + tiles_per_cta - 1) / tiles_per_cta, a.B);
   // W3 beyond the fp16 range: the fp16 engines fall back to the 3-pass bf16 kernel
   const int passes = !a.tc_f16_ok || ctx->engine == 1 ? 3 : (ctx->engine == 2 ? 2 : 1);
-  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
-  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
-  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta);
+#ifdef CG_EXPERIMENTS
+  static const bool timeline = getenv("CG_TRUNK_TIMELINE") && atoi(getenv("CG_TRUNK_TIMELINE")) != 0;
+  unsigned long long *tl = nullptr;
+  const size_t tl_words = (size_t)TL_CTAS * NCW * TL_REC;
+  if (timeline) {
+    CG_CUDA(ctx, cudaMallocAsync(&tl, tl_words * 8, ctx->stream));
+    CG_CUDA(ctx, cudaMemsetAsync(tl, 0, tl_words * 8, ctx->stream));
+  }
+#endif
+  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
+  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
+  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
   CG_LAUNCH_CHECK(ctx);
+#ifdef CG_EXPERIMENTS
+  if (timeline) {
+    std::vector<unsigned long long> h(tl_words);
+    CG_CUDA(ctx, cudaMemcpyAsync(h.data(), tl, tl_words * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CG_CUDA(ctx, cudaFreeAsync(tl, ctx->stream));
+    CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    // cycles per tile of one warp, averaged over the consumer warps of the sampled CTAs; the warps of a CTA run
+    // concurrently, so "total" is also the CTA's cycles per tile
+    double sum[TL_NPHASE + 1] = {}, tiles = 0;
+    int recs = 0;
+    for (int r = 0; r < TL_CTAS * NCW; r++) {
+      const unsigned long long *o = &h[(size_t)r * TL_REC];
+      if (o[TL_NPHASE] == 0) continue;
+      for (int p = 0; p < TL_NPHASE; p++) sum[p] += (double)o[p];
+      sum[TL_NPHASE] += (double)o[TL_NPHASE + 1];
+      tiles += (double)o[TL_NPHASE];
+      recs++;
+    }
+    if (recs > 0) {
+      // tensor-pipe cycles of one 128-point tile at 2048 dense fp16 / bf16 MAC per clock per SM
+      const double l3 = 128.0 * 128 * 1024 / 2048 * passes, l12 = 128.0 * 64 * (128 + (a.stage1_mode ? 64 : 0)) * 3 / 2048;
+      const double tot = sum[TL_NPHASE] / tiles;
+      fprintf(stderr,
+              "[trunk-timeline] passes=%d B=%d N=%d stage1=%d tiles/CTA=%.0f warps=%d  clk/tile: start %.0f  input %.0f  "
+              "front %.0f  l3 %.0f (wgmma-wait %.0f, ring-wait %.0f)  total %.0f  | tensor work %.0f clk/tile -> "
+              "busy %.1f%%\n",
+              passes, a.B, a.N, a.stage1_mode, tiles / recs, recs, sum[TL_START] / tiles, sum[TL_INPUT] / tiles,
+              sum[TL_FRONT] / tiles, sum[TL_L3] / tiles, sum[TL_L3_WAIT] / tiles, sum[TL_RING] / tiles, tot, l3 + l12,
+              100.0 * (l3 + l12) / tot);
+    }
+  }
+#endif
   return CG_OK;
 }
