@@ -18,9 +18,11 @@ __global__ void __launch_bounds__(256) linear_kernel(const float *__restrict__ X
                                                       float *__restrict__ Y) {
   __shared__ __align__(16) float xs[BK][BM + 4];
   __shared__ __align__(16) float ws[BK][BN + 4];
+  const long long tile = cg_row_tile();
+  if (tile * BM >= M) return;
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+  const int m0 = (int)tile * BM, n0 = blockIdx.x * BN;
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; i++)
@@ -99,9 +101,11 @@ __global__ void __launch_bounds__(256) linear_wide_kernel(const float *__restric
                                                            float *__restrict__ Y) {
   __shared__ __align__(16) float xs[2][LK][LM + 4];
   __shared__ __align__(16) float ws[2][LK][LN + 4];
+  const long long tile = cg_row_tile();
+  if (tile * LM >= M) return;
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;            // 16 x 16 threads: ty -> 4 rows, tx -> 8 cols (2 x float4)
-  const int m0 = blockIdx.y * LM, n0 = blockIdx.x * LN;
+  const int m0 = (int)tile * LM, n0 = blockIdx.x * LN;
   float acc[4][8];
 #pragma unroll
   for (int i = 0; i < 4; i++)
@@ -317,12 +321,12 @@ int cg_linear_launch(cg_ctx *ctx, const float *X, int M, int K, const float *Wt,
   }
   const long wide_ctas = (long)((N + LN - 1) / LN) * ((M + LM - 1) / LM);
   if (N >= 128 && (K % LK) == 0 && (K % 4) == 0 && wide_ctas >= ctx->num_sms) {
-    dim3 gridw((N + LN - 1) / LN, (M + LM - 1) / LM);
+    const dim3 gridw = cg_row_tile_grid((N + LN - 1) / LN, ((long long)M + LM - 1) / LM);
     linear_wide_kernel<<<gridw, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
     CG_LAUNCH_CHECK(ctx);
     return CG_OK;
   }
-  dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
+  const dim3 grid = cg_row_tile_grid((N + BN - 1) / BN, ((long long)M + BM - 1) / BM);
   linear_kernel<<<grid, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;

@@ -35,7 +35,9 @@ __global__ void __launch_bounds__(LT, 1) linear_tc_kernel(const float *__restric
   Bars &S = *reinterpret_cast<Bars *>(smem + STAGES * STAGE_BYTES);
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int g = lane >> 2, q = lane & 3;
-  const int n0 = blockIdx.x * 128, m0 = blockIdx.y * 128;
+  const long long tile = cg_row_tile();
+  if (tile * 128 >= M) return;                // before any barrier: the whole CTA leaves
+  const int n0 = blockIdx.x * 128, m0 = (int)tile * 128;
   const int nkb = K >> 6;
   const uint32_t smem_s = smem_u32(smem);
   const unsigned char *src = wimg + (size_t)blockIdx.x * nkb * STAGE_BYTES;   // this column tile's K-blocks
@@ -183,7 +185,7 @@ int cg_linear_tc_try(cg_ctx *ctx, const float *X, int M, int K, const float *Wt,
     CG_CUDA(ctx, cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LSMEM));
     attr_set[ctx->device] = true;
   }
-  dim3 grid((N + 127) / 128, (M + 127) / 128);
+  const dim3 grid = cg_row_tile_grid((N + 127) / 128, ((long long)M + 127) / 128);
   linear_tc_kernel<<<grid, LT, LSMEM, ctx->stream>>>(X, M, K, static_cast<const unsigned char *>(it->second), bias, N, relu,
                                                      bias_row_div, x_is_keys, Y);
   CG_LAUNCH_CHECK(ctx);

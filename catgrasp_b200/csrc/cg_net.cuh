@@ -67,6 +67,14 @@ size_t cg_tc_image_bytes();
 // Wt3 [128][1024], Wt2 [64][128], Wt1 [64][64] or nullptr (folded fp32, k-major rows, host)
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok);
 
+// Row tiles of the fully-connected kernels: gridDim.y is capped at 65535, so the tiles are spread over (y, z) and a
+// launch covers up to 2^31 rows.  tile = blockIdx.z * gridDim.y + blockIdx.y; CTAs past the last tile exit at once.
+inline dim3 cg_row_tile_grid(unsigned col_tiles, long long row_tiles) {
+  const unsigned y = row_tiles < 65535 ? (unsigned)row_tiles : 65535u;
+  return dim3(col_tiles, y, (unsigned)((row_tiles + y - 1) / y));
+}
+__device__ __forceinline__ long long cg_row_tile() { return (long long)blockIdx.z * gridDim.y + blockIdx.y; }
+
 // Y[M][N] = act(X[M][K] @ Wt[K][N] + bias[(row / bias_row_div)][N])
 // x_is_keys: X holds order-preserving uint keys (output of a trunk) to be decoded on load.
 int cg_linear_launch(cg_ctx *ctx, const float *X, int M, int K, const float *Wt, const float *bias,

@@ -39,6 +39,8 @@ __global__ void group_max_kernel(const float *__restrict__ x, int G, int K, int 
 // square_distance_kernel (cg_pn2.cu): dot = fma(z,z', fma(y,y', x*x')), d = ((-2*dot) + |a|^2) + |b|^2.
 // Selection = the first three entries of a stable ascending sort (ties -> lower index), which is what torch.sort
 // returns for distinct distances; exact ties between different sparse points are measure-zero for real clouds.
+// S == 2: the module family keeps the two neighbours it has (sort()[:, :, :3] of two columns), so the weights are
+// normalised over two and the third slot is written as index 0, weight 0.
 constexpr int NN_T = 128, NN_TILE = 1024;
 __global__ void three_nn_kernel(const float *__restrict__ xyz1, const float *__restrict__ xyz2, int N, int S,
                                 int32_t *__restrict__ out_idx, float *__restrict__ out_w) {
@@ -75,16 +77,21 @@ __global__ void three_nn_kernel(const float *__restrict__ xyz1, const float *__r
   }
   if (n >= N) return;
   // dist_recip = 1 / (d + 1e-8); weight = dist_recip / sum(dist_recip)   (fp32, torch operation order)
-  const float r0 = __fdiv_rn(1.f, __fadd_rn(d0, 1e-8f)), r1 = __fdiv_rn(1.f, __fadd_rn(d1, 1e-8f)),
-              r2 = __fdiv_rn(1.f, __fadd_rn(d2, 1e-8f));
-  const float norm = __fadd_rn(__fadd_rn(r0, r1), r2);
+  const float r0 = __fdiv_rn(1.f, __fadd_rn(d0, 1e-8f)), r1 = __fdiv_rn(1.f, __fadd_rn(d1, 1e-8f));
+  float norm = __fadd_rn(r0, r1), w2 = 0.f;
+  if (S >= 3) {
+    const float r2 = __fdiv_rn(1.f, __fadd_rn(d2, 1e-8f));
+    norm = __fadd_rn(norm, r2);
+    w2 = __fdiv_rn(r2, norm);
+  }
   const size_t o = ((size_t)b * N + n) * 3;
   out_idx[o] = i0; out_idx[o + 1] = i1; out_idx[o + 2] = i2;
-  out_w[o] = __fdiv_rn(r0, norm); out_w[o + 1] = __fdiv_rn(r1, norm); out_w[o + 2] = __fdiv_rn(r2, norm);
+  out_w[o] = __fdiv_rn(r0, norm); out_w[o + 1] = __fdiv_rn(r1, norm); out_w[o + 2] = w2;
 }
 
-// out[b][n][off + c] = sum_j w[b][n][j] * points2[b][idx[b][n][j]][c]   (sum order j = 0,1,2 like torch.sum over dim 2)
-// and out[b][n][c] = points1[b][n][c] for the skip features; one warp per dense point, lanes over channels.
+// out[b][n][off + c] = sum_j w[b][n][j] * points2[b][idx[b][n][j]][c]   (sum order j = 0,1,2 like torch.sum over dim 2;
+// j = 0,1 when S == 2) and out[b][n][c] = points1[b][n][c] for the skip features; one warp per dense point, lanes over
+// channels.
 __global__ void three_interp_kernel(const float *__restrict__ points1, int D1, const float *__restrict__ points2, int D2,
                                     const int32_t *__restrict__ idx, const float *__restrict__ w, int B, int N, int S,
                                     float *__restrict__ out) {
@@ -101,8 +108,10 @@ __global__ void three_interp_kernel(const float *__restrict__ points1, int D1, c
   float *o = out + (size_t)wid * (D1 + D2);
   if (points1)
     for (int c = lane; c < D1; c += 32) o[c] = points1[(size_t)wid * D1 + c];
-  for (int c = lane; c < D2; c += 32)
-    o[D1 + c] = __fadd_rn(__fadd_rn(__fmul_rn(p0[c], w0), __fmul_rn(p1[c], w1)), __fmul_rn(p2[c], w2));
+  for (int c = lane; c < D2; c += 32) {
+    const float v = __fadd_rn(__fmul_rn(p0[c], w0), __fmul_rn(p1[c], w1));
+    o[D1 + c] = S >= 3 ? __fadd_rn(v, __fmul_rn(p2[c], w2)) : v;
+  }
 }
 
 int run_mlp(cg_mlp *m, const float *x, long long R, float *out_last, float **last_buf) {
@@ -193,8 +202,8 @@ extern "C" int cg_three_interp_dev(cg_ctx *ctx, const float *xyz1, const float *
                                    const float *points2, int D2, int B, int N, int S, float *out, int32_t *out_idx,
                                    float *out_weight) {
   if (!ctx) return CG_EINVAL;
-  CG_REQUIRE(ctx, xyz1 && xyz2 && points2 && out && B > 0 && N > 0 && S >= 3 && D2 > 0 && D1 >= 0,
-             "three_interp: bad arguments (S >= 3 required; S == 1 is a plain broadcast)");
+  CG_REQUIRE(ctx, xyz1 && xyz2 && points2 && out && B > 0 && N > 0 && S >= 2 && D2 > 0 && D1 >= 0,
+             "three_interp: bad arguments (S >= 2 required; S == 1 is a plain broadcast)");
   CG_REQUIRE(ctx, (points1 != nullptr) == (D1 > 0), "three_interp: points1 / D1 mismatch");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   int32_t *idx = out_idx;

@@ -117,19 +117,10 @@ def sample_and_group_all(xyz, points):
 class _SharedMLP:
     def __init__(self, state_dict, nlayers, device=None):
         import ctypes as C
-        from .weights import _fold
+        from .weights import fold_mlp
         self.ctx = _lib.Context.get(device)
-        sd = {k.replace("module.", ""): v for k, v in state_dict.items()}
-        Wts, bs, dims = [], [], []
-        for i in range(nlayers):
-            w = {k: (v.detach().cpu().numpy() if torch.is_tensor(v) else np.asarray(v)) for k, v in sd.items()
-                 if k.startswith(f"mlp_convs.{i}.") or k.startswith(f"mlp_bns.{i}.")}
-            w[f"mlp_convs.{i}.weight"] = w[f"mlp_convs.{i}.weight"].reshape(w[f"mlp_convs.{i}.weight"].shape[0], -1, 1)
-            Wt, b = _fold(w, f"mlp_convs.{i}", f"mlp_bns.{i}")
-            Wts.append(np.ascontiguousarray(Wt, dtype=np.float32))
-            bs.append(np.ascontiguousarray(b, dtype=np.float32))
-            dims.append(Wt.shape[0])
-        dims.append(Wts[-1].shape[1])
+        Wts, bs = fold_mlp(state_dict, nlayers)
+        dims = [Wt.shape[0] for Wt in Wts] + [Wts[-1].shape[1]]
         self.dims = dims
         cdims = (C.c_int * len(dims))(*dims)
         cw = (C.c_void_p * nlayers)(*[w.ctypes.data for w in Wts])
@@ -203,6 +194,8 @@ class PointNetFeaturePropagation:
             w = torch.empty((B, N, 3), dtype=torch.float32, device=x1.device)
             ctx.check(ctx.lib.cg_three_interp_dev(ctx.h, _lib.ptr(x1), _lib.ptr(x2), _lib.ptr(p1), D1, _lib.ptr(p2), D2,
                                                   B, N, S, _lib.ptr(feat), _lib.ptr(idx), _lib.ptr(w)))
+            if S == 2:   # the module family's sort()[:, :, :3] of two columns: two neighbours
+                idx, w = idx[:, :, :2], w[:, :, :2]
         feat = feat.contiguous()
         out = torch.empty((B, N, self.mlp.dims[-1]), dtype=torch.float32, device=x1.device)
         ctx.check(ctx.lib.cg_shared_mlp_dev(self.mlp.h, _lib.ptr(feat), B * N, _lib.ptr(out)))

@@ -79,6 +79,20 @@ def _fold(sd, lin, bn):
     return W.T.copy(), b
 
 
+def fold_mlp(state_dict, nlayers):
+    """The fp32 (Wt [K][C], b [C]) of every layer of a PointNet++ shared-MLP stack (upstream layout mlp_convs.{i} +
+    mlp_bns.{i}, Conv1d or Conv2d 1x1), BatchNorm folded: the exact weights ``cg_mlp_create`` receives."""
+    sd = {k.replace("module.", ""): v for k, v in state_dict.items()}
+    Wts, bs = [], []
+    for i in range(nlayers):
+        w = {k: _np64(v) for k, v in sd.items() if k.startswith(f"mlp_convs.{i}.") or k.startswith(f"mlp_bns.{i}.")}
+        w[f"mlp_convs.{i}.weight"] = w[f"mlp_convs.{i}.weight"].reshape(w[f"mlp_convs.{i}.weight"].shape[0], -1, 1)
+        Wt, b = _fold(w, f"mlp_convs.{i}", f"mlp_bns.{i}")
+        Wts.append(np.ascontiguousarray(Wt, dtype=np.float32))
+        bs.append(np.ascontiguousarray(b, dtype=np.float32))
+    return Wts, bs
+
+
 def _pad64(a):
     a = np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
     n = (a.size + 63) // 64 * 64

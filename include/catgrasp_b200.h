@@ -343,7 +343,8 @@ typedef struct cg_mlp cg_mlp;
 int  cg_mlp_create(cg_ctx *ctx, int nlayers, const int *dims, const float *const *Wt_host,
                    const float *const *b_host, cg_mlp **out);
 void cg_mlp_destroy(cg_mlp *mlp);
-/* x (R, dims[0]) -> out (R, dims[nlayers]): the per-row MLP (feature-propagation tail).               */
+/* x (R, dims[0]) -> out (R, dims[nlayers]): the per-row MLP (feature-propagation tail).  R < 2^31 (also
+ * G*K below), any row count in that range.                                                          */
 int  cg_shared_mlp_dev(cg_mlp *mlp, const float *x, int64_t R, float *out);
 /* grouped (G, K, dims[0]) = output of cg_group_points_dev with G = B*S -> out (G, dims[nlayers]):
  * per-row MLP over all G*K rows, then max over the K rows of every group (set abstraction).           */
@@ -351,7 +352,11 @@ int  cg_group_mlp_max_dev(cg_mlp *mlp, const float *grouped, int G, int K, float
 /* Feature propagation, interpolation half: for every dense point xyz1[b][n] the 3 nearest of the S
  * sparse points xyz2[b] (expanded-form distances, ties -> lower index), weights (1/(d+1e-8))/sum, and
  *   out[b][n] = [points1[b][n] (D1 skip channels, optional) | sum_j w_j * points2[b][idx_j] (D2)]
- * out (B,N,D1+D2); out_idx (B,N,3) int32 / out_weight (B,N,3) optional (NULL: scratch).  S >= 3.      */
+ * out (B,N,D1+D2); out_idx (B,N,3) int32 / out_weight (B,N,3) optional (NULL: scratch).  S >= 2.
+ * S == 2 follows the module family, which keeps the first three of the sorted distances and so has two
+ * neighbours: weights (1/(d+1e-8)) / (r0+r1), out = w0*p0 + w1*p1, and the third slot of out_idx /
+ * out_weight is index 0 with weight 0 (the Python module returns (B,N,2)).  S == 1 is a plain broadcast
+ * and is left to the caller.                                                                            */
 int  cg_three_interp_dev(cg_ctx *ctx, const float *xyz1, const float *xyz2, const float *points1, int D1,
                          const float *points2, int D2, int B, int N, int S, float *out,
                          int32_t *out_idx, float *out_weight);

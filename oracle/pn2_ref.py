@@ -4,8 +4,13 @@ The floating-point forms are the reference's: FPS uses the direct form ((dx^2+dy
 the ball query the expanded form -2<s,d> + |s|^2 + |d|^2 (:30-32).  The dot product of the expanded
 form is accumulated as fma(sz,dz, fma(sy,dy, sx*dx)) which is what the BLAS sgemm behind
 ``torch.matmul`` does for K=3 on an FMA machine; tests/golden pins this against the reference itself.
+
+Also the exact fp32 contracts of the feature-propagation kernels (three_nn, three_interp), the FPS launch rule
+(fps_config) and a float64 reference of the shared-MLP stacks with an error bound (SharedMLP64).
 """
 import numpy as np
+
+from oracle.encoder_ref import FoldedNet, u_bf16x3, u_fp32
 
 f32 = np.float32
 
@@ -75,6 +80,90 @@ def query_ball_point(radius, nsample, xyz, new_xyz):
             row[: inb.size] = inb
             out[b, s] = row
     return out
+
+
+def fps_config(N, max_cluster=16):
+    """(cluster size, points per thread) that cg_fps_dev (csrc/cg_pn2.cu) launches for N points: the cheapest cluster
+    by its cost model base + 0.025 x points per thread, among the sizes whose points fit 32 per thread of 256; the
+    template is the smallest of 4 / 8 / 16 / 32 that holds them.  None when N does not fit."""
+    best, cfg = None, None
+    for size, base in ((2, 0.70), (4, 0.83), (8, 1.0), (16, 1.45)):
+        if size > max_cluster:
+            break
+        ppt = -(-N // (size * 256))
+        if ppt > 32:
+            continue
+        cost = base + 0.025 * ppt
+        if best is None or cost < best:
+            best, cfg = cost, (size, next(p for p in (4, 8, 16, 32) if ppt <= p))
+    return cfg
+
+
+def three_nn(xyz1, xyz2):
+    """The 3 nearest of the S sparse points xyz2 (B,S,3) for every dense point of xyz1 (B,N,3), as three_nn_kernel
+    (csrc/cg_sa.cu) states it: expanded-form fp32 distances (sq_expanded), the first three of a stable ascending sort
+    (ties -> lower index), weights (1/(d+1e-8)) / ((r0+r1)+r2) in fp32.  S == 2 keeps two neighbours, normalised
+    over two.  Returns idx (B,N,k) int64 and weight (B,N,k) fp32, k = min(S, 3)."""
+    B, N, _ = xyz1.shape
+    k = min(xyz2.shape[1], 3)
+    idx = np.zeros((B, N, k), dtype=np.int64)
+    w = np.zeros((B, N, k), dtype=f32)
+    for b in range(B):
+        d = sq_expanded(xyz1[b], xyz2[b])
+        i = np.argsort(d, axis=1, kind="stable")[:, :k]
+        r = f32(1.0) / (np.take_along_axis(d, i, 1) + f32(1e-8))
+        norm = r[:, 0] + r[:, 1]
+        if k == 3:
+            norm = norm + r[:, 2]
+        idx[b], w[b] = i, r / norm[:, None]
+    return idx, w
+
+
+def three_interp(points1, points2, idx, w):
+    """cat([points1, interpolated]) of three_interp_kernel: interpolated = (p0*w0 + p1*w1) + p2*w2 in fp32, every
+    product and sum rounded on its own (no fused multiply-add).  points1 (B,N,D1) or None, points2 (B,S,D2)."""
+    p = index_points(points2.astype(f32), idx)                 # (B,N,k,D2)
+    t = p * w[..., None]
+    out = t[:, :, 0] + t[:, :, 1]
+    if idx.shape[2] == 3:
+        out = out + t[:, :, 2]
+    return out if points1 is None else np.concatenate([points1.astype(f32), out], axis=-1)
+
+
+class SharedMLP64:
+    """Float64 reference of a cg_mlp stack (shared 1x1 conv + folded BN + ReLU per layer) with a per-value bound on
+    the GPU's error, built from the exact fp32 folded weights the GPU receives (weights.fold_mlp).  The bound follows
+    oracle/encoder_ref.py: e_out = |W|^T e_in + u (|W|^T (|x| + e_in) + |b|) per layer, u = u_bf16x3(K) where
+    cg_linear_launch puts the layer on tensor cores (engine >= 1, >= 64 rows, K % 64 == 0, C_out >= 64), else
+    u_fp32(K).  ReLU and the max over a group's members add no error: a group's bound is its members' largest."""
+
+    def __init__(self, state_dict, nlayers):
+        import torch
+        from catgrasp_b200.weights import fold_mlp
+        Wts, bs = fold_mlp(state_dict, nlayers)
+        self.W = [torch.from_numpy(W.astype(np.float64)) for W in Wts]
+        self.b = [torch.from_numpy(b.astype(np.float64)) for b in bs]
+        self.dims = [W.shape[0] for W in Wts] + [Wts[-1].shape[1]]
+
+    def on_tc(self, engine, rows):
+        return [FoldedNet.fc_on_tc(engine, rows, W.shape[0], W.shape[1]) for W in self.W]
+
+    def rows(self, x, engine, rows=None):
+        """x (R, dims[0]) -> y (R, dims[-1]) and its bound, both float64 numpy; ``rows`` is the row count of the GPU
+        call (it decides tensor cores or FMA), by default R."""
+        import torch
+        x = torch.as_tensor(np.asarray(x, dtype=np.float64))
+        e = torch.zeros_like(x)
+        for W, b, tc in zip(self.W, self.b, self.on_tc(engine, x.shape[0] if rows is None else rows)):
+            x, e = FoldedNet._lin(x, e, W, b, u_bf16x3(W.shape[0]) if tc else u_fp32(W.shape[0]))
+            x = x.clamp_min(0.0)
+        return x.numpy(), e.numpy()
+
+    def group_max(self, grouped, engine, rows=None):
+        """grouped (G,K,dims[0]) -> max over the K members (G,dims[-1]) and its bound; ``rows`` defaults to G*K."""
+        G, K, Cin = grouped.shape
+        y, e = self.rows(np.asarray(grouped).reshape(G * K, Cin), engine, G * K if rows is None else rows)
+        return y.reshape(G, K, -1).max(1), e.reshape(G, K, -1).max(1)
 
 
 def sample_and_group(npoint, radius, nsample, xyz, points, start_idx):

@@ -100,14 +100,19 @@ def test_sa_fp_stack_vs_golden(golden_dir):
 
 
 @pytest.mark.gpu
-def test_three_interp_error_paths():
+def test_three_interp_sparse_count_limit():
+    """S = 1 (a plain broadcast, left to the caller) is rejected with its message; S = 2 interpolates over two
+    neighbours like the module family; an empty MLP stack is rejected."""
     import ctypes as C
     from catgrasp_b200 import _lib
     ctx = _lib.Context.get(0)
+    ctx.use_torch_stream()
     x = torch.zeros((1, 8, 3), device="cuda")
     f = torch.zeros((1, 2, 4), device="cuda")
     out = torch.zeros((1, 8, 4), device="cuda")
+    rc = ctx.lib.cg_three_interp_dev(ctx.h, _lib.ptr(x), _lib.ptr(x), None, 0, _lib.ptr(f), 4, 1, 8, 1, _lib.ptr(out), None, None)
+    assert rc == _lib.CG_EINVAL and b"S >= 2" in ctx.lib.cg_last_error(ctx.h)
     rc = ctx.lib.cg_three_interp_dev(ctx.h, _lib.ptr(x), _lib.ptr(x), None, 0, _lib.ptr(f), 4, 1, 8, 2, _lib.ptr(out), None, None)
-    assert rc == _lib.CG_EINVAL and b"S >= 3" in ctx.lib.cg_last_error(ctx.h)
+    assert rc == _lib.CG_OK
     h = C.c_void_p()
     assert ctx.lib.cg_mlp_create(ctx.h, 0, None, None, None, C.byref(h)) == _lib.CG_EINVAL
