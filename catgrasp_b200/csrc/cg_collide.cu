@@ -33,7 +33,7 @@ struct SdfView {
   int nx, ny, nz;
   float ox, oy, oz;
   float inv_res;
-  int border_nonneg;
+  int border_nonneg;   // the out-of-box shortcut is exact for this view's margin (make_view)
 };
 
 __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
@@ -153,9 +153,11 @@ __device__ __forceinline__ bool point_hits(const SdfView &s, const float *G, int
   const float gy = fmaf(G[5], z, fmaf(G[4], y, fmaf(G[3], x, G[10])));
   const float gz = fmaf(G[8], z, fmaf(G[7], y, fmaf(G[6], x, G[11])));
   if (mode == CG_SDF_TRILINEAR) {
-    // Exact shortcut: a coordinate outside [0, dim-1] is clamped onto a boundary face (sdf.py:311-313) and then
-    // interpolates boundary cells only; when all of those are >= 0 the result cannot be < 0, so the eight gathers
-    // are skipped.  Most scene points are far from the gripper box, which makes this the common path.
+    // Out-of-box shortcut: a coordinate outside [0, dim-1] is clamped onto a boundary face (sdf.py:311-313) and then
+    // interpolates boundary cells only.  make_view() sets border_nonneg only where such a lookup provably cannot come
+    // out below the margin (all boundary cells >= 0 for margin 0; a slack of 32 ulps above a positive margin, see
+    // shortcut_exact()), so skipping the eight gathers changes no verdict.  Most scene points are far from the
+    // gripper box, which makes this the common path.
     if (s.border_nonneg && (gx < 0.f || gy < 0.f || gz < 0.f || gx > (float)(s.nx - 1) || gy > (float)(s.ny - 1) ||
                             gz > (float)(s.nz - 1)))
       return false;
@@ -352,13 +354,32 @@ __global__ void sdf_lookup_kernel(SdfView s, const float *__restrict__ gc, int P
   }
 }
 
+// Whether the out-of-box shortcut of point_hits() may be taken for this margin.
+//
+// margin 0: exact when every boundary cell is >= 0 -- a clamped lookup sums non-negative products.
+//
+// margin > 0: boundary cells >= margin is NOT enough.  A clamped lookup interpolates boundary cells only, with weights
+// that sum to 1 in real arithmetic, but sdf_trilinear() rounds them.  With u = 2^-24 and b = border_min > 0:
+//   * per axis, w0 = 1 - (c - l) and w1 = 1 - ((l + 1) - c) each carry at most one rounding of 2^-25 (c - l is exact;
+//     (l + 1) - c is exact unless l = 0 and c < 0.5, and then 1 - that is exact), so w0 + w1 >= 1 - u; on a clamped
+//     axis the weights are exactly (1, 0);
+//   * the two products per corner lose at most a factor (1 - u)^2, so the eight corner weights sum to at least
+//     (1 - u)^5 - 16 * 2^-150 (the absolute term covers subnormal products);
+//   * all eight terms are >= 0, so the chain of eight fmas loses at most a factor (1 - u)^8 and 8 * 2^-150.
+// Hence sd >= b (1 - u)^13 - 2^-146 b - 2^-147 > b (1 - 13 u) - 2^-140.  Requiring b (1 - 2^-19) - 2^-140 >= margin
+// (2^-19 = 32 u) keeps every clamped lookup >= margin; the check runs in double, where b (1 - 2^-19) is exact.  A
+// boundary within a few ulps of the margin really does interpolate below it, so such grids take the plain scan.
+int shortcut_exact(const cg_sdf *s, float margin) {
+  if (margin <= 0.f) return s->border_nonneg;
+  return ((double)s->border_min * (1.0 - 0x1p-19) - 0x1p-140 >= (double)margin) ? 1 : 0;   // false for a NaN border
+}
+
 SdfView make_view(const cg_sdf *s, float margin = 0.f) {
   SdfView v;
   v.grid = s->grid; v.nx = s->nx; v.ny = s->ny; v.nz = s->nz;
   v.ox = s->origin[0]; v.oy = s->origin[1]; v.oz = s->origin[2];
   v.inv_res = 1.0f / s->res;
-  // the out-of-box shortcut stays exact as long as no boundary cell can report a hit: boundary values >= margin
-  v.border_nonneg = (margin <= 0.f) ? s->border_nonneg : (s->border_min >= margin ? 1 : 0);
+  v.border_nonneg = shortcut_exact(s, margin);
   return v;
 }
 

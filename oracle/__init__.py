@@ -23,4 +23,7 @@ Pinning status (DESIGN.md section "Oracle"):
     tests/golden/make_golden_mycpp.py -> tests/golden/mycpp_*.npz).  The FCL / octomap boundary cannot be built
     here (libraries absent, versions unpinned) -> that part is parity UNPINNED; both sides use the gripper-SDF
     predicate of meshpy/sdf.py and a restatement of the octomap calls instead (oracle/ref_shim/).
+  * filter64.py                 : float64 statement of the filter's predicate on sdf_ref.py's lookups, with a rigorous
+    bound on the float32 pipeline; checks filter_ref.c and the kernel on every verdict the bound decides
+    (tests/test_filter_ref.py, tests/test_filter_kernel.py).
 """
