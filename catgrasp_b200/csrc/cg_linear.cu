@@ -307,13 +307,14 @@ __global__ void nunocs_post_kernel(const float *__restrict__ logits, int P, int 
 
 }  // namespace
 
-int cg_linear_launch(cg_ctx *ctx, const float *X, int M, int K, const float *Wt, const float *bias, int N,
-                     int relu, int bias_row_div, int x_is_keys, float *Y) {
+int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, float *Y, unsigned flags,
+                     const float *row_bias, int rows_per_bias) {
+  const int K = L.K, N = L.C;
   CG_REQUIRE(ctx, M > 0 && K > 0 && N > 0, "linear: bad shape");
-  {
-    const int rc = cg_linear_tc_try(ctx, X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
-    if (rc != 0) return rc < 0 ? rc : CG_OK;
-  }
+  const float *Wt = L.Wt, *bias = row_bias ? row_bias : L.b;
+  const int relu = (flags & CG_FC_RELU) != 0, x_is_keys = (flags & CG_FC_KEYS) != 0, bias_row_div = rows_per_bias;
+  if (ctx->engine >= 1 && L.tc && M >= 64)
+    return cg_linear_tc_launch(ctx, X, M, K, L.tc, bias, N, relu, bias_row_div, x_is_keys, Y);
   if (M <= RM) {
     linear_rows_kernel<<<(N + RC - 1) / RC, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
     CG_LAUNCH_CHECK(ctx);

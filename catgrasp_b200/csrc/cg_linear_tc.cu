@@ -7,7 +7,7 @@
 // through a 3-stage ring of 64-wide K-blocks: the weight block arrives as a bulk copy of the host-prepared swizzled
 // image (B operand), the activations are read as fp32 (or as the trunk's order-preserving keys) straight into the
 // A-operand register fragments, split into bf16 hi/lo on the way.
-#include <unordered_map>
+#include <algorithm>
 
 #include "cg_net.cuh"
 #include "cg_tc_ptx.cuh"
@@ -133,61 +133,45 @@ float bf16_to_f(unsigned short h) {
   return f;
 }
 
-std::unordered_map<const float *, void *> g_images;   // device Wt pointer -> device operand image
-
 }  // namespace
 
+void cg_pack_bf16x2_block(const float *Wt, int C, int c0, int rows, int k0, unsigned char *hi, unsigned char *lo) {
+  for (int r = 0; r < rows; r++)
+    for (int kk = 0; kk < 64; kk++) {
+      const float w = Wt[(size_t)(k0 + kk) * C + c0 + r];
+      const unsigned short h = bf16_rne(w), l = bf16_rne(w - bf16_to_f(h));
+      const size_t off = row_chunk_off(r, kk >> 3) + (size_t)(kk & 7) * 2;
+      memcpy(hi + off, &h, 2);
+      memcpy(lo + off, &l, 2);
+    }
+}
+
 // image layout: [column tile (128 outputs)][K-block][hi 16 KB | lo 16 KB], rows past N are zero
-int cg_linear_tc_register(cg_ctx *ctx, const float *Wt_dev, const float *Wt_host, int K, int N) {
+int cg_linear_tc_image(cg_ctx *ctx, const float *Wt_host, int K, int N, const void **img) {
+  *img = nullptr;
   if (K % 64 != 0 || N < 64) return CG_OK;
   const int ntile = (N + 127) / 128, nkb = K / 64;
   const size_t bytes = (size_t)ntile * nkb * 2 * PIECE;
-  std::vector<unsigned char> img(bytes, 0);
+  std::vector<unsigned char> h(bytes, 0);
   for (int t = 0; t < ntile; t++)
     for (int kb = 0; kb < nkb; kb++) {
-      unsigned char *hi = img.data() + ((size_t)t * nkb + kb) * 2 * PIECE, *lo = hi + PIECE;
-      for (int r = 0; r < 128; r++) {
-        const int n = t * 128 + r;
-        if (n >= N) continue;
-        for (int kk = 0; kk < 64; kk++) {
-          const float w = Wt_host[(size_t)(kb * 64 + kk) * N + n];
-          const unsigned short h = bf16_rne(w), l = bf16_rne(w - bf16_to_f(h));
-          const size_t off = row_chunk_off(r, kk >> 3) + (size_t)(kk & 7) * 2;
-          memcpy(hi + off, &h, 2);
-          memcpy(lo + off, &l, 2);
-        }
-      }
+      unsigned char *hi = h.data() + ((size_t)t * nkb + kb) * 2 * PIECE;
+      cg_pack_bf16x2_block(Wt_host, N, 128 * t, std::min(128, N - 128 * t), 64 * kb, hi, hi + PIECE);
     }
+  CG_CUDA(ctx, cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LSMEM));
   void *d = nullptr;
   CG_CUDA(ctx, cudaMalloc(&d, bytes));
-  CG_CUDA(ctx, cudaMemcpyAsync(d, img.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
-  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  g_images[Wt_dev] = d;
+  *img = d;
+  CG_CUDA(ctx, cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // h goes out of scope
   return CG_OK;
 }
 
-void cg_linear_tc_unregister(const float *Wt_dev) {
-  auto it = g_images.find(Wt_dev);
-  if (it != g_images.end()) {
-    cudaFree(it->second);
-    g_images.erase(it);
-  }
-}
-
-// returns 1 if the layer was launched on tensor cores, 0 if the caller should use the FMA kernels, < 0 on error
-int cg_linear_tc_try(cg_ctx *ctx, const float *X, int M, int K, const float *Wt, const float *bias, int N, int relu,
-                     int bias_row_div, int x_is_keys, float *Y) {
-  if (ctx->engine < 1 || M < 64 || (K % 64) != 0) return 0;
-  auto it = g_images.find(Wt);
-  if (it == g_images.end()) return 0;
-  static bool attr_set[CG_MAX_DEVICES] = {};   // the attribute is per device
-  if (!attr_set[ctx->device]) {
-    CG_CUDA(ctx, cudaFuncSetAttribute(linear_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LSMEM));
-    attr_set[ctx->device] = true;
-  }
+int cg_linear_tc_launch(cg_ctx *ctx, const float *X, int M, int K, const void *img, const float *bias, int N, int relu,
+                        int bias_row_div, int x_is_keys, float *Y) {
   const dim3 grid = cg_row_tile_grid((N + 127) / 128, ((long long)M + 127) / 128);
-  linear_tc_kernel<<<grid, LT, LSMEM, ctx->stream>>>(X, M, K, static_cast<const unsigned char *>(it->second), bias, N, relu,
+  linear_tc_kernel<<<grid, LT, LSMEM, ctx->stream>>>(X, M, K, static_cast<const unsigned char *>(img), bias, N, relu,
                                                      bias_row_div, x_is_keys, Y);
   CG_LAUNCH_CHECK(ctx);
-  return 1;
+  return CG_OK;
 }

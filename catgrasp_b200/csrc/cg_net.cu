@@ -7,6 +7,8 @@
 //   64-ch point feature; the 1088->512 conv is split into its global part
 //   (computed once per cloud and used as a per-cloud bias) and its 64-ch
 //   point part, which removes 4.29 of 9.72 GMAC without changing the math.
+#include <memory>
+
 #include "cg_net.cuh"
 
 namespace {
@@ -50,12 +52,12 @@ extern "C" int cg_net_create(cg_ctx *ctx, int kind, int n_out, const float *blob
   CG_REQUIRE(ctx, n_out > 0 && (kind == CG_NET_SEG || n_out <= 32), "n_out");
   CG_REQUIRE(ctx, blob_host && blob_floats == cg_net_blob_floats(kind, n_out), "weight blob size mismatch");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  cg_net *net = new cg_net();
+  // value-initialised (null blob, images and layers), so that every error return below frees what exists so far
+  std::unique_ptr<cg_net, void (*)(cg_net *)> net(new cg_net(), cg_net_destroy);
   net->ctx = ctx;
   net->kind = kind;
   net->n_out = n_out;
   net->blob_floats = blob_floats;
-  for (int i = 0; i < 3; i++) net->tc_img[i] = nullptr;
   CG_CUDA(ctx, cudaMalloc(&net->blob_dev, blob_floats * sizeof(float)));
   CG_CUDA(ctx, cudaMemcpyAsync(net->blob_dev, blob_host, blob_floats * sizeof(float), cudaMemcpyHostToDevice,
                                ctx->stream));
@@ -80,22 +82,21 @@ extern "C" int cg_net_create(cg_ctx *ctx, int kind, int n_out, const float *blob
                            l1[i] >= 0 ? blob_host + woff[l1[i]] : nullptr, net->tc_img[i], &net->tc_f16_ok[i]);
     if (rc != CG_OK) return rc;
   }
-  // tensor-core images of the FC / head layers
+  // tensor-core images of the FC / head layers (the trunk layers have theirs in tc_img)
   const int fc_layers[] = {L_S3_F1, L_S3_F2, L_SK_F1, L_SK_F2, L_SK_F3, L_HEAD0, L_HEAD1, L_HEAD2, L_HEAD3, L_HEAD4};
   for (int li : fc_layers) {
-    if (d[li].K == 0) continue;
-    int rc = cg_linear_tc_register(ctx, net->L[li].Wt, blob_host + woff[li], d[li].K, d[li].C);
+    int rc = cg_linear_tc_image(ctx, blob_host + woff[li], d[li].K, d[li].C, &net->L[li].tc);
     if (rc != CG_OK) return rc;
   }
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  *out = net;
+  *out = net.release();
   return CG_OK;
 }
 
 extern "C" void cg_net_destroy(cg_net *net) {
   if (!net) return;
   cudaSetDevice(net->ctx->device);
-  for (int i = 0; i < L_COUNT; i++) cg_linear_tc_unregister(net->L[i].Wt);
+  for (int i = 0; i < L_COUNT; i++) cudaFree(const_cast<void *>(net->L[i].tc));
   cudaFree(net->blob_dev);
   for (int i = 0; i < 3; i++) cudaFree(net->tc_img[i]);
   delete net;
@@ -142,6 +143,16 @@ void encoder_ws_carve(cg_arena &ar, int B, EncoderWs &w) {
   w.T64 = ar.take<float>((size_t)B * 4096);
 }
 
+// The FC chain after a trunk (STN3d, STNkd, cls head): layers L[l], L[l+1], L[l+2] =
+// 1024 -> 512 (ReLU, from the max-pool keys in w.gmax) -> 256 (ReLU) -> out (no ReLU)
+int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, float *out) {
+  int rc;
+  if ((rc = cg_linear_launch(ctx, L[l], reinterpret_cast<const float *>(w.gmax), B, w.f1, CG_FC_RELU | CG_FC_KEYS)))
+    return rc;
+  if ((rc = cg_linear_launch(ctx, L[l + 1], w.f1, B, w.f2, CG_FC_RELU))) return rc;
+  return cg_linear_launch(ctx, L[l + 2], w.f2, B, out, 0);
+}
+
 // Runs the PointNetEncoder (pointnet2.py:241-271) for B clouds; on return w.gmax holds the
 // (B,1024) global feature as order-preserving keys; pf_out (optional) the 64-ch point feature.
 // keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.
@@ -159,18 +170,14 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   a.l2 = L[L_S3_C2]; a.l3 = L[L_S3_C3]; a.tc_img = net->tc_img[0]; a.tc_f16_ok = net->tc_f16_ok[0]; a.relu3 = 1; a.gmax_keys = w.gmax; a.pf_out = nullptr;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_S3_F1].Wt, L[L_S3_F1].b, 512, 1, 0, 1, w.f1))) return rc;
-  if ((rc = cg_linear_launch(ctx, w.f1, B, 512, L[L_S3_F2].Wt, L[L_S3_F2].b, 256, 1, 0, 0, w.f2))) return rc;
-  if ((rc = cg_linear_launch(ctx, w.f2, B, 256, L[L_S3_F3].Wt, L[L_S3_F3].b, 9, 0, 0, 0, w.T3))) return rc;
+  if ((rc = fc_chain(ctx, L, L_S3_F1, B, w, w.T3))) return rc;
   // --- trunk B: encoder conv1 + STNkd convs + max (pointnet2.py:252, :208-213)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.T3 = w.T3; a.l0 = L[L_E_C1]; a.stage1_mode = 1; a.l1 = L[L_SK_C1];
   a.l2 = L[L_SK_C2]; a.l3 = L[L_SK_C3]; a.tc_img = net->tc_img[1]; a.tc_f16_ok = net->tc_f16_ok[1]; a.relu3 = 1;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out + (size_t)B * 1024, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_SK_F1].Wt, L[L_SK_F1].b, 512, 1, 0, 1, w.f1))) return rc;
-  if ((rc = cg_linear_launch(ctx, w.f1, B, 512, L[L_SK_F2].Wt, L[L_SK_F2].b, 256, 1, 0, 0, w.f2))) return rc;
-  if ((rc = cg_linear_launch(ctx, w.f2, B, 256, L[L_SK_F3].Wt, L[L_SK_F3].b, 4096, 0, 0, 0, w.T64))) return rc;
+  if ((rc = fc_chain(ctx, L, L_SK_F1, B, w, w.T64))) return rc;
   // --- trunk C: conv1, @T64, conv2, conv3(+BN, no ReLU), max (pointnet2.py:252-265)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.stage1_mode = 2; a.T64 = w.T64; a.l1 = cg_layer{nullptr, nullptr, 64, 64};
@@ -202,11 +209,8 @@ int cls_forward_impl(cg_net *net, const cg_input_src &in_all, int B_all, int N, 
     if (in.poses) in.poses += (size_t)b0 * 16;
     if (in.ids) in.ids += (size_t)b0 * N;
     if ((rc = encoder_forward(net, in, B, N, w, nullptr))) return rc;
-    const cg_layer *L = net->L;
-    if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_HEAD0].Wt, L[L_HEAD0].b, 512, 1, 0, 1, w.f1))) return rc;
-    if ((rc = cg_linear_launch(ctx, w.f1, B, 512, L[L_HEAD1].Wt, L[L_HEAD1].b, 256, 1, 0, 0, w.f2))) return rc;
     float *lg = out_logits ? out_logits + (size_t)b0 * n_out : logits_ws;
-    if ((rc = cg_linear_launch(ctx, w.f2, B, 256, L[L_HEAD2].Wt, L[L_HEAD2].b, n_out, 0, 0, 0, lg))) return rc;
+    if ((rc = fc_chain(ctx, net->L, L_HEAD0, B, w, lg))) return rc;
     if (out_probs || out_label) {
       if ((rc = cg_softmax_launch(ctx, lg, B, n_out, out_probs ? out_probs + (size_t)b0 * n_out : nullptr,
                                   out_label ? out_label + b0 : nullptr)))
@@ -245,11 +249,11 @@ int seg_forward_impl(cg_net *net, const float *x, int B, int N, float *out_logit
   if ((rc = encoder_forward(net, in, B, N, w, pf))) return rc;
   const cg_layer *L = net->L;
   // global half of conv1 (pointnet2.py:270-271 tiles the global feature over N; it is constant per cloud)
-  if ((rc = cg_linear_launch(ctx, reinterpret_cast<float *>(w.gmax), B, 1024, L[L_HEAD0].Wt, L[L_HEAD0].b, 512, 0, 0, 1, biasg))) return rc;
-  if ((rc = cg_linear_launch(ctx, pf, (int)P, 64, L[L_HEAD1].Wt, biasg, 512, 1, N, 0, y1))) return rc;
-  if ((rc = cg_linear_launch(ctx, y1, (int)P, 512, L[L_HEAD2].Wt, L[L_HEAD2].b, 256, 1, 0, 0, y2))) return rc;
-  if ((rc = cg_linear_launch(ctx, y2, (int)P, 256, L[L_HEAD3].Wt, L[L_HEAD3].b, 128, 1, 0, 0, y3))) return rc;
-  if ((rc = cg_linear_launch(ctx, y3, (int)P, 128, L[L_HEAD4].Wt, L[L_HEAD4].b, n_out, 0, 0, 0, lg))) return rc;
+  if ((rc = cg_linear_launch(ctx, L[L_HEAD0], reinterpret_cast<const float *>(w.gmax), B, biasg, CG_FC_KEYS))) return rc;
+  if ((rc = cg_linear_launch(ctx, L[L_HEAD1], pf, (int)P, y1, CG_FC_RELU, biasg, N))) return rc;
+  if ((rc = cg_linear_launch(ctx, L[L_HEAD2], y1, (int)P, y2, CG_FC_RELU))) return rc;
+  if ((rc = cg_linear_launch(ctx, L[L_HEAD3], y2, (int)P, y3, CG_FC_RELU))) return rc;
+  if ((rc = cg_linear_launch(ctx, L[L_HEAD4], y3, (int)P, lg, 0))) return rc;
   if (out_coords || out_conf || out_bins) {
     CG_REQUIRE(ctx, bins > 0 && bins * 3 == n_out, "nunocs: n_out != 3*bins");
     if ((rc = cg_nunocs_post_launch(ctx, lg, (int)P, bins, out_coords, out_conf, out_bins))) return rc;

@@ -1,12 +1,15 @@
-// cg_net.cuh -- network weight table + trunk launch interface (internal).
+// cg_net.cuh -- network weight table, trunk and fully-connected launch interfaces (internal).
 #pragma once
 #include "cg_common.cuh"
 
-// One folded (conv|linear)+BN layer: Wt is [K][C] row-major (k-major), b is [C].
+// One folded (conv|linear)+BN layer: Wt is [K][C] row-major (k-major), b is [C].  tc is the layer's own wgmma operand
+// image (cg_linear_tc_image), owned by the net / MLP that holds the layer; null for shapes the tensor-core FC kernel
+// does not take and for layers that are not launched through cg_linear_launch (the trunk layers).
 struct cg_layer {
   const float *Wt;
   const float *b;
   int K, C;
+  const void *tc;
 };
 
 // Weight order inside the blob (must match catgrasp_b200/weights.py:BLOB_ORDER).
@@ -64,8 +67,13 @@ struct cg_trunk_args {
 int cg_trunk_launch_simt(cg_ctx *ctx, const cg_trunk_args &a);
 int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a);   // engines 1-3 (wgmma)
 size_t cg_tc_image_bytes();
-// Wt3 [128][1024], Wt2 [64][128], Wt1 [64][64] or nullptr (folded fp32, k-major rows, host)
+// Wt3 [128][1024], Wt2 [64][128], Wt1 [64][64] or nullptr (folded fp32, k-major rows, host).  Also sets the trunk
+// kernels' shared-memory limit on the current device, so it runs there before any trunk launch that uses the image.
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok);
+
+// Packs rows c0 .. c0+rows-1 (output channels) of the K-block k0 .. k0+63 of a host weight Wt [K][C] (k-major) into
+// the swizzled [rows x 64] bf16 hi / lo operand pieces of the wgmma kernels (w = hi + lo, both round-to-nearest-even).
+void cg_pack_bf16x2_block(const float *Wt, int C, int c0, int rows, int k0, unsigned char *hi, unsigned char *lo);
 
 // Row tiles of the fully-connected kernels: gridDim.y is capped at 65535, so the tiles are spread over (y, z) and a
 // launch covers up to 2^31 rows.  tile = blockIdx.z * gridDim.y + blockIdx.y; CTAs past the last tile exit at once.
@@ -75,15 +83,20 @@ inline dim3 cg_row_tile_grid(unsigned col_tiles, long long row_tiles) {
 }
 __device__ __forceinline__ long long cg_row_tile() { return (long long)blockIdx.z * gridDim.y + blockIdx.y; }
 
-// Y[M][N] = act(X[M][K] @ Wt[K][N] + bias[(row / bias_row_div)][N])
-// x_is_keys: X holds order-preserving uint keys (output of a trunk) to be decoded on load.
-int cg_linear_launch(cg_ctx *ctx, const float *X, int M, int K, const float *Wt, const float *bias,
-                     int N, int relu, int bias_row_div, int x_is_keys, float *Y);
-// tensor-core FC path (cg_linear_tc.cu)
-int cg_linear_tc_register(cg_ctx *ctx, const float *Wt_dev, const float *Wt_host, int K, int N);
-void cg_linear_tc_unregister(const float *Wt_dev);
-int cg_linear_tc_try(cg_ctx *ctx, const float *X, int M, int K, const float *Wt, const float *bias, int N, int relu,
-                     int bias_row_div, int x_is_keys, float *Y);
+// Y[M][C] = act(X[M][K] @ L.Wt[K][C] + bias[(row / rows_per_bias)][C]), bias = row_bias if given, else L.b.
+// Runs on tensor cores when the engine is >= 1, the layer has an image (L.tc) and M >= 64; else on the FMA kernels.
+enum : unsigned {
+  CG_FC_RELU = 1u,   // ReLU after the bias
+  CG_FC_KEYS = 2u,   // X holds order-preserving uint keys (a trunk's max-pool output), decoded on load
+};
+int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, float *Y, unsigned flags,
+                     const float *row_bias = nullptr, int rows_per_bias = 0);
+// tensor-core FC path (cg_linear_tc.cu).  The image builder returns nullptr in *img for shapes the kernel does not take
+// (K % 64 != 0 or N < 64); otherwise a device image the caller frees with cudaFree.  It also sets the kernel's
+// shared-memory limit on the current device.
+int cg_linear_tc_image(cg_ctx *ctx, const float *Wt_host, int K, int N, const void **img);
+int cg_linear_tc_launch(cg_ctx *ctx, const float *X, int M, int K, const void *img, const float *bias, int N, int relu,
+                        int bias_row_div, int x_is_keys, float *Y);
 int cg_softmax_launch(cg_ctx *ctx, const float *logits, int B, int C, float *probs, int32_t *label);
 int cg_nunocs_post_launch(cg_ctx *ctx, const float *logits, int P, int bins, float *coords,
                           float *conf_z, int32_t *out_bins);

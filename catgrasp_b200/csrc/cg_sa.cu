@@ -8,17 +8,17 @@
 //   SA:  sample_and_group -> (B,S,K,3+D) -> [1x1 conv + BN + ReLU] x L over all B*S*K rows -> max over K -> (B,S,C_L)
 //   FP:  3 nearest neighbours of every dense point among the S sparse points (expanded-form square_distance, :14-33),
 //        weights (1/(d+1e-8)) / sum, weighted sum of their features -> concat skip features -> [conv + BN + ReLU] x L
-// A layer whose K is a multiple of 64 and that has >= 64 rows runs on wgmma (linear_tc_kernel, bf16 hi/lo x3, fp32
-// accumulate); the first layer of an SA stack (K = 3 + D, typically 6) is an FMA kernel -- it is not a tensor-core shape.
+// Every layer is launched through cg_linear_launch: a layer with a tensor-core image (K a multiple of 64, >= 64 output
+// channels) and >= 64 rows runs on wgmma (linear_tc_kernel, bf16 hi/lo x3, fp32 accumulate); the first layer of an SA
+// stack (K = 3 + D, typically 6) is an FMA kernel -- it is not a tensor-core shape.
 #include <float.h>
+#include <memory>
 
 #include "cg_net.cuh"
 
 struct cg_mlp {
   cg_ctx *ctx;
-  int nlayers;
-  std::vector<int> dims;        // nlayers + 1
-  std::vector<float *> Wt, b;   // device, Wt[i] is [dims[i]][dims[i+1]] k-major (BN folded by the host)
+  std::vector<cg_layer> L;   // device weights (BN folded by the host), each layer's tensor-core image owned here
 };
 
 namespace {
@@ -116,17 +116,18 @@ __global__ void three_interp_kernel(const float *__restrict__ points1, int D1, c
 
 int run_mlp(cg_mlp *m, const float *x, long long R, float *out_last, float **last_buf) {
   cg_ctx *ctx = m->ctx;
+  const int nlayers = (int)m->L.size();
   int maxc = 0;
-  for (int i = 1; i <= m->nlayers; i++) maxc = m->dims[i] > maxc ? m->dims[i] : maxc;
+  for (const cg_layer &l : m->L) maxc = l.C > maxc ? l.C : maxc;
   const size_t buf = cg_arena::pad((size_t)R * maxc * sizeof(float));
   int rc = cg_ws_reserve(ctx, 2 * buf + 4096);
   if (rc) return rc;
   cg_arena ar(ctx->ws);
   float *pp[2] = {ar.take<float>((size_t)R * maxc), ar.take<float>((size_t)R * maxc)};
   const float *cur = x;
-  for (int i = 0; i < m->nlayers; i++) {
-    float *dst = (i == m->nlayers - 1 && out_last) ? out_last : pp[i & 1];
-    if ((rc = cg_linear_launch(ctx, cur, (int)R, m->dims[i], m->Wt[i], m->b[i], m->dims[i + 1], 1, 0, 0, dst))) return rc;
+  for (int i = 0; i < nlayers; i++) {
+    float *dst = (i == nlayers - 1 && out_last) ? out_last : pp[i & 1];
+    if ((rc = cg_linear_launch(ctx, m->L[i], cur, (int)R, dst, CG_FC_RELU))) return rc;
     cur = dst;
   }
   if (last_buf) *last_buf = const_cast<float *>(cur);
@@ -141,37 +142,38 @@ extern "C" int cg_mlp_create(cg_ctx *ctx, int nlayers, const int *dims, const fl
   CG_REQUIRE(ctx, nlayers >= 1 && nlayers <= 8 && dims && Wt_host && b_host, "mlp_create: bad arguments");
   for (int i = 0; i <= nlayers; i++) CG_REQUIRE(ctx, dims[i] > 0 && dims[i] <= 4096, "mlp_create: channel count out of range");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  cg_mlp *m = new cg_mlp();
+  // null layers, so that every error return below frees what exists so far
+  std::unique_ptr<cg_mlp, void (*)(cg_mlp *)> m(new cg_mlp(), cg_mlp_destroy);
   m->ctx = ctx;
-  m->nlayers = nlayers;
-  m->dims.assign(dims, dims + nlayers + 1);
+  m->L.assign(nlayers, cg_layer{});
   for (int i = 0; i < nlayers; i++) {
+    cg_layer &l = m->L[i];
+    l.K = dims[i];
+    l.C = dims[i + 1];
     float *W = nullptr, *b = nullptr;
-    const size_t nw = (size_t)dims[i] * dims[i + 1];
+    const size_t nw = (size_t)l.K * l.C;
     CG_CUDA(ctx, cudaMalloc(&W, nw * sizeof(float)));
-    CG_CUDA(ctx, cudaMalloc(&b, (size_t)dims[i + 1] * sizeof(float)));
+    l.Wt = W;
+    CG_CUDA(ctx, cudaMalloc(&b, (size_t)l.C * sizeof(float)));
+    l.b = b;
     CG_CUDA(ctx, cudaMemcpyAsync(W, Wt_host[i], nw * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    CG_CUDA(ctx, cudaMemcpyAsync(b, b_host[i], (size_t)dims[i + 1] * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    m->Wt.push_back(W);
-    m->b.push_back(b);
-    if (dims[i] % 64 == 0) {   // tensor-core image (bf16 hi/lo) for layers that are a dense contraction
-      const int rc = cg_linear_tc_register(ctx, W, Wt_host[i], dims[i], dims[i + 1]);
-      if (rc != CG_OK) return rc;
-    }
+    CG_CUDA(ctx, cudaMemcpyAsync(b, b_host[i], (size_t)l.C * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    const int rc = cg_linear_tc_image(ctx, Wt_host[i], l.K, l.C, &l.tc);
+    if (rc != CG_OK) return rc;
   }
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  *out = m;
+  *out = m.release();
   return CG_OK;
 }
 
 extern "C" void cg_mlp_destroy(cg_mlp *m) {
   if (!m) return;
   cudaSetDevice(m->ctx->device);
-  for (float *W : m->Wt) {
-    cg_linear_tc_unregister(W);
-    cudaFree(W);
+  for (const cg_layer &l : m->L) {
+    cudaFree(const_cast<float *>(l.Wt));
+    cudaFree(const_cast<float *>(l.b));
+    cudaFree(const_cast<void *>(l.tc));
   }
-  for (float *b : m->b) cudaFree(b);
   delete m;
 }
 
@@ -191,7 +193,7 @@ extern "C" int cg_group_mlp_max_dev(cg_mlp *m, const float *grouped, int G, int 
   float *last = nullptr;
   int rc = run_mlp(m, grouped, (long long)G * K, nullptr, &last);
   if (rc) return rc;
-  const int C = m->dims[m->nlayers];
+  const int C = m->L.back().C;
   const long long total = (long long)G * C;
   group_max_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(last, G, K, C, out);
   CG_LAUNCH_CHECK(ctx);

@@ -519,38 +519,14 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   }
 }
 
-unsigned short bf16_rne(float f) {
-  uint32_t x;
-  memcpy(&x, &f, 4);
-  const uint32_t lsb = (x >> 16) & 1u;
-  x += 0x7fffu + lsb;
-  return (unsigned short)(x >> 16);
-}
-float bf16_to_f(unsigned short h) {
-  uint32_t x = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &x, 4);
-  return f;
-}
-
-// One [rows x 64] K-block (k0 .. k0+63) of a folded layer as bf16 hi / lo swizzled images; rows = output channels
-// c0 .. c0+rows-1.  Wt is [K][C] (k-major rows, as in the weight blob).
-void pack_block(const float *Wt, int C, int c0, int rows, int k0, unsigned char *hi, unsigned char *lo) {
-  for (int r = 0; r < rows; r++)
-    for (int kk = 0; kk < 64; kk++) {
-      const float w = Wt[(size_t)(k0 + kk) * C + c0 + r];
-      const unsigned short h = bf16_rne(w), l = bf16_rne(w - bf16_to_f(h));
-      const size_t off = row_chunk_off(r, kk >> 3) + (size_t)(kk & 7) * 2;
-      memcpy(hi + off, &h, 2);
-      memcpy(lo + off, &l, 2);
-    }
-}
-
 }  // namespace
 
 size_t cg_tc_image_bytes() { return (size_t)IMG_W3H_OFF + IMG_W3H; }
 
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok) {
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   float wmax = 0.f;
   for (size_t i = 0; i < (size_t)128 * 1024; i++) wmax = fmaxf(wmax, fabsf(Wt3[i]));
   *f16_ok = (wmax < 65504.f) ? 1 : 0;   // otherwise the fp16 image would hold infinities
@@ -558,10 +534,10 @@ int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *
   for (int ch = 0; ch < NCHUNK; ch++)
     for (int kb = 0; kb < 2; kb++) {
       unsigned char *hi = img.data() + (size_t)(ch * 2 + kb) * 2 * PIECE;
-      pack_block(Wt3, 1024, ch * 128, 128, kb * 64, hi, hi + PIECE);
+      cg_pack_bf16x2_block(Wt3, 1024, ch * 128, 128, kb * 64, hi, hi + PIECE);
     }
-  pack_block(Wt2, 128, 0, 128, 0, img.data() + IMG_W2_OFF, img.data() + IMG_W2_OFF + PIECE);
-  if (Wt1) pack_block(Wt1, 64, 0, 64, 0, img.data() + IMG_W1_OFF, img.data() + IMG_W1_OFF + 8192);
+  cg_pack_bf16x2_block(Wt2, 128, 0, 128, 0, img.data() + IMG_W2_OFF, img.data() + IMG_W2_OFF + PIECE);
+  if (Wt1) cg_pack_bf16x2_block(Wt1, 64, 0, 64, 0, img.data() + IMG_W1_OFF, img.data() + IMG_W1_OFF + 8192);
   // fp16 single-term W3 for the fp16 engines: [chunk][kb] 16 KB
   for (int ch = 0; ch < NCHUNK; ch++)
     for (int r = 0; r < 128; r++)
@@ -582,13 +558,6 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
   CG_REQUIRE(ctx, a.B > 0 && a.N > 0, "trunk: B,N must be positive");
   CG_REQUIRE(ctx, a.B <= 65535, "trunk: B > 65535 must be chunked by the caller");
   CG_REQUIRE(ctx, a.tc_img != nullptr, "trunk: tensor-core weight image missing");
-  static bool attr_set[CG_MAX_DEVICES] = {};   // the attribute is per device
-  if (!attr_set[ctx->device]) {
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    attr_set[ctx->device] = true;
-  }
   // split a candidate's tiles over CTAs only while there are fewer than ~4 CTAs per SM
   const int ntiles = (a.N + TP - 1) / TP;
   int splits = 1;

@@ -186,7 +186,8 @@ class FoldedNet:
 
     @staticmethod
     def fc_on_tc(engine, M, K, C):
-        """cg_linear_launch runs a layer on tensor cores when all of these hold (cg_linear_tc.cu, cg_linear_tc_try)."""
+        """cg_linear_launch runs a layer on tensor cores when all of these hold (cg_linear.cu): engine >= 1, at least
+        64 rows, and the layer has a tensor-core image, which cg_linear_tc_image builds for K % 64 == 0 and C >= 64."""
         return engine >= 1 and M >= 64 and K % 64 == 0 and C >= 64
 
     # ------------------------------------------------------------------------------------------------ trunks
