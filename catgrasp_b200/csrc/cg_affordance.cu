@@ -99,6 +99,10 @@ __global__ void __launch_bounds__(AT) affordance_kernel(const double *__restrict
     __syncthreads();
     int jstar = sh_i[0];
     for (int w = 1; w < AT / 32; w++) jstar = min(jstar, sh_i[w]);
+    if (jstar == 0x7fffffff) {                       // empty patch: tol < 0 or NaN (contact_mask.sum()==0, :268-269)
+      if (tid == 0) out_contacts[g * MAXF + f] = 0;
+      continue;
+    }
     sum = block_sum(sum, sh);
     cnt = block_sum(cnt, sh);
     // normal at the closest point, rotated into the finger frame; only the sign of its y component matters (:277-281)

@@ -1,7 +1,8 @@
 // cg_ransac.cu -- hypothesis scoring of the NUNOCS 9-DoF RANSAC (SURVEY.md 8f F1).
 //
 // Replaces the loop body of aligning.py:36-81 (estimate9DTransform_worker) for all hypotheses at once:
-//   4-point affine (cv2.estimateAffine3D on 4 correspondences = the exact affine through them, aligning.py:23-33)
+//   4-point affine (cv2.estimateAffine3D on 4 correspondences = the exact affine through them, or the minimum-norm
+//   least-squares affine when the 4 points are affinely dependent, aligning.py:23-33)
 //   -> per-axis scales and scale gates (:41-43) -> R = A / scales, singular values in [0.8, 1.2] (:45-49)
 //   -> R := U V^T, det > 0 (:51-53) -> T = [R diag(scales) | t] (:55)
 //   -> extent of inv(T) target <= max_dimensions (:58-62) -> inlier ratio |T src - tgt| <= threshold (:64-67).
@@ -38,6 +39,53 @@ __device__ bool solve4(double M[4][4], double B[4][3], double X[4][3]) {
       X[c][k] = s / M[perm[c]][c];
     }
   return true;
+}
+
+// Minimum-norm least-squares solution X = pinv(M) B, the answer cv2.estimateAffine3D gives on 4 points when M is
+// singular: it solves the 12x12 system (M's singular values, each three times) with DECOMP_SVD, which drops singular
+// values <= 2 DBL_EPSILON * (sum of the 12) = 6 DBL_EPSILON * sum_j sigma_j(M) (OpenCV 4.13, bisected on cv2).
+// One-sided (Hestenes) Jacobi on the columns of M: M V = W with orthogonal columns w_j = sigma_j u_j, so
+// pinv(M) B = sum over kept j of v_j (w_j^T B) / sigma_j^2.  Small singular values come out to ~eps * sigma_max
+// (an eigen-decomposition of M^T M would give sqrt(eps) * sigma_max, above the threshold).
+__device__ void minnorm4(const double Min[4][4], const double B[4][3], double X[4][3]) {
+  double W[4][4], V[4][4];
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++) { W[i][j] = Min[i][j]; V[i][j] = (i == j) ? 1.0 : 0.0; }
+  for (int sweep = 0; sweep < 30; sweep++) {
+    bool rotated = false;
+    for (int p = 0; p < 3; p++)
+      for (int q = p + 1; q < 4; q++) {
+        double a = 0.0, b = 0.0, g = 0.0;
+        for (int i = 0; i < 4; i++) { a += W[i][p] * W[i][p]; b += W[i][q] * W[i][q]; g += W[i][p] * W[i][q]; }
+        if (fabs(g) <= 1e-300 || fabs(g) <= 2.220446049250313e-16 * sqrt(a * b)) continue;
+        rotated = true;
+        const double zeta = (b - a) / (2.0 * g);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+        for (int i = 0; i < 4; i++) {
+          const double wp = W[i][p], wq = W[i][q];
+          W[i][p] = c * wp - s * wq; W[i][q] = s * wp + c * wq;
+          const double vp = V[i][p], vq = V[i][q];
+          V[i][p] = c * vp - s * vq; V[i][q] = s * vp + c * vq;
+        }
+      }
+    if (!rotated) break;
+  }
+  double sig2[4], sum = 0.0;
+  for (int j = 0; j < 4; j++) {
+    sig2[j] = W[0][j] * W[0][j] + W[1][j] * W[1][j] + W[2][j] * W[2][j] + W[3][j] * W[3][j];
+    sum += sqrt(sig2[j]);
+  }
+  const double cut = 6.0 * 2.220446049250313e-16 * sum;
+  for (int r = 0; r < 4; r++)
+    for (int k = 0; k < 3; k++) X[r][k] = 0.0;
+  for (int j = 0; j < 4; j++) {
+    if (!(sqrt(sig2[j]) > cut)) continue;
+    for (int k = 0; k < 3; k++) {
+      const double proj = (W[0][j] * B[0][k] + W[1][j] * B[1][k] + W[2][j] * B[2][k] + W[3][j] * B[3][k]) / sig2[j];
+      for (int r = 0; r < 4; r++) X[r][k] += V[r][j] * proj;
+    }
+  }
 }
 
 // symmetric 3x3 eigen-decomposition by cyclic Jacobi: A = V diag(w) V^T
@@ -86,20 +134,23 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
   const int h = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   if (tid == 0) {
     ok = 0;
-    double M[4][4], B[4][3], X[4][3];
+    double M[4][4], B[4][3], X[4][3], M0[4][4], B0[4][3];
     for (int i = 0; i < 4; i++) {
       const int id = ids[h * 4 + i];
       // cv2.estimateAffine3D (aligning.py:27) narrows its inputs to CV_32F before the double-precision solve:
       // the four sample points go through float, the residual pass below keeps the caller's float64.
       for (int k = 0; k < 3; k++) {
-        M[i][k] = (double)(float)src[(size_t)id * 3 + k];
-        B[i][k] = (double)(float)tgt[(size_t)id * 3 + k];
+        M[i][k] = M0[i][k] = (double)(float)src[(size_t)id * 3 + k];
+        B[i][k] = B0[i][k] = (double)(float)tgt[(size_t)id * 3 + k];
       }
-      M[i][3] = 1.0;
+      M[i][3] = M0[i][3] = 1.0;
     }
-    bool good = solve4(M, B, X);   // X[j][k]: dst_k = sum_j X[j][k] * [src,1]_j  -> A[k][j] = X[j][k]
+    // X[j][k]: dst_k = sum_j X[j][k] * [src,1]_j  -> A[k][j] = X[j][k].  A pivot below 1e-12 (duplicate, coplanar or
+    // nearly so) sends the subset to the minimum-norm solve; it is as rare as such subsets are.
+    if (!solve4(M, B, X)) minnorm4(M0, B0, X);
+    bool good = true;
     double A[3][3], t[3], sc[3];
-    if (good) {
+    {
       for (int k = 0; k < 3; k++) {
         for (int j = 0; j < 3; j++) A[k][j] = X[j][k];
         t[k] = X[3][k];

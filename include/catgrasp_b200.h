@@ -264,8 +264,14 @@ int cg_occupancy_from_scan_host(cg_ctx *ctx, const float *pts_host, int P, float
 /* ---- NUNOCS 9-DoF RANSAC hypothesis scoring -------------------------------------
  * Replaces: aligning.py:36-81 (estimate9DTransform_worker) for H hypotheses at once.
  *   source, target (N,3) float64 correspondences; ids (H,4) int32 = the 4-subsets (host numpy RNG, aligning.py:91-97)
+ *   The 4-point affine is cv2.estimateAffine3D's: the exact solution when the float32-narrowed points are affinely
+ *   independent, else the minimum-norm least-squares one (singular values <= 6 DBL_EPSILON * their sum dropped).
+ *   The minimum-norm solve runs when the LU solve meets a pivot < 1e-12; a system that is nonsingular by that test
+ *   but whose smallest singular value is under cv2's cut (large coordinates; not for points in the unit cube)
+ *   keeps the LU answer where cv2 would truncate.
  *   out_valid[h] = hypothesis passed the scale / singular-value / det / max_dimensions gates
- *   out_ratio[h] = inlier ratio at pass_threshold, out_T[h] = (4,4) float64 transform R diag(scales) | t           */
+ *   out_ratio[h] = inlier ratio at pass_threshold, out_T[h] = (4,4) float64 transform R diag(scales) | t;
+ *   where out_valid[h] = 0: out_ratio[h] = 0 and out_T[h] is all zeros                                              */
 int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids, int H,
                      double pass_threshold, const double min_scale[3], const double max_scale[3],
                      const double *max_dims, double *out_ratio, double *out_T, unsigned char *out_valid);
@@ -293,7 +299,10 @@ int cg_center_grasps_dev(cg_ctx *ctx, double *poses64, float *poses32, int P, co
  *   canonical point (:62-63, gathered once per object on the host)
  *   finger_boxes (F,4) = x min, x max, z min, z max of each finger mesh (:252); grip_dirs (F) = +1 / -1 for a finger closing
  *   along +y / -y (:261-266); 1 <= F <= 4
- *   out_p (G) = p(T|G), NaN where the reference drops the grasp; out_contacts (G,4) = contact-patch sizes per finger.   */
+ *   surface_tol: a point is in the patch when |y - extreme y| <= surface_tol; a negative or NaN tolerance leaves every
+ *   patch empty, which drops the finger (:268-269) without reading a normal
+ *   out_p (G) = p(T|G), NaN where the reference drops the grasp; out_contacts (G,4) = contact-patch sizes per finger
+ *   (0 for a dropped finger).                                                                                          */
 int cg_grasp_affordance_dev(cg_ctx *ctx, const double *cam_in_finger, int G, const double *pts, const double *nrm,
                             const double *affordance, int P, const double *finger_boxes, const int *grip_dirs, int F,
                             double surface_tol, double *out_p, int *out_contacts);

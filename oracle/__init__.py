@@ -26,4 +26,6 @@ Pinning status (DESIGN.md section "Oracle"):
   * filter64.py                 : float64 statement of the filter's predicate on sdf_ref.py's lookups, with a rigorous
     bound on the float32 pipeline; checks filter_ref.c and the kernel on every verdict the bound decides
     (tests/test_filter_ref.py, tests/test_filter_kernel.py).
+  * ransac64.py                 : one RANSAC hypothesis in high precision (cv2's 4-point affine, gate margins, a bound on
+    the kernel's T, the inlier count as an interval); pinned to cv2 via aligning_ref._hypothesis (tests/test_ransac_ref.py).
 """
