@@ -18,11 +18,20 @@
 // On both fp16 engines X3 values above the fp16 range are clamped to 65504 AND reported through
 // cg_trunk_args::ovf_flag so that the host can re-run on engine 1.
 //
-// CTA = 288 threads, 1 per SM: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the
-// whole layer chain for its points) and one producer warp.  The two warpgroups are independent except for the shared
-// W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core work; warpgroup 1
-// starts one front (input + FMA + L1 + L2) behind warpgroup 0 so that their fronts do not coincide.
+// Persistent grid: one CTA per SM.  The B x ntiles tiles are numbered candidate-major and CTA i runs the contiguous
+// range [i T / G, (i + 1) T / G), so ranges differ by at most one tile and may start or end inside a candidate (the
+// global max is an atomicMax on order-preserving keys, so a candidate split over CTAs needs nothing else).
+//
+// CTA = 384 threads: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the whole layer
+// chain for its points), one producer warp and three helper warps.  The two consumer warpgroups are independent except
+// for the shared W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core
+// work; warpgroup 1 starts one front (input + FMA + L1 + L2) behind warpgroup 0 so that their fronts do not coincide.
+// The helpers keep per-candidate work off the consumers' path: the next candidate's pose inverse, T3 and T64 operand
+// image, and the global fold (bias, ReLU, atomicMax) of each finished candidate's running max.
+#include <limits.h>
 #include <stdlib.h>
+
+#include <algorithm>
 
 #include "cg_tc_ptx.cuh"
 #include "cg_trunk_common.cuh"
@@ -33,17 +42,21 @@ using namespace cg_ptx;
 
 constexpr int NCW = 8;                      // consumer warps (two warpgroups)
 constexpr int PROD_WARP = NCW;              // warp 8: W1 / W2 / W3 producer
-constexpr int NTC = (NCW + 1) * 32;         // 288 threads
+constexpr int HELP_WARP = NCW + 1;          // warps 9-11: per-candidate helpers
+constexpr int NHELP = 3 * 32;
+constexpr int NTC = (NCW + 4) * 32;         // 384 threads
 constexpr int NCHUNK = 8;                   // 1024 output channels / 128
 constexpr uint32_t PIECE = 16384;           // [128 rows x 64 x 16-bit] one swizzled K-block
 // shared-memory map
-constexpr uint32_t W1_OFF = 0;              // [hi 8 KB | lo 8 KB]: shared W1, or the per-candidate T64 operand
+constexpr uint32_t W1_OFF = 0;              // [hi 8 KB | lo 8 KB]: shared W1, or the current candidate's T64 operand
 constexpr uint32_t W2_OFF = PIECE;          // [hi 16 KB | lo 16 KB]
 constexpr uint32_t RING_OFF = 3 * PIECE;    // 128 KB of W3 slots (one slot = one 64-wide K-block of a 128-channel chunk)
 constexpr uint32_t RING_BYTES = 8 * PIECE;
 constexpr uint32_t SACC_OFF = RING_OFF + RING_BYTES;   // running max: float2 per (warpgroup, half-chunk, warp, lane)
 constexpr uint32_t SACC_BYTES = 2 * 2 * NCHUNK * 4 * 32 * 8;
-constexpr uint32_t MISC_OFF = SACC_OFF + SACC_BYTES;
+constexpr uint32_t KEYS_OFF = SACC_OFF + SACC_BYTES;   // per-candidate max keys [2][1024], by candidate parity
+constexpr uint32_t KEYS_BYTES = 2 * 1024 * 4;
+constexpr uint32_t MISC_OFF = KEYS_OFF + KEYS_BYTES;
 constexpr int NSLOT_MAX = 8;
 // operand image built by cg_tc_prepare
 constexpr uint32_t IMG_W3B = NCHUNK * 2 * 2 * PIECE;   // bf16: [chunk][kb][hi 16 KB | lo 16 KB]
@@ -64,12 +77,15 @@ struct Misc {
   unsigned long long full_bar[NSLOT_MAX];    // producer -> consumers: W3 slot landed
   unsigned long long empty_bar[NSLOT_MAX];   // consumers -> producer: every consumer warp is done reading the slot
   unsigned long long w_bar;                  // resident W1 / W2 landed
+  // Per-candidate hand-offs; k counts the candidates of the CTA's range.  pinv, T3 and the T64 image exist once: the
+  // helpers rewrite them for candidate k + 1 between the consumers' last front of candidate k and their first of k + 1.
+  unsigned long long cand_bar;               // helpers -> consumers: pinv / T3 / T64 image of candidate k written
+  unsigned long long front_bar;              // consumers -> helpers: every consumer is past the last front of k
+  unsigned long long keys_bar[2];            // consumers -> helpers: candidate k's max is in keys[k & 1]
 };
 
 constexpr size_t SMEM_BYTES = MISC_OFF + sizeof(Misc);
 static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_90");
-
-__device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // One step of the transposing column-max butterfly of the L3 reduction: the lanes with bit STEP set keep the upper
 // half of their STEP columns, the others the lower half, and each takes the max with its partner's copy.  STEP is a
@@ -86,9 +102,9 @@ __device__ __forceinline__ void max_butterfly_step(float *x, int lane) {
 }
 
 #ifdef CG_EXPERIMENTS
-// Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer warp of TL_CTAS sampled CTAs (blockIdx.x 0,
-// candidates spread over the batch) sums clock64() cycles per phase over its tiles and writes one record of
-// TL_REC words: the TL_NPHASE sums, its tile count and its total cycles.  TL_L3_WAIT and TL_RING lie inside TL_L3.
+// Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer warp of TL_CTAS sampled CTAs (spread over
+// the grid) sums clock64() cycles per phase over its tiles and writes one record of TL_REC words: the TL_NPHASE
+// sums, its tile count and its total cycles.  TL_L3_WAIT and TL_RING lie inside TL_L3.
 enum { TL_START, TL_INPUT, TL_FRONT, TL_L3, TL_L3_WAIT, TL_RING, TL_NPHASE };
 constexpr int TL_CTAS = 8, TL_REC = 8;
 __host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / TL_CTAS : 1; }
@@ -100,7 +116,7 @@ __host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / T
 #endif
 
 template <int PASSES>
-__global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a, int tiles_per_cta TL_PARAM) {
+__global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a TL_PARAM) {
   constexpr int NSLOT = PASSES == 3 ? 4 : 8;
   constexpr uint32_t SLOT_BYTES = PASSES == 3 ? 2 * PIECE : PIECE;
   constexpr bool F16 = PASSES < 3;
@@ -109,15 +125,18 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   if ((smem_u32(smem) & 1023u) != 0u) __trap();
   Misc &S = *reinterpret_cast<Misc *>(smem + MISC_OFF);
   float2 *sacc = reinterpret_cast<float2 *>(smem + SACC_OFF);
+  uint32_t *keys = reinterpret_cast<uint32_t *>(smem + KEYS_OFF);
   // warp index through a shuffle: the compiler then knows it is warp-uniform and the role branches are not divergent
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
-  const int b = blockIdx.y;
   const int N = a.N;
   const int ntiles = (N + TP - 1) / TP;
-  const int tile_begin = blockIdx.x * tiles_per_cta;
-  const int tile_end = min(ntiles, tile_begin + tiles_per_cta);
-  if (tile_begin >= tile_end) return;
-  const int my_tiles = tile_end - tile_begin;
+  // this CTA's tiles [t_begin, t_begin + my_tiles) of the candidate-major numbering t = b * ntiles + j; the launch
+  // makes gridDim.x <= B * ntiles, so every range holds at least one tile
+  const long long T = (long long)a.B * ntiles;
+  const int t_begin = (int)(blockIdx.x * T / gridDim.x);
+  const int my_tiles = (int)((blockIdx.x + 1) * T / gridDim.x) - t_begin;
+  const int b_first = t_begin / ntiles;
+  const int ncand = (t_begin + my_tiles - 1) / ntiles - b_first + 1;
   const unsigned char *img = static_cast<const unsigned char *>(a.tc_img);
   const bool has_l1 = a.stage1_mode != 0;
   const uint32_t smem_s = smem_u32(smem);
@@ -125,6 +144,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   const uint32_t misc_s = smem_s + MISC_OFF;
   const uint32_t full_s = misc_s + (uint32_t)offsetof(Misc, full_bar), empty_s = misc_s + (uint32_t)offsetof(Misc, empty_bar);
   const uint32_t wbar_s = misc_s + (uint32_t)offsetof(Misc, w_bar);
+  const uint32_t cand_s = misc_s + (uint32_t)offsetof(Misc, cand_bar), front_s = misc_s + (uint32_t)offsetof(Misc, front_bar);
+  const uint32_t keys_s = misc_s + (uint32_t)offsetof(Misc, keys_bar);
 
   // ---- one-time setup --------------------------------------------------------------------------------------
   for (int i = tid; i < 6 * 64; i += NTC) S.w0[i] = a.l0.Wt[i];
@@ -133,42 +154,29 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     S.bias1[tid] = (a.stage1_mode == 1) ? a.l1.b[tid] : 0.f;
   }
   if (tid < 128) S.bias2[tid] = a.l2.b[tid];
-  if (tid < 9) S.T3[tid] = a.T3 ? a.T3[b * 9 + tid] : 0.f;
-  if (a.in.x_direct == nullptr) {
-    if (tid == 0) pose_inverse(a.in.poses + (size_t)b * 16, S.pinv);
-    if (tid < 6) {
-      S.mean[tid] = a.in.mean ? a.in.mean[tid] : 0.0;
-      S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: the hot loop multiplies
-    }
+  if (a.in.x_direct == nullptr && tid < 6) {
+    S.mean[tid] = a.in.mean ? a.in.mean[tid] : 0.0;
+    S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: the hot loop multiplies
   }
   for (int i = tid; i < (int)(SACC_BYTES / 8); i += NTC) sacc[i] = make_float2(-INFINITY, -INFINITY);
-  if (a.stage1_mode == 2) {
-    // per-candidate feature transform as the B operand of L1:  B[j][k] = T64[k][j]   (pointnet2.py:257)
-    const float *T = a.T64 + (size_t)b * 4096;
-    unsigned char *w1 = smem + W1_OFF;
-    for (int idx = tid; idx < 4096; idx += NTC) {
-      const int k = idx >> 6, j = idx & 63;
-      const float v = __ldg(T + idx);
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
-      const uint32_t off = row_chunk_off(j, k >> 3) + (uint32_t)(k & 7) * 2u;
-      *reinterpret_cast<__nv_bfloat16 *>(w1 + off) = h;
-      *reinterpret_cast<__nv_bfloat16 *>(w1 + 8192 + off) = l;
-    }
-    fence_proxy_async();
-  }
+  for (int i = tid; i < 2 * 1024; i += NTC) keys[i] = 0u;   // below the key of every float
   if (tid == 0) {
     for (int i = 0; i < NSLOT; i++) {
       mbar_init(full_s + 8u * i, 1);
       mbar_init(empty_s + 8u * i, NCW);
     }
     mbar_init(wbar_s, 1);
+    mbar_init(cand_s, NHELP);
+    mbar_init(front_s, NCW * 32);
+    mbar_init(keys_s, NCW * 32);
+    mbar_init(keys_s + 8u, NCW * 32);
     mbar_init_fence();
   }
   __syncthreads();
 
   if (warp == PROD_WARP) {
     // ======================= producer: resident W2 (+ shared W1), then W3 slot by slot =======================
+    // one W3 stream over the whole range: the ring does not drain at candidate boundaries
     if (lane == 0) {
       mbar_expect_tx(wbar_s, IMG_W2 + (a.stage1_mode == 1 ? IMG_W1 : 0u));
       bulk_g2s(w2_s, img + IMG_W2_OFF, IMG_W2, wbar_s);
@@ -186,13 +194,84 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     return;
   }
 
+  if (warp >= HELP_WARP) {
+    // ======================= helpers: per-candidate constants and the global fold =======================
+    // Candidate k's inputs are loaded (and T64 converted) before waiting for the consumers to leave candidate k - 1,
+    // so that only the shared-memory stores sit between the consumers' last front of k - 1 and their first of k.
+    // The fold of candidate k - 1 follows the hand-over of k; the consumers cannot fill keys[(k - 1) & 1] again
+    // before the hand-over of k + 1, which comes after that fold.
+    const int ht = tid - HELP_WARP * 32;
+    for (int k = 0; k <= ncand; k++) {
+      if (k < ncand) {
+        const int b = b_first + k;
+        // T64 as the B operand of L1:  B[j][kk] = T64[kk][j]  (pointnet2.py:257).  Unit u = (row j, 8-wide K chunk
+        // kc) is one 16-byte chunk of the hi and of the lo image; a warp's 32 rows read 32 consecutive floats.
+        constexpr int TU = (64 * 8 + NHELP - 1) / NHELP;
+        uint32_t t64h[TU][4], t64l[TU][4];
+        if (a.stage1_mode == 2) {
+          const float *Tb = a.T64 + (size_t)b * 4096;
+#pragma unroll
+          for (int i = 0; i < TU; i++) {
+            const int u = ht + NHELP * i;
+            if (u < 512) {
+              float v[8];
+#pragma unroll
+              for (int e = 0; e < 8; e++) v[e] = __ldg(Tb + (8 * (u >> 6) + e) * 64 + (u & 63));
+#pragma unroll
+              for (int e = 0; e < 4; e++) split_bf16x2(v[2 * e], v[2 * e + 1], t64h[i][e], t64l[i][e]);
+            }
+          }
+        }
+        double pinv[12];
+        const bool do_pinv = a.in.x_direct == nullptr && ht == 0;
+        if (do_pinv) pose_inverse(a.in.poses + (size_t)b * 16, pinv);
+        const float t3 = (a.T3 && ht < 9) ? a.T3[b * 9 + ht] : 0.f;
+        if (k > 0) mbar_wait(front_s, (uint32_t)(k - 1) & 1u);
+        if (a.stage1_mode == 2) {
+#pragma unroll
+          for (int i = 0; i < TU; i++) {
+            const int u = ht + NHELP * i;
+            if (u < 512) {
+              const uint32_t off = row_chunk_off(u & 63, u >> 6);
+              *reinterpret_cast<uint4 *>(smem + W1_OFF + off) =
+                  make_uint4(t64h[i][0], t64h[i][1], t64h[i][2], t64h[i][3]);
+              *reinterpret_cast<uint4 *>(smem + W1_OFF + 8192 + off) =
+                  make_uint4(t64l[i][0], t64l[i][1], t64l[i][2], t64l[i][3]);
+            }
+          }
+          fence_proxy_async();
+        }
+        if (do_pinv) {
+#pragma unroll
+          for (int i = 0; i < 12; i++) S.pinv[i] = pinv[i];
+        }
+        if (ht < 9) S.T3[ht] = t3;
+        mbar_arrive(cand_s);
+      }
+      if (k > 0) {
+        // candidate k - 1: bias and ReLU commute with the max (both are monotone), so they follow it
+        const int kp = k - 1;
+        mbar_wait(keys_s + 8u * (kp & 1), ((uint32_t)kp >> 1) & 1u);
+        uint32_t *kb = keys + (kp & 1) * 1024;
+        uint32_t *g = a.gmax_keys + (size_t)(b_first + kp) * 1024;
+        for (int ch = ht; ch < 1024; ch += NHELP) {
+          float m = cg_key2f(kb[ch]) + __ldg(&a.l3.b[ch]);
+          if (a.relu3) m = fmaxf(m, 0.f);
+          atomicMax(&g[ch], cg_f2key(m));
+          kb[ch] = 0u;
+        }
+      }
+    }
+    return;
+  }
+
   // ======================= consumer warpgroups =======================
   const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, q = lane & 3;
   float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU, fp16 engines): reported if beyond the fp16 range
 #ifdef CG_EXPERIMENTS
   // phase timeline of the sampled CTAs (scripts/trunk_timeline.py): cycles per phase summed over this warp's tiles
-  const bool tl_on = tl != nullptr && blockIdx.x == 0 && blockIdx.y % TL_STRIDE(a.B) == TL_STRIDE(a.B) / 2 &&
-                     (int)(blockIdx.y / TL_STRIDE(a.B)) < TL_CTAS;
+  const bool tl_on = tl != nullptr && blockIdx.x % TL_STRIDE(gridDim.x) == 0 &&
+                     (int)(blockIdx.x / TL_STRIDE(gridDim.x)) < TL_CTAS;
   unsigned long long tl_sum[TL_NPHASE] = {}, tl_t0 = clock64(), tl_t = tl_t0, tl_s;
 #define TL_MARK(phase)                   \
   do {                                   \
@@ -211,12 +290,13 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
 
   // The input of a point row is fetched one tile ahead (fetch_id / fetch_row during the previous tile's L3) and
   // finished (finish_row) when its tile starts, so the dependent id -> cloud-row loads are off the critical path.
-  // Row n >= N duplicates a valid point: it cannot change a max.  x_direct rows travel as exact float -> double.
-  auto fetch_id = [&](int n) -> int {
+  // Row n >= N of candidate b duplicates a valid point of b: it cannot change a max.  x_direct rows travel as exact
+  // float -> double.
+  auto fetch_id = [&](int b, int n) -> int {
     if (n >= N) n = N - 1;
     return (a.in.x_direct == nullptr && a.in.ids) ? __ldg(a.in.ids + (size_t)b * N + n) : n;
   };
-  auto fetch_row = [&](int id, double *r) {
+  auto fetch_row = [&](int b, int id, double *r) {
     if (a.in.x_direct) {
       const float *xr = a.in.x_direct + ((size_t)b * N + id) * 6;
 #pragma unroll
@@ -269,24 +349,33 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
   constexpr int L3_GROUP = PASSES == 1 ? 8 : 4;
   constexpr bool ROW_PREFETCH = PASSES == 1;
   double r0[6], r1[6];   // raw input rows of the next tile
-  int id0 = fetch_id(tile_begin * TP + prow), id1 = fetch_id(tile_begin * TP + prow + 8);
-  if (ROW_PREFETCH) {
-    fetch_row(id0, r0);
-    fetch_row(id1, r1);
+  int id0, id1;
+  {
+    const int j = t_begin - b_first * ntiles;
+    id0 = fetch_id(b_first, j * TP + prow);
+    id1 = fetch_id(b_first, j * TP + prow + 8);
+    if (ROW_PREFETCH) {
+      fetch_row(b_first, id0, r0);
+      fetch_row(b_first, id1, r1);
+    }
   }
   // Warpgroup 1 starts its first tile when warpgroup 0 has finished the front layers of its own (named barrier 2), so
   // that one warpgroup's front runs under the other's L3 instead of leaving the tensor pipe idle for both.
   if (wg == 1) asm volatile("bar.sync 2, 256;" ::: "memory");
   TL_MARK(TL_START);
   for (int it = 0; it < my_tiles; it++) {
-    const int p0 = (tile_begin + it) * TP + prow;   // this thread's rows: points p0 and p0 + 8
+    // tile j of candidate b, candidate ci of the range; the candidate's first / last tile in this range
+    const int b = (t_begin + it) / ntiles, j = t_begin + it - b * ntiles, ci = b - b_first;
+    const bool cand_first = it == 0 || j == 0, cand_last = it + 1 == my_tiles || j + 1 == ntiles;
+    const int p0 = j * TP + prow;   // this thread's rows: points p0 and p0 + 8
+    if (cand_first) mbar_wait(cand_s, (uint32_t)ci & 1u);   // pinv / T3 / T64 image of candidate b
     // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
     float d64[32];
     {
       float v0[6], v1[6];
       if (!ROW_PREFETCH) {
-        fetch_row(id0, r0);
-        fetch_row(id1, r1);
+        fetch_row(b, id0, r0);
+        fetch_row(b, id1, r1);
       }
       finish_row(r0, v0);
       finish_row(r1, v1);
@@ -344,6 +433,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
         }
       }
     }
+    // the last read of candidate b's pinv / T3 / T64 image in this range is done: the helpers may replace them
+    if (cand_last) mbar_arrive(front_s);
     // ---- L2: 64 -> 128 ----
     float acc[64];
     d_to_a<4, false>(d64, xh, xl);
@@ -460,14 +551,15 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     // warpgroup: 288 threads count as 384).
     // The next tile's input is fetched where nothing is in flight: the ids before the first group, the dependent
     // rows before the second (a last tile re-reads its own rows, clamped to the candidate's points).
-    const int pn = p0 + (it + 1 < my_tiles ? TP : 0);
-    id0 = fetch_id(pn);
-    id1 = fetch_id(pn + 8);
+    const int nt = t_begin + it + (it + 1 < my_tiles ? 1 : 0);
+    const int nb = nt / ntiles, pn = (nt - nb * ntiles) * TP + prow;
+    id0 = fetch_id(nb, pn);
+    id1 = fetch_id(nb, pn + 8);
 #pragma unroll 1
     for (int h0 = 0; h0 < 2 * NCHUNK; h0 += L3_GROUP) {
       if (ROW_PREFETCH && h0 == L3_GROUP) {
-        fetch_row(id0, r0);
-        fetch_row(id1, r1);
+        fetch_row(nb, id0, r0);
+        fetch_row(nb, id1, r1);
       }
       float acc3[2][32];   // even / odd half-chunks
       issue(h0, acc3[0]);
@@ -486,12 +578,25 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
     wg_fence_regs<32>(xh[0]);
     if (PASSES != 1) wg_fence_regs<32>(xl[0]);
     gslot += 2u * NCHUNK;
+    if (cand_last) {
+      // hand candidate b's running max to the helpers (keys by candidate parity) and start the next one at -inf
+      uint32_t *kk = keys + (ci & 1) * 1024;
+#pragma unroll 4
+      for (int h = 0; h < 2 * NCHUNK; h++) {
+        float2 &slot = sacc[((wg * 2 * NCHUNK + h) * 4 + w4) * 32 + lane];
+        const float2 v = slot;
+        atomicMax(&kk[64 * h + 2 * lane], cg_f2key(v.x));   // thread (g, q) holds columns 8g + 2q + {0, 1}
+        atomicMax(&kk[64 * h + 2 * lane + 1], cg_f2key(v.y));
+        slot = make_float2(-INFINITY, -INFINITY);
+      }
+      mbar_arrive(keys_s + 8u * (ci & 1));
+    }
     TL_MARK(TL_L3);
   }
   if (F16 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
 #ifdef CG_EXPERIMENTS
   if (tl_on && lane == 0) {
-    unsigned long long *o = tl + ((size_t)(blockIdx.y / TL_STRIDE(a.B)) * NCW + warp) * TL_REC;
+    unsigned long long *o = tl + ((size_t)(blockIdx.x / TL_STRIDE(gridDim.x)) * NCW + warp) * TL_REC;
 #pragma unroll
     for (int p = 0; p < TL_NPHASE; p++) o[p] = tl_sum[p];
     o[TL_NPHASE] = (unsigned long long)my_tiles;
@@ -501,22 +606,6 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a,
 #undef TL_MARK
 #undef TL_SPAN_BEGIN
 #undef TL_SPAN_END
-
-  // ---- fold the eight warps' running maxima of every channel into the global feature ----
-  bar_consumers();
-  for (int ch = tid; ch < 1024; ch += NCW * 32) {
-    const int h = ch >> 6, col = ch & 63;
-    const int ln = 4 * (col >> 3) + ((col & 7) >> 1), k = col & 1;
-    float m = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < 8; w++) {
-      const float *sv = reinterpret_cast<const float *>(&sacc[(((w >> 2) * 2 * NCHUNK + h) * 4 + (w & 3)) * 32 + ln]);
-      m = fmaxf(m, sv[k]);
-    }
-    m += __ldg(&a.l3.b[ch]);   // bias is constant over points: add after the max
-    if (a.relu3) m = fmaxf(m, 0.f);
-    atomicMax(&a.gmax_keys[(size_t)b * 1024 + ch], cg_f2key(m));
-  }
 }
 
 }  // namespace
@@ -556,14 +645,11 @@ int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *
 
 int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
   CG_REQUIRE(ctx, a.B > 0 && a.N > 0, "trunk: B,N must be positive");
-  CG_REQUIRE(ctx, a.B <= 65535, "trunk: B > 65535 must be chunked by the caller");
   CG_REQUIRE(ctx, a.tc_img != nullptr, "trunk: tensor-core weight image missing");
-  // split a candidate's tiles over CTAs only while there are fewer than ~4 CTAs per SM
-  const int ntiles = (a.N + TP - 1) / TP;
-  int splits = 1;
-  while ((long)a.B * splits < 4L * ctx->num_sms && splits < ntiles) splits *= 2;
-  const int tiles_per_cta = (ntiles + splits - 1) / splits;
-  dim3 grid((ntiles + tiles_per_cta - 1) / tiles_per_cta, a.B);
+  // persistent: one CTA per SM (or per tile, if there are fewer tiles), each over a balanced range of tiles
+  const long long tiles = (long long)a.B * ((a.N + TP - 1) / TP);
+  CG_REQUIRE(ctx, tiles <= INT_MAX, "trunk: too many tiles in one launch");
+  const int grid = (int)std::min<long long>(ctx->num_sms, tiles);
   // W3 beyond the fp16 range: the fp16 engines fall back to the 3-pass bf16 kernel
   const int passes = !a.tc_f16_ok || ctx->engine == 1 ? 3 : (ctx->engine == 2 ? 2 : 1);
 #ifdef CG_EXPERIMENTS
@@ -575,9 +661,9 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
     CG_CUDA(ctx, cudaMemsetAsync(tl, 0, tl_words * 8, ctx->stream));
   }
 #endif
-  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
-  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
-  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a, tiles_per_cta TL_ARG(tl));
+  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
+  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
+  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
   CG_LAUNCH_CHECK(ctx);
 #ifdef CG_EXPERIMENTS
   if (timeline) {
