@@ -73,6 +73,9 @@ SIGNATURES = {
     "cg_sdf_create": (_i, [_vp, _vp, _i, _i, _i, C.POINTER(_f), _f, C.POINTER(_vp)]),
     "cg_sdf_destroy": (None, [_vp]),
     "cg_sdf_lookup_dev": (_i, [_vp, _vp, _i, _i, _vp]),
+    "cg_sdf_from_mesh": (_i, [_vp, _vp, _i, _vp, _i, _f, _i, C.POINTER(_vp)]),
+    "cg_sdf_geometry": (_i, [_vp, C.POINTER(_i), C.POINTER(_f), C.POINTER(_f)]),
+    "cg_sdf_download": (_i, [_vp, _vp]),
     "cg_filter_grasp_pose_host": (_i, [_vp, C.POINTER(FilterParams), _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _i,
                                        _vp, _vp, _vp]),
     "cg_filter_grasp_pose_dev": (_i, [_vp, C.POINTER(FilterParams), _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _i,

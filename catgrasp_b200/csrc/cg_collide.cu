@@ -16,16 +16,6 @@
 // result bit for bit.
 #include "cg_common.cuh"
 
-struct cg_sdf {
-  cg_ctx *ctx;
-  float *grid;  // device, data[i][j][k]
-  int nx, ny, nz;
-  float origin[3];
-  float res;
-  int border_nonneg;   // every cell on the six boundary faces is >= 0 (true for padded grids, make_sdf.py:30)
-  float border_min;    // smallest value on the six boundary faces
-};
-
 namespace {
 
 struct SdfView {
@@ -385,15 +375,8 @@ SdfView make_view(const cg_sdf *s, float margin = 0.f) {
 
 }  // namespace
 
-extern "C" int cg_sdf_create(cg_ctx *ctx, const float *grid_host, int nx, int ny, int nz, const float origin[3],
-                             float resolution, cg_sdf **out) {
-  if (!ctx || !out) return CG_EINVAL;
-  CG_REQUIRE(ctx, grid_host && nx > 0 && ny > 0 && nz > 0 && resolution > 0.f, "sdf: bad grid");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  cg_sdf *s = new cg_sdf();
-  s->ctx = ctx; s->nx = nx; s->ny = ny; s->nz = nz; s->res = resolution;
-  for (int k = 0; k < 3; k++) s->origin[k] = origin[k];
-  const size_t bytes = (size_t)nx * ny * nz * sizeof(float);
+void cg_sdf_border_stats(cg_sdf *s, const float *grid_host) {
+  const int nx = s->nx, ny = s->ny, nz = s->nz;
   s->border_nonneg = 1;
   s->border_min = 3.0e38f;
   for (int i = 0; i < nx; i++)
@@ -404,6 +387,18 @@ extern "C" int cg_sdf_create(cg_ctx *ctx, const float *grid_host, int nx, int ny
         if (!(v >= 0.f)) s->border_nonneg = 0;
         if (!(v >= s->border_min)) s->border_min = v;   // NaN counts as "smallest"
       }
+}
+
+extern "C" int cg_sdf_create(cg_ctx *ctx, const float *grid_host, int nx, int ny, int nz, const float origin[3],
+                             float resolution, cg_sdf **out) {
+  if (!ctx || !out) return CG_EINVAL;
+  CG_REQUIRE(ctx, grid_host && nx > 0 && ny > 0 && nz > 0 && resolution > 0.f, "sdf: bad grid");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  cg_sdf *s = new cg_sdf();
+  s->ctx = ctx; s->nx = nx; s->ny = ny; s->nz = nz; s->res = resolution;
+  for (int k = 0; k < 3; k++) s->origin[k] = origin[k];
+  const size_t bytes = (size_t)nx * ny * nz * sizeof(float);
+  cg_sdf_border_stats(s, grid_host);
   CG_CUDA(ctx, cudaMalloc(&s->grid, bytes));
   CG_CUDA(ctx, cudaMemcpyAsync(s->grid, grid_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

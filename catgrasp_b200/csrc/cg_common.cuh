@@ -75,6 +75,20 @@ void cg_trace_mark(cg_ctx *ctx, const char *where);
     }                                                                             \
   } while (0)
 
+// one Sdf3D grid resident in HBM: made by cg_sdf_create (cg_collide.cu) from a host grid or by cg_sdf_from_mesh
+// (cg_sdf_build.cu) from a triangle mesh
+struct cg_sdf {
+  cg_ctx *ctx;
+  float *grid;  // device, data[i][j][k]
+  int nx, ny, nz;
+  float origin[3];
+  float res;
+  int border_nonneg;   // every cell on the six boundary faces is >= 0 (true for padded grids, make_sdf.py:30)
+  float border_min;    // smallest value on the six boundary faces
+};
+// border_nonneg / border_min of a host copy of the grid (decides the filter's out-of-box shortcut)
+void cg_sdf_border_stats(cg_sdf *s, const float *grid_host);
+
 int cg_ws_reserve(cg_ctx *ctx, size_t bytes);
 int cg_io_reserve(cg_ctx *ctx, size_t bytes);
 int cg_hs_reserve(cg_ctx *ctx, size_t bytes);

@@ -5,8 +5,9 @@
 of (4,4) float32 arrays.  Differences, all documented in INTEGRATION.md:
 
 * geometry predicate = gripper SDF vs scene points (sdf.py:292-389) instead of
-  FCL mesh-vs-octree; the SDFs of the two gripper meshes must be registered
-  once with :func:`register_gripper_sdf` (the reference loads the same grids
+  FCL mesh-vs-octree; the SDF of each gripper mesh is built from the mesh on
+  first use (Sdf3D.from_mesh, 1 mm cells, 5 cells of padding) unless one was
+  registered with :func:`register_gripper_sdf` (the reference loads the grids
   from ``gripper*.sdf``, dexnet/grasping/gripper.py:120-129);
 * survivors come back in deterministic (pose, symmetry) order, not in OpenMP
   thread-arrival order (common.cpp:303-313);
@@ -20,8 +21,12 @@ import numpy as np
 import torch
 
 from . import _lib
+from .sdf import Sdf3D
 
 _SDF_REGISTRY = {}
+# cell size (m) and padding (cells) of the grids built for unregistered gripper meshes: make_sdf.py:30's defaults
+GRIPPER_SDF_RESOLUTION = 0.001
+GRIPPER_SDF_PADDING = 5
 _IK_SOLVER = None
 DEFAULT_SDF_MODE = _lib.CG_SDF_TRILINEAR
 # Which geometry predicate filterGraspPose uses for "the posed gripper touches a scene point":
@@ -57,10 +62,11 @@ def set_ik_solver(fn):
 
 
 def _sdf_for(vertices, faces):
+    """The registered Sdf3D of a gripper mesh; unregistered meshes get a grid built from the mesh on the current
+    device (make_sdf.py:30's cell size and padding), cached under the same key."""
     key = _digest(vertices, faces)
     if key not in _SDF_REGISTRY:
-        raise _lib.CgError("no SDF registered for this gripper mesh: call "
-                           "catgrasp_b200.my_cpp.register_gripper_sdf(vertices, faces, Sdf3D) first")
+        _SDF_REGISTRY[key] = Sdf3D.from_mesh(vertices, faces, GRIPPER_SDF_RESOLUTION, GRIPPER_SDF_PADDING)
     return _SDF_REGISTRY[key]
 
 
@@ -270,7 +276,8 @@ def augmentGraspPoses(R0, selected_point, sphere_pts, inplane_rot_step, hand_dep
 
 class CollisionManager:
     """my_cpp/collision_manager.h:33-52 (exported by pybind.cpp:13-18, no Python caller): one posed mesh against one
-    point set.  The mesh is represented by its registered SDF (see register_gripper_sdf); isAnyCollision() evaluates
+    point set.  The mesh is represented by its SDF (registered with register_gripper_sdf, else built from the mesh on
+    first use); isAnyCollision() evaluates
     the same predicate as filterGraspPose for the single transform set with setTransform()."""
 
     def __init__(self):

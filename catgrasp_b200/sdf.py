@@ -30,6 +30,40 @@ class Sdf3D:
                                                   C.c_float(self.resolution_), C.byref(h)))
         self.h = h
 
+    @classmethod
+    def from_mesh(cls, vertices, faces, resolution=0.001, padding=5, device=None, ctx=None):
+        """Signed-distance grid of a closed triangle mesh, built on the GPU (replaces make_sdf.py:30-36 / SDFGen).
+
+        vertices (N,3), faces (M,3); ``resolution`` is the cell size and ``padding`` the number of cells added on
+        every side of the mesh's bounding box (make_sdf.py's defaults: 1 mm, 5 cells).  Values are exact distances to
+        the nearest triangle, negative inside.  ``write_sdf_file(path, s.data_, s.origin_, s.resolution_)`` stores the
+        result as a ``.sdf`` file.  Raises CgError for an open mesh or invalid input."""
+        V = np.ascontiguousarray(vertices, dtype=np.float64)
+        F = np.asarray(faces)
+        if V.ndim != 2 or V.shape[1] != 3 or F.ndim != 2 or F.shape[1] != 3:
+            raise ValueError(f"from_mesh: vertices and faces must be (N,3), got {V.shape} and {F.shape}")
+        if F.size and (F.min() < np.iinfo(np.int32).min or F.max() > np.iinfo(np.int32).max):
+            raise ValueError("from_mesh: face index out of the int32 range")
+        F = np.ascontiguousarray(F, dtype=np.int32)
+        self = cls.__new__(cls)
+        self.ctx = ctx if ctx is not None else _lib.Context.get(device)
+        self.h = None
+        h = C.c_void_p()
+        self.ctx.use_own_stream()   # blocking host call
+        self.ctx.check(self.ctx.lib.cg_sdf_from_mesh(self.ctx.h, _lib.ptr(V), V.shape[0], _lib.ptr(F), F.shape[0],
+                                                     C.c_float(float(resolution)), int(padding), C.byref(h)))
+        self.h = h
+        dims = (C.c_int * 3)()
+        org = (C.c_float * 3)()
+        res = C.c_float()
+        self.ctx.check(self.ctx.lib.cg_sdf_geometry(self.h, dims, org, C.byref(res)))
+        self.data_ = np.empty((dims[0], dims[1], dims[2]), np.float32)
+        self.ctx.check(self.ctx.lib.cg_sdf_download(self.h, _lib.ptr(self.data_)))
+        self.origin_ = np.array(org[:], dtype=np.float32)
+        self.resolution_ = float(res.value)
+        self.dims_ = np.array(self.data_.shape)
+        return self
+
     def __del__(self):
         try:
             if getattr(self, "h", None):

@@ -322,6 +322,73 @@ def _box_mesh(lo, hi):
     return V, F
 
 
+def tessellated_box_mesh(lo, hi, m):
+    """Closed mesh of the box [lo, hi] with every face split into m x m quads (2 m^2 triangles per face, outward
+    winding).  Vertices are not shared between faces, but a coordinate along an axis is always lo + (hi - lo) * (t / m)
+    for the same t, so shared edges coincide exactly."""
+    lo, hi = np.asarray(lo, np.float64), np.asarray(hi, np.float64)
+    lin = [lo[a] + (hi[a] - lo[a]) * (np.arange(m + 1) / m) for a in range(3)]
+    Vs, Fs, off = [], [], 0
+    for a in range(3):
+        b, c = (a + 1) % 3, (a + 2) % 3          # (b, c, a) is right-handed: b x c = +a
+        for side, val in ((0, lo[a]), (1, hi[a])):
+            gb, gc = np.meshgrid(lin[b], lin[c], indexing="ij")
+            V = np.zeros(((m + 1) * (m + 1), 3))
+            V[:, a], V[:, b], V[:, c] = val, gb.reshape(-1), gc.reshape(-1)
+            q = (np.arange(m)[:, None] * (m + 1) + np.arange(m)[None, :]).reshape(-1)
+            v00, v10, v01, v11 = q, q + (m + 1), q + 1, q + m + 2
+            if side == 1:                          # normal +a: counter-clockwise in (b, c)
+                F = np.concatenate([np.stack([v00, v10, v11], 1), np.stack([v00, v11, v01], 1)])
+            else:
+                F = np.concatenate([np.stack([v00, v11, v10], 1), np.stack([v00, v01, v11], 1)])
+            Vs.append(V); Fs.append(F + off); off += V.shape[0]
+    return np.concatenate(Vs), np.concatenate(Fs).astype(np.int32)
+
+
+def make_hex_nut_mesh(across_flats=0.020, height=0.008, bore=0.010, n_seg=48):
+    """Closed genus-1 mesh of a hex nut (the solid of sample_hex_nut) whose bore is a regular n_seg-gon inscribed in
+    the bore circle (n_seg a multiple of 6).  Returns (V, F); see hex_nut_mesh_inside for the exact solid."""
+    assert n_seg % 6 == 0
+    R = across_flats / np.sqrt(3.0)
+    s = n_seg // 6
+    outer = []
+    for k in range(6):                             # hexagon sides, each split into s segments
+        p0 = R * np.array([np.cos(k * np.pi / 3), np.sin(k * np.pi / 3)])
+        p1 = R * np.array([np.cos((k + 1) * np.pi / 3), np.sin((k + 1) * np.pi / 3)])
+        outer += [p0 + (p1 - p0) * (t / s) for t in range(s)]
+    outer = np.array(outer)
+    th = 2 * np.pi * np.arange(n_seg) / n_seg
+    inner = bore / 2 * np.stack([np.cos(th), np.sin(th)], 1)
+    h = height / 2
+    # vertex blocks: outer bottom, outer top, inner bottom, inner top
+    V = np.concatenate([np.c_[outer, np.full(n_seg, -h)], np.c_[outer, np.full(n_seg, h)],
+                        np.c_[inner, np.full(n_seg, -h)], np.c_[inner, np.full(n_seg, h)]])
+    ob, ot, ib, it = 0, n_seg, 2 * n_seg, 3 * n_seg
+    F = []
+    for i in range(n_seg):
+        j = (i + 1) % n_seg
+        F += [[ob + i, ob + j, ot + j], [ob + i, ot + j, ot + i]]     # outer wall, normal outward
+        F += [[ib + i, it + j, ib + j], [ib + i, it + i, it + j]]     # bore wall, normal towards the axis
+        F += [[ot + i, ot + j, it + j], [ot + i, it + j, it + i]]     # top cap, +z
+        F += [[ob + i, ib + j, ob + j], [ob + i, ib + i, ib + j]]     # bottom cap, -z
+    return V, np.array(F, np.int32)
+
+
+def hex_nut_mesh_inside(p, across_flats=0.020, height=0.008, bore=0.010, n_seg=48):
+    """Analytic inside test of make_hex_nut_mesh's solid: |z| < h/2, inside the hexagon, outside the bore polygon."""
+    p = np.asarray(p, np.float64)
+    x, y, z = p[..., 0], p[..., 1], p[..., 2]
+    ok = np.abs(z) < height / 2
+    for k in range(6):                             # hexagon: apothem across_flats/2 at angles 30 + 60k deg
+        a = np.pi / 6 + k * np.pi / 3
+        ok &= x * np.cos(a) + y * np.sin(a) < across_flats / 2
+    in_bore = np.ones_like(ok)
+    for i in range(n_seg):                         # bore polygon: edge i between angles th_i and th_{i+1}
+        a = 2 * np.pi * (i + 0.5) / n_seg
+        in_bore &= x * np.cos(a) + y * np.sin(a) < bore / 2 * np.cos(np.pi / n_seg)
+    return ok & ~in_bore
+
+
 def make_gripper_proxy(res=0.001, pad_cells=5):
     """Two-finger box gripper (SURVEY.md 8d): palm 40x60x30 mm, fingers 45x8x20 mm, opening 50 mm.
 

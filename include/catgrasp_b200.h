@@ -191,6 +191,27 @@ void cg_sdf_destroy(cg_sdf *sdf);
 int cg_sdf_lookup_dev(cg_sdf *sdf, const float *grid_coords, int P, int mode,
                       float *out_sd);
 
+/* ---- SDF grid from a triangle mesh ---------------------------------------
+ * Replaces: make_sdf.py:30-36 (the external SDFGen binary run on a gripper
+ * mesh) and the .sdf files it writes, sdf_file.py:59-87.
+ * vertices (nv,3) float64 and faces (nf,3) int32 are HOST arrays of a closed
+ * mesh; the call is blocking.  Grid geometry, per axis a:
+ *   n_a      = ceil((max_a - min_a) / resolution - 1e-4) + 1 + 2 * padding
+ *   origin_a = float32(min_a - padding * resolution)   (float64 arithmetic)
+ * Node (i,j,k) lies at origin + (i,j,k) * resolution (float64 from the float32
+ * values).  Each value is the exact distance from the node to the nearest
+ * triangle, computed in float64 and rounded once to float32, negative inside
+ * (ray parity along x).  Errors (CG_EINVAL, no handle created): nv or nf <= 0,
+ * an index out of range, a non-finite vertex, resolution <= 0 or not finite,
+ * padding < 0, more than 2048 nodes along an axis, a mesh that is not closed.
+ * CG_ENOMEM when the device is out of memory.                              */
+int cg_sdf_from_mesh(cg_ctx *ctx, const double *vertices, int nv, const int32_t *faces, int nf,
+                     float resolution, int padding, cg_sdf **out);
+/* dims (nx,ny,nz), origin and resolution of a grid (sdf_file.py:59-87 header) */
+int cg_sdf_geometry(const cg_sdf *sdf, int dims[3], float origin[3], float *resolution);
+/* copy the grid to host memory, data[i][j][k] (k fastest); blocking          */
+int cg_sdf_download(cg_sdf *sdf, float *grid_host);
+
 /* ---- collision filter --------------------------------------------------
  * Replaces: my_cpp/common.cpp:156-321 (filterGraspPose) with the FCL
  * mesh-vs-octree test (collision_manager.cpp:93-111) substituted by the
