@@ -1,13 +1,15 @@
 // cg_tc_ptx.cuh -- inline-PTX wrappers for the sm_90a tensor-core kernels (wgmma / mbarrier / bulk copies).
 // Shared by the trunk kernel (cg_trunk_tc.cu) and the fully-connected kernel (cg_linear_tc.cu).
 //
-// Operand conventions of every wgmma below: D (fp32, registers) = A (registers) x B (shared memory).
+// Operand conventions of the wgmma below: D (fp32, registers) = A (registers, or shared memory for wg_ss_*) x B
+// (shared memory).
 // A and D use the m64nNk16 register fragments of the PTX ISA: warp w of the warpgroup owns rows 16w .. 16w+15;
 // with g = lane / 4 and q = lane % 4 a thread holds
 //   D: d[4i + e] = (row g, col 8i + 2q + e),  d[4i + 2 + e] = (row g + 8, col 8i + 2q + e)      i < N/8, e < 2
 //   A (k-step of 16): r0 = (row g, k 2q..2q+1), r1 = (row g+8, k 2q..), r2 = (row g, k 8+2q..), r3 = (row g+8, k 8+2q..)
 // so the D of one layer is the A of the next without any data movement (d_to_a below).
-// B is an [N rows x 64] K-block in the canonical K-major SWIZZLE_128B layout (row_chunk_off), 1024-byte aligned.
+// B (and a shared-memory A) is an [N (M) rows x 64] K-block in the canonical K-major SWIZZLE_128B layout
+// (row_chunk_off), 1024-byte aligned.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -134,6 +136,37 @@ __device__ __forceinline__ void wg_m64n128(float *d, const uint32_t *a, uint64_t
         "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
         : CG_WG_D8(0), CG_WG_D8(8), CG_WG_D8(16), CG_WG_D8(24), CG_WG_D8(32), CG_WG_D8(40), CG_WG_D8(48), CG_WG_D8(56)
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+        : "memory");
+  }
+}
+// D[64 x 128] (+)= A[64 x 16] (shared, K-major) . B[128 x 16] (shared, K-major); both operands by descriptor
+template <bool F16>
+__device__ __forceinline__ void wg_ss_m64n128(float *d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if (F16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : CG_WG_D8(0), CG_WG_D8(8), CG_WG_D8(16), CG_WG_D8(24), CG_WG_D8(32), CG_WG_D8(40), CG_WG_D8(48), CG_WG_D8(56)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : CG_WG_D8(0), CG_WG_D8(8), CG_WG_D8(16), CG_WG_D8(24), CG_WG_D8(32), CG_WG_D8(40), CG_WG_D8(48), CG_WG_D8(56)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
   }
 }

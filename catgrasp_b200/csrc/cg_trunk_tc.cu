@@ -4,30 +4,33 @@
 //   layer            wgmma (m64nNk16, fp32 accumulators in registers)                          epilogue
 //   6 -> 64          fp32 FMA (K = 6 is not a tensor-core shape), computed in the A-fragment layout -> X1
 //   64 -> 64 (L1)    D1[pt][ch] = X1[pt][k] (registers) . W1[ch][k] (smem)   bf16 hi/lo x3, N = 64    bias/ReLU -> X2
-//   64 -> 128 (L2)   D2[pt][ch] = X2[pt][k] (registers) . W2[ch][k] (smem)   bf16 hi/lo x3, N = 128   bias/ReLU -> X3
-//   128 -> 1024 (L3) D3[pt][ch] = X3[pt][k] (registers) . W3[ch][k] (smem ring), 8 chunks of 128   max over points
+//   64 -> 128 (L2)   D2[pt][ch] = X2[pt][k] (registers) . W2[ch][k] (smem)   bf16 hi/lo x3, N = 128   bias/ReLU -> X3 smem
+//   128 -> 1024 (L3) D3[ch][pt] = W3[ch][k] (smem ring) . X3[pt][k] (smem), 8 chunks of 128 channels  max over points
 //
-// The accumulator fragment of one layer is the A-operand fragment of the next (cg_tc_ptx.cuh), so the activations of a
-// tile never touch shared memory: shared memory holds only the resident W1 / W2 and a ring through which a producer
-// warp streams W3 with cp.async.bulk, completion counted on mbarriers.
+// The front (FMA, L1, L2) runs point-major: the accumulator fragment of one layer is the A-operand fragment of the
+// next (cg_tc_ptx.cuh), so X1 and X2 stay in registers.  Only X3 is staged, once per tile: L2's epilogue stores it into
+// a [points x 128] K-major swizzled image that is the B operand of L3.  L3 runs channel-major with W3 as the A operand,
+// straight from the ring through which a producer warp streams W3 with cp.async.bulk (completion counted on
+// mbarriers), so one W3 fetch serves every point of the tile, and a channel's max over points is a row reduction
+// inside the accumulator fragment.
 //
 // Precision of L3 (PASSES, the template parameter; L1 / L2 are always near-fp32):
-//   3 (engine 1)  W3 and X3 split x = hi + lo in bf16, products lo*hi + hi*lo + hi*hi (lo*lo ~ 2^-16 dropped): near-fp32
+//   3 (engine 1)  W3 and X3 split x = hi + lo in bf16, products hi*lo + lo*hi + hi*hi (lo*lo ~ 2^-16 dropped): near-fp32
 //   2 (engine 2)  W3 one fp16 term, X3 fp16 hi + lo
 //   1 (engine 3)  W3 and X3 one fp16 term each.
 // On both fp16 engines X3 values above the fp16 range are clamped to 65504 AND reported through
 // cg_trunk_args::ovf_flag so that the host can re-run on engine 1.
 //
+// Tiles: 256 points on engine 3 (the fp16 X3 image is 64 KB), 128 points on engines 1 and 2 (hi + lo images, 64 KB).
 // Persistent grid: one CTA per SM.  The B x ntiles tiles are numbered candidate-major and CTA i runs the contiguous
 // range [i T / G, (i + 1) T / G), so ranges differ by at most one tile and may start or end inside a candidate (the
 // global max is an atomicMax on order-preserving keys, so a candidate split over CTAs needs nothing else).
 //
-// CTA = 384 threads: two consumer warpgroups (points 0-63 / 64-127 of each 128-point tile; each runs the whole layer
-// chain for its points), one producer warp and three helper warps.  The two consumer warpgroups are independent except
-// for the shared W3 ring, so one warpgroup's FMA layer, epilogues and max reduction overlap the other's tensor-core
-// work; warpgroup 1 starts one front (input + FMA + L1 + L2) behind warpgroup 0 so that their fronts do not coincide.
-// The helpers keep per-candidate work off the consumers' path: the next candidate's pose inverse, T3 and T64 operand
-// image, and the global fold (bias, ReLU, atomicMax) of each finished candidate's running max.
+// CTA = 384 threads: two consumer warpgroups, one producer warp and three helper warps.  Warpgroup w builds the front
+// of the tile's points [w TILE / 2, (w + 1) TILE / 2) in 64-row blocks, and in L3 computes the channels 64w .. 64w+63
+// of every 128-channel chunk over all the tile's points.  The helpers keep per-candidate work off the consumers' path:
+// the next candidate's pose inverse, T3 and T64 operand image, and the global fold (bias, ReLU, atomicMax) of each
+// finished candidate's max.
 #include <limits.h>
 #include <stdlib.h>
 
@@ -47,17 +50,19 @@ constexpr int NHELP = 3 * 32;
 constexpr int NTC = (NCW + 4) * 32;         // 384 threads
 constexpr int NCHUNK = 8;                   // 1024 output channels / 128
 constexpr uint32_t PIECE = 16384;           // [128 rows x 64 x 16-bit] one swizzled K-block
+// points per tile: engine 3 stages one fp16 X3 term, engines 1 and 2 a hi and a lo term in the same 64 KB
+__host__ __device__ constexpr int tile_points(int passes) { return passes == 1 ? 256 : 128; }
 // shared-memory map
 constexpr uint32_t W1_OFF = 0;              // [hi 8 KB | lo 8 KB]: shared W1, or the current candidate's T64 operand
 constexpr uint32_t W2_OFF = PIECE;          // [hi 16 KB | lo 16 KB]
-constexpr uint32_t RING_OFF = 3 * PIECE;    // 128 KB of W3 slots (one slot = one 64-wide K-block of a 128-channel chunk)
-constexpr uint32_t RING_BYTES = 8 * PIECE;
-constexpr uint32_t SACC_OFF = RING_OFF + RING_BYTES;   // running max: float2 per (warpgroup, half-chunk, warp, lane)
-constexpr uint32_t SACC_BYTES = 2 * 2 * NCHUNK * 4 * 32 * 8;
-constexpr uint32_t KEYS_OFF = SACC_OFF + SACC_BYTES;   // per-candidate max keys [2][1024], by candidate parity
+constexpr uint32_t X3_OFF = 3 * PIECE;      // 64 KB X3 image: [kb][TILE rows x 64] (engine 3), [hi | lo][kb][128 x 64]
+constexpr uint32_t X3_BYTES = 4 * PIECE;
+constexpr uint32_t RING_OFF = X3_OFF + X3_BYTES;   // 96 KB of W3 slots (one slot = one 64-wide K-block of a chunk)
+constexpr uint32_t RING_BYTES = 6 * PIECE;
+constexpr uint32_t KEYS_OFF = RING_OFF + RING_BYTES;   // per-candidate max keys [2][1024], by candidate parity
 constexpr uint32_t KEYS_BYTES = 2 * 1024 * 4;
 constexpr uint32_t MISC_OFF = KEYS_OFF + KEYS_BYTES;
-constexpr int NSLOT_MAX = 8;
+constexpr int NSLOT_MAX = 6;
 // operand image built by cg_tc_prepare
 constexpr uint32_t IMG_W3B = NCHUNK * 2 * 2 * PIECE;   // bf16: [chunk][kb][hi 16 KB | lo 16 KB]
 constexpr uint32_t IMG_W2 = 2 * PIECE, IMG_W1 = PIECE;
@@ -87,26 +92,12 @@ struct Misc {
 constexpr size_t SMEM_BYTES = MISC_OFF + sizeof(Misc);
 static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_90");
 
-// One step of the transposing column-max butterfly of the L3 reduction: the lanes with bit STEP set keep the upper
-// half of their STEP columns, the others the lower half, and each takes the max with its partner's copy.  STEP is a
-// template parameter so that every index into x is a constant and x stays in registers.
-template <int STEP>
-__device__ __forceinline__ void max_butterfly_step(float *x, int lane) {
-  const bool up = (lane & STEP) != 0;
-#pragma unroll
-  for (int k = 0; k < STEP / 2; k++) {
-    const float send = up ? x[k] : x[k + STEP / 2];
-    const float keep = up ? x[k + STEP / 2] : x[k];
-    x[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, STEP));
-  }
-}
-
 #ifdef CG_EXPERIMENTS
 // Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer warp of TL_CTAS sampled CTAs (spread over
 // the grid) sums clock64() cycles per phase over its tiles and writes one record of TL_REC words: the TL_NPHASE
 // sums, its tile count and its total cycles.  TL_L3_WAIT and TL_RING lie inside TL_L3.
-enum { TL_START, TL_INPUT, TL_FRONT, TL_L3, TL_L3_WAIT, TL_RING, TL_NPHASE };
-constexpr int TL_CTAS = 8, TL_REC = 8;
+enum { TL_START, TL_INPUT, TL_FRONT, TL_X3, TL_L3, TL_L3_WAIT, TL_RING, TL_NPHASE };
+constexpr int TL_CTAS = 8, TL_REC = TL_NPHASE + 2;
 __host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / TL_CTAS : 1; }
 #define TL_PARAM , unsigned long long *tl
 #define TL_ARG(p) , p
@@ -117,19 +108,24 @@ __host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / T
 
 template <int PASSES>
 __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a TL_PARAM) {
-  constexpr int NSLOT = PASSES == 3 ? 4 : 8;
+  constexpr int TILE = tile_points(PASSES);
+  constexpr int NBLK = TILE / 128;            // 64-row front blocks per warpgroup = 128-point L3 units per chunk
+  constexpr int NSLOT = PASSES == 3 ? 3 : 6;
   constexpr uint32_t SLOT_BYTES = PASSES == 3 ? 2 * PIECE : PIECE;
+  static_assert(NSLOT * SLOT_BYTES == RING_BYTES, "ring");
   constexpr bool F16 = PASSES < 3;
+  constexpr uint32_t X3_KB = TILE * 128;      // one [TILE x 64] K-block of the X3 image
+  constexpr uint32_t X3_LO = 2 * X3_KB;       // the lo term (engines 1 and 2)
+  static_assert((PASSES == 1 ? 2 : 4) * X3_KB == X3_BYTES, "X3 image");
   // the operand tiles need 1024-byte alignment (SWIZZLE_128B atoms); the kernel has no static shared memory
   extern __shared__ __align__(1024) unsigned char smem[];
   if ((smem_u32(smem) & 1023u) != 0u) __trap();
   Misc &S = *reinterpret_cast<Misc *>(smem + MISC_OFF);
-  float2 *sacc = reinterpret_cast<float2 *>(smem + SACC_OFF);
   uint32_t *keys = reinterpret_cast<uint32_t *>(smem + KEYS_OFF);
   // warp index through a shuffle: the compiler then knows it is warp-uniform and the role branches are not divergent
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int N = a.N;
-  const int ntiles = (N + TP - 1) / TP;
+  const int ntiles = (N + TILE - 1) / TILE;
   // this CTA's tiles [t_begin, t_begin + my_tiles) of the candidate-major numbering t = b * ntiles + j; the launch
   // makes gridDim.x <= B * ntiles, so every range holds at least one tile
   const long long T = (long long)a.B * ntiles;
@@ -140,7 +136,7 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
   const unsigned char *img = static_cast<const unsigned char *>(a.tc_img);
   const bool has_l1 = a.stage1_mode != 0;
   const uint32_t smem_s = smem_u32(smem);
-  const uint32_t w1_s = smem_s + W1_OFF, w2_s = smem_s + W2_OFF, ring_s = smem_s + RING_OFF;
+  const uint32_t w1_s = smem_s + W1_OFF, w2_s = smem_s + W2_OFF, x3_s = smem_s + X3_OFF, ring_s = smem_s + RING_OFF;
   const uint32_t misc_s = smem_s + MISC_OFF;
   const uint32_t full_s = misc_s + (uint32_t)offsetof(Misc, full_bar), empty_s = misc_s + (uint32_t)offsetof(Misc, empty_bar);
   const uint32_t wbar_s = misc_s + (uint32_t)offsetof(Misc, w_bar);
@@ -158,8 +154,6 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
     S.mean[tid] = a.in.mean ? a.in.mean[tid] : 0.0;
     S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: the hot loop multiplies
   }
-  for (int i = tid; i < (int)(SACC_BYTES / 8); i += NTC) sacc[i] = make_float2(-INFINITY, -INFINITY);
-  for (int i = tid; i < 2 * 1024; i += NTC) keys[i] = 0u;   // below the key of every float
   if (tid == 0) {
     for (int i = 0; i < NSLOT; i++) {
       mbar_init(full_s + 8u * i, 1);
@@ -249,16 +243,16 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
         mbar_arrive(cand_s);
       }
       if (k > 0) {
-        // candidate k - 1: bias and ReLU commute with the max (both are monotone), so they follow it
+        // candidate k - 1: bias and ReLU commute with the max (both are monotone), so they follow it.  Every one of
+        // the 1024 keys was stored by its channel's owner before the consumers arrived on keys_bar.
         const int kp = k - 1;
         mbar_wait(keys_s + 8u * (kp & 1), ((uint32_t)kp >> 1) & 1u);
-        uint32_t *kb = keys + (kp & 1) * 1024;
+        const uint32_t *kb = keys + (kp & 1) * 1024;
         uint32_t *g = a.gmax_keys + (size_t)(b_first + kp) * 1024;
         for (int ch = ht; ch < 1024; ch += NHELP) {
           float m = cg_key2f(kb[ch]) + __ldg(&a.l3.b[ch]);
           if (a.relu3) m = fmaxf(m, 0.f);
           atomicMax(&g[ch], cg_f2key(m));
-          kb[ch] = 0u;
         }
       }
     }
@@ -288,10 +282,9 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
 #endif
   mbar_wait(wbar_s, 0u);
 
-  // The input of a point row is fetched one tile ahead (fetch_id / fetch_row during the previous tile's L3) and
-  // finished (finish_row) when its tile starts, so the dependent id -> cloud-row loads are off the critical path.
-  // Row n >= N of candidate b duplicates a valid point of b: it cannot change a max.  x_direct rows travel as exact
-  // float -> double.
+  // The ids of a tile's point rows are fetched one tile ahead (during the previous tile's L3) and the dependent
+  // cloud rows at the start of each 64-row block (the rows of both blocks do not fit beside the front's registers).  Row n >= N of candidate b duplicates a valid point of b: it cannot change a max.
+  // x_direct rows travel as exact float -> double.
   auto fetch_id = [&](int b, int n) -> int {
     if (n >= N) n = N - 1;
     return (a.in.x_direct == nullptr && a.in.ids) ? __ldg(a.in.ids + (size_t)b * N + n) : n;
@@ -343,254 +336,254 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
   auto slot_of = [&](int c, int kb) { return (gslot + 2u * c + kb) % NSLOT; };
   auto phase_of = [&](int c, int kb) { return ((gslot + 2u * c + kb) / NSLOT) & 1u; };
 
-  const int prow = wg * 64 + w4 * 16 + g;   // this thread's rows of a tile: prow and prow + 8
-  // Half-chunks per unrolled L3 group (below), and whether the whole input rows of the next tile are prefetched during
-  // L3 or only their ids: the 24 registers of two float64 rows fit beside the L3 pipeline of engine 3 only.
-  constexpr int L3_GROUP = PASSES == 1 ? 8 : 4;
-  constexpr bool ROW_PREFETCH = PASSES == 1;
-  double r0[6], r1[6];   // raw input rows of the next tile
-  int id0, id1;
+  // this thread's front rows of a tile: prow(blk) and prow(blk) + 8 of each 64-row block blk
+  auto prow = [&](int blk) { return wg * (TILE / 2) + blk * 64 + w4 * 16 + g; };
+  int ids[NBLK][2];
   {
     const int j = t_begin - b_first * ntiles;
-    id0 = fetch_id(b_first, j * TP + prow);
-    id1 = fetch_id(b_first, j * TP + prow + 8);
-    if (ROW_PREFETCH) {
-      fetch_row(b_first, id0, r0);
-      fetch_row(b_first, id1, r1);
-    }
+#pragma unroll
+    for (int blk = 0; blk < NBLK; blk++)
+#pragma unroll
+      for (int r = 0; r < 2; r++) ids[blk][r] = fetch_id(b_first, j * TILE + prow(blk) + 8 * r);
   }
-  // Warpgroup 1 starts its first tile when warpgroup 0 has finished the front layers of its own (named barrier 2), so
-  // that one warpgroup's front runs under the other's L3 instead of leaving the tensor pipe idle for both.
-  if (wg == 1) asm volatile("bar.sync 2, 256;" ::: "memory");
   TL_MARK(TL_START);
   for (int it = 0; it < my_tiles; it++) {
     // tile j of candidate b, candidate ci of the range; the candidate's first / last tile in this range
     const int b = (t_begin + it) / ntiles, j = t_begin + it - b * ntiles, ci = b - b_first;
     const bool cand_first = it == 0 || j == 0, cand_last = it + 1 == my_tiles || j + 1 == ntiles;
-    const int p0 = j * TP + prow;   // this thread's rows: points p0 and p0 + 8
     if (cand_first) mbar_wait(cand_s, (uint32_t)ci & 1u);   // pinv / T3 / T64 image of candidate b
-    // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
-    float d64[32];
-    {
-      float v0[6], v1[6];
-      if (!ROW_PREFETCH) {
-        fetch_row(b, id0, r0);
-        fetch_row(b, id1, r1);
-      }
-      finish_row(r0, v0);
-      finish_row(r1, v1);
-      TL_MARK(TL_INPUT);
+#pragma unroll 1
+    for (int blk = 0; blk < NBLK; blk++) {
+      const int p0 = j * TILE + prow(blk);   // this thread's rows: points p0 and p0 + 8
+      // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
+      float d64[32];
+      {
+        double r0[6], r1[6];
+        fetch_row(b, blk == 0 ? ids[0][0] : ids[NBLK - 1][0], r0);   // constant indices: ids stays in registers
+        fetch_row(b, blk == 0 ? ids[0][1] : ids[NBLK - 1][1], r1);
+        float v0[6], v1[6];
+        finish_row(r0, v0);
+        finish_row(r1, v1);
+        TL_MARK(TL_INPUT);
 #pragma unroll
-      for (int m = 0; m < 8; m++)
+        for (int m = 0; m < 8; m++)
 #pragma unroll
-        for (int e = 0; e < 2; e++) {
-          const int c = 8 * m + 2 * q + e;
-          float o0 = S.bias0[c], o1 = o0;
+          for (int e = 0; e < 2; e++) {
+            const int c = 8 * m + 2 * q + e;
+            float o0 = S.bias0[c], o1 = o0;
 #pragma unroll
-          for (int k = 0; k < 6; k++) {
-            const float w = S.w0[k * 64 + c];
-            o0 = fmaf(v0[k], w, o0);
-            o1 = fmaf(v1[k], w, o1);
+            for (int k = 0; k < 6; k++) {
+              const float w = S.w0[k * 64 + c];
+              o0 = fmaf(v0[k], w, o0);
+              o1 = fmaf(v1[k], w, o1);
+            }
+            d64[4 * m + e] = fmaxf(o0, 0.f);
+            d64[4 * m + 2 + e] = fmaxf(o1, 0.f);
           }
-          d64[4 * m + e] = fmaxf(o0, 0.f);
-          d64[4 * m + 2 + e] = fmaxf(o1, 0.f);
+      }
+      uint32_t xh[4][4], xl[4][4];   // A fragments of the layer input (K = 64), bf16 hi + lo
+      // ---- L1: 64 -> 64 (STNkd shared conv, or the per-candidate T64 feature transform) ----
+      if (has_l1) {
+        d_to_a<4, false>(d64, xh, xl);
+        wg_fence_regs<16>(xh[0]);
+        wg_fence_regs<16>(xl[0]);
+        wg_fence_regs<32>(d64);
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ks++) {
+          const uint64_t bh = wg_desc(w1_s + 32u * ks), bl = wg_desc(w1_s + 8192u + 32u * ks);
+          wg_m64n64<false>(d64, xl[ks], bh, ks > 0 ? 1u : 0u);
+          wg_m64n64<false>(d64, xh[ks], bl, 1u);
+          wg_m64n64<false>(d64, xh[ks], bh, 1u);
         }
-    }
-    uint32_t xh[8][4], xl[8][4];   // A fragments of the current layer input (up to K = 128), bf16 / fp16 hi + lo
-    // ---- L1: 64 -> 64 (STNkd shared conv, or the per-candidate T64 feature transform) ----
-    if (has_l1) {
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_regs<32>(d64);
+        wg_fence_regs<16>(xh[0]);
+        wg_fence_regs<16>(xl[0]);
+#pragma unroll
+        for (int i = 0; i < 32; i++) {
+          if (a.stage1_mode == 1) d64[i] = fmaxf(d64[i] + S.bias1[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
+        }
+        if (a.pf_out) {   // PointNetSeg point feature (pointnet2.py:261)
+#pragma unroll
+          for (int r = 0; r < 2; r++) {
+            const int n = p0 + 8 * r;
+            if (n < N) {
+              float *dst = a.pf_out + ((size_t)b * N + n) * 64 + 2 * q;
+#pragma unroll
+              for (int m = 0; m < 8; m++)
+                *reinterpret_cast<float2 *>(dst + 8 * m) = make_float2(d64[4 * m + 2 * r], d64[4 * m + 2 * r + 1]);
+            }
+          }
+        }
+      }
+      // the last read of candidate b's pinv / T3 / T64 image in this range is done: the helpers may replace them
+      if (cand_last && blk == NBLK - 1) mbar_arrive(front_s);
+      // ---- L2: 64 -> 128 ----
+      float acc[64];
       d_to_a<4, false>(d64, xh, xl);
       wg_fence_regs<16>(xh[0]);
       wg_fence_regs<16>(xl[0]);
-      wg_fence_regs<32>(d64);
+      wg_fence_regs<64>(acc);
       wg_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ks++) {
-        const uint64_t bh = wg_desc(w1_s + 32u * ks), bl = wg_desc(w1_s + 8192u + 32u * ks);
-        wg_m64n64<false>(d64, xl[ks], bh, ks > 0 ? 1u : 0u);
-        wg_m64n64<false>(d64, xh[ks], bl, 1u);
-        wg_m64n64<false>(d64, xh[ks], bh, 1u);
+        const uint64_t bh = wg_desc(w2_s + 32u * ks), bl = wg_desc(w2_s + PIECE + 32u * ks);
+        wg_m64n128<false>(acc, xl[ks], bh, ks > 0 ? 1u : 0u);
+        wg_m64n128<false>(acc, xh[ks], bl, 1u);
+        wg_m64n128<false>(acc, xh[ks], bh, 1u);
       }
       wg_commit();
       wg_wait<0>();
-      wg_fence_regs<32>(d64);
+      wg_fence_regs<64>(acc);
       wg_fence_regs<16>(xh[0]);
       wg_fence_regs<16>(xl[0]);
 #pragma unroll
-      for (int i = 0; i < 32; i++) {
-        if (a.stage1_mode == 1) d64[i] = fmaxf(d64[i] + S.bias1[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
-      }
-      if (a.pf_out) {   // PointNetSeg point feature (pointnet2.py:261)
+      for (int i = 0; i < 64; i++) acc[i] = fmaxf(acc[i] + S.bias2[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
+      TL_MARK(TL_FRONT);
+      // Both warpgroups' L3 wgmma of the previous tile are complete (each waited for its own before getting here):
+      // the X3 image may be overwritten.  The first block's front ran under the other warpgroup's L3.
+      if (blk == 0) asm volatile("bar.sync 1, 256;" ::: "memory");
+      // ---- X3 -> the [TILE x 128] K-major image: accumulator pair i (channels 8i + 2q, +1) of row g (+ 8) is one
+      // 32-bit word of 16-byte chunk i & 7 of K-block i >> 3 (conflict-free: the 8 rows of a step hit 8 chunks) ----
 #pragma unroll
-        for (int r = 0; r < 2; r++) {
-          const int n = p0 + 8 * r;
-          if (n < N) {
-            float *dst = a.pf_out + ((size_t)b * N + n) * 64 + 2 * q;
+      for (int r = 0; r < 2; r++) {
+        const int pr = prow(blk) + 8 * r;
 #pragma unroll
-            for (int m = 0; m < 8; m++)
-              *reinterpret_cast<float2 *>(dst + 8 * m) = make_float2(d64[4 * m + 2 * r], d64[4 * m + 2 * r + 1]);
+        for (int i = 0; i < 16; i++) {
+          const float x0 = acc[4 * i + 2 * r], x1 = acc[4 * i + 2 * r + 1];
+          const uint32_t off = X3_OFF + (uint32_t)(i >> 3) * X3_KB + row_chunk_off(pr, i & 7) + 4u * q;
+          uint32_t h, l;
+          if (PASSES == 1) {
+            vmax = fmaxf(vmax, fmaxf(x0, x1));
+            // values beyond the fp16 range saturate to 65504 instead of becoming inf (x0 -> low half)
+            asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(x1), "f"(x0));
+          } else if (PASSES == 2) {   // split_f16x2 clamps to the fp16 range: record what it clamps
+            vmax = fmaxf(vmax, fmaxf(x0, x1));
+            split_f16x2(x0, x1, h, l);
+          } else {
+            split_bf16x2(x0, x1, h, l);
           }
+          *reinterpret_cast<uint32_t *>(smem + off) = h;
+          if (PASSES != 1) *reinterpret_cast<uint32_t *>(smem + off + X3_LO) = l;
         }
       }
     }
-    // the last read of candidate b's pinv / T3 / T64 image in this range is done: the helpers may replace them
-    if (cand_last) mbar_arrive(front_s);
-    // ---- L2: 64 -> 128 ----
-    float acc[64];
-    d_to_a<4, false>(d64, xh, xl);
-    wg_fence_regs<16>(xh[0]);
-    wg_fence_regs<16>(xl[0]);
-    wg_fence_regs<64>(acc);
-    wg_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ks++) {
-      const uint64_t bh = wg_desc(w2_s + 32u * ks), bl = wg_desc(w2_s + PIECE + 32u * ks);
-      wg_m64n128<false>(acc, xl[ks], bh, ks > 0 ? 1u : 0u);
-      wg_m64n128<false>(acc, xh[ks], bl, 1u);
-      wg_m64n128<false>(acc, xh[ks], bh, 1u);
-    }
-    wg_commit();
-    wg_wait<0>();
-    wg_fence_regs<64>(acc);
-    wg_fence_regs<16>(xh[0]);
-    wg_fence_regs<16>(xl[0]);
-    // warpgroup 0's front of the first tile is done: release warpgroup 1 (see above)
-    if (it == 0 && wg == 0) asm volatile("bar.arrive 2, 256;" ::: "memory");
-    TL_MARK(TL_FRONT);
-#pragma unroll
-    for (int i = 0; i < 64; i++) acc[i] = fmaxf(acc[i] + S.bias2[8 * (i >> 2) + 2 * q + (i & 1)], 0.f);
-    if (PASSES == 1) {
-#pragma unroll
-      for (int j = 0; j < 8; j++)
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-          const float x0 = acc[8 * j + 2 * r], x1 = acc[8 * j + 2 * r + 1];
-          vmax = fmaxf(vmax, fmaxf(x0, x1));
-          // values beyond the fp16 range saturate to 65504 instead of becoming inf (x0 -> low half)
-          asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(xh[j][r]) : "f"(x1), "f"(x0));
-        }
-    } else {
-      if (PASSES == 2) {   // split_f16x2 clamps to the fp16 range: record what it clamps
-#pragma unroll
-        for (int i = 0; i < 64; i++) vmax = fmaxf(vmax, acc[i]);
-      }
-      d_to_a<8, F16>(acc, xh, xl);
-    }
-    wg_fence_regs<32>(xh[0]);
-    if (PASSES != 1) wg_fence_regs<32>(xl[0]);
-    // ---- L3: 128 -> 1024 in 16 half-chunks of 64 channels; max over the tile's points ----
-    // Two 32-register accumulators: half-chunk h + 1 is issued before half-chunk h is reduced, so the reduction
-    // overlaps the tensor cores.  Half-chunk h = channels 64h .. 64h+63 = rows 64 (h & 1) .. of chunk h / 2's W3 slots.
-    // The 16 half-chunks are unrolled so that both accumulators are fixed registers: with operand fences around every
-    // issue and wait ptxas then keeps exactly one wgmma group in flight during each reduction.
-    auto issue = [&](int h, float *d) {
-      const int c = h >> 1;
-      if ((h & 1) == 0) {
+    // X3 is complete once every consumer thread has stored its part: make it visible to the wgmma (async) proxy
+    fence_proxy_async();
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    TL_MARK(TL_X3);
+    // ---- L3: 128 -> 1024, channel-major: D[ch][pt] = W3 (ring slot rows 64 wg ..) . X3^T ----
+    // 8 * NBLK units; unit u = 128-point block u % NBLK of chunk u / NBLK, one m64n128 accumulator of 64 registers.
+    // Two accumulators: unit u + 1 is issued before unit u is reduced, so the reduction overlaps the tensor cores.
+    // The units of a group are unrolled so that both accumulators are fixed registers; with operand fences around
+    // every issue and wait ptxas keeps exactly one wgmma group in flight during each reduction.
+    // The units run in unrolled groups that end with a full wait, so that no wgmma is in flight across the loop's
+    // back edge (ptxas would otherwise serialise the loop); larger groups do not fit the 168-register budget of a
+    // 384-thread CTA.  Issuing the next chunk's unit while a chunk is in flight holds 4 W3 slots: the 6 fp16 slots
+    // allow it, the 3 bf16 slots of engine 1 do not, so engine 1 runs unit by unit and relies on the other
+    // warpgroup's wgmma to cover its reductions.  Its ring holds only 1.5 chunks, so engine 1 commits each K-block
+    // as a group of its own and hands K-block 0's slot back as soon as that group is complete: the producer then
+    // fetches the next chunk's second slot under the current chunk's second half.
+    constexpr int NU = NCHUNK * NBLK, GROUP = PASSES == 1 ? 8 : (PASSES == 2 ? 4 : 1);
+    constexpr bool EARLY_RELEASE = GROUP == 1;
+    static_assert(GROUP == 1 || NSLOT >= 4, "a unit issued ahead needs the next chunk's slots as well");
+    auto issue = [&](int u, float *d) {
+      const int c = u / NBLK, hb = u % NBLK;
+      if (hb == 0) {
         TL_SPAN_BEGIN();
         mbar_wait(full_s + 8u * slot_of(c, 0), phase_of(c, 0));
         mbar_wait(full_s + 8u * slot_of(c, 1), phase_of(c, 1));
         TL_SPAN_END(TL_RING);
       }
-      wg_fence_regs<32>(d);
+      wg_fence_regs<64>(d);
       wg_fence();
 #pragma unroll
       for (int kb = 0; kb < 2; kb++) {
-        const uint32_t ws = ring_s + slot_of(c, kb) * SLOT_BYTES + (uint32_t)(h & 1) * (PIECE / 2);
+        const uint32_t ws = ring_s + slot_of(c, kb) * SLOT_BYTES + (uint32_t)wg * (PIECE / 2);
+        const uint32_t xs = x3_s + (uint32_t)kb * X3_KB + (uint32_t)hb * PIECE;
 #pragma unroll
         for (int ks = 0; ks < 4; ks++) {
-          const int j = kb * 4 + ks;
           const uint32_t first = (kb | ks) ? 1u : 0u;
-          const uint64_t bw = wg_desc(ws + 32u * ks);
+          const uint64_t aw = wg_desc(ws + 32u * ks), bx = wg_desc(xs + 32u * ks);
           if (PASSES == 3) {
-            const uint64_t bl = wg_desc(ws + PIECE + 32u * ks);
-            wg_m64n64<false>(d, xl[j], bw, first);   // x_lo * w_hi
-            wg_m64n64<false>(d, xh[j], bl, 1u);      // x_hi * w_lo
-            wg_m64n64<false>(d, xh[j], bw, 1u);      // x_hi * w_hi
+            const uint64_t al = wg_desc(ws + PIECE + 32u * ks), bxl = wg_desc(xs + X3_LO + 32u * ks);
+            wg_ss_m64n128<false>(d, aw, bxl, first);   // w_hi * x_lo
+            wg_ss_m64n128<false>(d, al, bx, 1u);       // w_lo * x_hi
+            wg_ss_m64n128<false>(d, aw, bx, 1u);       // w_hi * x_hi
           } else if (PASSES == 2) {
-            wg_m64n64<true>(d, xl[j], bw, first);
-            wg_m64n64<true>(d, xh[j], bw, 1u);
+            wg_ss_m64n128<true>(d, aw, wg_desc(xs + X3_LO + 32u * ks), first);
+            wg_ss_m64n128<true>(d, aw, bx, 1u);
           } else {
-            wg_m64n64<true>(d, xh[j], bw, first);
+            wg_ss_m64n128<true>(d, aw, bx, first);
           }
         }
+        if (EARLY_RELEASE && kb == 0) wg_commit();   // K-block 0 as a group of its own (see below)
       }
       wg_commit();
-      wg_fence_regs<32>(d);
+      wg_fence_regs<64>(d);
     };
-    // half-chunk h is complete in this warp: fold its column max into the running max; after the second half of a
-    // chunk hand the chunk's two W3 slots back
-    auto reduce = [&](int h, const float *d) {
-      const int c = h >> 1;
-      if (h & 1) {
+    // unit u is complete in this warpgroup: the max over its points of each of this thread's rows (channels
+    // 128 c + 64 wg + 16 w4 + g + 8 r) is folded over the row's quad, and the q = 0 lane, the channel's only owner in
+    // the CTA, keeps the candidate's running max as a key in keys[ci & 1] (stored on the candidate's first unit of
+    // the range).  After the chunk's last unit hand its two W3 slots back.
+    uint32_t *kk = keys + (ci & 1) * 1024 + wg * 64 + w4 * 16 + g;
+    auto reduce = [&](int u, const float *d) {
+      const int c = u / NBLK, hb = u % NBLK;
+      if (hb == NBLK - 1) {
         __syncwarp();
         if (lane == 0) {
-          mbar_arrive(empty_s + 8u * slot_of(c, 0));
+          if (!EARLY_RELEASE) mbar_arrive(empty_s + 8u * slot_of(c, 0));
           mbar_arrive(empty_s + 8u * slot_of(c, 1));
         }
       }
-      // column max over this warp's 16 rows: own two rows, then a transposing butterfly over lane bits 4, 3, 2
-      // (each step halves the columns a thread is responsible for).  Afterwards thread (g, q) holds the columns
-      // 8g + 2q + {0, 1} of the half-chunk.
-      float x[16];
 #pragma unroll
-      for (int i = 0; i < 8; i++) {
-        x[2 * i] = fmaxf(d[4 * i], d[4 * i + 2]);
-        x[2 * i + 1] = fmaxf(d[4 * i + 1], d[4 * i + 3]);
+      for (int r = 0; r < 2; r++) {
+        float m = fmaxf(d[2 * r], d[2 * r + 1]);
+#pragma unroll
+        for (int i = 1; i < 16; i++) m = fmaxf(m, fmaxf(d[4 * i + 2 * r], d[4 * i + 2 * r + 1]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        if (q == 0) {
+          const uint32_t key = cg_f2key(m);
+          uint32_t &slot = kk[128 * c + 8 * r];
+          slot = (cand_first && hb == 0) ? key : max(slot, key);
+        }
       }
-      max_butterfly_step<16>(x, lane);
-      max_butterfly_step<8>(x, lane);
-      max_butterfly_step<4>(x, lane);
-      float2 &slot = sacc[((wg * 2 * NCHUNK + h) * 4 + w4) * 32 + lane];   // private to this thread
-      const float2 old = slot;
-      slot = make_float2(fmaxf(old.x, x[0]), fmaxf(old.y, x[1]));
     };
-    // The half-chunks run in groups of L3_GROUP, unrolled so that the two accumulators are fixed registers.  Inside a
-    // group one wgmma group is in flight during each reduction; a group ends with a full wait, so that no wgmma is in
-    // flight across the loop's back edge (ptxas would otherwise serialise the loop).  A fully unrolled L3 does not fit
-    // the 168-register budget of a 288-thread CTA (registers are allocated per
-    // warpgroup: 288 threads count as 384).
-    // The next tile's input is fetched where nothing is in flight: the ids before the first group, the dependent
-    // rows before the second (a last tile re-reads its own rows, clamped to the candidate's points).
-    const int nt = t_begin + it + (it + 1 < my_tiles ? 1 : 0);
-    const int nb = nt / ntiles, pn = (nt - nb * ntiles) * TP + prow;
-    id0 = fetch_id(nb, pn);
-    id1 = fetch_id(nb, pn + 8);
-#pragma unroll 1
-    for (int h0 = 0; h0 < 2 * NCHUNK; h0 += L3_GROUP) {
-      if (ROW_PREFETCH && h0 == L3_GROUP) {
-        fetch_row(nb, id0, r0);
-        fetch_row(nb, id1, r1);
-      }
-      float acc3[2][32];   // even / odd half-chunks
-      issue(h0, acc3[0]);
+    // the next tile's ids are loaded while nothing depends on them (a last tile re-reads its own)
+    {
+      const int nt = t_begin + it + (it + 1 < my_tiles ? 1 : 0);
+      const int nb = nt / ntiles, pn = (nt - nb * ntiles) * TILE;
 #pragma unroll
-      for (int j = 0; j < L3_GROUP; j++) {
-        if (j + 1 < L3_GROUP) issue(h0 + j + 1, acc3[(j + 1) & 1]);
+      for (int blk = 0; blk < NBLK; blk++)
+#pragma unroll
+        for (int r = 0; r < 2; r++) ids[blk][r] = fetch_id(nb, pn + prow(blk) + 8 * r);
+    }
+#pragma unroll 1
+    for (int u0 = 0; u0 < NU; u0 += GROUP) {
+      float acc3[2][64];   // even / odd units
+      issue(u0, acc3[0]);
+#pragma unroll
+      for (int j = 0; j < GROUP; j++) {
+        if (j + 1 < GROUP) issue(u0 + j + 1, acc3[(j + 1) & 1]);
         TL_SPAN_BEGIN();
-        if (j + 1 < L3_GROUP) wg_wait<1>();
+        if (EARLY_RELEASE) {
+          wg_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_s + 8u * slot_of((u0 + j) / NBLK, 0));
+        }
+        if (j + 1 < GROUP) wg_wait<1>();
         else wg_wait<0>();
         TL_SPAN_END(TL_L3_WAIT);
-        wg_fence_regs<32>(acc3[j & 1]);
-        reduce(h0 + j, acc3[j & 1]);
+        wg_fence_regs<64>(acc3[j & 1]);
+        reduce(u0 + j, acc3[j & 1]);
       }
     }
-    // the last wgmma that read the A fragments is complete: the next tile's front may overwrite them
-    wg_fence_regs<32>(xh[0]);
-    if (PASSES != 1) wg_fence_regs<32>(xl[0]);
     gslot += 2u * NCHUNK;
-    if (cand_last) {
-      // hand candidate b's running max to the helpers (keys by candidate parity) and start the next one at -inf
-      uint32_t *kk = keys + (ci & 1) * 1024;
-#pragma unroll 4
-      for (int h = 0; h < 2 * NCHUNK; h++) {
-        float2 &slot = sacc[((wg * 2 * NCHUNK + h) * 4 + w4) * 32 + lane];
-        const float2 v = slot;
-        atomicMax(&kk[64 * h + 2 * lane], cg_f2key(v.x));   // thread (g, q) holds columns 8g + 2q + {0, 1}
-        atomicMax(&kk[64 * h + 2 * lane + 1], cg_f2key(v.y));
-        slot = make_float2(-INFINITY, -INFINITY);
-      }
-      mbar_arrive(keys_s + 8u * (ci & 1));
-    }
+    // candidate b's max is complete in keys[ci & 1]: hand it to the helpers
+    if (cand_last) mbar_arrive(keys_s + 8u * (ci & 1));
     TL_MARK(TL_L3);
   }
   if (F16 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
@@ -646,12 +639,13 @@ int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *
 int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
   CG_REQUIRE(ctx, a.B > 0 && a.N > 0, "trunk: B,N must be positive");
   CG_REQUIRE(ctx, a.tc_img != nullptr, "trunk: tensor-core weight image missing");
-  // persistent: one CTA per SM (or per tile, if there are fewer tiles), each over a balanced range of tiles
-  const long long tiles = (long long)a.B * ((a.N + TP - 1) / TP);
-  CG_REQUIRE(ctx, tiles <= INT_MAX, "trunk: too many tiles in one launch");
-  const int grid = (int)std::min<long long>(ctx->num_sms, tiles);
   // W3 beyond the fp16 range: the fp16 engines fall back to the 3-pass bf16 kernel
   const int passes = !a.tc_f16_ok || ctx->engine == 1 ? 3 : (ctx->engine == 2 ? 2 : 1);
+  // persistent: one CTA per SM (or per tile, if there are fewer tiles), each over a balanced range of tiles
+  const int tp = tile_points(passes);
+  const long long tiles = (long long)a.B * ((a.N + tp - 1) / tp);
+  CG_REQUIRE(ctx, tiles <= INT_MAX, "trunk: too many tiles in one launch");
+  const int grid = (int)std::min<long long>(ctx->num_sms, tiles);
 #ifdef CG_EXPERIMENTS
   static const bool timeline = getenv("CG_TRUNK_TIMELINE") && atoi(getenv("CG_TRUNK_TIMELINE")) != 0;
   unsigned long long *tl = nullptr;
@@ -671,8 +665,8 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
     CG_CUDA(ctx, cudaMemcpyAsync(h.data(), tl, tl_words * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CG_CUDA(ctx, cudaFreeAsync(tl, ctx->stream));
     CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    // cycles per tile of one warp, averaged over the consumer warps of the sampled CTAs; the warps of a CTA run
-    // concurrently, so "total" is also the CTA's cycles per tile
+    // cycles of one warp, averaged over the consumer warps of the sampled CTAs; the warps of a CTA run
+    // concurrently, so "total" is also the CTA's cycles
     double sum[TL_NPHASE + 1] = {}, tiles = 0;
     int recs = 0;
     for (int r = 0; r < TL_CTAS * NCW; r++) {
@@ -684,16 +678,18 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
       recs++;
     }
     if (recs > 0) {
-      // tensor-pipe cycles of one 128-point tile at 2048 dense fp16 / bf16 MAC per clock per SM
+      // per 128 points, so that tiles of 128 and 256 points compare directly; tensor-pipe cycles of 128 points at
+      // 2048 dense fp16 / bf16 MAC per clock per SM
+      const double p128 = tiles * (tp / 128);
       const double l3 = 128.0 * 128 * 1024 / 2048 * passes, l12 = 128.0 * 64 * (128 + (a.stage1_mode ? 64 : 0)) * 3 / 2048;
-      const double tot = sum[TL_NPHASE] / tiles;
+      const double tot = sum[TL_NPHASE] / p128;
       fprintf(stderr,
-              "[trunk-timeline] passes=%d B=%d N=%d stage1=%d tiles/CTA=%.0f warps=%d  clk/tile: start %.0f  input %.0f  "
-              "front %.0f  l3 %.0f (wgmma-wait %.0f, ring-wait %.0f)  total %.0f  | tensor work %.0f clk/tile -> "
-              "busy %.1f%%\n",
-              passes, a.B, a.N, a.stage1_mode, tiles / recs, recs, sum[TL_START] / tiles, sum[TL_INPUT] / tiles,
-              sum[TL_FRONT] / tiles, sum[TL_L3] / tiles, sum[TL_L3_WAIT] / tiles, sum[TL_RING] / tiles, tot, l3 + l12,
-              100.0 * (l3 + l12) / tot);
+              "[trunk-timeline] passes=%d B=%d N=%d stage1=%d tile=%d tiles/CTA=%.0f warps=%d  clk/128 pts: start %.0f  "
+              "input %.0f  front %.0f  x3 %.0f  l3 %.0f (wgmma-wait %.0f, ring-wait %.0f)  total %.0f  | tensor work "
+              "%.0f clk/128 pts -> busy %.1f%%\n",
+              passes, a.B, a.N, a.stage1_mode, tp, tiles / recs, recs, sum[TL_START] / p128, sum[TL_INPUT] / p128,
+              sum[TL_FRONT] / p128, sum[TL_X3] / p128, sum[TL_L3] / p128, sum[TL_L3_WAIT] / p128, sum[TL_RING] / p128,
+              tot, l3 + l12, 100.0 * (l3 + l12) / tot);
     }
   }
 #endif

@@ -2,13 +2,16 @@
 
 Builds a developer copy of the library (CG_EXPERIMENTS, in a temporary directory; the package's own build is not
 touched), then runs one K2-sized grasp-Q forward (B candidates x N points: the STN3d, STNkd and encoder trunks) per
-engine with CG_TRUNK_TIMELINE=1.  Every trunk launch prints one line to stderr: clock64() cycles per 128-point tile of
-one consumer warp, averaged over the warps of 8 sampled CTAs, split into
-  start   W2 landed / warpgroup offset (once per CTA, spread over its tiles)
-  input   the float64 input transform of the tile's rows (plus their loads where they are not prefetched)
+engine with CG_TRUNK_TIMELINE=1.  Every trunk launch prints one line to stderr: clock64() cycles of one consumer warp
+per 128 points (engine 3 runs 256-point tiles, engines 1 and 2 128-point tiles), averaged over the warps of 8 sampled
+CTAs, split into
+  start   W2 landed (once per CTA, spread over its tiles)
+  input   the cloud-row loads and the float64 input transform of the rows
   front   6->64 FMA, L1, L2
+  x3      waiting for the other warpgroup to leave the previous tile's L3, storing X3, and the barrier after it
   l3      128->1024 and the max; of which wgmma-wait = waiting for a wgmma group, ring-wait = waiting for W3 slots
-and the tensor-busy estimate: the tile's tensor work at 2048 dense fp16 / bf16 MAC per clock per SM over its cycles.
+and the tensor-busy estimate: the tensor work of 128 points at 2048 dense fp16 / bf16 MAC per clock per SM over their
+cycles.
 
     python scripts/trunk_timeline.py [--engines 3,1] [-B 4096] [-N 1024]
 """
