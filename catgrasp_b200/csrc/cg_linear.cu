@@ -247,7 +247,9 @@ __global__ void __launch_bounds__(256) linear_rows_kernel(const float *__restric
   }
 }
 
-// softmax over C <= 32 classes, one warp per row (predicter.py:86-90)
+// softmax over C <= 32 classes, one warp per row (predicter.py:86-90).  The label is the argmax of the probabilities
+// as written, the lowest class winning a tie, as the reference takes it (softmax, then argmax): logits closer than
+// expf resolves, such as 0 and 1e-30, give equal probabilities and so the lower class, not the larger logit.
 __global__ void softmax_kernel(const float *__restrict__ logits, int B, int C, float *__restrict__ probs,
                                int32_t *__restrict__ label) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -255,19 +257,25 @@ __global__ void softmax_kernel(const float *__restrict__ logits, int B, int C, f
   if (row >= B) return;
   const float v = (lane < C) ? logits[(size_t)row * C + lane] : -INFINITY;
   float m = v;
-  int am = (lane < C) ? lane : 0x7fffffff;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float om = __shfl_xor_sync(0xffffffffu, m, o);
-    const int oa = __shfl_xor_sync(0xffffffffu, am, o);
-    if (om > m || (om == m && oa < am)) { m = om; am = oa; }
-  }
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   const float e = (lane < C) ? expf(v - m) : 0.f;
   float s = e;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane < C && probs) probs[(size_t)row * C + lane] = e / s;
-  if (lane == 0 && label) label[row] = am;
+  const float p = e / s;
+  if (lane < C && probs) probs[(size_t)row * C + lane] = p;
+  if (label) {
+    float pm = (lane < C) ? p : -1.f;   // lanes past C never win: every probability is >= 0
+    int am = lane;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float op = __shfl_xor_sync(0xffffffffu, pm, o);
+      const int oa = __shfl_xor_sync(0xffffffffu, am, o);
+      if (op > pm || (op == pm && oa < am)) { pm = op; am = oa; }
+    }
+    if (lane == 0) label[row] = am;
+  }
 }
 
 // NUNOCS post-processing (predicter.py:144-150): one warp per (point, axis)

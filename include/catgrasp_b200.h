@@ -100,6 +100,10 @@ size_t cg_net_blob_floats(int kind, int n_out);
  *   cloud_xyz, cloud_nrm : (M,3) float64      poses : (B,4,4) float64
  *   ids : (B,N) int32 in [0,M)                mean,std : (6,) float64 or NULL
  *   out_probs : (B,n_out) float32             out_label : (B,) int32 or NULL
+ * out_label[b] is the argmax of the float32 probabilities written to
+ * out_probs[b], the lowest class winning a tie (predicter.py:86-89 takes
+ * the argmax after the softmax): logits too close for expf to separate give
+ * equal probabilities and the lower class.
  */
 int cg_graspq_forward_host(cg_net *net,
                            const double *cloud_xyz, const double *cloud_nrm, int M,
