@@ -86,7 +86,15 @@ SIGNATURES = {
     "cg_cone_poses_dev": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, C.c_double, _vp, _vp]),
     "cg_center_grasps_dev": (_i, [_vp, _vp, _vp, _i, _vp, _i]),
     "cg_grasp_affordance_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, C.c_double, _vp, _vp]),
-    "cg_square_distance_dev": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
+    "cg_depth2xyz_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "cg_cloud_index_create": (_i, [_vp, _vp, _i, C.c_double, C.POINTER(_vp)]),
+    "cg_cloud_index_destroy": (None, [_vp]),
+    "cg_cloud_index_info": (_i, [_vp, C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "cg_voxel_down_sample_dev": (_i, [_vp, _vp, _vp, _vp]),
+    "cg_cloud_nearest_dev": (_i, [_vp, _vp, _i, C.c_double, _vp, _vp]),
+    "cg_cloud_radius_mask_dev": (_i, [_vp, _vp, _i, C.c_double, _i, _vp]),
+    "cg_cloud_normals_dev": (_i, [_vp, C.c_double, _i, _vp, _vp, _vp, _vp]),
+    "cg_square_distance_dev":(_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "cg_index_points_dev": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "cg_fps_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "cg_fps_single_cta_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

@@ -270,6 +270,34 @@ def make_pile(n_points, n_objects=8, seed=0, bin_size=0.10, floor_z=0.70, max_ti
             "object_id": ids[sel], "object_poses": np.stack(poses)}
 
 
+def render_depth(K, H, W, n_objects=8, seed=0, bin_size=0.10, floor_z=0.70, oversample=10.0):
+    """A z-buffer of a make_pile scene seen by a pinhole camera K (3x3) at the origin: the nuts over a bin floor that
+    fills the image at camera z = floor_z (a fronto-parallel plane, so its points lie on an exact lattice).
+
+    The nuts are splatted from their surface samples, about ``oversample`` samples per covered pixel, each to its
+    nearest pixel; the nearest sample wins.  Returns (depth (H,W) float32, object id (H,W) int32 with -1 on the floor).
+    The id map stands in for PointGroup's segmentation in tests and timing."""
+    K = np.asarray(K, np.float64)
+    pitch = floor_z / K[0, 0]
+    n_points = int(oversample * n_objects * 4e-4 / (pitch * pitch))
+    scene = make_pile(n_points, n_objects=n_objects, seed=seed, bin_size=bin_size, floor_z=floor_z)
+    p = scene["cloud_xyz"]
+    u = np.rint(K[0, 0] * p[:, 0] / p[:, 2] + K[0, 2]).astype(np.int64)
+    v = np.rint(K[1, 1] * p[:, 1] / p[:, 2] + K[1, 2]).astype(np.int64)
+    ok = (u >= 0) & (u < W) & (v >= 0) & (v < H)
+    pix, z, oid = v[ok] * W + u[ok], p[ok, 2], scene["object_id"][ok]
+    order = np.lexsort((z, pix))
+    first = np.ones(len(order), bool)
+    first[1:] = pix[order][1:] != pix[order][:-1]
+    sel = order[first]
+    depth = np.full(H * W, floor_z, np.float32)
+    ids = np.full(H * W, -1, np.int32)
+    near = z[sel] < floor_z
+    depth[pix[sel][near]] = z[sel][near].astype(np.float32)
+    ids[pix[sel][near]] = oid[sel][near]
+    return depth.reshape(H, W), ids.reshape(H, W)
+
+
 def _rot_x(a):
     c, s = np.cos(a), np.sin(a)
     return np.array([[1, 0, 0], [0, c, -s], [0, s, c]])

@@ -332,6 +332,47 @@ int cg_grasp_affordance_dev(cg_ctx *ctx, const double *cam_in_finger, int G, con
                             const double *affordance, int P, const double *finger_boxes, const int *grip_dirs, int F,
                             double surface_tol, double *out_p, int *out_contacts);
 
+/* ---- point-cloud preparation ---- */
+/* Replaces the open3d / scipy steps of the per-pick path: Utils.py:239-251 (depth2xyzmap), open3d VoxelDownSample and
+ * EstimateNormals (run_grasp_simulation.py:97, :114, :137, :173, :209, :246-247), Utils.py:205-213
+ * (correct_pcd_normal_direction), cKDTree.query (:120, :131) and query_ball_point (Utils.py:482-488).
+ * Points are float64 (N,3) device arrays.  Distances are d2 = (dx*dx + dy*dy) + dz*dz in float64 without FMA,
+ * bit-equal to scipy's; a tie goes to the smaller point index.  No result depends on atomic arrival order.        */
+#define CG_CLOUD_MAX_NN 64
+typedef struct cg_cloud_index cg_cloud_index;
+/* depth (H,W) float32 (depth_is_f64 = 0) or float64 -> out_xyz (H,W,3) float32: x = (u - K[2]) * z / K[0],
+ * y = (v - K[5]) * z / K[4] in float64 left to right, then narrowed; depth < 0.1 in the depth's own type gives
+ * (0,0,0).  K is a host array of 9 doubles (row-major 3x3).                                                        */
+int cg_depth2xyz_dev(cg_ctx *ctx, const void *depth, int depth_is_f64, int H, int W, const double *K, float *out_xyz);
+/* Bins pts (P,3) into cells of size `cell` with origin min_bound - cell/2 (cell = floor((p - origin) / cell)), sorts
+ * the points by (cell, index) and builds the ascending cell table.  The index copies the points, so pts may be freed
+ * afterwards.  Synchronises the context's stream twice (the bounds, then the cell count).  Fails with CG_EINVAL on a
+ * non-finite coordinate or when the cloud spans 2^21 or more cells on an axis.                                     */
+int  cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, double cell, cg_cloud_index **out);
+void cg_cloud_index_destroy(cg_cloud_index *index);
+/* P, number of occupied cells (= the voxel count of cg_voxel_down_sample_dev), cell size, origin[3]; any may be NULL */
+int  cg_cloud_index_info(const cg_cloud_index *index, int *out_points, int *out_cells, double *out_cell, double *out_origin);
+/* open3d VoxelDownSample with voxel_size = the index's cell: one output per occupied cell, in ascending (ix, iy, iz)
+ * order; mean = members summed in ascending point index, divided by the count; normals (P,3) or NULL: the summed
+ * normal divided by its norm (a zero sum stays zero).  out_pts / out_normals hold cg_cloud_index_info's cell count. */
+int  cg_voxel_down_sample_dev(const cg_cloud_index *index, const double *normals, double *out_pts, double *out_normals);
+/* cKDTree(indexed points).query(query (Q,3)) restricted to max_dist: out_idx (Q) int32 = nearest point (smallest
+ * index on a tie), out_dist = sqrt(d2); -1 / +inf when no point has sqrt(d2) <= max_dist.                          */
+int  cg_cloud_nearest_dev(const cg_cloud_index *index, const double *query, int Q, double max_dist, int32_t *out_idx,
+                          double *out_dist);
+/* out_mask[i] = 1 when some indexed point has d2 <= r*r (compare_sqrt = 0, query_ball_point's test) or
+ * sqrt(d2) <= r (compare_sqrt = 1, the `dists <= R` test on cKDTree.query's distances), else 0.                   */
+int  cg_cloud_radius_mask_dev(const cg_cloud_index *index, const double *query, int Q, double r, int compare_sqrt,
+                              uint8_t *out_mask);
+/* Normals of the indexed points: the max_nn (<= CG_CLOUD_MAX_NN) nearest points with d2 <= radius*radius, ordered
+ * by (d2, index) and including the point itself; the unit eigenvector of the smallest eigenvalue of their float64
+ * covariance about the mean; (0,0,1) for fewer than 3 neighbours or a zero covariance; then oriented towards
+ * view_point (host double[3]) exactly as correct_pcd_normal_direction does (n / (|n| + 1e-10), flipped when the dot
+ * product with the unit view direction is < 0).  out_normals (P,3) in the caller's point order; out_nbr (P,max_nn)
+ * int32 (neighbours in order, -1 padded) and out_nbr_count (P) may be NULL.                                      */
+int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point,
+                          double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count);
+
 /* ---- PointNet++ primitives (device pointers) ---------------------------
  * Replace the free functions of pointnet2.py:14-149.  Indices are int32 on
  * the device (the Python mirror widens to int64 like the reference).        */
