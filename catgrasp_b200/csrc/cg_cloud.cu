@@ -619,7 +619,7 @@ extern "C" int cg_cloud_nearest_dev(const cg_cloud_index *ix, const double *quer
                                     double *out_dist) {
   if (!ix) return CG_EINVAL;
   cg_ctx *ctx = ix->ctx;
-  CG_REQUIRE(ctx, query && out_idx && out_dist && Q >= 0, "cloud_nearest: bad arguments");
+  CG_REQUIRE(ctx, Q >= 0 && (Q == 0 || (query && out_idx && out_dist)), "cloud_nearest: bad arguments");   // empty: NULL allowed
   CG_REQUIRE(ctx, max_dist >= 0.0 && std::isfinite(max_dist), "cloud_nearest: max_dist must be finite and >= 0");
   if (Q == 0) return CG_OK;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -632,7 +632,7 @@ extern "C" int cg_cloud_radius_mask_dev(const cg_cloud_index *ix, const double *
                                         uint8_t *out_mask) {
   if (!ix) return CG_EINVAL;
   cg_ctx *ctx = ix->ctx;
-  CG_REQUIRE(ctx, query && out_mask && Q >= 0, "cloud_radius_mask: bad arguments");
+  CG_REQUIRE(ctx, Q >= 0 && (Q == 0 || (query && out_mask)), "cloud_radius_mask: bad arguments");   // empty: NULL allowed
   CG_REQUIRE(ctx, r >= 0.0 && std::isfinite(r), "cloud_radius_mask: r must be finite and >= 0");
   if (Q == 0) return CG_OK;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));

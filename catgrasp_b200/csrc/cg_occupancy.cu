@@ -5,10 +5,14 @@
 // cast from the sensor origin through the sample; the sample is reported when the first occupied cell on that ray is
 // not farther than the sample itself (i.e. the sample is on or behind the observed surface).
 //
-// octomap is not available (SURVEY.md 8c): this file and oracle/occupancy_ref.c restate the semantic with one fixed
-// arithmetic so that they agree bit for bit -- occupied set = cells floor(p / res) of the scan points (dense bit mask
-// over their bounding box); the ray is a 3-D DDA from the origin cell whose next-boundary parameters are recomputed
-// from the integer cell index at every step (no accumulation); a hit counts when |cell centre| <= |sample|.
+// octomap is not available (SURVEY.md 8c): this file and oracle/occupancy_ref.c restate the semantic with the same
+// operations in the same order so that they agree bit for bit -- occupied set = cells floor(p / res) of the scan points
+// (dense bit mask over their bounding box); the ray is a 3-D DDA from the origin cell whose next-boundary parameters
+// are recomputed from the integer cell index at every step (no accumulation); a hit counts when |cell centre| <=
+// |sample|.  The oracle is compiled with -ffp-contract=off; nvcc contracts a*b + c into an FMA by default, so every
+// floating-point operation of the cast kernel is written as an explicit round-to-nearest intrinsic, which nvcc never
+// fuses (tests/test_bitexact_codegen.py checks the PTX for FMAs).  An exact rational statement of the rule, without
+// the kernel's arithmetic or its early exit, is oracle/occupancy_exact.py.
 // The reference's own function, compiled against a restatement of the octomap calls it makes (oracle/build_ref.py,
 // oracle/ref_shim/octomap/octomap.h), returns exactly the same samples (tests/test_mycpp_golden.py); parity with the
 // octomap library itself stays unpinned (not installed, version not pinned by the reference).
@@ -60,17 +64,19 @@ __global__ void occ_cast_kernel(OccGrid g, const unsigned *__restrict__ mask, un
     for (int a = 0; a < 3; a++) step[a] = (d[a] > 0.0) - (d[a] < 0.0);
     // the origin cell itself (octomap's castRay tests the start node first)
     bool hit = occ_test(mask, g, 0, 0, 0);
-    double cdist = sqrt(3.0 * 0.25 * r * r);
+    double cdist = sqrt(__dmul_rn(__dmul_rn(0.75, r), r));    // 3.0 * 0.25 * r * r
+    const double reach = __dadd_rn(dist_q, __dmul_rn(2.0, r));
     while (!hit) {
       double tmax[3];
       for (int a = 0; a < 3; a++)
-        tmax[a] = step[a] ? ((double)(k[a] + (step[a] > 0 ? 1 : 0)) * r) / d[a] : 1e300;
+        tmax[a] = step[a] ? __ddiv_rn(__dmul_rn((double)(k[a] + (step[a] > 0 ? 1 : 0)), r), d[a]) : 1e300;
       const int dim = (tmax[0] < tmax[1]) ? ((tmax[0] < tmax[2]) ? 0 : 2) : ((tmax[1] < tmax[2]) ? 1 : 2);
-      if (tmax[dim] > dist_q + 2.0 * r) break;   // any later cell centre is farther than the sample
+      if (tmax[dim] > reach) break;   // any later cell centre is farther than the sample
       k[dim] += step[dim];
       if (occ_test(mask, g, k[0], k[1], k[2])) {
-        const double cx = ((double)k[0] + 0.5) * r, cy = ((double)k[1] + 0.5) * r, cz = ((double)k[2] + 0.5) * r;
-        cdist = sqrt(cx * cx + cy * cy + cz * cz);
+        const double cx = __dmul_rn(__dadd_rn((double)k[0], 0.5), r), cy = __dmul_rn(__dadd_rn((double)k[1], 0.5), r),
+                     cz = __dmul_rn(__dadd_rn((double)k[2], 0.5), r);
+        cdist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz)));
         hit = true;
       }
     }
@@ -92,7 +98,9 @@ extern "C" int cg_occupancy_grid_geometry(const float *pts_host, int P, float re
     }
   const float pad = 0.005f;
   for (int a = 0; a < 3; a++) {
-    dims[a] = (int)((mx[a] + pad - (mn[a] - pad)) / resolution);   // int max_xi = (xmax+pad-(xmin-pad))/resolution
+    const float n = (mx[a] + pad - (mn[a] - pad)) / resolution;     // int max_xi = (xmax+pad-(xmin-pad))/resolution
+    if (!(n < 2147483648.f)) return CG_EINVAL;                        // the conversion to int would overflow
+    dims[a] = (int)n;
     origin[a] = mn[a] - pad;
   }
   return CG_OK;

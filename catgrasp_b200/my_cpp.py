@@ -209,12 +209,16 @@ def makeOccupancyGridFromCloudScan(pts, K, resolution):
         raise ValueError(f"pts must be (N,3), got {p.shape}")     # assert(pts.cols()==3), common.cpp:329
     ctx = _lib.Context.get()
     res = float(np.float32(resolution))
+    if not res > 0.0:
+        raise _lib.CgError(f"makeOccupancyGridFromCloudScan: resolution must be > 0 in float32, got {resolution!r}")
     dims = (C.c_int * 3)()
     org = (C.c_float * 3)()
     ctx.check(ctx.lib.cg_occupancy_grid_geometry(_lib.ptr(p), p.shape[0], C.c_float(res), dims, org))
     nx, ny, nz = int(dims[0]), int(dims[1]), int(dims[2])
     if nx * ny * nz == 0:
         return np.zeros((0, 3), np.float32)
+    if nx * ny * nz >= 1 << 31:      # refused before the (nx, ny, nz) flag array is allocated
+        raise _lib.CgError(f"makeOccupancyGridFromCloudScan: a {nx} x {ny} x {nz} grid has 2^31 or more samples")
     flags = np.empty(nx * ny * nz, np.uint8)
     ctx.use_own_stream()   # blocking host call
     ctx.check(ctx.lib.cg_occupancy_from_scan_host(ctx.h, _lib.ptr(p), p.shape[0], C.c_float(res), _lib.ptr(flags)))

@@ -357,7 +357,8 @@ int  cg_cloud_index_info(const cg_cloud_index *index, int *out_points, int *out_
  * normal divided by its norm (a zero sum stays zero).  out_pts / out_normals hold cg_cloud_index_info's cell count. */
 int  cg_voxel_down_sample_dev(const cg_cloud_index *index, const double *normals, double *out_pts, double *out_normals);
 /* cKDTree(indexed points).query(query (Q,3)) restricted to max_dist: out_idx (Q) int32 = nearest point (smallest
- * index on a tie), out_dist = sqrt(d2); -1 / +inf when no point has sqrt(d2) <= max_dist.                          */
+ * index on a tie), out_dist = sqrt(d2); -1 / +inf when no point has sqrt(d2) <= max_dist.  Here and in
+ * cg_cloud_radius_mask_dev, Q = 0 is a no-op whose pointers may be NULL (an empty torch tensor has no storage).    */
 int  cg_cloud_nearest_dev(const cg_cloud_index *index, const double *query, int Q, double max_dist, int32_t *out_idx,
                           double *out_dist);
 /* out_mask[i] = 1 when some indexed point has d2 <= r*r (compare_sqrt = 0, query_ball_point's test) or

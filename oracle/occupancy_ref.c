@@ -4,8 +4,10 @@
  * Restates my_cpp/common.cpp:324-431 (makeOccupancyGridFromCloudScan): grid geometry :352-366,:375-377, ray
  * direction :378-380, "first occupied cell not farther than the sample" :383-393.  octomap (OcTree::insertPointCloud,
  * castRay) is not in /root/reference nor installed: the traversal below is a restatement of the SEMANTIC (occupied set
- * = cells floor(p/res) containing a scan point; 3-D DDA from the origin cell; hit reported at the cell centre) with a
- * fixed arithmetic shared with the CUDA kernel.  PARITY with octomap itself is UNPINNED; the control flow is pinned:
+ * = cells floor(p/res) containing a scan point; 3-D DDA from the origin cell; hit reported at the cell centre) with
+ * the CUDA kernel's operations in the kernel's order, none contracted (-ffp-contract=off here, explicit _rn intrinsics
+ * there).  oracle/occupancy_exact.py states the same rule in exact rationals, without this arithmetic or the early
+ * exit.  PARITY with octomap itself is UNPINNED; the control flow is pinned:
  * the reference's compiled function on oracle/ref_shim/octomap/octomap.h returns the same samples (tests/test_mycpp_golden.py).
  */
 #include <limits.h>
