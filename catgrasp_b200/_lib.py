@@ -33,6 +33,15 @@ class FilterParams(C.Structure):
     ]
 
 
+class IkParams(C.Structure):
+    _fields_ = [
+        ("cam_in_world", C.c_float * 16),
+        ("ee_in_grasp", C.c_float * 16),
+        ("upper", C.c_double * 7),
+        ("lower", C.c_double * 7),
+    ]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol of include/catgrasp_b200.h
@@ -80,6 +89,9 @@ SIGNATURES = {
                                        _vp, _vp, _vp]),
     "cg_filter_grasp_pose_dev": (_i, [_vp, C.POINTER(FilterParams), _vp, _i, _vp, _i, _vp, _vp, _i, _vp, _vp, _i,
                                       _vp, _vp, _vp]),
+    "cg_iiwa14_ik_dev": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "cg_filter_apply_ik_dev": (_i, [_vp, C.POINTER(FilterParams), _vp, _i, _vp, _i, C.POINTER(IkParams), _vp, _vp,
+                                    _vp]),
     "cg_occupancy_grid_geometry": (_i, [_vp, _i, _f, C.POINTER(_i), C.POINTER(_f)]),
     "cg_occupancy_from_scan_host": (_i, [_vp, _vp, _i, _f, _vp]),
     "cg_ransac9d_host": (_i, [_vp, _vp, _vp, _i, _vp, _i, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -11,8 +11,10 @@ of (4,4) float32 arrays.  Differences, all documented in INTEGRATION.md:
   from ``gripper*.sdf``, dexnet/grasping/gripper.py:120-129);
 * survivors come back in deterministic (pose, symmetry) order, not in OpenMP
   thread-arrival order (common.cpp:303-313);
-* ``filter_ik=True`` needs a host IK predicate registered with
-  :func:`set_ik_solver` (the generated ikfast solver stays on the CPU).
+* ``filter_ik=True`` runs the closed-form KUKA iiwa14 solver of csrc/cg_ik.cu on
+  the GPU (the reference's generated ikfast solver, reproduced outside the
+  singular bands of DESIGN.md X5), unless a host IK predicate was registered
+  with :func:`set_ik_solver`.
 """
 import ctypes as C
 import hashlib
@@ -21,6 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .ik import joint_limits
 from .sdf import Sdf3D
 
 _SDF_REGISTRY = {}
@@ -56,7 +59,8 @@ def register_gripper_sdf(vertices, faces, sdf):
 
 
 def set_ik_solver(fn):
-    """fn(ee_in_base (4,4) float32, upper, lower) -> bool (True = some IK solution within limits)."""
+    """fn(ee_in_base (4,4) float32, upper, lower) -> bool (True = some IK solution within limits), called per pose on
+    the host in place of the built-in GPU solver; None selects the built-in solver again."""
     global _IK_SOLVER
     _IK_SOLVER = fn
 
@@ -77,11 +81,23 @@ def _m16(m):
 
 def filter_grasp_pose_raw(grasp_poses, symmetry_tfs, nocs_pose, canonical_to_nocs, gripper_in_grasp,
                           filter_approach_dir_face_camera, adjust_collision_pose, sdf_open, open_pts,
-                          sdf_enclosed, enclosed_pts, sdf_mode=None, device_out=False, sdf_margin=0.0, split_status=False):
+                          sdf_enclosed, enclosed_pts, sdf_mode=None, device_out=False, sdf_margin=0.0, split_status=False,
+                          ik=None):
     """Array-level entry: returns (status (Q,) u8, offset (Q,) i8, poses (Q,4,4) f32) with Q = G*S.
     ``split_status`` (only meaningful without pose adjustment): CG_ST_REJ_COLL = open gripper vs object points,
-    CG_ST_REJ_COLL_ENCL = enclosed gripper vs background (the reference's two verbose counters)."""
+    CG_ST_REJ_COLL_ENCL = enclosed gripper vs background (the reference's two verbose counters).
+    ``ik = (cam_in_world, ee_in_grasp, upper, lower)`` adds the reference's IK test (common.cpp:214-226) on the GPU:
+    a pair that passed the approach test and has no iiwa14 solution within the limits gets CG_ST_REJ_IK, offset -1 and
+    an all-zero pose."""
     ctx = sdf_open.ctx
+    if ik is not None and not (isinstance(grasp_poses, torch.Tensor) and grasp_poses.is_cuda):
+        # the IK pass works on device buffers: run the device route and bring the results back
+        gp = torch.from_numpy(np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).astype(np.float32)))
+        st, of, po = filter_grasp_pose_raw(gp.to(f"cuda:{ctx.device}"), symmetry_tfs, nocs_pose, canonical_to_nocs,
+                                           gripper_in_grasp, filter_approach_dir_face_camera, adjust_collision_pose,
+                                           sdf_open, open_pts, sdf_enclosed, enclosed_pts, sdf_mode=sdf_mode,
+                                           sdf_margin=sdf_margin, split_status=split_status, ik=ik)
+        return st.cpu().numpy(), of.cpu().numpy(), po.cpu().numpy()
     prm = _lib.FilterParams()
     prm.nocs_pose = _m16(nocs_pose)
     prm.canonical_to_nocs = _m16(canonical_to_nocs)
@@ -107,6 +123,16 @@ def filter_grasp_pose_raw(grasp_poses, symmetry_tfs, nocs_pose, canonical_to_noc
             ctx.h, C.byref(prm), _lib.ptr(gp), G, _lib.ptr(st), S, sdf_open.h, _lib.ptr(p1), p1.shape[0],
             sdf_enclosed.h if sdf_enclosed is not None else None, _lib.ptr(p2), p2.shape[0],
             _lib.ptr(status), _lib.ptr(offset), _lib.ptr(poses)))
+        if ik is not None:
+            cam_in_world, ee_in_grasp, upper, lower = ik
+            up, lo = joint_limits(upper, lower)
+            ikp = _lib.IkParams()
+            ikp.cam_in_world = _m16(cam_in_world)
+            ikp.ee_in_grasp = _m16(ee_in_grasp)
+            ikp.upper = (C.c_double * 7)(*up.tolist())
+            ikp.lower = (C.c_double * 7)(*lo.tolist())
+            ctx.check(ctx.lib.cg_filter_apply_ik_dev(ctx.h, C.byref(prm), _lib.ptr(gp), G, _lib.ptr(st), S, C.byref(ikp),
+                                                     _lib.ptr(status), _lib.ptr(offset), _lib.ptr(poses)))
         return status, offset, poses
     gp = np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).astype(np.float32)).reshape(-1, 16)
     st = np.ascontiguousarray(np.asarray(symmetry_tfs, dtype=np.float64).astype(np.float32)).reshape(-1, 16)
@@ -166,18 +192,22 @@ def filterGraspPose(grasp_poses, symmetry_tfs, nocs_pose, canonical_to_nocs_tran
             raise ValueError(f"{name} must be (N,3), got {a.shape}")
     sdf_open = _sdf_for(gripper_vertices, gripper_faces)
     sdf_encl = _sdf_for(gripper_enclosed_vertices, gripper_enclosed_faces)
-    if filter_ik and _IK_SOLVER is None:
-        raise NotImplementedError("filter_ik=True requires catgrasp_b200.my_cpp.set_ik_solver(fn); "
-                                  "the generated ikfast solver is a host stage (INTEGRATION.md)")
+    builtin_ik = bool(filter_ik) and _IK_SOLVER is None
+    if builtin_ik:
+        joint_limits(upper, lower)      # ValueError before any GPU work
     status, offset, poses = filter_grasp_pose_raw(
         grasp_poses, symmetry_tfs, nocs_pose, canonical_to_nocs_transform, gripper_in_grasp,
         filter_approach_dir_face_camera, adjust_collision_pose, sdf_open,
         np.asarray(gripper_collision_pts).reshape(-1, 3), sdf_encl,
         np.asarray(gripper_enclosed_collision_pts).reshape(-1, 3),
-        sdf_margin=voxel_margin(octo_resolution) if COLLISION_PREDICATE == "voxel" else 0.0, split_status=bool(verbose))
+        sdf_margin=voxel_margin(octo_resolution) if COLLISION_PREDICATE == "voxel" else 0.0, split_status=bool(verbose),
+        ik=(cam_in_world, ee_in_grasp, upper, lower) if builtin_ik else None)
+    if isinstance(status, torch.Tensor):
+        status, poses = status.cpu().numpy(), poses.cpu().numpy()
     keep = status == _lib.CG_ST_ACCEPT
-    ik_fail = np.zeros(status.shape[0], bool)
-    if filter_ik:
+    # the built-in pass already attributed IK rejections the reference's way (CG_ST_REJ_IK, before collision)
+    ik_fail = status == _lib.CG_ST_REJ_IK
+    if filter_ik and not builtin_ik:
         # common.cpp:214-226: IK is evaluated on the UN-shifted grasp_in_cam, after the approach test and before the
         # collision tests.  The rejections are independent, so running IK on the collision survivors only keeps the
         # same set; verbose mode evaluates it wherever the reference does, so that its counters come out the same.

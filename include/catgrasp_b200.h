@@ -221,8 +221,8 @@ int cg_sdf_download(cg_sdf *sdf, float *grid_host);
  * mesh-vs-octree test (collision_manager.cpp:93-111) substituted by the
  * gripper-SDF predicate of sdf.py:377-389 (is_any_points_inside, nearest
  * mode) or its trilinear form (sdf.py:292-343).  IK (common.cpp:214-226) is
- * NOT evaluated here (see INTEGRATION.md): pass filter results to the host
- * ikfast stage.
+ * NOT evaluated here: cg_filter_apply_ik_dev (below) applies it to these
+ * outputs.
  *   grasp_poses (G,4,4), symmetry_tfs (S,4,4), the five 4x4 matrices:
  *       float32 row-major (the reference narrows float64 -> float at the
  *       pybind boundary, common.h:51,60).
@@ -274,6 +274,43 @@ int cg_filter_grasp_pose_dev(cg_ctx *ctx, const cg_filter_params *prm,
                              cg_sdf *sdf_open, const float *open_pts, int P1,
                              cg_sdf *sdf_enclosed, const float *enclosed_pts, int P2,
                              uint8_t *out_status, int8_t *out_offset, float *out_poses);
+
+/* ---- IK feasibility (KUKA iiwa14) ----------------------------------------
+ * Replaces: my_cpp/common.cpp:9-72 (get_ik_within_limits over the generated
+ * ikfast solver, free joint 2 fixed at 0) and its use in filterGraspPose
+ * (:214-226).  A closed-form float64 solver of the same chain (DESIGN.md X5).
+ *
+ * cg_iiwa14_ik_dev: ee_in_base (Q,4,4) float32 (device), upper / lower: HOST
+ *   arrays of 7 doubles.  out_count[i] (int8) = number of solutions with
+ *   lower[k] <= q[k] <= upper[k] for all 7 joints (0 for a non-finite pose and
+ *   whenever lower > upper).  out_solutions (Q,8,7) float64 or NULL: every
+ *   solution regardless of the limits, slot 4*s + 2*e + w with
+ *     s: 0 = q0 towards the wrist centre, 1 = q0 + pi (shoulder flip)
+ *     e: 0 = q3 >= 0, 1 = q3 < 0 (elbow)
+ *     w: 0 = q5 >= 0 (or the lumped singular wrist), 1 = flipped wrist,
+ *   angles in [-pi, pi], q2 = 0, unused slots NaN.  Q = 0 is a no-op.
+ *
+ * cg_filter_apply_ik_dev: the IK test of filterGraspPose as a pass over the
+ *   outputs of cg_filter_grasp_pose_dev (same prm, poses, symmetries; same
+ *   stream, after it).  For every pair whose status is not CG_ST_REJ_DIR it
+ *   composes ee_in_base = cam_in_world * grasp_in_cam * ee_in_grasp from the
+ *   UN-shifted pose in the filter's float32 order and, when no solution is
+ *   within the limits, sets status CG_ST_REJ_IK, offset -1 and an all-zero pose
+ *   (IK precedes the collision tests in the reference).                      */
+typedef struct cg_ik_params {
+  float  cam_in_world[16];
+  float  ee_in_grasp[16];
+  double upper[7];
+  double lower[7];
+} cg_ik_params;
+int cg_iiwa14_ik_dev(cg_ctx *ctx, const float *ee_in_base, int Q,
+                     const double upper[7], const double lower[7],
+                     int8_t *out_count, double *out_solutions);
+int cg_filter_apply_ik_dev(cg_ctx *ctx, const cg_filter_params *prm,
+                           const float *grasp_poses, int G,
+                           const float *symmetry_tfs, int S,
+                           const cg_ik_params *ik,
+                           uint8_t *status, int8_t *offset, float *out_poses);
 
 /* ---- occupancy / occlusion grid from a depth scan ----------------------------
  * Replaces: my_cpp/common.cpp:324-431 (makeOccupancyGridFromCloudScan; the K
