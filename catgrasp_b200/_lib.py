@@ -106,6 +106,7 @@ SIGNATURES = {
     "cg_cloud_nearest_dev": (_i, [_vp, _vp, _i, C.c_double, _vp, _vp]),
     "cg_cloud_radius_mask_dev": (_i, [_vp, _vp, _i, C.c_double, _i, _vp]),
     "cg_cloud_normals_dev": (_i, [_vp, C.c_double, _i, _vp, _vp, _vp, _vp]),
+    "cg_meanshift_dev": (_i, [_vp, _vp, _i, C.c_double, _i, _vp, _vp, _vp, _vp, _vp]),
     "cg_square_distance_dev":(_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
     "cg_index_points_dev": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "cg_fps_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

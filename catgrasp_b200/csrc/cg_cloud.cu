@@ -7,7 +7,8 @@
 // points are radix-sorted by (key, index), so a cell's members are contiguous and in ascending point index.  The unique
 // keys, ascending, with each cell's first sorted point, form the cell table; a query binary-searches it once per (x, y)
 // column of its cell range, because the cells of a column are consecutive keys and their points one contiguous run.
-// Nothing depends on atomic arrival order: the results are a function of the inputs alone.
+// Nothing depends on atomic arrival order: the results are a function of the inputs alone.  The index structure and
+// its query helpers are in cg_cloud_index.cuh, shared with cg_meanshift.cu.
 //
 // Decisions are float64 with the reference's operation order and no FMA contraction:
 //   d2 = (dx*dx + dy*dy) + dz*dz     scipy's sqeuclidean_distance_double (cKDTree.query, query_ball_point)
@@ -16,92 +17,9 @@
 #include <algorithm>
 #include <cmath>
 #include <cub/cub.cuh>
-#include "cg_common.cuh"
-
-struct cg_cloud_index {
-  cg_ctx *ctx = nullptr;
-  int P = 0, U = 0;            // points, occupied cells
-  double cell = 0.0;
-  double origin[3] = {0, 0, 0};
-  int bits = 1;                // bits per axis in a key
-  int64_t maxc[3] = {0, 0, 0}; // largest occupied cell coordinate per axis
-  double *spts = nullptr;      // (P,3) points in key order
-  int32_t *perm = nullptr;     // (P) original index of each sorted point
-  uint64_t *ukey = nullptr;    // (U) ascending unique keys
-  int32_t *start = nullptr;    // (U+1) first sorted point of each cell; start[U] = P
-};
+#include "cg_cloud_index.cuh"
 
 namespace {
-
-constexpr int MAX_AXIS_BITS = 21;
-constexpr double RANGE_SLACK = 1e-6;   // cells
-
-struct IndexView {
-  const double *spts;
-  const int32_t *perm;
-  const uint64_t *ukey;
-  const int32_t *start;
-  int U, bits;
-  double cell, ox, oy, oz;
-  int64_t mx, my, mz;
-};
-
-IndexView view_of(const cg_cloud_index *ix) {
-  return IndexView{ix->spts, ix->perm, ix->ukey, ix->start, ix->U, ix->bits, ix->cell, ix->origin[0], ix->origin[1],
-                   ix->origin[2], ix->maxc[0], ix->maxc[1], ix->maxc[2]};
-}
-
-__device__ __forceinline__ double dist2(double ax, double ay, double az, double bx, double by, double bz) {
-  const double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
-  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-
-__device__ __forceinline__ uint64_t pack(int64_t x, int64_t y, int64_t z, int b) {
-  return ((uint64_t)x << (2 * b)) | ((uint64_t)y << b) | (uint64_t)z;
-}
-
-// cells [lo, hi] on one axis that can hold a point within R of q; false when none of them is occupied
-__device__ __forceinline__ bool axis_range(double q, double o, double R, double cell, int64_t maxc, int64_t &lo, int64_t &hi) {
-  const double d = __dsub_rn(q, o);
-  const double flo = floor(__ddiv_rn(__dsub_rn(d, R), cell) - RANGE_SLACK);
-  const double fhi = floor(__ddiv_rn(__dadd_rn(d, R), cell) + RANGE_SLACK);
-  if (!(flo <= (double)maxc) || !(fhi >= 0.0)) return false;   // also false for NaN
-  lo = flo < 0.0 ? 0 : (int64_t)flo;
-  hi = fhi > (double)maxc ? maxc : (int64_t)fhi;
-  return true;
-}
-
-__device__ __forceinline__ int lower_bound(const uint64_t *a, int lo, int hi, uint64_t k) {
-  while (lo < hi) {
-    const int m = (lo + hi) >> 1;
-    if (a[m] < k) lo = m + 1; else hi = m;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ int upper_bound(const uint64_t *a, int lo, int hi, uint64_t k) {
-  while (lo < hi) {
-    const int m = (lo + hi) >> 1;
-    if (a[m] <= k) lo = m + 1; else hi = m;
-  }
-  return lo;
-}
-
-// The cell range of a query: per (x, y) column, the contiguous run [s, e) of sorted points in cells z_lo..z_hi.
-struct Columns {
-  int64_t x0, x1, y0, y1, z0, z1;
-  bool any;
-  __device__ Columns(const IndexView &V, double qx, double qy, double qz, double R) {
-    any = axis_range(qx, V.ox, R, V.cell, V.mx, x0, x1) && axis_range(qy, V.oy, R, V.cell, V.my, y0, y1) &&
-          axis_range(qz, V.oz, R, V.cell, V.mz, z0, z1);
-  }
-  __device__ __forceinline__ void run(const IndexView &V, int64_t cx, int64_t cy, int &s, int &e) const {
-    const int a = lower_bound(V.ukey, 0, V.U, pack(cx, cy, z0, V.bits));
-    const int b = upper_bound(V.ukey, a, V.U, pack(cx, cy, z1, V.bits));
-    s = V.start[a];
-    e = V.start[b];
-  }
-};
 
 // ---- index construction ------------------------------------------------------------------------------------------
 
@@ -539,6 +457,7 @@ extern "C" int cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, doub
   int64_t maxc = 0;
   for (int a = 0; a < 3; a++) {
     ix->origin[a] = hb[a] - cell * 0.5;                               // open3d: min_bound - voxel_size * 0.5
+    ix->hi[a] = hb[3 + a];
     const double top = floor((hb[3 + a] - ix->origin[a]) / cell);     // the largest point's cell (floor is monotone)
     if (!(top < (double)(1 << MAX_AXIS_BITS))) {
       delete ix;

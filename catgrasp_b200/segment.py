@@ -1,0 +1,154 @@
+"""Clustering of the segmentation's shifted points on the device (csrc/cg_meanshift.cu): sklearn's MeanShift as
+PointGroupPredictor.predict uses it (predicter.py:332), and the label propagation around it (:308-338).
+
+Follows the cloud.py convention: numpy in, numpy out; CUDA tensor in, CUDA tensor out.  Centres keep X's dtype
+(float32 or float64); labels are int64.  Labels are the nearest kept centre in float64 d2, ties to the smaller centre
+index.  Centres are summed in int64 fixed point, so they do not depend on the order of X's rows; sklearn's own
+centres move by a few float32 ulps when the rows are permuted, its labels do not.
+"""
+import ctypes as C
+import numbers
+
+import numpy as np
+import torch
+
+from . import _lib
+from .cloud import CloudIndex, _ctx, _dev, _device_of, _out, _query_cell
+
+MEANSHIFT_BANDWIDTH = {"hnm": 0.005, "nut": 0.007, "screw": 0.009}   # predicter.py:317-330
+DOWNSAMPLE = 0.002                                                     # predicter.py:309
+LABEL_REACH = 4.0      # first nearest-centre query bound, in bandwidths; points beyond it are queried again unbounded
+
+
+def _as_points(X):
+    """X as an (N,3) float32 / float64 numpy array or tensor (other dtypes widened to float64, as sklearn does);
+    ValueError for a wrong shape, no rows or a non-finite value."""
+    if isinstance(X, torch.Tensor):
+        if X.dtype not in (torch.float32, torch.float64):
+            X = X.to(torch.float64)
+        finite = lambda a: bool(torch.isfinite(a).all())      # noqa: E731
+    else:
+        X = np.asarray(X)
+        if X.dtype not in (np.float32, np.float64):
+            X = X.astype(np.float64)
+        finite = lambda a: bool(np.isfinite(a).all())         # noqa: E731
+    if X.ndim != 2 or X.shape[1] != 3:
+        raise ValueError(f"Expected a 2D array of shape (n_samples, 3), got shape {tuple(X.shape)}")
+    if X.shape[0] == 0:
+        raise ValueError("Found array with 0 sample(s) (shape=(0, 3)) while a minimum of 1 is required")
+    if not finite(X):
+        raise ValueError("Input X contains NaN or infinity")
+    return X
+
+
+def _nearest(ref, query, reach):
+    """Index of the nearest ref point for every query (ref, query: float64 device tensors): first within `reach`,
+    then, for the queries with nothing that close, within the diagonal of the joint bounding box, so none goes
+    unanswered.  Either way the answer is the global nearest point with ties to the smaller index."""
+    _, idx = CloudIndex(ref, _query_cell(ref, reach), ref.device.index).nearest(query, reach)
+    miss = torch.nonzero(idx < 0).reshape(-1)
+    if miss.numel():
+        q = query[miss]
+        span = torch.maximum(ref.amax(0), q.amax(0)) - torch.minimum(ref.amin(0), q.amin(0))
+        bound = float(torch.linalg.norm(span)) * (1 + 1e-9)
+        _, far = CloudIndex(ref, _query_cell(ref, bound), ref.device.index).nearest(q, bound)
+        if bool((far < 0).any()):
+            raise _lib.CgError("nearest: a query found no point within the joint bounding box's diagonal")
+        idx[miss] = far
+    return idx.to(torch.int64)
+
+
+class MeanShift:
+    """sklearn.cluster.MeanShift for the arguments the reference passes: every point seeds an ascent (seeds=None,
+    bin_seeding=False) and every point is labelled (cluster_all=True).  n_jobs is accepted and ignored.
+
+    fit(X) sets cluster_centers_ (K,3) in X's dtype, labels_ (N,) int64 and n_iter_, and also the per-seed results
+    seed_centers_ (N,3), seed_counts_ (N,) (points within bandwidth of the final centre, 0 when none) and
+    seed_iters_ (N,).  X holds at most 2^21 points."""
+
+    def __init__(self, bandwidth=None, cluster_all=True, n_jobs=None, seeds=None, bin_seeding=False, max_iter=300):
+        self.bandwidth = bandwidth
+        self.cluster_all = cluster_all
+        self.n_jobs = n_jobs
+        self.seeds = seeds
+        self.bin_seeding = bin_seeding
+        self.max_iter = max_iter
+
+    def _check_params(self):
+        if self.bandwidth is None:
+            raise NotImplementedError("MeanShift: bandwidth=None (estimate_bandwidth) is not supported")
+        if self.seeds is not None:
+            raise NotImplementedError("MeanShift: explicit seeds are not supported")
+        if self.bin_seeding:
+            raise NotImplementedError("MeanShift: bin_seeding=True is not supported")
+        if not self.cluster_all:
+            raise NotImplementedError("MeanShift: cluster_all=False is not supported")
+        bw = self.bandwidth
+        if isinstance(bw, bool) or not isinstance(bw, numbers.Real) or not (np.isfinite(bw) and bw > 0):
+            raise ValueError(f"MeanShift: bandwidth must be a positive finite number, got {bw!r}")
+        it = self.max_iter
+        if isinstance(it, bool) or not isinstance(it, numbers.Integral) or not 0 <= it < 2 ** 31:
+            raise ValueError(f"MeanShift: max_iter must be an integer >= 0, got {it!r}")
+
+    def fit(self, X, y=None):
+        self._check_params()
+        X = _as_points(X)
+        like = isinstance(X, torch.Tensor)
+        device = _device_of(X)
+        ctx = _ctx(device)
+        f64 = X.dtype in (torch.float64, np.float64)
+        x = _dev(X, torch.float64 if f64 else torch.float32, device)
+        bw = float(self.bandwidth)
+        index = CloudIndex(x, bw, device)
+        P = x.shape[0]
+        seed_c = torch.empty_like(x)
+        seed_n = torch.empty((P,), dtype=torch.int32, device=x.device)
+        seed_it = torch.empty_like(seed_n)
+        cen = torch.empty_like(x)
+        nc = torch.empty((1,), dtype=torch.int32, device=x.device)
+        ctx.use_torch_stream()
+        ctx.check(ctx.lib.cg_meanshift_dev(index.h, _lib.ptr(x), int(f64), C.c_double(bw), int(self.max_iter),
+                                           _lib.ptr(seed_c), _lib.ptr(seed_n), _lib.ptr(seed_it), _lib.ptr(cen),
+                                           _lib.ptr(nc)))
+        centres = cen[:int(nc.item())].contiguous()
+        labels = _nearest(centres.to(torch.float64), x.to(torch.float64), LABEL_REACH * bw)
+        self.n_iter_ = int(seed_it.max().item())
+        self.cluster_centers_ = _out(centres, like)
+        self.labels_ = _out(labels, like)
+        self.seed_centers_ = _out(seed_c, like)
+        self.seed_counts_ = _out(seed_n.to(torch.int64), like)
+        self.seed_iters_ = _out(seed_it.to(torch.int64), like)
+        return self
+
+    def fit_predict(self, X, y=None):
+        return self.fit(X).labels_
+
+
+def pointgroup_labels(xyz_original_all, pt_offsets, cloud_xyz, bandwidth):
+    """predicter.py:308-338 after the network: the 2 mm voxel down-sampling of the network's points, each voxel mean
+    snapped to its nearest point, those points moved by their offsets (float32), clustered by MeanShift, and every
+    point of cloud_xyz labelled with its nearest snapped point's cluster.  Returns (labels_all (M,) int64,
+    xyz_shifted (U,3) float32)."""
+    like = isinstance(xyz_original_all, torch.Tensor)
+    xo = _as_points(xyz_original_all)
+    off = _as_points(pt_offsets)
+    cloud = _as_points(cloud_xyz)
+    if off.shape[0] != xo.shape[0]:
+        raise ValueError("pt_offsets must have one row per point of xyz_original_all")
+    device = _device_of(xo, off, cloud)
+    _ctx(device)
+    xo = _dev(xo, torch.float32, device)
+    off = _dev(off, torch.float32, device)
+    down, _ = CloudIndex(xo, DOWNSAMPLE, device).voxel_means()                          # :308-310
+    # :311-313 snap: a voxel mean and its members share a voxel, so the nearest member is within the diagonal; the
+    # bound is widened by 1e-9 relative so rounding at a voxel face cannot exclude it
+    snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)
+    _, ids = CloudIndex(xo, snap, device).nearest(down, snap)
+    if bool((ids < 0).any()):
+        raise _lib.CgError("pointgroup_labels: a voxel mean has no point within its voxel's diagonal")
+    ids = ids.to(torch.int64)
+    xyz_down = xo[ids]
+    xyz_shifted = xyz_down + off[ids]                                                    # :314, float32
+    labels = MeanShift(bandwidth=bandwidth).fit_predict(xyz_shifted)                      # :332
+    nearest = _nearest(xyz_down.to(torch.float64), _dev(cloud, torch.float64, device), LABEL_REACH * DOWNSAMPLE)
+    return _out(labels[nearest], like), _out(xyz_shifted, like)                           # :334-336

@@ -411,6 +411,21 @@ int  cg_cloud_radius_mask_dev(const cg_cloud_index *index, const double *query, 
 int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point,
                           double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count);
 
+/* ---- mean-shift clustering ---- */
+/* sklearn MeanShift(bandwidth, seeds=None, bin_seeding=False, cluster_all=True) up to its labels (predicter.py:332).
+ * index: a cg_cloud_index over X built with cell = bandwidth (its origin anchors the fixed point; an ascent step scans
+ * at most 4 x 4 x 4 cells), else CG_EINVAL; X (P,3): the same points, float32 (x_is_f64 = 0) or float64, in the dtype every centre is returned in.  P <= 2^21, else
+ * CG_EINVAL.  One flat-kernel ascent per point: the set d2 = (dx*dx + dy*dy) + dz*dz <= bandwidth^2 (float64, no
+ * FMA), its mean summed in int64 fixed point (order-free; see cg_meanshift.cu), stopping on an empty set, on a step
+ * of at most 1e-3 * bandwidth or after max_iter (>= 0) steps.  Outputs, all device memory:
+ *   out_seed_centres (P,3), out_seed_counts (P) = final set size (0: empty), out_seed_iters (P) = completed steps;
+ *   out_centres (P,3 capacity) = the kept modes, in (count, x, y, z) descending order after sklearn's greedy
+ *   suppression of modes within bandwidth; out_n_centres (1) = how many.
+ * Labels are the nearest kept centre (cg_cloud_nearest_dev over an index of out_centres).  Never synchronises.     */
+int  cg_meanshift_dev(const cg_cloud_index *index, const void *X, int x_is_f64, double bandwidth, int max_iter,
+                      void *out_seed_centres, int32_t *out_seed_counts, int32_t *out_seed_iters, void *out_centres,
+                      int32_t *out_n_centres);
+
 /* ---- PointNet++ primitives (device pointers) ---------------------------
  * Replace the free functions of pointnet2.py:14-149.  Indices are int32 on
  * the device (the Python mirror widens to int64 like the reference).        */
