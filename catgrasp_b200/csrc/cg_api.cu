@@ -56,7 +56,6 @@ extern "C" void cg_ctx_destroy(cg_ctx *ctx) {
   if (ctx->ovf_flag) cudaFree(ctx->ovf_flag);
   if (ctx->ws) cudaFree(ctx->ws);
   if (ctx->io) cudaFree(ctx->io);
-  if (ctx->hs) cudaFreeHost(ctx->hs);
   cudaStreamDestroy(ctx->own_stream);
   delete ctx;
 }
@@ -108,22 +107,22 @@ extern "C" int cg_ctx_set_engine(cg_ctx *ctx, int engine) {
 }
 extern "C" int cg_ctx_get_engine(cg_ctx *ctx) { return ctx ? ctx->engine : CG_EINVAL; }
 
-static int grow(cg_ctx *ctx, void **p, size_t *cur, size_t bytes, bool host) {
+static int grow(cg_ctx *ctx, void **p, size_t *cur, size_t bytes) {
   if (bytes <= *cur) return CG_OK;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   // the arena may still be in use by enqueued work
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (*p) {
-    if (host) cudaFreeHost(*p); else cudaFree(*p);
+    cudaFree(*p);
     *p = nullptr;
     *cur = 0;
   }
   size_t want = bytes + bytes / 4;
-  cudaError_t e = host ? cudaMallocHost(p, want) : cudaMalloc(p, want);
+  cudaError_t e = cudaMalloc(p, want);
   if (e != cudaSuccess) {
     cudaGetLastError();
     want = bytes;
-    e = host ? cudaMallocHost(p, want) : cudaMalloc(p, want);
+    e = cudaMalloc(p, want);
   }
   if (e != cudaSuccess) {
     ctx->err = std::string("workspace allocation failed: ") + cudaGetErrorString(e);
@@ -134,9 +133,8 @@ static int grow(cg_ctx *ctx, void **p, size_t *cur, size_t bytes, bool host) {
   return CG_OK;
 }
 
-int cg_ws_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->ws, &ctx->ws_bytes, bytes, false); }
-int cg_io_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->io, &ctx->io_bytes, bytes, false); }
-int cg_hs_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->hs, &ctx->hs_bytes, bytes, true); }
+int cg_ws_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->ws, &ctx->ws_bytes, bytes); }
+int cg_io_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->io, &ctx->io_bytes, bytes); }
 
 // CG_TRACE diagnostics: durations between consecutive post-launch events on the context's stream, grouped by call site
 void cg_trace_mark(cg_ctx *ctx, const char *where) {

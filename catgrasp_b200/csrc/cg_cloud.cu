@@ -429,17 +429,16 @@ extern "C" int cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, doub
                                                (int32_t *)nullptr, P, 0, 3 * MAX_AXIS_BITS, ctx->stream));
   CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int32_t *)nullptr, (int32_t *)nullptr, P, ctx->stream));
   const size_t tmp = std::max(sort_tmp, scan_tmp);
-  const size_t need = cg_arena::pad(sizeof(double) * (7 * (size_t)nb + 7)) + 2 * cg_arena::pad(sizeof(uint64_t) * (size_t)P) +
-                      3 * cg_arena::pad(sizeof(int32_t) * (size_t)P) + cg_arena::pad(sizeof(int)) + cg_arena::pad(tmp) + 256;
-  int rc = cg_ws_reserve(ctx, need);
+  double *part; uint64_t *kin, *kout; int32_t *vin, *flag, *cid, *dU; void *dtmp;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    part = ar.take<double>(7 * (size_t)nb + 7);
+    kin = ar.take<uint64_t>(P); kout = ar.take<uint64_t>(P);
+    vin = ar.take<int32_t>(P); flag = ar.take<int32_t>(P); cid = ar.take<int32_t>(P);
+    dU = ar.take<int32_t>(1);
+    dtmp = ar.take<char>(tmp);
+  });
   if (rc != CG_OK) return rc;
-  cg_arena ar(ctx->ws);
-  double *part = ar.take<double>(7 * (size_t)nb + 7);
   double *bnd = part + 7 * (size_t)nb;
-  uint64_t *kin = ar.take<uint64_t>(P), *kout = ar.take<uint64_t>(P);
-  int32_t *vin = ar.take<int32_t>(P), *flag = ar.take<int32_t>(P), *cid = ar.take<int32_t>(P);
-  int *dU = ar.take<int>(1);
-  void *dtmp = ar.take<char>(tmp);
 
   bounds_kernel<<<nb, BT, 0, ctx->stream>>>(pts, P, part);
   CG_LAUNCH_CHECK(ctx);
@@ -450,56 +449,45 @@ extern "C" int cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, doub
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   CG_REQUIRE(ctx, hb[6] == 0.0, "cloud_index: a coordinate is NaN or infinite");
 
-  cg_cloud_index *ix = new cg_cloud_index;
-  ix->ctx = ctx;
-  ix->P = P;
-  ix->cell = cell;
+  cg_cloud_index ix;   // goes to the heap only when every step below has succeeded
+  ix.ctx = ctx;
+  ix.P = P;
+  ix.cell = cell;
   int64_t maxc = 0;
   for (int a = 0; a < 3; a++) {
-    ix->origin[a] = hb[a] - cell * 0.5;                               // open3d: min_bound - voxel_size * 0.5
-    ix->hi[a] = hb[3 + a];
-    const double top = floor((hb[3 + a] - ix->origin[a]) / cell);     // the largest point's cell (floor is monotone)
-    if (!(top < (double)(1 << MAX_AXIS_BITS))) {
-      delete ix;
-      CG_REQUIRE(ctx, false, "cloud_index: the cloud spans 2^21 or more cells on an axis; use a larger cell");
-    }
-    ix->maxc[a] = (int64_t)top;
-    maxc = std::max(maxc, ix->maxc[a]);
+    ix.origin[a] = hb[a] - cell * 0.5;                               // open3d: min_bound - voxel_size * 0.5
+    ix.hi[a] = hb[3 + a];
+    const double top = floor((hb[3 + a] - ix.origin[a]) / cell);     // the largest point's cell (floor is monotone)
+    CG_REQUIRE(ctx, top < (double)(1 << MAX_AXIS_BITS),
+               "cloud_index: the cloud spans 2^21 or more cells on an axis; use a larger cell");
+    ix.maxc[a] = (int64_t)top;
+    maxc = std::max(maxc, ix.maxc[a]);
   }
   int bits = 1;
   while ((int64_t(1) << bits) <= maxc) bits++;
-  ix->bits = bits;
-  auto fail = [&](cudaError_t e, const char *what) {
-    ctx->err = std::string(what) + ": " + cudaGetErrorString(e);
-    cudaFree(ix->spts); cudaFree(ix->perm); cudaFree(ix->ukey); cudaFree(ix->start);
-    delete ix;
-    return CG_ECUDA;
-  };
-  cudaError_t e;
-  if ((e = cudaMalloc(&ix->spts, sizeof(double) * 3 * (size_t)P)) != cudaSuccess) return fail(e, "cudaMalloc");
-  if ((e = cudaMalloc(&ix->perm, sizeof(int32_t) * (size_t)P)) != cudaSuccess) return fail(e, "cudaMalloc");
-  if ((e = cudaMalloc(&ix->ukey, sizeof(uint64_t) * (size_t)P)) != cudaSuccess) return fail(e, "cudaMalloc");
-  if ((e = cudaMalloc(&ix->start, sizeof(int32_t) * ((size_t)P + 1))) != cudaSuccess) return fail(e, "cudaMalloc");
+  ix.bits = bits;
+  DevBuf spts, perm, ukey, start;
+  if ((rc = dev_alloc(ctx, spts, sizeof(double) * 3 * (size_t)P))) return rc;
+  if ((rc = dev_alloc(ctx, perm, sizeof(int32_t) * (size_t)P))) return rc;
+  if ((rc = dev_alloc(ctx, ukey, sizeof(uint64_t) * (size_t)P))) return rc;
+  if ((rc = dev_alloc(ctx, start, sizeof(int32_t) * ((size_t)P + 1)))) return rc;
+  ix.spts = static_cast<double *>(spts.p); ix.perm = static_cast<int32_t *>(perm.p);
+  ix.ukey = static_cast<uint64_t *>(ukey.p); ix.start = static_cast<int32_t *>(start.p);
 
-  key_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(pts, P, ix->origin[0], ix->origin[1], ix->origin[2], cell, bits, kin, vin);
-  if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, "key_kernel");
-  ctx->launches++;
+  key_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(pts, P, ix.origin[0], ix.origin[1], ix.origin[2], cell, bits, kin, vin);
+  CG_LAUNCH_CHECK(ctx);
   size_t tb = tmp;
-  if ((e = cub::DeviceRadixSort::SortPairs(dtmp, tb, kin, kout, vin, ix->perm, P, 0, 3 * bits, ctx->stream)) != cudaSuccess)
-    return fail(e, "DeviceRadixSort::SortPairs");
+  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(dtmp, tb, kin, kout, vin, ix.perm, P, 0, 3 * bits, ctx->stream));
   head_flag_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, P, flag);
-  if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, "head_flag_kernel");
+  CG_LAUNCH_CHECK(ctx);
   tb = tmp;
-  if ((e = cub::DeviceScan::ExclusiveSum(dtmp, tb, flag, cid, P, ctx->stream)) != cudaSuccess)
-    return fail(e, "DeviceScan::ExclusiveSum");
-  table_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, ix->perm, cid, pts, P, ix->ukey, ix->start, ix->spts, dU);
-  if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, "table_kernel");
-  ctx->launches += 2;
-  int hU = 0;
-  if ((e = cudaMemcpyAsync(&hU, dU, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream)) != cudaSuccess) return fail(e, "cudaMemcpyAsync");
-  if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) return fail(e, "cudaStreamSynchronize");
-  ix->U = hU;
-  *out = ix;
+  CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(dtmp, tb, flag, cid, P, ctx->stream));
+  table_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, ix.perm, cid, pts, P, ix.ukey, ix.start, ix.spts, dU);
+  CG_LAUNCH_CHECK(ctx);
+  CG_CUDA(ctx, cudaMemcpyAsync(&ix.U, dU, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  spts.release(); perm.release(); ukey.release(); start.release();   // owned by the index now
+  *out = new cg_cloud_index(ix);
   return CG_OK;
 }
 

@@ -367,14 +367,17 @@ extern "C" int cg_sdf_create(cg_ctx *ctx, const float *grid_host, int nx, int ny
   if (!ctx || !out) return CG_EINVAL;
   CG_REQUIRE(ctx, grid_host && nx > 0 && ny > 0 && nz > 0 && resolution > 0.f, "sdf: bad grid");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t bytes = (size_t)nx * ny * nz * sizeof(float);
+  DevBuf grid;
+  int rc = dev_alloc(ctx, grid, bytes);
+  if (rc) return rc;
+  CG_CUDA(ctx, cudaMemcpyAsync(grid.p, grid_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   cg_sdf *s = new cg_sdf();
   s->ctx = ctx; s->nx = nx; s->ny = ny; s->nz = nz; s->res = resolution;
   for (int k = 0; k < 3; k++) s->origin[k] = origin[k];
-  const size_t bytes = (size_t)nx * ny * nz * sizeof(float);
   cg_sdf_border_stats(s, grid_host);
-  CG_CUDA(ctx, cudaMalloc(&s->grid, bytes));
-  CG_CUDA(ctx, cudaMemcpyAsync(s->grid, grid_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  s->grid = static_cast<float *>(grid.release());
   *out = s;
   return CG_OK;
 }
@@ -427,18 +430,17 @@ extern "C" int cg_filter_grasp_pose_host(cg_ctx *ctx, const cg_filter_params *pr
   CG_REQUIRE(ctx, out_status && out_offset && out_poses, "filter_host: outputs");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t Q = (size_t)G * S;
-  const size_t need = cg_arena::pad((size_t)G * 64) + cg_arena::pad((size_t)S * 64) + cg_arena::pad((size_t)P1 * 12) +
-                      cg_arena::pad((size_t)P2 * 12) + cg_arena::pad(Q) * 2 + cg_arena::pad(Q * 64) + 4096;
-  int rc = cg_io_reserve(ctx, need);
+  float *d_g, *d_s, *d_p1, *d_p2, *d_po; uint8_t *d_st; int8_t *d_of;
+  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
+    d_g = ar.take<float>((size_t)G * 16);
+    d_s = ar.take<float>((size_t)S * 16);
+    d_p1 = ar.take<float>((size_t)P1 * 3 + 1);
+    d_p2 = ar.take<float>((size_t)P2 * 3 + 1);
+    d_st = ar.take<uint8_t>(Q);
+    d_of = ar.take<int8_t>(Q);
+    d_po = ar.take<float>(Q * 16);
+  });
   if (rc) return rc;
-  cg_arena ar(ctx->io);
-  float *d_g = ar.take<float>((size_t)G * 16);
-  float *d_s = ar.take<float>((size_t)S * 16);
-  float *d_p1 = ar.take<float>((size_t)P1 * 3 + 1);
-  float *d_p2 = ar.take<float>((size_t)P2 * 3 + 1);
-  uint8_t *d_st = ar.take<uint8_t>(Q);
-  int8_t *d_of = ar.take<int8_t>(Q);
-  float *d_po = ar.take<float>(Q * 16);
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemcpyAsync(d_g, grasp_poses, (size_t)G * 64, cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemcpyAsync(d_s, symmetry_tfs, (size_t)S * 64, cudaMemcpyHostToDevice, st));

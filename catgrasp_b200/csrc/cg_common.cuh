@@ -35,9 +35,6 @@ struct cg_ctx {
   // grow-only device workspace, carved per call
   void *ws = nullptr;
   size_t ws_bytes = 0;
-  // grow-only pinned host staging for the *_host entry points
-  void *hs = nullptr;
-  size_t hs_bytes = 0;
   // second device arena for *_host entry points' device copies of I/O
   void *io = nullptr;
   size_t io_bytes = 0;
@@ -89,11 +86,11 @@ struct cg_sdf {
 // border_nonneg / border_min of a host copy of the grid (decides the filter's out-of-box shortcut)
 void cg_sdf_border_stats(cg_sdf *s, const float *grid_host);
 
-int cg_ws_reserve(cg_ctx *ctx, size_t bytes);
+int cg_ws_reserve(cg_ctx *ctx, size_t bytes);   // grow-only (cg_api.cu); call sites use cg_ws_carve / cg_io_carve
 int cg_io_reserve(cg_ctx *ctx, size_t bytes);
-int cg_hs_reserve(cg_ctx *ctx, size_t bytes);
 
-// bump allocator over a reserved arena (256-byte aligned pieces)
+// Bump allocator over an arena: each piece starts at the next multiple of 256 bytes from the base.  An arena over
+// nullptr only measures: take() returns nullptr, and `off` ends at the bytes the same takes need in a real arena.
 struct cg_arena {
   char *base;
   size_t off = 0;
@@ -101,12 +98,52 @@ struct cg_arena {
   template <typename T>
   T *take(size_t n) {
     off = (off + 255) & ~size_t(255);
-    T *p = reinterpret_cast<T *>(base + off);
+    T *p = base ? reinterpret_cast<T *>(base + off) : nullptr;
     off += n * sizeof(T);
     return p;
   }
-  static size_t pad(size_t bytes) { return (bytes + 255) & ~size_t(255); }
 };
+
+// cg_ws_carve / cg_io_carve(ctx, layout): layout(cg_arena &) makes one call's take()s and stores the pointers.  It runs
+// over a measuring arena, the context's ws (*_dev internals) or io (*_host staging) arena grows to the bytes measured,
+// and it runs again over that arena.  Growing frees the arena: code that holds pieces of a carve must not call anything
+// that carves the same arena (a *_host call holds its io pieces across the *_dev call it wraps, which carves ws only).
+template <typename Layout>
+int cg_carve(cg_ctx *ctx, bool io, Layout &layout) {
+  cg_arena measure(nullptr);
+  layout(measure);
+  const int rc = io ? cg_io_reserve(ctx, measure.off) : cg_ws_reserve(ctx, measure.off);
+  if (rc) return rc;
+  cg_arena ar(io ? ctx->io : ctx->ws);
+  layout(ar);
+  if (ar.off == measure.off) return CG_OK;
+  ctx->err = "internal error: a workspace layout carved a different size than it measured";
+  return CG_EINVAL;
+}
+template <typename Layout> int cg_ws_carve(cg_ctx *ctx, Layout &&layout) { return cg_carve(ctx, false, layout); }
+template <typename Layout> int cg_io_carve(cg_ctx *ctx, Layout &&layout) { return cg_carve(ctx, true, layout); }
+
+// one owning device allocation: freed when it goes out of scope unless release() hands it on
+struct DevBuf {
+  void *p = nullptr;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  void *release() { return std::exchange(p, nullptr); }
+};
+
+// cudaMalloc into b: CG_ENOMEM when the device is out of memory, CG_ECUDA on any other error
+inline int dev_alloc(cg_ctx *ctx, DevBuf &b, size_t bytes) {
+  const cudaError_t e = cudaMalloc(&b.p, bytes);
+  if (e == cudaErrorMemoryAllocation) {
+    cudaGetLastError();
+    ctx->err = "out of device memory";
+    return CG_ENOMEM;
+  }
+  CG_CUDA(ctx, e);
+  return CG_OK;
+}
 
 // ---- order-preserving float <-> uint key (for atomicMax on floats) --------
 __host__ __device__ __forceinline__ uint32_t cg_f2key(float f) {

@@ -268,19 +268,19 @@ int meanshift(const cg_cloud_index *ix, const T *X, double bw, int max_iter, T *
   CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int32_t *)nullptr, (int32_t *)nullptr, P, ctx->stream));
   const size_t tmp = std::max(sort_tmp, scan_tmp);
   const size_t Pz = (size_t)P;
-  const size_t need = 2 * cg_arena::pad(sizeof(long long) * 3 * Pz) + 2 * cg_arena::pad(sizeof(uint64_t) * Pz) +
-                      9 * cg_arena::pad(sizeof(int32_t) * Pz) + cg_arena::pad(sizeof(int32_t)) + cg_arena::pad(tmp) + 256;
-  int rc_ = cg_ws_reserve(ctx, need);
+  long long *q; double *rc; uint64_t *kA, *kB; void *dtmp;
+  int32_t *vA, *vB, *head, *gid, *gseed, *gcount, *rseed, *supp, *kept, *nmodes;
+  const int rc_ = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    q = ar.take<long long>(3 * Pz);
+    rc = ar.take<double>(3 * Pz);
+    kA = ar.take<uint64_t>(Pz); kB = ar.take<uint64_t>(Pz);
+    vA = ar.take<int32_t>(Pz); vB = ar.take<int32_t>(Pz); head = ar.take<int32_t>(Pz);
+    gid = ar.take<int32_t>(Pz); gseed = ar.take<int32_t>(Pz); gcount = ar.take<int32_t>(Pz);
+    rseed = ar.take<int32_t>(Pz); supp = ar.take<int32_t>(Pz); kept = ar.take<int32_t>(Pz);
+    nmodes = ar.take<int32_t>(1);
+    dtmp = ar.take<char>(tmp);
+  });
   if (rc_ != CG_OK) return rc_;
-  cg_arena ar(ctx->ws);
-  long long *q = ar.take<long long>(3 * Pz);
-  double *rc = ar.take<double>(3 * Pz);
-  uint64_t *kA = ar.take<uint64_t>(Pz), *kB = ar.take<uint64_t>(Pz);
-  int32_t *vA = ar.take<int32_t>(Pz), *vB = ar.take<int32_t>(Pz), *head = ar.take<int32_t>(Pz);
-  int32_t *gid = ar.take<int32_t>(Pz), *gseed = ar.take<int32_t>(Pz), *gcount = ar.take<int32_t>(Pz);
-  int32_t *rseed = ar.take<int32_t>(Pz), *supp = ar.take<int32_t>(Pz), *kept = ar.take<int32_t>(Pz);
-  int32_t *nmodes = ar.take<int32_t>(1);
-  void *dtmp = ar.take<char>(tmp);
   cudaStream_t st = ctx->stream;
   const unsigned g256 = blocks(P, 256);
 

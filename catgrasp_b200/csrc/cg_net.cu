@@ -129,12 +129,6 @@ struct EncoderWs {
   float *T64;       // (B,4096)
 };
 
-size_t encoder_ws_bytes(int B) {
-  return cg_arena::pad((size_t)B * 1024 * 4) + cg_arena::pad((size_t)B * 512 * 4) +
-         cg_arena::pad((size_t)B * 256 * 4) + cg_arena::pad((size_t)B * 9 * 4) +
-         cg_arena::pad((size_t)B * 4096 * 4) + 4096;
-}
-
 void encoder_ws_carve(cg_arena &ar, int B, EncoderWs &w) {
   w.gmax = ar.take<uint32_t>((size_t)B * 1024);
   w.f1 = ar.take<float>((size_t)B * 512);
@@ -195,15 +189,15 @@ int cls_forward_impl(cg_net *net, const cg_input_src &in_all, int B_all, int N, 
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const int n_out = net->n_out;
   const int Bc_max = B_all < CHUNK_B ? B_all : CHUNK_B;
-  const size_t need = encoder_ws_bytes(Bc_max) + cg_arena::pad((size_t)Bc_max * n_out * 4) + 1024;
-  int rc = cg_ws_reserve(ctx, need);
+  EncoderWs w;
+  float *logits_ws;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    encoder_ws_carve(ar, Bc_max, w);
+    logits_ws = ar.take<float>((size_t)Bc_max * n_out);
+  });
   if (rc) return rc;
   for (int b0 = 0; b0 < B_all; b0 += CHUNK_B) {
     const int B = (B_all - b0 < CHUNK_B) ? (B_all - b0) : CHUNK_B;
-    cg_arena ar(ctx->ws);
-    EncoderWs w;
-    encoder_ws_carve(ar, B, w);
-    float *logits_ws = ar.take<float>((size_t)B * n_out);
     cg_input_src in = in_all;
     if (in.x_direct) in.x_direct += (size_t)b0 * N * 6;
     if (in.poses) in.poses += (size_t)b0 * 16;
@@ -229,20 +223,18 @@ int seg_forward_impl(cg_net *net, const float *x, int B, int N, float *out_logit
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t P = (size_t)B * N;
   const int n_out = net->n_out;
-  const size_t need = encoder_ws_bytes(B) + cg_arena::pad(P * 64 * 4) + cg_arena::pad((size_t)B * 512 * 4) +
-                      cg_arena::pad(P * 512 * 4) + cg_arena::pad(P * 256 * 4) + cg_arena::pad(P * 128 * 4) +
-                      cg_arena::pad(P * n_out * 4) + 4096;
-  int rc = cg_ws_reserve(ctx, need);
-  if (rc) return rc;
-  cg_arena ar(ctx->ws);
   EncoderWs w;
-  encoder_ws_carve(ar, B, w);
-  float *pf = ar.take<float>(P * 64);
-  float *biasg = ar.take<float>((size_t)B * 512);
-  float *y1 = ar.take<float>(P * 512);
-  float *y2 = ar.take<float>(P * 256);
-  float *y3 = ar.take<float>(P * 128);
-  float *lg = out_logits ? out_logits : ar.take<float>(P * n_out);
+  float *pf, *biasg, *y1, *y2, *y3, *lg;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    encoder_ws_carve(ar, B, w);
+    pf = ar.take<float>(P * 64);
+    biasg = ar.take<float>((size_t)B * 512);
+    y1 = ar.take<float>(P * 512);
+    y2 = ar.take<float>(P * 256);
+    y3 = ar.take<float>(P * 128);
+    lg = out_logits ? out_logits : ar.take<float>(P * n_out);
+  });
+  if (rc) return rc;
   cg_input_src in;
   memset(&in, 0, sizeof(in));
   in.x_direct = x;
@@ -287,20 +279,18 @@ extern "C" int cg_graspq_forward_host(cg_net *net, const double *cloud_xyz, cons
   CG_REQUIRE(ctx, M > 0 && B > 0 && N > 0, "graspq_host: bad shape");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const int n_out = net->n_out;
-  const size_t need = cg_arena::pad((size_t)M * 3 * 8) * 2 + cg_arena::pad((size_t)B * 16 * 8) +
-                      cg_arena::pad((size_t)B * N * 4) + cg_arena::pad(6 * 8) * 2 +
-                      cg_arena::pad((size_t)B * n_out * 4) + cg_arena::pad((size_t)B * 4) + 4096;
-  int rc = cg_io_reserve(ctx, need);
+  double *d_xyz, *d_nrm, *d_pose, *d_mean, *d_std; int32_t *d_ids, *d_label; float *d_probs;
+  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
+    d_xyz = ar.take<double>((size_t)M * 3);
+    d_nrm = ar.take<double>((size_t)M * 3);
+    d_pose = ar.take<double>((size_t)B * 16);
+    d_ids = ar.take<int32_t>((size_t)B * N);
+    d_mean = ar.take<double>(6);
+    d_std = ar.take<double>(6);
+    d_probs = ar.take<float>((size_t)B * n_out);
+    d_label = ar.take<int32_t>(B);
+  });
   if (rc) return rc;
-  cg_arena ar(ctx->io);
-  double *d_xyz = ar.take<double>((size_t)M * 3);
-  double *d_nrm = ar.take<double>((size_t)M * 3);
-  double *d_pose = ar.take<double>((size_t)B * 16);
-  int32_t *d_ids = ar.take<int32_t>((size_t)B * N);
-  double *d_mean = ar.take<double>(6);
-  double *d_std = ar.take<double>(6);
-  float *d_probs = ar.take<float>((size_t)B * n_out);
-  int32_t *d_label = ar.take<int32_t>(B);
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemcpyAsync(d_xyz, cloud_xyz, (size_t)M * 24, cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemcpyAsync(d_nrm, cloud_nrm, (size_t)M * 24, cudaMemcpyHostToDevice, st));
@@ -366,11 +356,9 @@ extern "C" int cg_encoder_probe_dev(cg_net *net, const float *x, const double *c
     in.mean = mean; in.stdv = stdv; in.M = M;
   }
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  int rc = cg_ws_reserve(ctx, encoder_ws_bytes(B) + 1024);
-  if (rc) return rc;
-  cg_arena ar(ctx->ws);
   EncoderWs w;
-  encoder_ws_carve(ar, B, w);
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) { encoder_ws_carve(ar, B, w); });
+  if (rc) return rc;
   if ((rc = encoder_forward(net, in, B, N, w, out_pf, out_keys))) return rc;
   CG_CUDA(ctx, cudaMemcpyAsync(out_T3, w.T3, (size_t)B * 9 * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   CG_CUDA(ctx, cudaMemcpyAsync(out_T64, w.T64, (size_t)B * 4096 * 4, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -389,14 +377,14 @@ extern "C" int cg_nunocs_forward_host(cg_net *net, const float *x_host, int N, i
   cg_ctx *ctx = net->ctx;
   CG_REQUIRE(ctx, x_host && N > 0 && out_coords, "nunocs_host: bad arguments");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t need = cg_arena::pad((size_t)N * 24) + cg_arena::pad((size_t)N * 12) * 2 + cg_arena::pad((size_t)N * 4) + 4096;
-  int rc = cg_io_reserve(ctx, need);
+  float *d_x, *d_c, *d_z; int32_t *d_b;
+  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
+    d_x = ar.take<float>((size_t)N * 6);
+    d_c = ar.take<float>((size_t)N * 3);
+    d_b = ar.take<int32_t>((size_t)N * 3);
+    d_z = ar.take<float>(N);
+  });
   if (rc) return rc;
-  cg_arena ar(ctx->io);
-  float *d_x = ar.take<float>((size_t)N * 6);
-  float *d_c = ar.take<float>((size_t)N * 3);
-  int32_t *d_b = ar.take<int32_t>((size_t)N * 3);
-  float *d_z = ar.take<float>(N);
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemcpyAsync(d_x, x_host, (size_t)N * 24, cudaMemcpyHostToDevice, st));
   rc = cg_nunocs_forward_dev(net, d_x, N, bins, d_c, d_z, d_b);

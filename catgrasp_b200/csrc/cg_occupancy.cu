@@ -133,12 +133,13 @@ extern "C" int cg_occupancy_from_scan_host(cg_ctx *ctx, const float *pts_host, i
   CG_REQUIRE(ctx, bits < (size_t(1) << 33), "occupancy: occupied-cell bounding box too large");
   const size_t words = (bits + 31) / 32;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  rc = cg_io_reserve(ctx, cg_arena::pad((size_t)P * 12) + cg_arena::pad(words * 4) + cg_arena::pad((size_t)total) + 4096);
+  float *d_pts; unsigned *d_mask; unsigned char *d_flags;
+  rc = cg_io_carve(ctx, [&](cg_arena &ar) {
+    d_pts = ar.take<float>((size_t)P * 3);
+    d_mask = ar.take<unsigned>(words);
+    d_flags = ar.take<unsigned char>((size_t)total);
+  });
   if (rc) return rc;
-  cg_arena ar(ctx->io);
-  float *d_pts = ar.take<float>((size_t)P * 3);
-  unsigned *d_mask = ar.take<unsigned>(words);
-  unsigned char *d_flags = ar.take<unsigned char>((size_t)total);
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemcpyAsync(d_pts, pts_host, (size_t)P * 12, cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemsetAsync(d_mask, 0, words * 4, st));

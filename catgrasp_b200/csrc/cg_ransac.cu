@@ -266,18 +266,17 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
   CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && min_scale && max_scale, "ransac9d: bad arguments");
   CG_REQUIRE(ctx, out_ratio && out_T && out_valid, "ransac9d: outputs");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t need = cg_arena::pad((size_t)N * 24) * 2 + cg_arena::pad((size_t)H * 16) + cg_arena::pad(9 * 8) +
-                      cg_arena::pad((size_t)H * 8) + cg_arena::pad((size_t)H * 128) + cg_arena::pad(H) + 4096;
-  int rc = cg_io_reserve(ctx, need);
+  double *d_src, *d_tgt, *d_par, *d_ratio, *d_T; int32_t *d_ids; unsigned char *d_valid;
+  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
+    d_src = ar.take<double>((size_t)N * 3);
+    d_tgt = ar.take<double>((size_t)N * 3);
+    d_ids = ar.take<int32_t>((size_t)H * 4);
+    d_par = ar.take<double>(9);
+    d_ratio = ar.take<double>(H);
+    d_T = ar.take<double>((size_t)H * 16);
+    d_valid = ar.take<unsigned char>(H);
+  });
   if (rc) return rc;
-  cg_arena ar(ctx->io);
-  double *d_src = ar.take<double>((size_t)N * 3);
-  double *d_tgt = ar.take<double>((size_t)N * 3);
-  int32_t *d_ids = ar.take<int32_t>((size_t)H * 4);
-  double *d_par = ar.take<double>(9);
-  double *d_ratio = ar.take<double>(H);
-  double *d_T = ar.take<double>((size_t)H * 16);
-  unsigned char *d_valid = ar.take<unsigned char>(H);
   double par[9];
   for (int k = 0; k < 3; k++) { par[k] = min_scale[k]; par[3 + k] = max_scale[k]; par[6 + k] = max_dims ? max_dims[k] : 0.0; }
   cudaStream_t st = ctx->stream;

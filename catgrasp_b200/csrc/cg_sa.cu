@@ -119,11 +119,9 @@ int run_mlp(cg_mlp *m, const float *x, long long R, float *out_last, float **las
   const int nlayers = (int)m->L.size();
   int maxc = 0;
   for (const cg_layer &l : m->L) maxc = l.C > maxc ? l.C : maxc;
-  const size_t buf = cg_arena::pad((size_t)R * maxc * sizeof(float));
-  int rc = cg_ws_reserve(ctx, 2 * buf + 4096);
+  float *pp[2];
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) { for (float *&p : pp) p = ar.take<float>((size_t)R * maxc); });
   if (rc) return rc;
-  cg_arena ar(ctx->ws);
-  float *pp[2] = {ar.take<float>((size_t)R * maxc), ar.take<float>((size_t)R * maxc)};
   const float *cur = x;
   for (int i = 0; i < nlayers; i++) {
     float *dst = (i == nlayers - 1 && out_last) ? out_last : pp[i & 1];
@@ -212,11 +210,9 @@ extern "C" int cg_three_interp_dev(cg_ctx *ctx, const float *xyz1, const float *
   float *w = out_weight;
   if (!idx || !w) {
     const size_t n3 = (size_t)B * N * 3;
-    int rc = cg_ws_reserve(ctx, cg_arena::pad(n3 * 4) * 2 + 1024);
+    int32_t *ti; float *tw;
+    int rc = cg_ws_carve(ctx, [&](cg_arena &ar) { ti = ar.take<int32_t>(n3); tw = ar.take<float>(n3); });
     if (rc) return rc;
-    cg_arena ar(ctx->ws);
-    int32_t *ti = ar.take<int32_t>(n3);
-    float *tw = ar.take<float>(n3);
     if (!idx) idx = ti;
     if (!w) w = tw;
   }

@@ -297,23 +297,6 @@ __global__ void sdf_parity_kernel(const Geom g, const int *__restrict__ cnt, flo
   if (run & 1) atomicOr(open_flag, 1);
 }
 
-// device allocations of one build; freed on every return path
-struct DevBuf {
-  void *p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-};
-
-int dev_alloc(cg_ctx *ctx, DevBuf &b, size_t bytes) {
-  const cudaError_t e = cudaMalloc(&b.p, bytes);
-  if (e == cudaErrorMemoryAllocation) {
-    cudaGetLastError();
-    ctx->err = "sdf_from_mesh: out of device memory";
-    return CG_ENOMEM;
-  }
-  CG_CUDA(ctx, e);
-  return CG_OK;
-}
-
 }  // namespace
 
 extern "C" int cg_sdf_from_mesh(cg_ctx *ctx, const double *vertices, int nv, const int32_t *faces, int nf,
@@ -441,8 +424,7 @@ extern "C" int cg_sdf_from_mesh(cg_ctx *ctx, const double *vertices, int nv, con
   s->ctx = ctx; s->nx = g.nx; s->ny = g.ny; s->nz = g.nz; s->res = resolution;
   for (int a = 0; a < 3; a++) s->origin[a] = (float)g.o[a];
   cg_sdf_border_stats(s, host.data());
-  s->grid = grid;
-  d_grid.p = nullptr;   // owned by s now
+  s->grid = static_cast<float *>(d_grid.release());
   *out = s;
   return CG_OK;
 }
