@@ -6,8 +6,6 @@ down-sampled point the affordance of its nearest canonical point (the kd-tree qu
 depend on the grasp: contact points are a subset of the down-sampled cloud).  Device (per grasp): finger-frame transform,
 finger-extent test, contact patch, normal test, mean affordance.
 """
-import ctypes as C
-
 import numpy as np
 import torch
 from scipy.spatial import cKDTree
@@ -26,8 +24,6 @@ def compute_grasp_affordance(grasp_poses, finger_mesh_in_grasp, canonical_pts_in
                              device=0):
     """Returns (p_T_given_G (G,) float64 with NaN where the reference drops the grasp (run_grasp_simulation.py:66-67),
     contact-patch sizes (G, F) int32)."""
-    if not torch.cuda.is_available():
-        raise _lib.CgError("catgrasp_b200.affordance needs a CUDA device (no CPU fallback)")
     poses = np.asarray(grasp_poses, dtype=np.float64).reshape(-1, 4, 4)
     G = poses.shape[0]
     boxes = np.ascontiguousarray(finger_boxes, dtype=np.float64).reshape(-1, 4)
@@ -47,15 +43,10 @@ def compute_grasp_affordance(grasp_poses, finger_mesh_in_grasp, canonical_pts_in
     _, nn = cKDTree(np.asarray(canonical_cloud_in_cam, dtype=np.float64)).query(pts)       # :62, once per object
     aff = np.ascontiguousarray(np.asarray(canonical_affordance, dtype=np.float64)[nn])
     cam_in_finger = np.linalg.inv(np.asarray(finger_mesh_in_grasp, np.float64)) @ np.linalg.inv(poses)   # :52
-    ctx = _lib.Context.get(device)
-    ctx.use_torch_stream()
-    dev = torch.device("cuda", device)
-    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)       # noqa: E731
-    d_T, d_pts, d_nrm, d_aff = up(cam_in_finger), up(pts), up(np.asarray(canonical_normals_in_cam, np.float64)), up(aff)
-    out_p = torch.empty((G,), dtype=torch.float64, device=dev)
-    out_c = torch.zeros((G, 4), dtype=torch.int32, device=dev)
-    dirs_c = (C.c_int * F)(*dirs)
-    ctx.check(ctx.lib.cg_grasp_affordance_dev(ctx.h, _lib.ptr(d_T), G, _lib.ptr(d_pts), _lib.ptr(d_nrm), _lib.ptr(d_aff),
-                                              pts.shape[0], _lib.ptr(boxes), dirs_c, F, C.c_double(float(surface_tol)),
-                                              _lib.ptr(out_p), _lib.ptr(out_c)))
+    ctx, d_T, d_pts, d_nrm, d_aff = _lib.inputs(cam_in_finger, pts, canonical_normals_in_cam, aff, dtype=torch.float64,
+                                                ctx=_lib.Context.get(device))
+    out_p = torch.empty((G,), dtype=torch.float64, device=d_T.device)
+    out_c = torch.zeros((G, 4), dtype=torch.int32, device=d_T.device)
+    ctx.call("cg_grasp_affordance_dev", ctx.h, d_T, G, d_pts, d_nrm, d_aff, pts.shape[0], boxes,
+             np.array(dirs, dtype=np.intc), F, float(surface_tol), out_p, out_c)
     return out_p.cpu().numpy(), out_c.cpu().numpy()[:, :F]

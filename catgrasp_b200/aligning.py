@@ -5,8 +5,6 @@ The host keeps exactly the reference's RNG consumption -- one ``np.random.choice
 iteration, all drawn up front (aligning.py:91-97) -- and the reference's selection rule (first maximum of the inlier
 ratio over the hypotheses that survive the gates, aligning.py:105-117).
 """
-import ctypes as C
-
 import numpy as np
 
 from . import _lib
@@ -31,10 +29,8 @@ def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree
     ratio = np.empty(max_iter, np.float64)
     T = np.empty((max_iter, 4, 4), np.float64)
     valid = np.empty(max_iter, np.uint8)
-    ctx.use_own_stream()   # blocking host call
-    ctx.check(ctx.lib.cg_ransac9d_host(ctx.h, _lib.ptr(source), _lib.ptr(target), N, _lib.ptr(ids), max_iter,
-                                       C.c_double(float(PassThreshold)), _lib.ptr(mins), _lib.ptr(maxs), _lib.ptr(mdim),
-                                       _lib.ptr(ratio), _lib.ptr(T), _lib.ptr(valid)))
+    ctx.call("cg_ransac9d_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs, mdim, ratio,
+             T, valid)
     keep = np.nonzero(valid)[0]
     if keep.size == 0:
         return None, None

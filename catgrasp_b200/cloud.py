@@ -1,9 +1,8 @@
 """Point-cloud preparation on the device (csrc/cg_cloud.cu): the open3d and scipy calls that feed the ported stages.
 
-Each function replaces one reference call site and takes numpy arrays or CUDA tensors; it returns numpy arrays for
-numpy input and CUDA tensors for tensor input.  Points are float64 (scipy works in float64 and open3d stores
-Vector3d); float32 input is widened exactly.  Distances are float64 ``(dx*dx + dy*dy) + dz*dz``, bit-equal to scipy's
-cKDTree; a tie goes to the smaller point index.
+Each function replaces one reference call site and takes numpy arrays or CUDA tensors (numpy in, numpy out; see
+_lib).  Points are float64 (scipy works in float64 and open3d stores Vector3d); float32 input is widened exactly.
+Distances are float64 ``(dx*dx + dy*dy) + dz*dz``, bit-equal to scipy's cKDTree; a tie goes to the smaller point index.
 
 Voxel outputs come in ascending (ix, iy, iz) voxel order.  open3d returns them in the iteration order of its hash
 map, which is not reproducible, so callers must not depend on the order.
@@ -16,98 +15,65 @@ import torch
 from . import _lib
 
 
-def _ctx(device):
-    if not torch.cuda.is_available():
-        raise _lib.CgError("catgrasp_b200.cloud needs a CUDA device (no CPU fallback)")
-    ctx = _lib.Context.get(device)
-    ctx.use_torch_stream()
-    return ctx
-
-
-def _device_of(*arrays):
-    for a in arrays:
-        if isinstance(a, torch.Tensor) and a.is_cuda:
-            return a.device.index
-    return torch.cuda.current_device()
-
-
-def _dev(a, dtype, device, cols=3):
-    """Contiguous (N, cols) device tensor of ``dtype`` (exact widening of float32 points)."""
-    t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
-    t = t.to(device=torch.device("cuda", device), dtype=dtype)
-    if cols:
-        t = t.reshape(-1, cols)
-    return t.contiguous()
-
-
-def _out(t, like_torch):
-    return t if like_torch else t.cpu().numpy()
-
-
 class CloudIndex:
     """Points binned into cells of size ``cell`` (origin min_bound - cell/2) and sorted by (cell, index); built once
     and shared by every query on the same cloud and cell size.  Holds its own copy of the points."""
 
     def __init__(self, pts, cell, device=None):
-        device = _device_of(pts) if device is None else device
-        self.ctx = _ctx(device)
-        self.device = device
-        p = _dev(pts, torch.float64, device)
+        self.ctx, p = _lib.inputs(pts, dtype=torch.float64, ctx=None if device is None else _lib.Context.get(device))
+        p = p.reshape(-1, 3)
+        self.device = self.ctx.device
         if p.shape[0] == 0:
             raise ValueError("CloudIndex needs at least one point")
         h = C.c_void_p()
-        self.ctx.check(self.ctx.lib.cg_cloud_index_create(self.ctx.h, _lib.ptr(p), p.shape[0], C.c_double(float(cell)),
-                                                          C.byref(h)))
+        self.ctx.call("cg_cloud_index_create", self.ctx.h, p, p.shape[0], float(cell), C.byref(h))
         self.h = h
         n, u = C.c_int(), C.c_int()
-        self.ctx.check(self.ctx.lib.cg_cloud_index_info(h, C.byref(n), C.byref(u), None, None))
+        self.ctx.call("cg_cloud_index_info", h, C.byref(n), C.byref(u), None, None)
         self.n_points, self.n_cells = n.value, u.value
 
     def __del__(self):
         h = getattr(self, "h", None)
         if h is not None and h.value:
-            self.ctx.lib.cg_cloud_index_destroy(h)
+            self.ctx.call("cg_cloud_index_destroy", h)
             self.h = None
+
+    def _query(self, query):
+        return _lib.inputs(query, dtype=torch.float64, ctx=self.ctx)[1].reshape(-1, 3)
+
+    def _empty(self, *shape, dtype=torch.float64):
+        return torch.empty(shape, dtype=dtype, device=torch.device("cuda", self.device))
 
     def voxel_means(self, normals=None):
         """open3d VoxelDownSample with voxel_size = cell: (U,3) means (and (U,3) normals) as device tensors."""
-        dev = torch.device("cuda", self.device)
-        out = torch.empty((self.n_cells, 3), dtype=torch.float64, device=dev)
-        nrm = None if normals is None else _dev(normals, torch.float64, self.device)
+        out = self._empty(self.n_cells, 3)
+        nrm = None if normals is None else self._query(normals)
         out_n = None if normals is None else torch.empty_like(out)
-        self.ctx.use_torch_stream()
-        self.ctx.check(self.ctx.lib.cg_voxel_down_sample_dev(self.h, _lib.ptr(nrm), _lib.ptr(out), _lib.ptr(out_n)))
+        self.ctx.call("cg_voxel_down_sample_dev", self.h, nrm, out, out_n)
         return out, out_n
 
     def nearest(self, query, max_dist):
-        q = _dev(query, torch.float64, self.device)
-        idx = torch.empty((q.shape[0],), dtype=torch.int32, device=q.device)
-        dist = torch.empty((q.shape[0],), dtype=torch.float64, device=q.device)
-        self.ctx.use_torch_stream()
-        self.ctx.check(self.ctx.lib.cg_cloud_nearest_dev(self.h, _lib.ptr(q), q.shape[0], C.c_double(float(max_dist)),
-                                                         _lib.ptr(idx), _lib.ptr(dist)))
+        q = self._query(query)
+        idx = self._empty(q.shape[0], dtype=torch.int32)
+        dist = self._empty(q.shape[0])
+        self.ctx.call("cg_cloud_nearest_dev", self.h, q, q.shape[0], float(max_dist), idx, dist)
         return dist, idx
 
     def within(self, query, r, compare_sqrt):
         """uint8 mask: some indexed point has d2 <= r*r (compare_sqrt False) or sqrt(d2) <= r (True)."""
-        q = _dev(query, torch.float64, self.device)
-        mask = torch.empty((q.shape[0],), dtype=torch.uint8, device=q.device)
-        self.ctx.use_torch_stream()
-        self.ctx.check(self.ctx.lib.cg_cloud_radius_mask_dev(self.h, _lib.ptr(q), q.shape[0], C.c_double(float(r)),
-                                                             int(bool(compare_sqrt)), _lib.ptr(mask)))
+        q = self._query(query)
+        mask = self._empty(q.shape[0], dtype=torch.uint8)
+        self.ctx.call("cg_cloud_radius_mask_dev", self.h, q, q.shape[0], float(r), int(bool(compare_sqrt)), mask)
         return mask
 
     def normals(self, radius, max_nn, view_port=(0.0, 0.0, 0.0), neighbours=False):
         """Oriented normals of the indexed points (N,3); with neighbours=True also the (N,max_nn) int32 neighbour
         lists in (d2, index) order, -1 padded, and their (N,) sizes."""
-        dev = torch.device("cuda", self.device)
-        out = torch.empty((self.n_points, 3), dtype=torch.float64, device=dev)
-        nbr = torch.empty((self.n_points, max_nn), dtype=torch.int32, device=dev) if neighbours else None
-        cnt = torch.empty((self.n_points,), dtype=torch.int32, device=dev) if neighbours else None
-        vp = np.ascontiguousarray(np.asarray(view_port, dtype=np.float64).reshape(3))
-        self.ctx.use_torch_stream()
-        self.ctx.check(self.ctx.lib.cg_cloud_normals_dev(self.h, C.c_double(float(radius)), int(max_nn), _lib.ptr(vp),
-                                                         _lib.ptr(out), _lib.ptr(nbr), _lib.ptr(cnt)))
+        out = self._empty(self.n_points, 3)
+        nbr = self._empty(self.n_points, max_nn, dtype=torch.int32) if neighbours else None
+        cnt = self._empty(self.n_points, dtype=torch.int32) if neighbours else None
+        vp = np.ascontiguousarray(view_port, dtype=np.float64).reshape(3)
+        self.ctx.call("cg_cloud_normals_dev", self.h, float(radius), int(max_nn), vp, out, nbr, cnt)
         return (out, nbr, cnt) if neighbours else out
 
 
@@ -125,42 +91,31 @@ def _query_cell(pts, r):
 def depth2xyzmap(depth, K):
     """Utils.py:239-251 (called at run_grasp_simulation.py:198): (H,W) depth, float32 or float64 -> (H,W,3) float32
     camera-frame points; pixels with depth < 0.1 are (0,0,0)."""
-    like = isinstance(depth, torch.Tensor)
-    device = _device_of(depth)
-    ctx = _ctx(device)
-    d = depth if like else torch.from_numpy(np.ascontiguousarray(depth))
-    if d.dtype not in (torch.float32, torch.float64):
-        d = d.to(torch.float64)
-    d = d.to(torch.device("cuda", device)).contiguous()
+    d = depth if isinstance(depth, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(depth))
+    ctx, d = _lib.inputs(d, dtype=d.dtype if d.dtype in (torch.float32, torch.float64) else torch.float64)
     H, W = d.shape[:2]
-    Kh = np.ascontiguousarray(np.asarray(K, dtype=np.float64).reshape(9))
     out = torch.empty((H, W, 3), dtype=torch.float32, device=d.device)
-    ctx.check(ctx.lib.cg_depth2xyz_dev(ctx.h, _lib.ptr(d), int(d.dtype == torch.float64), H, W, _lib.ptr(Kh), _lib.ptr(out)))
-    return _out(out, like)
+    ctx.call("cg_depth2xyz_dev", ctx.h, d, int(d.dtype == torch.float64), H, W,
+             np.ascontiguousarray(K, dtype=np.float64).reshape(9), out)
+    return _lib.returned(depth, out)
 
 
 def voxel_down_sample(pts, voxel_size, normals=None):
     """open3d ``PointCloud.voxel_down_sample(voxel_size)`` (run_grasp_simulation.py:97, :114, :137, :173, :246):
     voxel means (and normalised summed normals when ``normals`` is given), in ascending (ix, iy, iz) order."""
-    like = isinstance(pts, torch.Tensor)
-    n = pts.shape[0]
-    if n == 0:
+    if pts.shape[0] == 0:
         z = np.zeros((0, 3))
-        z = torch.from_numpy(z).cuda() if like else z
+        z = torch.from_numpy(z).to(pts.device) if getattr(pts, "is_cuda", False) else z
         return z if normals is None else (z, z)
-    idx = CloudIndex(pts, voxel_size)
-    p, nrm = idx.voxel_means(normals)
-    return _out(p, like) if normals is None else (_out(p, like), _out(nrm, like))
+    p, nrm = CloudIndex(pts, voxel_size).voxel_means(normals)
+    return _lib.returned(pts, p) if normals is None else _lib.returned(pts, p, nrm)
 
 
 def nearest(ref_pts, query_pts, max_dist):
     """``cKDTree(ref_pts).query(query_pts)`` (run_grasp_simulation.py:120, :131) for answers within ``max_dist``:
     (dists (Q,) float64, indices (Q,) int64), -1 / inf where no point lies within max_dist (inclusive)."""
-    like = isinstance(query_pts, torch.Tensor)
-    idx = CloudIndex(ref_pts, _query_cell(ref_pts, max_dist))
-    d, i = idx.nearest(query_pts, max_dist)
-    i = i.to(torch.int64)
-    return _out(d, like), _out(i, like)
+    d, i = CloudIndex(ref_pts, _query_cell(ref_pts, max_dist)).nearest(query_pts, max_dist)
+    return _lib.returned(query_pts, d, i.to(torch.int64))
 
 
 def cloudA_minus_cloudB(ptsA, ptsB, thres):
@@ -183,11 +138,10 @@ def cloudA_minus_cloudB(ptsA, ptsB, thres):
 def estimate_normals(pts, radius, max_nn, view_port=(0.0, 0.0, 0.0)):
     """open3d ``estimate_normals(KDTreeSearchParamHybrid(radius, max_nn))`` followed by Utils.py:205-213
     ``correct_pcd_normal_direction(pcd, view_port)`` (run_grasp_simulation.py:209-210, :247-248): (N,3) float64."""
-    like = isinstance(pts, torch.Tensor)
     if pts.shape[0] == 0:
         z = np.zeros((0, 3))
-        return torch.from_numpy(z).cuda() if like else z
-    return _out(CloudIndex(pts, _query_cell(pts, radius)).normals(radius, max_nn, view_port), like)
+        return torch.from_numpy(z).to(pts.device) if getattr(pts, "is_cuda", False) else z
+    return _lib.returned(pts, CloudIndex(pts, _query_cell(pts, radius)).normals(radius, max_nn, view_port))
 
 
 def prepare_object(ob_pts, ob_normals, scene_pts, gripper_diameter, octo_resolution=0.001, K=None):

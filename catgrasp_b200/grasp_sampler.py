@@ -12,7 +12,6 @@ Split of work (file:line = dexnet/grasping/grasp_sampler.py unless stated):
 
 ``cone_grasp_poses`` consumes the global numpy RNG exactly like ``sample_grasps`` (:131-158).
 """
-import ctypes as C
 import math
 
 import numpy as np
@@ -184,11 +183,6 @@ def enumerate_poses(surface_pts, R0s, sphere_pts, hand_depth, approach_step, ini
     """Device part: (S,3) samples with frames (S,3,3) -> poses ((P,4,4) float64 cuda, (P,4,4) float32 cuda),
     P = S * (1 + len(sphere_pts) * len(inplane_deg)) * len(np.arange(0, hand_depth, approach_step)), in the reference's
     order.  ``points_for_center`` (M,3) applies center_ob_between_gripper (:191-203)."""
-    if not torch.cuda.is_available():
-        raise _lib.CgError("catgrasp_b200.grasp_sampler needs a CUDA device (no CPU fallback)")
-    ctx = _lib.Context.get(device)
-    ctx.use_torch_stream()
-    dev = torch.device("cuda", device)
     ref = np.array([1, 0, 0])
     R_sphere = np.stack([directionVecToRotation(direction=sp.copy(), ref=ref) for sp in sphere_pts]) \
         if len(sphere_pts) else np.zeros((0, 3, 3))
@@ -196,17 +190,15 @@ def enumerate_poses(surface_pts, R0s, sphere_pts, hand_depth, approach_step, ini
     depths = np.arange(0, hand_depth, approach_step).astype(np.float64)
     S, NS, NI, ND = len(surface_pts), len(R_sphere), len(R_inplane), len(depths)
     P = S * (1 + NS * NI) * ND
-    up = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)      # noqa: E731
-    d_surf, d_R0, d_sph, d_inp, d_dep = up(surface_pts), up(R0s), up(R_sphere), up(R_inplane), up(depths)
-    out64 = torch.empty((P, 4, 4), dtype=torch.float64, device=dev)
-    out32 = torch.empty((P, 4, 4), dtype=torch.float32, device=dev)
+    ctx, d_surf, d_R0, d_sph, d_inp, d_dep, d_pts = _lib.inputs(
+        surface_pts, R0s, R_sphere, R_inplane, depths, points_for_center, dtype=torch.float64, ctx=_lib.Context.get(device))
+    out64 = torch.empty((P, 4, 4), dtype=torch.float64, device=d_surf.device)
+    out32 = torch.empty((P, 4, 4), dtype=torch.float32, device=d_surf.device)
     if P == 0:
         return out64, out32
-    ctx.check(ctx.lib.cg_cone_poses_dev(ctx.h, _lib.ptr(d_surf), _lib.ptr(d_R0), S, _lib.ptr(d_sph), NS, _lib.ptr(d_inp), NI,
-                                        _lib.ptr(d_dep), ND, C.c_double(float(init_bite)), _lib.ptr(out64), _lib.ptr(out32)))
-    if points_for_center is not None:
-        d_pts = up(points_for_center)
-        ctx.check(ctx.lib.cg_center_grasps_dev(ctx.h, _lib.ptr(out64), _lib.ptr(out32), P, _lib.ptr(d_pts), d_pts.shape[0]))
+    ctx.call("cg_cone_poses_dev", ctx.h, d_surf, d_R0, S, d_sph, NS, d_inp, NI, d_dep, ND, float(init_bite), out64, out32)
+    if d_pts is not None:
+        ctx.call("cg_center_grasps_dev", ctx.h, out64, out32, P, d_pts, d_pts.shape[0])
     return out64, out32
 
 

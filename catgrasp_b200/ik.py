@@ -1,7 +1,5 @@
 """IK feasibility of the KUKA iiwa14 on the GPU (csrc/cg_ik.cu): the closed-form replacement of the reference's
 get_ik_within_limits (my_cpp/common.cpp:9-72) over its generated ikfast solver, free joint 2 fixed at 0."""
-import ctypes as C
-
 import numpy as np
 import torch
 
@@ -26,30 +24,13 @@ def iiwa14_ik(ee_in_base, upper, lower, solutions=False):
     include/catgrasp_b200.h (NaN where a branch has none).  numpy in -> numpy out; a CUDA tensor in -> CUDA tensors
     out on the same device and stream."""
     up, lo = joint_limits(upper, lower)
-    cuda = isinstance(ee_in_base, torch.Tensor) and ee_in_base.is_cuda
-    if cuda:
-        dev = ee_in_base.device
-        ctx = _lib.Context.get(dev.index)
-        ee = ee_in_base.to(torch.float32).contiguous().reshape(-1, 16)
-        Q = ee.shape[0]
-        count = torch.empty((Q,), dtype=torch.int8, device=dev)
-        sol = torch.empty((Q, 8, 7), dtype=torch.float64, device=dev) if solutions else None
-        ctx.use_torch_stream()
-    else:
-        ctx = _lib.Context.get()
-        host = np.ascontiguousarray(np.asarray(ee_in_base, dtype=np.float64).astype(np.float32)).reshape(-1, 16)
-        Q = host.shape[0]
-        ctx.use_torch_stream()
-        ee = torch.from_numpy(host).to(f"cuda:{ctx.device}")
-        count = torch.empty((Q,), dtype=torch.int8, device=ee.device)
-        sol = torch.empty((Q, 8, 7), dtype=torch.float64, device=ee.device) if solutions else None
-    ctx.check(ctx.lib.cg_iiwa14_ik_dev(ctx.h, _lib.ptr(ee) if Q else None, Q, up.ctypes.data_as(C.c_void_p),
-                                       lo.ctypes.data_as(C.c_void_p), _lib.ptr(count) if Q else None,
-                                       _lib.ptr(sol) if (solutions and Q) else None))
-    if not cuda:
-        count = count.cpu().numpy()
-        sol = sol.cpu().numpy() if solutions else None
-    return (count, sol) if solutions else count
+    ctx, ee = _lib.inputs(ee_in_base, dtype=torch.float32)
+    ee = ee.reshape(-1, 16)
+    Q = ee.shape[0]
+    count = torch.empty((Q,), dtype=torch.int8, device=ee.device)
+    sol = torch.empty((Q, 8, 7), dtype=torch.float64, device=ee.device) if solutions else None
+    ctx.call("cg_iiwa14_ik_dev", ctx.h, ee, Q, up, lo, count, sol)
+    return _lib.returned(ee_in_base, count, sol) if solutions else _lib.returned(ee_in_base, count)
 
 
 def iiwa14_fk(q):

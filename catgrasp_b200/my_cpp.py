@@ -90,14 +90,6 @@ def filter_grasp_pose_raw(grasp_poses, symmetry_tfs, nocs_pose, canonical_to_noc
     a pair that passed the approach test and has no iiwa14 solution within the limits gets CG_ST_REJ_IK, offset -1 and
     an all-zero pose."""
     ctx = sdf_open.ctx
-    if ik is not None and not (isinstance(grasp_poses, torch.Tensor) and grasp_poses.is_cuda):
-        # the IK pass works on device buffers: run the device route and bring the results back
-        gp = torch.from_numpy(np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).astype(np.float32)))
-        st, of, po = filter_grasp_pose_raw(gp.to(f"cuda:{ctx.device}"), symmetry_tfs, nocs_pose, canonical_to_nocs,
-                                           gripper_in_grasp, filter_approach_dir_face_camera, adjust_collision_pose,
-                                           sdf_open, open_pts, sdf_enclosed, enclosed_pts, sdf_mode=sdf_mode,
-                                           sdf_margin=sdf_margin, split_status=split_status, ik=ik)
-        return st.cpu().numpy(), of.cpu().numpy(), po.cpu().numpy()
     prm = _lib.FilterParams()
     prm.nocs_pose = _m16(nocs_pose)
     prm.canonical_to_nocs = _m16(canonical_to_nocs)
@@ -107,48 +99,33 @@ def filter_grasp_pose_raw(grasp_poses, symmetry_tfs, nocs_pose, canonical_to_noc
     prm.sdf_mode = DEFAULT_SDF_MODE if sdf_mode is None else int(sdf_mode)
     prm.sdf_margin = float(sdf_margin)
     prm.split_coll_status = int(bool(split_status))
-    if isinstance(grasp_poses, torch.Tensor) and grasp_poses.is_cuda:
-        dev = grasp_poses.device
-        gp = grasp_poses.to(torch.float32).contiguous().reshape(-1, 16)
-        st = torch.as_tensor(np.asarray(symmetry_tfs)).to(device=dev, dtype=torch.float32).contiguous().reshape(-1, 16)
-        p1 = torch.as_tensor(open_pts).to(device=dev, dtype=torch.float32).contiguous().reshape(-1, 3)
-        p2 = torch.as_tensor(enclosed_pts).to(device=dev, dtype=torch.float32).contiguous().reshape(-1, 3)
-        G, S = gp.shape[0], st.shape[0]
-        Q = G * S
-        status = torch.empty((Q,), dtype=torch.uint8, device=dev)
-        offset = torch.empty((Q,), dtype=torch.int8, device=dev)
-        poses = torch.empty((Q, 4, 4), dtype=torch.float32, device=dev)
-        ctx.use_torch_stream()
-        ctx.check(ctx.lib.cg_filter_grasp_pose_dev(
-            ctx.h, C.byref(prm), _lib.ptr(gp), G, _lib.ptr(st), S, sdf_open.h, _lib.ptr(p1), p1.shape[0],
-            sdf_enclosed.h if sdf_enclosed is not None else None, _lib.ptr(p2), p2.shape[0],
-            _lib.ptr(status), _lib.ptr(offset), _lib.ptr(poses)))
-        if ik is not None:
-            cam_in_world, ee_in_grasp, upper, lower = ik
-            up, lo = joint_limits(upper, lower)
-            ikp = _lib.IkParams()
-            ikp.cam_in_world = _m16(cam_in_world)
-            ikp.ee_in_grasp = _m16(ee_in_grasp)
-            ikp.upper = (C.c_double * 7)(*up.tolist())
-            ikp.lower = (C.c_double * 7)(*lo.tolist())
-            ctx.check(ctx.lib.cg_filter_apply_ik_dev(ctx.h, C.byref(prm), _lib.ptr(gp), G, _lib.ptr(st), S, C.byref(ikp),
-                                                     _lib.ptr(status), _lib.ptr(offset), _lib.ptr(poses)))
-        return status, offset, poses
-    gp = np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).astype(np.float32)).reshape(-1, 16)
-    st = np.ascontiguousarray(np.asarray(symmetry_tfs, dtype=np.float64).astype(np.float32)).reshape(-1, 16)
-    p1 = np.ascontiguousarray(np.asarray(open_pts, dtype=np.float64).astype(np.float32)).reshape(-1, 3)
-    p2 = np.ascontiguousarray(np.asarray(enclosed_pts, dtype=np.float64).astype(np.float32)).reshape(-1, 3)
+    arrays = (grasp_poses, symmetry_tfs, open_pts, enclosed_pts)
+    if ik is None and not getattr(grasp_poses, "is_cuda", False):
+        # host arrays without IK: the blocking host entry stages them itself (the reference narrows float64 -> float)
+        route, dev = "host", "cpu"
+        gp, st, p1, p2 = (torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.float64), dtype=np.float32))
+                          for a in arrays)
+    else:
+        route, dev = "dev", torch.device("cuda", ctx.device)
+        _, gp, st, p1, p2 = _lib.inputs(*arrays, dtype=torch.float32, ctx=ctx)
+    gp, st, p1, p2 = gp.reshape(-1, 16), st.reshape(-1, 16), p1.reshape(-1, 3), p2.reshape(-1, 3)
     G, S = gp.shape[0], st.shape[0]
     Q = G * S
-    status = np.empty((Q,), np.uint8)
-    offset = np.empty((Q,), np.int8)
-    poses = np.empty((Q, 4, 4), np.float32)
-    ctx.use_own_stream()   # blocking host call
-    ctx.check(ctx.lib.cg_filter_grasp_pose_host(
-        ctx.h, C.byref(prm), _lib.ptr(gp), G, _lib.ptr(st), S, sdf_open.h, _lib.ptr(p1), p1.shape[0],
-        sdf_enclosed.h if sdf_enclosed is not None else None, _lib.ptr(p2), p2.shape[0],
-        _lib.ptr(status), _lib.ptr(offset), _lib.ptr(poses)))
-    return status, offset, poses
+    status = torch.empty((Q,), dtype=torch.uint8, device=dev)
+    offset = torch.empty((Q,), dtype=torch.int8, device=dev)
+    poses = torch.empty((Q, 4, 4), dtype=torch.float32, device=dev)
+    ctx.call(f"cg_filter_grasp_pose_{route}", ctx.h, C.byref(prm), gp, G, st, S, sdf_open.h, p1, p1.shape[0],
+             sdf_enclosed.h if sdf_enclosed is not None else None, p2, p2.shape[0], status, offset, poses)
+    if ik is not None:
+        cam_in_world, ee_in_grasp, upper, lower = ik
+        up, lo = joint_limits(upper, lower)
+        ikp = _lib.IkParams()
+        ikp.cam_in_world = _m16(cam_in_world)
+        ikp.ee_in_grasp = _m16(ee_in_grasp)
+        ikp.upper = (C.c_double * 7)(*up.tolist())
+        ikp.lower = (C.c_double * 7)(*lo.tolist())
+        ctx.call("cg_filter_apply_ik_dev", ctx.h, C.byref(prm), gp, G, st, S, C.byref(ikp), status, offset, poses)
+    return _lib.returned(grasp_poses, status, offset, poses)
 
 
 def _mm4_f32(A, B):
@@ -241,17 +218,16 @@ def makeOccupancyGridFromCloudScan(pts, K, resolution):
     res = float(np.float32(resolution))
     if not res > 0.0:
         raise _lib.CgError(f"makeOccupancyGridFromCloudScan: resolution must be > 0 in float32, got {resolution!r}")
-    dims = (C.c_int * 3)()
-    org = (C.c_float * 3)()
-    ctx.check(ctx.lib.cg_occupancy_grid_geometry(_lib.ptr(p), p.shape[0], C.c_float(res), dims, org))
+    dims = np.empty(3, np.int32)
+    org = np.empty(3, np.float32)
+    ctx.call("cg_occupancy_grid_geometry", p, p.shape[0], res, dims, org)
     nx, ny, nz = int(dims[0]), int(dims[1]), int(dims[2])
     if nx * ny * nz == 0:
         return np.zeros((0, 3), np.float32)
     if nx * ny * nz >= 1 << 31:      # refused before the (nx, ny, nz) flag array is allocated
         raise _lib.CgError(f"makeOccupancyGridFromCloudScan: a {nx} x {ny} x {nz} grid has 2^31 or more samples")
     flags = np.empty(nx * ny * nz, np.uint8)
-    ctx.use_own_stream()   # blocking host call
-    ctx.check(ctx.lib.cg_occupancy_from_scan_host(ctx.h, _lib.ptr(p), p.shape[0], C.c_float(res), _lib.ptr(flags)))
+    ctx.call("cg_occupancy_from_scan_host", ctx.h, p, p.shape[0], res, flags)
     idx = np.nonzero(flags)[0]
     xi, yi, zi = idx // (ny * nz), (idx // nz) % ny, idx % nz
     r32 = np.float32(res)

@@ -16,27 +16,24 @@ class _Net:
         self.ctx = _lib.Context.get(device)
         blob, n_out = pack_blob(state_dict, self.kind)
         self.n_out = n_out
-        lib = self.ctx.lib
-        expect = lib.cg_net_blob_floats(self.kind_id, n_out)
+        expect = self.ctx.call("cg_net_blob_floats", self.kind_id, n_out)
         if expect != blob.size:
             raise _lib.CgError(f"weight blob has {blob.size} floats, library expects {expect}")
         h = C.c_void_p()
-        self.ctx.check(lib.cg_net_create(self.ctx.h, self.kind_id, n_out, _lib.ptr(blob), blob.size, C.byref(h)))
+        self.ctx.call("cg_net_create", self.ctx.h, self.kind_id, n_out, blob, blob.size, C.byref(h))
         self.h = h
         self.device = torch.device("cuda", self.ctx.device)
 
     def __del__(self):
         try:
             if getattr(self, "h", None):
-                self.ctx.lib.cg_net_destroy(self.h)
+                self.ctx.call("cg_net_destroy", self.h)
                 self.h = None
         except Exception:
             pass
 
-    def _dev(self, a, dtype):
-        if isinstance(a, np.ndarray):
-            a = torch.from_numpy(np.ascontiguousarray(a))
-        return a.to(device=self.device, dtype=dtype).contiguous()
+    def _empty(self, *shape, dtype=torch.float32):
+        return torch.empty(shape, dtype=dtype, device=self.device)
 
 
 class PointNetCls(_Net):
@@ -44,23 +41,20 @@ class PointNetCls(_Net):
     kind, kind_id = "cls", _lib.CG_NET_CLS
 
     def forward(self, x, return_probs=False):
-        x = self._dev(x, torch.float32)
+        _, x = _lib.inputs(x, dtype=torch.float32, ctx=self.ctx)
         B, N, D = x.shape
         assert D == 6
-        self.ctx.use_torch_stream()
-        logits = torch.empty((B, self.n_out), dtype=torch.float32, device=self.device)
+        logits = self._empty(B, self.n_out)
         probs = torch.empty_like(logits) if return_probs else None
-        self.ctx.check(self.ctx.lib.cg_cls_forward_dev(self.h, _lib.ptr(x), B, N, _lib.ptr(logits), _lib.ptr(probs)))
+        self.ctx.call("cg_cls_forward_dev", self.h, x, B, N, logits, probs)
         return (logits, probs) if return_probs else logits
 
     __call__ = forward
 
     def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0):
         """Counter-based subset draw on the device (cg_draw_ids_dev): (count, n_pts) int32 cuda tensor."""
-        self.ctx.use_torch_stream()
-        ids = torch.empty((count, n_pts), dtype=torch.int32, device=self.device)
-        self.ctx.check(self.ctx.lib.cg_draw_ids_dev(self.ctx.h, int(M), int(n_pts), int(count), C.c_uint64(int(seed)),
-                                                    C.c_int64(int(first_candidate)), _lib.ptr(ids)))
+        ids = self._empty(count, n_pts, dtype=torch.int32)
+        self.ctx.call("cg_draw_ids_dev", self.ctx.h, int(M), int(n_pts), int(count), int(seed), int(first_candidate), ids)
         return ids
 
     def graspq_dev(self, cloud_xyz, cloud_nrm, poses, ids, mean=None, std=None, out=None):
@@ -68,16 +62,8 @@ class PointNetCls(_Net):
         M = cloud_xyz.shape[0]
         B = poses.shape[0]
         N = ids.shape[1]
-        self.ctx.use_torch_stream()
-        if out is not None:
-            probs, label = out
-            assert probs.is_contiguous() and label.is_contiguous() and poses.is_contiguous() and ids.is_contiguous()
-        else:
-            probs = torch.empty((B, self.n_out), dtype=torch.float32, device=self.device)
-            label = torch.empty((B,), dtype=torch.int32, device=self.device)
-        self.ctx.check(self.ctx.lib.cg_graspq_forward_dev(
-            self.h, _lib.ptr(cloud_xyz), _lib.ptr(cloud_nrm), M, _lib.ptr(poses), B, _lib.ptr(ids), N,
-            _lib.ptr(mean), _lib.ptr(std), _lib.ptr(probs), _lib.ptr(label)))
+        probs, label = out if out is not None else (self._empty(B, self.n_out), self._empty(B, dtype=torch.int32))
+        self.ctx.call("cg_graspq_forward_dev", self.h, cloud_xyz, cloud_nrm, M, poses, B, ids, N, mean, std, probs, label)
         return probs, label
 
     def graspq_host(self, cloud_xyz, cloud_nrm, poses, ids, mean=None, std=None, out_probs=None, out_label=None):
@@ -89,10 +75,8 @@ class PointNetCls(_Net):
             out_probs = np.empty((B, self.n_out), dtype=np.float32)
         if out_label is None:
             out_label = np.empty((B,), dtype=np.int32)
-        self.ctx.use_own_stream()      # blocking host call: never on a (possibly freed) torch stream of an earlier _dev call
-        self.ctx.check(self.ctx.lib.cg_graspq_forward_host(
-            self.h, _lib.ptr(cloud_xyz), _lib.ptr(cloud_nrm), M, _lib.ptr(poses), B, _lib.ptr(ids), N,
-            _lib.ptr(mean), _lib.ptr(std), _lib.ptr(out_probs), _lib.ptr(out_label)))
+        self.ctx.call("cg_graspq_forward_host", self.h, cloud_xyz, cloud_nrm, M, poses, B, ids, N, mean, std, out_probs,
+                      out_label)
         return out_probs, out_label
 
 
@@ -101,12 +85,11 @@ class PointNetSeg(_Net):
     kind, kind_id = "seg", _lib.CG_NET_SEG
 
     def forward(self, x):
-        x = self._dev(x, torch.float32)
+        _, x = _lib.inputs(x, dtype=torch.float32, ctx=self.ctx)
         B, N, D = x.shape
         assert D == 6
-        self.ctx.use_torch_stream()
-        out = torch.empty((B, N, self.n_out), dtype=torch.float32, device=self.device)
-        self.ctx.check(self.ctx.lib.cg_seg_forward_dev(self.h, _lib.ptr(x), B, N, _lib.ptr(out)))
+        out = self._empty(B, N, self.n_out)
+        self.ctx.call("cg_seg_forward_dev", self.h, x, B, N, out)
         return out
 
     __call__ = forward
@@ -118,18 +101,14 @@ class PointNetSeg(_Net):
         coords = np.empty((N, 3), np.float32)
         conf = np.empty((N,), np.float32)
         b = np.empty((N, 3), np.int32)
-        self.ctx.use_own_stream()
-        self.ctx.check(self.ctx.lib.cg_nunocs_forward_host(self.h, _lib.ptr(x), N, int(bins), _lib.ptr(coords),
-                                                           _lib.ptr(conf), _lib.ptr(b)))
+        self.ctx.call("cg_nunocs_forward_host", self.h, x, N, int(bins), coords, conf, b)
         return coords, conf, b
 
     def nunocs_dev(self, x, bins):
-        x = self._dev(x, torch.float32)
+        _, x = _lib.inputs(x, dtype=torch.float32, ctx=self.ctx)
         N = x.shape[0]
-        self.ctx.use_torch_stream()
-        coords = torch.empty((N, 3), dtype=torch.float32, device=self.device)
-        conf = torch.empty((N,), dtype=torch.float32, device=self.device)
-        b = torch.empty((N, 3), dtype=torch.int32, device=self.device)
-        self.ctx.check(self.ctx.lib.cg_nunocs_forward_dev(self.h, _lib.ptr(x), N, int(bins), _lib.ptr(coords),
-                                                          _lib.ptr(conf), _lib.ptr(b)))
+        coords = self._empty(N, 3)
+        conf = self._empty(N)
+        b = self._empty(N, 3, dtype=torch.int32)
+        self.ctx.call("cg_nunocs_forward_dev", self.h, x, N, int(bins), coords, conf, b)
         return coords, conf, b

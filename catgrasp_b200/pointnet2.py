@@ -11,39 +11,32 @@ from . import _lib
 from .net import PointNetCls, PointNetSeg  # noqa: F401  (pointnet2.py:275,302)
 
 
-def _ctx(t):
-    if not t.is_cuda:
-        raise _lib.CgError("catgrasp_b200.pointnet2 operates on CUDA tensors only (no CPU fallback)")
-    ctx = _lib.Context.get(t.device.index)
-    ctx.use_torch_stream()
-    return ctx
-
-
-def _f32(t):
-    return t.to(torch.float32).contiguous()
+def _f32(*tensors):
+    """(ctx, *tensors): the context of the first tensor's device, and the tensors as contiguous float32 where they are
+    (Context.call refuses a CPU tensor, or one on another device, before any launch)."""
+    return (_lib.Context.get(tensors[0].device.index), *[None if t is None else t.to(torch.float32).contiguous()
+                                                         for t in tensors])
 
 
 def square_distance(src, dst):
     """pointnet2.py:14-33. src (B,N,3), dst (B,M,3) -> (B,N,M) in the expanded form."""
-    src, dst = _f32(src), _f32(dst)
-    ctx = _ctx(src)
+    ctx, src, dst = _f32(src, dst)
     B, N, _ = src.shape
     M = dst.shape[1]
     out = torch.empty((B, N, M), dtype=torch.float32, device=src.device)
-    ctx.check(ctx.lib.cg_square_distance_dev(ctx.h, _lib.ptr(src), _lib.ptr(dst), B, N, M, _lib.ptr(out)))
+    ctx.call("cg_square_distance_dev", ctx.h, src, dst, B, N, M, out)
     return out
 
 
 def index_points(points, idx):
     """pointnet2.py:35-51. points (B,N,C), idx (B,S) or (B,S,K) -> (B,S[,K],C)."""
-    points = _f32(points)
-    ctx = _ctx(points)
+    ctx, points = _f32(points)
     B, N, Cc = points.shape
     shape = list(idx.shape)
     idx32 = idx.reshape(B, -1).to(torch.int32).contiguous()
     S = idx32.shape[1]
     out = torch.empty((B, S, Cc), dtype=torch.float32, device=points.device)
-    ctx.check(ctx.lib.cg_index_points_dev(ctx.h, _lib.ptr(points), _lib.ptr(idx32), B, N, Cc, S, _lib.ptr(out)))
+    ctx.call("cg_index_points_dev", ctx.h, points, idx32, B, N, Cc, S, out)
     return out.reshape(shape + [Cc])
 
 
@@ -53,34 +46,30 @@ def farthest_point_sample(xyz, npoint, start_idx=None):
     ``start_idx`` (B,) makes the reference's ``torch.randint`` start (:66) explicit;
     when None it is drawn with torch.randint exactly like the reference.
     """
-    xyz = _f32(xyz)
-    ctx = _ctx(xyz)
+    ctx, xyz = _f32(xyz)
     B, N, _ = xyz.shape
     if start_idx is None:
         start_idx = torch.randint(0, N, (B,), dtype=torch.long).to(xyz.device)
     start = torch.as_tensor(start_idx).to(device=xyz.device, dtype=torch.int32).contiguous()
     out = torch.empty((B, npoint), dtype=torch.int32, device=xyz.device)
-    ctx.check(ctx.lib.cg_fps_dev(ctx.h, _lib.ptr(xyz), B, N, int(npoint), _lib.ptr(start), _lib.ptr(out)))
+    ctx.call("cg_fps_dev", ctx.h, xyz, B, N, int(npoint), start, out)
     return out.long()
 
 
 def query_ball_point(radius, nsample, xyz, new_xyz):
     """pointnet2.py:78-98. -> (B,S,nsample) int64, nsample smallest in-ball indices, padded with the first."""
-    xyz, new_xyz = _f32(xyz), _f32(new_xyz)
-    ctx = _ctx(xyz)
+    ctx, xyz, new_xyz = _f32(xyz, new_xyz)
     B, N, _ = xyz.shape
     S = new_xyz.shape[1]
     out = torch.empty((B, S, nsample), dtype=torch.int32, device=xyz.device)
     r2 = float(np.float32(radius ** 2))   # torch compares the fp32 tensor against float32(radius**2), :93
-    ctx.check(ctx.lib.cg_ball_query_dev(ctx.h, r2, int(nsample), _lib.ptr(xyz), _lib.ptr(new_xyz), B, N, S,
-                                        _lib.ptr(out)))
+    ctx.call("cg_ball_query_dev", ctx.h, r2, int(nsample), xyz, new_xyz, B, N, S, out)
     return out.long()
 
 
 def sample_and_group(npoint, radius, nsample, xyz, points, returnfps=False, start_idx=None):
     """pointnet2.py:101-129."""
-    xyz = _f32(xyz)
-    ctx = _ctx(xyz)
+    ctx, xyz, pts = _f32(xyz, points)
     B, N, Cc = xyz.shape
     S = npoint
     fps_idx = farthest_point_sample(xyz, npoint, start_idx=start_idx)
@@ -88,10 +77,8 @@ def sample_and_group(npoint, radius, nsample, xyz, points, returnfps=False, star
     idx = query_ball_point(radius, nsample, xyz, new_xyz)
     idx32 = idx.to(torch.int32).contiguous()
     D = 0 if points is None else points.shape[-1]
-    pts = None if points is None else _f32(points)
     new_points = torch.empty((B, S, nsample, 3 + D), dtype=torch.float32, device=xyz.device)
-    ctx.check(ctx.lib.cg_group_points_dev(ctx.h, _lib.ptr(xyz), _lib.ptr(pts), _lib.ptr(new_xyz), _lib.ptr(idx32),
-                                          B, N, D, S, nsample, _lib.ptr(new_points)))
+    ctx.call("cg_group_points_dev", ctx.h, xyz, pts, new_xyz, idx32, B, N, D, S, nsample, new_points)
     if returnfps:
         grouped_xyz = index_points(xyz, idx)
         return new_xyz, new_points, grouped_xyz, fps_idx
@@ -126,13 +113,13 @@ class _SharedMLP:
         cw = (C.c_void_p * nlayers)(*[w.ctypes.data for w in Wts])
         cb = (C.c_void_p * nlayers)(*[b.ctypes.data for b in bs])
         h = C.c_void_p()
-        self.ctx.check(self.ctx.lib.cg_mlp_create(self.ctx.h, nlayers, cdims, cw, cb, C.byref(h)))
+        self.ctx.call("cg_mlp_create", self.ctx.h, nlayers, cdims, cw, cb, C.byref(h))
         self.h = h
 
     def __del__(self):
         try:
             if getattr(self, "h", None):
-                self.ctx.lib.cg_mlp_destroy(self.h)
+                self.ctx.call("cg_mlp_destroy", self.h)
                 self.h = None
         except Exception:
             pass
@@ -150,17 +137,15 @@ class PointNetSetAbstraction:
         assert self.mlp.dims[0] == in_channel and list(self.mlp.dims[1:]) == list(mlp), (self.mlp.dims, in_channel, mlp)
 
     def forward(self, xyz, points, start_idx=None):
-        xyz = _f32(xyz.permute(0, 2, 1))
-        pts = None if points is None else _f32(points.permute(0, 2, 1))
+        _, xyz, pts = _f32(xyz.permute(0, 2, 1), None if points is None else points.permute(0, 2, 1))
         if self.group_all:
             new_xyz, new_points = sample_and_group_all(xyz, pts)
         else:
             new_xyz, new_points = sample_and_group(self.npoint, self.radius, self.nsample, xyz, pts, start_idx=start_idx)
-        new_points = _f32(new_points)
+        new_points = new_points.to(torch.float32).contiguous()
         B, S, K, Cin = new_points.shape
-        ctx = _ctx(new_points)
         out = torch.empty((B, S, self.mlp.dims[-1]), dtype=torch.float32, device=xyz.device)
-        ctx.check(ctx.lib.cg_group_mlp_max_dev(self.mlp.h, _lib.ptr(new_points), B * S, K, _lib.ptr(out)))
+        self.mlp.ctx.call("cg_group_mlp_max_dev", self.mlp.h, new_points, B * S, K, out)
         return new_xyz.permute(0, 2, 1), out.permute(0, 2, 1)
 
     __call__ = forward
@@ -177,13 +162,11 @@ class PointNetFeaturePropagation:
         assert self.mlp.dims[0] == in_channel and list(self.mlp.dims[1:]) == list(mlp), (self.mlp.dims, in_channel, mlp)
 
     def forward(self, xyz1, xyz2, points1, points2, return_nn=False):
-        x1, x2 = _f32(xyz1.permute(0, 2, 1)), _f32(xyz2.permute(0, 2, 1))
-        p2 = _f32(points2.permute(0, 2, 1))
-        p1 = None if points1 is None else _f32(points1.permute(0, 2, 1))
+        ctx, x1, x2, p1, p2 = _f32(xyz1.permute(0, 2, 1), xyz2.permute(0, 2, 1),
+                                   None if points1 is None else points1.permute(0, 2, 1), points2.permute(0, 2, 1))
         B, N, _ = x1.shape
         S, D2 = p2.shape[1], p2.shape[2]
         D1 = 0 if p1 is None else p1.shape[2]
-        ctx = _ctx(x1)
         idx = w = None
         if S == 1:
             interp = p2.repeat(1, N, 1)
@@ -192,13 +175,12 @@ class PointNetFeaturePropagation:
             feat = torch.empty((B, N, D1 + D2), dtype=torch.float32, device=x1.device)
             idx = torch.empty((B, N, 3), dtype=torch.int32, device=x1.device)
             w = torch.empty((B, N, 3), dtype=torch.float32, device=x1.device)
-            ctx.check(ctx.lib.cg_three_interp_dev(ctx.h, _lib.ptr(x1), _lib.ptr(x2), _lib.ptr(p1), D1, _lib.ptr(p2), D2,
-                                                  B, N, S, _lib.ptr(feat), _lib.ptr(idx), _lib.ptr(w)))
+            ctx.call("cg_three_interp_dev", ctx.h, x1, x2, p1, D1, p2, D2, B, N, S, feat, idx, w)
             if S == 2:   # the module family's sort()[:, :, :3] of two columns: two neighbours
                 idx, w = idx[:, :, :2], w[:, :, :2]
         feat = feat.contiguous()
         out = torch.empty((B, N, self.mlp.dims[-1]), dtype=torch.float32, device=x1.device)
-        ctx.check(ctx.lib.cg_shared_mlp_dev(self.mlp.h, _lib.ptr(feat), B * N, _lib.ptr(out)))
+        self.mlp.ctx.call("cg_shared_mlp_dev", self.mlp.h, feat, B * N, out)
         out = out.permute(0, 2, 1)
         return (out, idx.long(), w) if return_nn else out
 

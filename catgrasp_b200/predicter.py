@@ -64,20 +64,15 @@ class _LegacyDraw:
         self.pos = C.c_int32(int(st[2]))
 
     def draw(self, M, n_pts, count, out=None, nthreads=0):
-        C = self._C
         if out is None:
             out = np.empty((count, n_pts), dtype=np.int32)
-        ptr = out.data_ptr() if hasattr(out, "data_ptr") else out.ctypes.data
-        rc = self._lib.cg_host_legacy_choice(C.c_void_p(self.key.ctypes.data), C.byref(self.pos), C.c_int64(M),
-                                             C.c_int32(n_pts), C.c_int32(count), C.c_void_p(ptr), C.c_int32(nthreads))
+        rc = self._lib.cg_host_legacy_choice(self.key, self._C.byref(self.pos), M, n_pts, count, out, nthreads)
         if rc != 0:
             raise ValueError(f"cg_host_legacy_choice({M}, {n_pts}, {count}) failed with {rc}")
         return out
 
     def skip(self, M, n_pts, count):
-        C = self._C
-        rc = self._lib.cg_host_legacy_skip(C.c_void_p(self.key.ctypes.data), C.byref(self.pos), C.c_int64(M),
-                                           C.c_int32(n_pts), C.c_int32(count))
+        rc = self._lib.cg_host_legacy_skip(self.key, self._C.byref(self.pos), M, n_pts, count)
         if rc != 0:
             raise ValueError(f"cg_host_legacy_skip({M}, {n_pts}, {count}) failed with {rc}")
 

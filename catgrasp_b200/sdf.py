@@ -17,17 +17,15 @@ class Sdf3D:
     def __init__(self, sdf_data, origin, resolution, device=None, ctx=None):
         self.data_ = np.ascontiguousarray(sdf_data, dtype=np.float32)
         assert self.data_.ndim == 3
-        self.origin_ = np.asarray(origin, dtype=np.float32).reshape(3)
+        self.origin_ = np.ascontiguousarray(origin, dtype=np.float32).reshape(3)
         self.resolution_ = float(np.float32(resolution))
         self.dims_ = np.array(self.data_.shape)
         # ``ctx``: a library context of its own (= its own stream and workspace) lets the collision filter run
         # concurrently with the networks of the per-device default context (bench.py does this)
         self.ctx = ctx if ctx is not None else _lib.Context.get(device)
         h = C.c_void_p()
-        org = (C.c_float * 3)(*[float(v) for v in self.origin_])
-        nx, ny, nz = self.data_.shape
-        self.ctx.check(self.ctx.lib.cg_sdf_create(self.ctx.h, _lib.ptr(self.data_), nx, ny, nz, org,
-                                                  C.c_float(self.resolution_), C.byref(h)))
+        self.ctx.call("cg_sdf_create", self.ctx.h, self.data_, *self.data_.shape, self.origin_, self.resolution_,
+                      C.byref(h))
         self.h = h
 
     @classmethod
@@ -49,17 +47,15 @@ class Sdf3D:
         self.ctx = ctx if ctx is not None else _lib.Context.get(device)
         self.h = None
         h = C.c_void_p()
-        self.ctx.use_own_stream()   # blocking host call
-        self.ctx.check(self.ctx.lib.cg_sdf_from_mesh(self.ctx.h, _lib.ptr(V), V.shape[0], _lib.ptr(F), F.shape[0],
-                                                     C.c_float(float(resolution)), int(padding), C.byref(h)))
+        self.ctx.call("cg_sdf_from_mesh", self.ctx.h, V, V.shape[0], F, F.shape[0], float(resolution), int(padding),
+                      C.byref(h))
         self.h = h
-        dims = (C.c_int * 3)()
-        org = (C.c_float * 3)()
+        dims = np.empty(3, np.int32)
+        self.origin_ = np.empty(3, np.float32)
         res = C.c_float()
-        self.ctx.check(self.ctx.lib.cg_sdf_geometry(self.h, dims, org, C.byref(res)))
-        self.data_ = np.empty((dims[0], dims[1], dims[2]), np.float32)
-        self.ctx.check(self.ctx.lib.cg_sdf_download(self.h, _lib.ptr(self.data_)))
-        self.origin_ = np.array(org[:], dtype=np.float32)
+        self.ctx.call("cg_sdf_geometry", self.h, dims, self.origin_, C.byref(res))
+        self.data_ = np.empty(tuple(dims), np.float32)
+        self.ctx.call("cg_sdf_download", self.h, self.data_)
         self.resolution_ = float(res.value)
         self.dims_ = np.array(self.data_.shape)
         return self
@@ -67,19 +63,17 @@ class Sdf3D:
     def __del__(self):
         try:
             if getattr(self, "h", None):
-                self.ctx.lib.cg_sdf_destroy(self.h)
+                self.ctx.call("cg_sdf_destroy", self.h)
                 self.h = None
         except Exception:
             pass
 
     def _lookup(self, coords, mode):
-        dev = torch.device("cuda", self.ctx.device)
-        c = torch.as_tensor(coords).to(device=dev, dtype=torch.float32)
+        _, c = _lib.inputs(coords, dtype=torch.float32, ctx=self.ctx)
         c = c.reshape(3, -1).t().contiguous()          # reference passes (3,N)
         P = c.shape[0]
-        out = torch.empty((P,), dtype=torch.float32, device=dev)
-        self.ctx.use_torch_stream()
-        self.ctx.check(self.ctx.lib.cg_sdf_lookup_dev(self.h, _lib.ptr(c), P, mode, _lib.ptr(out)))
+        out = torch.empty((P,), dtype=torch.float32, device=c.device)
+        self.ctx.call("cg_sdf_lookup_dev", self.h, c, P, mode, out)
         return out
 
     def _signed_distance(self, coords, fast=False):

@@ -1,19 +1,18 @@
 """Clustering of the segmentation's shifted points on the device (csrc/cg_meanshift.cu): sklearn's MeanShift as
 PointGroupPredictor.predict uses it (predicter.py:332), and the label propagation around it (:308-338).
 
-Follows the cloud.py convention: numpy in, numpy out; CUDA tensor in, CUDA tensor out.  Centres keep X's dtype
-(float32 or float64); labels are int64.  Labels are the nearest kept centre in float64 d2, ties to the smaller centre
-index.  Centres are summed in int64 fixed point, so they do not depend on the order of X's rows; sklearn's own
-centres move by a few float32 ulps when the rows are permuted, its labels do not.
+Numpy in, numpy out; CUDA tensor in, CUDA tensor out (see _lib).  Centres keep X's dtype (float32 or float64); labels
+are int64.  Labels are the nearest kept centre in float64 d2, ties to the smaller centre index.  Centres are summed in
+int64 fixed point, so they do not depend on the order of X's rows; sklearn's own centres move by a few float32 ulps
+when the rows are permuted, its labels do not.
 """
-import ctypes as C
 import numbers
 
 import numpy as np
 import torch
 
 from . import _lib
-from .cloud import CloudIndex, _ctx, _dev, _device_of, _out, _query_cell
+from .cloud import CloudIndex, _query_cell
 
 MEANSHIFT_BANDWIDTH = {"hnm": 0.005, "nut": 0.007, "screw": 0.009}   # predicter.py:317-330
 DOWNSAMPLE = 0.002                                                     # predicter.py:309
@@ -93,31 +92,22 @@ class MeanShift:
     def fit(self, X, y=None):
         self._check_params()
         X = _as_points(X)
-        like = isinstance(X, torch.Tensor)
-        device = _device_of(X)
-        ctx = _ctx(device)
         f64 = X.dtype in (torch.float64, np.float64)
-        x = _dev(X, torch.float64 if f64 else torch.float32, device)
+        ctx, x = _lib.inputs(X, dtype=torch.float64 if f64 else torch.float32)
         bw = float(self.bandwidth)
-        index = CloudIndex(x, bw, device)
+        index = CloudIndex(x, bw)
         P = x.shape[0]
         seed_c = torch.empty_like(x)
         seed_n = torch.empty((P,), dtype=torch.int32, device=x.device)
         seed_it = torch.empty_like(seed_n)
         cen = torch.empty_like(x)
         nc = torch.empty((1,), dtype=torch.int32, device=x.device)
-        ctx.use_torch_stream()
-        ctx.check(ctx.lib.cg_meanshift_dev(index.h, _lib.ptr(x), int(f64), C.c_double(bw), int(self.max_iter),
-                                           _lib.ptr(seed_c), _lib.ptr(seed_n), _lib.ptr(seed_it), _lib.ptr(cen),
-                                           _lib.ptr(nc)))
+        ctx.call("cg_meanshift_dev", index.h, x, int(f64), bw, int(self.max_iter), seed_c, seed_n, seed_it, cen, nc)
         centres = cen[:int(nc.item())].contiguous()
         labels = _nearest(centres.to(torch.float64), x.to(torch.float64), LABEL_REACH * bw)
         self.n_iter_ = int(seed_it.max().item())
-        self.cluster_centers_ = _out(centres, like)
-        self.labels_ = _out(labels, like)
-        self.seed_centers_ = _out(seed_c, like)
-        self.seed_counts_ = _out(seed_n.to(torch.int64), like)
-        self.seed_iters_ = _out(seed_it.to(torch.int64), like)
+        (self.cluster_centers_, self.labels_, self.seed_centers_, self.seed_counts_,
+         self.seed_iters_) = _lib.returned(X, centres, labels, seed_c, seed_n.to(torch.int64), seed_it.to(torch.int64))
         return self
 
     def fit_predict(self, X, y=None):
@@ -129,26 +119,22 @@ def pointgroup_labels(xyz_original_all, pt_offsets, cloud_xyz, bandwidth):
     snapped to its nearest point, those points moved by their offsets (float32), clustered by MeanShift, and every
     point of cloud_xyz labelled with its nearest snapped point's cluster.  Returns (labels_all (M,) int64,
     xyz_shifted (U,3) float32)."""
-    like = isinstance(xyz_original_all, torch.Tensor)
     xo = _as_points(xyz_original_all)
     off = _as_points(pt_offsets)
     cloud = _as_points(cloud_xyz)
     if off.shape[0] != xo.shape[0]:
         raise ValueError("pt_offsets must have one row per point of xyz_original_all")
-    device = _device_of(xo, off, cloud)
-    _ctx(device)
-    xo = _dev(xo, torch.float32, device)
-    off = _dev(off, torch.float32, device)
-    down, _ = CloudIndex(xo, DOWNSAMPLE, device).voxel_means()                          # :308-310
+    _, xo_d, off, cloud = _lib.inputs(xo, off, cloud, dtype=(torch.float32, torch.float32, torch.float64))
+    down, _ = CloudIndex(xo_d, DOWNSAMPLE).voxel_means()                                # :308-310
     # :311-313 snap: a voxel mean and its members share a voxel, so the nearest member is within the diagonal; the
     # bound is widened by 1e-9 relative so rounding at a voxel face cannot exclude it
     snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)
-    _, ids = CloudIndex(xo, snap, device).nearest(down, snap)
+    _, ids = CloudIndex(xo_d, snap).nearest(down, snap)
     if bool((ids < 0).any()):
         raise _lib.CgError("pointgroup_labels: a voxel mean has no point within its voxel's diagonal")
     ids = ids.to(torch.int64)
-    xyz_down = xo[ids]
+    xyz_down = xo_d[ids]
     xyz_shifted = xyz_down + off[ids]                                                    # :314, float32
     labels = MeanShift(bandwidth=bandwidth).fit_predict(xyz_shifted)                      # :332
-    nearest = _nearest(xyz_down.to(torch.float64), _dev(cloud, torch.float64, device), LABEL_REACH * DOWNSAMPLE)
-    return _out(labels[nearest], like), _out(xyz_shifted, like)                           # :334-336
+    nearest = _nearest(xyz_down.to(torch.float64), cloud, LABEL_REACH * DOWNSAMPLE)
+    return _lib.returned(xyz_original_all, labels[nearest], xyz_shifted)                 # :334-336

@@ -12,8 +12,10 @@
  *            itself on the context stream and returns after the result is in
  *            the host output buffer (the reference-facing, blocking call).
  *   *_dev  : all data pointers are DEVICE pointers owned by the caller
- *            (e.g. torch allocations); the call enqueues work on the context
- *            stream and returns without synchronising.
+ *            (e.g. torch allocations), except parameters marked host; the
+ *            call enqueues work on the context stream and returns without
+ *            synchronising.
+ * A parameter marked host or device is read there whatever the entry's name.
  * Row-major everywhere.  Poses are 4x4 row-major.
  */
 #ifndef CATGRASP_B200_H
@@ -268,7 +270,7 @@ int cg_filter_grasp_pose_host(cg_ctx *ctx, const cg_filter_params *prm,
                               cg_sdf *sdf_open, const float *open_pts, int P1,
                               cg_sdf *sdf_enclosed, const float *enclosed_pts, int P2,
                               uint8_t *out_status, int8_t *out_offset, float *out_poses);
-int cg_filter_grasp_pose_dev(cg_ctx *ctx, const cg_filter_params *prm,
+int cg_filter_grasp_pose_dev(cg_ctx *ctx, const cg_filter_params *prm /* host */,
                              const float *grasp_poses, int G,
                              const float *symmetry_tfs, int S,
                              cg_sdf *sdf_open, const float *open_pts, int P1,
@@ -304,12 +306,12 @@ typedef struct cg_ik_params {
   double lower[7];
 } cg_ik_params;
 int cg_iiwa14_ik_dev(cg_ctx *ctx, const float *ee_in_base, int Q,
-                     const double upper[7], const double lower[7],
+                     const double upper[7] /* host */, const double lower[7] /* host */,
                      int8_t *out_count, double *out_solutions);
-int cg_filter_apply_ik_dev(cg_ctx *ctx, const cg_filter_params *prm,
+int cg_filter_apply_ik_dev(cg_ctx *ctx, const cg_filter_params *prm /* host */,
                            const float *grasp_poses, int G,
                            const float *symmetry_tfs, int S,
-                           const cg_ik_params *ik,
+                           const cg_ik_params *ik /* host */,
                            uint8_t *status, int8_t *offset, float *out_poses);
 
 /* ---- occupancy / occlusion grid from a depth scan ----------------------------
@@ -366,7 +368,8 @@ int cg_center_grasps_dev(cg_ctx *ctx, double *poses64, float *poses32, int P, co
  *   out_p (G) = p(T|G), NaN where the reference drops the grasp; out_contacts (G,4) = contact-patch sizes per finger
  *   (0 for a dropped finger).                                                                                          */
 int cg_grasp_affordance_dev(cg_ctx *ctx, const double *cam_in_finger, int G, const double *pts, const double *nrm,
-                            const double *affordance, int P, const double *finger_boxes, const int *grip_dirs, int F,
+                            const double *affordance, int P, const double *finger_boxes /* host */,
+                            const int *grip_dirs /* host */, int F,
                             double surface_tol, double *out_p, int *out_contacts);
 
 /* ---- point-cloud preparation ---- */
@@ -380,12 +383,13 @@ typedef struct cg_cloud_index cg_cloud_index;
 /* depth (H,W) float32 (depth_is_f64 = 0) or float64 -> out_xyz (H,W,3) float32: x = (u - K[2]) * z / K[0],
  * y = (v - K[5]) * z / K[4] in float64 left to right, then narrowed; depth < 0.1 in the depth's own type gives
  * (0,0,0).  K is a host array of 9 doubles (row-major 3x3).                                                        */
-int cg_depth2xyz_dev(cg_ctx *ctx, const void *depth, int depth_is_f64, int H, int W, const double *K, float *out_xyz);
+int cg_depth2xyz_dev(cg_ctx *ctx, const void *depth, int depth_is_f64, int H, int W, const double *K /* host */,
+                     float *out_xyz);
 /* Bins pts (P,3) into cells of size `cell` with origin min_bound - cell/2 (cell = floor((p - origin) / cell)), sorts
  * the points by (cell, index) and builds the ascending cell table.  The index copies the points, so pts may be freed
  * afterwards.  Synchronises the context's stream twice (the bounds, then the cell count).  Fails with CG_EINVAL on a
  * non-finite coordinate or when the cloud spans 2^21 or more cells on an axis.                                     */
-int  cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, double cell, cg_cloud_index **out);
+int  cg_cloud_index_create(cg_ctx *ctx, const double *pts /* device */, int P, double cell, cg_cloud_index **out);
 void cg_cloud_index_destroy(cg_cloud_index *index);
 /* P, number of occupied cells (= the voxel count of cg_voxel_down_sample_dev), cell size, origin[3]; any may be NULL */
 int  cg_cloud_index_info(const cg_cloud_index *index, int *out_points, int *out_cells, double *out_cell, double *out_origin);
@@ -408,7 +412,7 @@ int  cg_cloud_radius_mask_dev(const cg_cloud_index *index, const double *query, 
  * view_point (host double[3]) exactly as correct_pcd_normal_direction does (n / (|n| + 1e-10), flipped when the dot
  * product with the unit view direction is < 0).  out_normals (P,3) in the caller's point order; out_nbr (P,max_nn)
  * int32 (neighbours in order, -1 padded) and out_nbr_count (P) may be NULL.                                      */
-int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point,
+int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point /* host */,
                           double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count);
 
 /* ---- mean-shift clustering ---- */
