@@ -151,6 +151,9 @@ SIGNATURES = {
     "cg_cloud_radius_mask_dev": (_i, [_vp, _D, _i, _d, _i, _D], TORCH),
     "cg_cloud_normals_dev": (_i, [_vp, _d, _i, _H, _D, _D, _D], TORCH),
     "cg_meanshift_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
+    "cg_spconv_index_dev": (_i, [_vp, _D, _i, _D, _D, _D, _D], TORCH),
+    "cg_spconv_down_dev": (_i, [_vp, _D, _D, _i, _H, _i, _D, _D, _D, _D, _D], TORCH),
+    "cg_spconv_conv_dev": (_i, [_vp, _D, _i, _D, _i, _D, _i, _D, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_square_distance_dev": (_i, [_vp, _D, _D, _i, _i, _i, _D], TORCH),
     "cg_index_points_dev": (_i, [_vp, _D, _D, _i, _i, _i, _i, _D], TORCH),
     "cg_fps_dev": (_i, [_vp, _D, _i, _i, _i, _D, _D], TORCH),

@@ -430,6 +430,35 @@ int  cg_meanshift_dev(const cg_cloud_index *index, const void *X, int x_is_f64, 
                       void *out_seed_centres, int32_t *out_seed_counts, int32_t *out_seed_iters, void *out_centres,
                       int32_t *out_n_centres);
 
+/* ---- sparse 3-D convolution (spconv 1.x semantics; cg_spconv.cu) ----
+ * The layer types of PointGroup's U-Net (PointGroup/model/pointgroup/pointgroup.py): SubMConv3d k3 and k1,
+ * SparseConv3d k2 s2 and SparseInverseConv3d k2.  A level is a set of distinct sites (x, y, z), each in [0, 2^21), in
+ * ascending (x, y, z) order, z fastest.  Rows are int32 indices into a level; -1 is "absent".  Every output is sized
+ * from a row bound the caller gives; the true count is written to a device word, and no entry synchronises.        */
+/* coords (N,3) int32, each in [0, 2^21) (not checked) -> the level of its distinct sites: out_vox (N,3 capacity),
+ * out_nvox (1) = V, out_p2v (N) = each point's site, out_nbr (N,27): for site v < V and k = 9 kx + 3 ky + kz the site
+ * v + (kx-1, ky-1, kz-1) or -1; rows from V on are -1.                                                            */
+int  cg_spconv_index_dev(cg_ctx *ctx, const int32_t *coords, int N, int32_t *out_vox, int32_t *out_nvox,
+                         int32_t *out_p2v, int32_t *out_nbr);
+/* The coarser level of a level with *nvox sites (rows of vox, M >= *nvox) on the spatial shape shape[3] (host): the
+ * parents c >> 1 of the sites whose parent index is below (S - 2) / 2 + 1 on every axis (an odd axis drops its last
+ * plane).  out_rows bounds the parents: at least min(M, the coarse shape's cell count), else CG_EINVAL.  out_vox
+ * (out_rows,3 capacity), out_nvox (1) and out_nbr (out_rows,27) as cg_spconv_index_dev gives them for the parents;
+ * out_down (out_rows,8): for parent p and k = 4 kx + 2 ky + kz the child 2 p + (kx, ky, kz) or -1; out_up (M,8): for
+ * child c the parent at k = c - 2 parent(c) and -1 at the other seven (all eight -1 for a dropped child).          */
+int  cg_spconv_down_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *nvox, int M, const int32_t *shape /* host */,
+                        int out_rows, int32_t *out_vox, int32_t *out_nvox, int32_t *out_nbr, int32_t *out_down,
+                        int32_t *out_up);
+/* out (M,Cout) rows r < *nout: (sum over k, then input channel, of W[k][ci][co] * act(in[nbr[r][k]][ci]) + bias[co])
+ * + residual[r][co], one fp32 FMA chain per output, so two runs are bitwise equal.  in (rows,Cin); nbr (M,K), or NULL
+ * with K = 1 for the 1x1 convolution (row r reads row r); W (K,Cin,Cout) as spconv stores (k..., Cin, Cout).  act(v) =
+ * max(v * bn_scale[ci] + bn_shift[ci], 0) when both are given (the BN + ReLU before a conv), else v; an absent row
+ * contributes nothing.  bias (Cout) and residual (M,Cout) may be NULL.  Rows from min(*nout, M) on are not written.
+ * Every index in the first min(*nout, M) rows of nbr must be a row of in (not checked).                          */
+int  cg_spconv_conv_dev(cg_ctx *ctx, const float *in, int Cin, const int32_t *nbr, int K, const int32_t *nout, int M,
+                        const float *W, int Cout, const float *bn_scale, const float *bn_shift, const float *bias,
+                        const float *residual, float *out);
+
 /* ---- PointNet++ primitives (device pointers) ---------------------------
  * Replace the free functions of pointnet2.py:14-149.  Indices are int32 on
  * the device (the Python mirror widens to int64 like the reference).        */
