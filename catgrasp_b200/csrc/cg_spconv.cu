@@ -246,6 +246,80 @@ __global__ void __launch_bounds__(CT_THREADS) spconv_kernel(
   }
 }
 
+// ---- PointGroup's voxelisation (pointgroup_ops mode 4) and offset head around the U-Net ----
+
+// each point's site as a sort key; a point naming no site below *nvox sorts last as ~0u
+__global__ void site_key_kernel(const int32_t *__restrict__ p2v, int N, const int32_t *__restrict__ nvox, int V,
+                                uint32_t *__restrict__ key, int32_t *__restrict__ val) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int v = p2v[i];
+  key[i] = v >= 0 && v < min(*nvox, V) ? (uint32_t)v : ~0u;
+  val[i] = i;
+}
+
+// the sorted keys' runs: site v's points are sorted positions [first[v], last[v]); both were set to 0 before
+__global__ void site_run_kernel(const uint32_t *__restrict__ key, int N, int32_t *__restrict__ first,
+                                int32_t *__restrict__ last) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N || key[j] == ~0u) return;
+  if (j == 0 || key[j - 1] != key[j]) first[key[j]] = j;
+  if (j == N - 1 || key[j + 1] != key[j]) last[key[j]] = j + 1;
+}
+
+// one thread per (site, channel): out = 0; for each point in ascending index out = fl(out + fl(fl(1/n) * x)), the
+// arithmetic of voxelize_fp_cuda_ with average = true, whose atomicAdd rules out a fused multiply-add
+__global__ void voxel_mean_kernel(const float *__restrict__ feats, int C, const int32_t *__restrict__ perm,
+                                  const int32_t *__restrict__ first, const int32_t *__restrict__ last,
+                                  const int32_t *__restrict__ nvox, int V, float *__restrict__ out) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)min(*nvox, V) * C) return;
+  const int v = (int)(t / C), c = (int)(t % C);
+  const int b = first[v], e = last[v];
+  const float mult = e > b ? __fdiv_rn(1.f, (float)(e - b)) : 1.f;
+  float acc = 0.f;
+  for (int j = b; j < e; j++) acc = __fadd_rn(acc, __fmul_rn(mult, feats[(size_t)perm[j] * C + c]));
+  out[t] = acc;
+}
+
+constexpr int HD_WARPS = 8;   // offset head: sites (one warp each) per CTA
+
+// one warp per site: a = ReLU(x * s0 + t0) (output_layer), h = ReLU(W1^T a + b1) (Linear with its BN folded in),
+// out = W2^T h + b2; each output one fp32 FMA chain over the input channels ascending, then the bias
+__global__ void __launch_bounds__(HD_WARPS * 32) offset_head_kernel(
+    const float *__restrict__ in, int m, const int32_t *__restrict__ nvox, int V, const float *__restrict__ s0,
+    const float *__restrict__ t0, const float *__restrict__ W1, const float *__restrict__ b1,
+    const float *__restrict__ W2, const float *__restrict__ b2, float *__restrict__ out) {
+  extern __shared__ float hd_sh[];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int v = blockIdx.x * HD_WARPS + w;
+  if (v >= min(*nvox, V)) return;   // the whole warp leaves together
+  float *a = hd_sh + (size_t)w * 2 * m, *h = a + m;
+  for (int c = lane; c < m; c += 32) a[c] = fmaxf(fmaf(in[(size_t)v * m + c], s0[c], t0[c]), 0.f);
+  __syncwarp();
+  for (int o = lane; o < m; o += 32) {
+    float acc = 0.f;
+    for (int c = 0; c < m; c++) acc = fmaf(a[c], W1[(size_t)c * m + o], acc);
+    h[o] = fmaxf(__fadd_rn(acc, b1[o]), 0.f);
+  }
+  __syncwarp();
+  if (lane < 3) {
+    float acc = 0.f;
+    for (int c = 0; c < m; c++) acc = fmaf(h[c], W2[3 * c + lane], acc);
+    out[3 * (size_t)v + lane] = __fadd_rn(acc, b2[lane]);
+  }
+}
+
+// out[i] = site[p2v[i]] (3 floats), NaN for a point naming no site below *nvox
+__global__ void gather3_kernel(const float *__restrict__ site, const int32_t *__restrict__ p2v, int N,
+                               const int32_t *__restrict__ nvox, int V, float *__restrict__ out) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= 3 * (int64_t)N) return;
+  const int i = (int)(t / 3), j = (int)(t % 3);
+  const int v = p2v[i];
+  out[t] = v >= 0 && v < min(*nvox, V) ? site[3 * (size_t)v + j] : __int_as_float(0x7fc00000);
+}
+
 }  // namespace
 
 extern "C" int cg_spconv_index_dev(cg_ctx *ctx, const int32_t *coords, int N, int32_t *out_vox, int32_t *out_nvox,
@@ -321,6 +395,65 @@ extern "C" int cg_spconv_conv_dev(cg_ctx *ctx, const float *in, int Cin, const i
   auto kernel = nj == 1 ? spconv_kernel<1> : nj == 2 ? spconv_kernel<2> : spconv_kernel<4>;
   kernel<<<grid, CT_THREADS, 0, ctx->stream>>>(in, Cin, nbr, K, nout, M, W, Cout, bn_scale, bn_shift, bias, residual,
                                                out);
+  CG_LAUNCH_CHECK(ctx);
+  return CG_OK;
+}
+
+extern "C" int cg_pointgroup_voxel_mean_dev(cg_ctx *ctx, const float *feats, int N, int C, const int32_t *p2v,
+                                            const int32_t *nvox, int V, float *out) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, N >= 1 && C >= 1 && V >= 1, "pointgroup_voxel_mean: N, C and V must be >= 1");
+  CG_REQUIRE(ctx, (int64_t)V * C < ((int64_t)1 << 40) && (int64_t)N * C < ((int64_t)1 << 40),
+             "pointgroup_voxel_mean: features too large");
+  CG_REQUIRE(ctx, feats && p2v && nvox && out, "pointgroup_voxel_mean: null argument");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  size_t sort_tmp = 0;
+  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (uint32_t *)nullptr, (uint32_t *)nullptr,
+                                               (int32_t *)nullptr, (int32_t *)nullptr, N, 0, 32, st));
+  uint32_t *kA, *kB;
+  int32_t *rA, *rB, *first, *last;
+  void *tmp;
+  const size_t Nz = (size_t)N, Vz = (size_t)V;
+  const int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    kA = ar.take<uint32_t>(Nz); kB = ar.take<uint32_t>(Nz);
+    rA = ar.take<int32_t>(Nz); rB = ar.take<int32_t>(Nz);
+    first = ar.take<int32_t>(Vz); last = ar.take<int32_t>(Vz);
+    tmp = ar.take<char>(sort_tmp);
+  });
+  if (rc != CG_OK) return rc;
+  site_key_kernel<<<blocks(N, 256), 256, 0, st>>>(p2v, N, nvox, V, kA, rA);
+  CG_LAUNCH_CHECK(ctx);
+  // a stable sort: each site's points stay in ascending index order
+  size_t tb = sort_tmp;
+  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp, tb, kA, kB, rA, rB, N, 0, 32, st));
+  CG_CUDA(ctx, cudaMemsetAsync(first, 0, sizeof(int32_t) * Vz, st));
+  CG_CUDA(ctx, cudaMemsetAsync(last, 0, sizeof(int32_t) * Vz, st));
+  site_run_kernel<<<blocks(N, 256), 256, 0, st>>>(kB, N, first, last);
+  CG_LAUNCH_CHECK(ctx);
+  voxel_mean_kernel<<<blocks((int64_t)V * C, 256), 256, 0, st>>>(feats, C, rB, first, last, nvox, V, out);
+  CG_LAUNCH_CHECK(ctx);
+  return CG_OK;
+}
+
+extern "C" int cg_pointgroup_head_dev(cg_ctx *ctx, const float *in, int m, const int32_t *nvox, int V,
+                                      const float *bn_scale, const float *bn_shift, const float *W1, const float *b1,
+                                      const float *W2, const float *b2, const int32_t *p2v, int N, float *out_site,
+                                      float *out) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, m >= 1 && m <= 512, "pointgroup_head: m must be in [1, 512]");
+  CG_REQUIRE(ctx, V >= 1 && N >= 1 && (int64_t)V * m < ((int64_t)1 << 40), "pointgroup_head: V and N must be >= 1");
+  CG_REQUIRE(ctx, in && nvox && bn_scale && bn_shift && W1 && b1 && W2 && b2 && p2v && out_site && out,
+             "pointgroup_head: null argument");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t shm = sizeof(float) * HD_WARPS * 2 * (size_t)m;
+  if (shm > 48 * 1024)
+    CG_CUDA(ctx, cudaFuncSetAttribute(offset_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm));
+  offset_head_kernel<<<blocks(V, HD_WARPS), HD_WARPS * 32, shm, st>>>(in, m, nvox, V, bn_scale, bn_shift, W1, b1, W2,
+                                                                      b2, out_site);
+  CG_LAUNCH_CHECK(ctx);
+  gather3_kernel<<<blocks(3 * (int64_t)N, 256), 256, 0, st>>>(out_site, p2v, N, nvox, V, out);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
 }

@@ -376,3 +376,108 @@ class NunocsPredicter:
         self.nocs_pose = transform.copy()
         nocs_cloud = (best_symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
         return nocs_cloud, transform
+
+
+def flatten_config(cfg, out=None):
+    """PointGroup/util/config.py key_to_attr: every leaf of the nested config sections as one flat dict (a later
+    section's key overwrites an earlier one's, as setattr does)."""
+    out = {} if out is None else out
+    for k, v in cfg.items():
+        if isinstance(v, dict):
+            flatten_config(v, out)
+        else:
+            out[k] = v
+    return out
+
+
+def slice_keep_mask(xyz):
+    """predicter.py:246-249 with n_slice_per_side = 1, in the input's dtype as the reference writes it: in float32
+    xmin + (xmax - xmin) can round below xmax, and a point at xmax is then dropped."""
+    x, y = xyz[:, 0], xyz[:, 1]
+    xmin, xmax, ymin, ymax = x.min(), x.max(), y.min(), y.max()
+    xlen, ylen = (xmax - xmin) / 1, (ymax - ymin) / 1
+    return (x >= xmin) & (x <= xmin + xlen) & (y >= ymin) & (y <= ymin + ylen)
+
+
+class PointGroupPredictor:
+    """predicter.py:206-338: the segmentation of a pile into instances.  The host front runs in numpy and on the
+    device's cloud kernels, the network (voxelisation, U-Net, offset head) on the device (catgrasp_b200.pointgroup),
+    the clustering after it in segment.pointgroup_labels.  Only the shipped structure is implemented: mode 4,
+    use_coords, residual blocks, input_channel 3 and n_slice_per_side 1; any m and block_reps 1 or 2."""
+
+    class_name_to_artifact_id = {"nut": 40, "hnm": 68, "screw": 77}
+
+    def __init__(self, class_name, artifact_dir=None, device=None):
+        from .pointgroup import PointGroupNet
+        from .segment import MEANSHIFT_BANDWIDTH
+        if class_name not in MEANSHIFT_BANDWIDTH:
+            raise NotImplementedError(f"PointGroupPredictor: no clustering bandwidth for class {class_name!r}")
+        self.class_name = class_name
+        if artifact_dir is None:
+            artifact_dir = f"{_CODE_DIR}/artifacts/artifacts-{self.class_name_to_artifact_id[class_name]}"
+        print("PointGroupPredictor artifact_dir", artifact_dir)
+        with open(f"{artifact_dir}/config_pointgroup.yaml", "r") as ff:
+            self.cfg = yaml.safe_load(ff)
+        self.cfg_pg = flatten_config(self.cfg)
+        self.n_slice_per_side = 1
+        self._check_structure()
+        sd = load_checkpoint(f"{artifact_dir}/best_val.pth.tar")
+        self.model = PointGroupNet(sd, int(self.cfg_pg["m"]), int(self.cfg_pg["block_reps"]), device=device)
+
+    def _check_structure(self):
+        c = self.cfg_pg
+        for key, want in (("mode", 4), ("use_coords", True), ("block_residual", True), ("input_channel", 3)):
+            if c.get(key) != want:
+                raise NotImplementedError(f"PointGroupPredictor: {key} = {c.get(key)!r}; only the shipped {key} = "
+                                          f"{want!r} is implemented")
+        if self.n_slice_per_side != 1:
+            raise NotImplementedError("PointGroupPredictor: n_slice_per_side must be 1 (the site tables hold one "
+                                      "batch)")
+        if int(c["block_reps"]) not in (1, 2):
+            raise NotImplementedError(f"PointGroupPredictor: block_reps = {c['block_reps']}; only 1 and 2 build")
+
+    def host_front(self, data):
+        """predicter.py:234-300 with n_slice_per_side = 1: (xyz_original_all (N,3) float32, locs (N,3) int64,
+        feats (N,6) float32, spatial_shape (3 ints)), numpy."""
+        import torch
+        from .cloud import CloudIndex
+        from . import _lib
+        self._check_structure()
+        xyz, nrm = np.asarray(data["cloud_xyz"]), np.asarray(data["cloud_normal"])
+        keep = slice_keep_mask(xyz)
+        xo, no = xyz[keep], nrm[keep]
+        ds = float(self.cfg["downsample_size"])
+        dev = self.model.ctx.device
+        down, _ = CloudIndex(xo, ds, dev).voxel_means()
+        # the snap (cKDTree.query): a voxel mean and its members share a voxel, so the nearest member is within the
+        # diagonal, widened by 1e-9 relative against rounding at a voxel face
+        snap = ds * np.sqrt(3.0) * (1 + 1e-9)
+        _, ids = CloudIndex(xo, snap, dev).nearest(down, snap)
+        ids = ids.cpu().numpy()
+        if (ids < 0).any():
+            raise _lib.CgError("PointGroupPredictor: a voxel mean has no point within its voxel's diagonal")
+        xo, no = xo[ids], no[ids]
+        s = xo * self.cfg_pg["scale"]
+        s -= s.min(0)
+        locs = torch.from_numpy(s).long().numpy()
+        shape = tuple(int(v) for v in np.maximum(locs.max(0) + 1, int(self.cfg_pg["full_scale"][0])))
+        feats = np.concatenate([no.astype(np.float32), xo.astype(np.float32)], 1)
+        return xo.astype(np.float32), locs, feats, shape
+
+    def offsets(self, data):
+        """The host front and the network: (xyz_original_all (N,3) float32 numpy, pt_offsets (N,3) float32 CUDA)."""
+        import torch
+        from . import spconv
+        xo, locs, feats, shape = self.host_front(data)
+        dev = self.model.device
+        level, p2v = spconv.index(torch.from_numpy(locs).to(dev), shape)
+        return xo, self.model.offsets(level, p2v, torch.from_numpy(feats).to(dev))
+
+    def predict(self, data):
+        """predicter.py:232-338: labels_all (M,) int64, one per point of data['cloud_xyz']; sets self.xyz_shifted."""
+        from .segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
+        xo, off = self.offsets(data)
+        labels_all, xyz_shifted = pointgroup_labels(xo, off.cpu().numpy(), data["cloud_xyz"],
+                                                    MEANSHIFT_BANDWIDTH[self.class_name])
+        self.xyz_shifted = xyz_shifted
+        return labels_all

@@ -154,3 +154,130 @@ def pack_blob(sd, kind):
     else:
         raise ValueError(kind)
     return np.concatenate(parts).astype(np.float32), int(n_out)
+
+
+# ---- PointGroup (PointGroup/model/pointgroup/pointgroup.py) ----
+# spconv 1.x stores a convolution's weight as (k, k, k, Cin, Cout).  Every BatchNorm1d sits in front of a convolution
+# (BN, ReLU, conv), so it cannot be folded into the conv's weights; it is kept as a per-channel (scale, shift), which
+# the conv kernel applies to present rows only.  The offset head's BN follows its first Linear and is folded into it.
+
+PG_INPUT_C = 6          # normals + coordinates (input_channel 3, use_coords)
+PG_LEVELS = 7           # UBlock([m, 2m, ..., 7m])
+
+
+def _pg_bn(keys, p, C):
+    for s in (".weight", ".bias", ".running_mean", ".running_var"):
+        keys[p + s] = (C,)
+
+
+def _pg_conv(keys, p, k, cin, cout):
+    keys[p + ".weight"] = (k, k, k, cin, cout)
+    keys[p + ".bias"] = (cout,)
+
+
+def _pg_resblock(keys, p, cin, cout):
+    if cin != cout:
+        _pg_conv(keys, p + "i_branch.0", 1, cin, cout)
+    _pg_bn(keys, p + "conv_branch.0", cin)
+    _pg_conv(keys, p + "conv_branch.2", 3, cin, cout)
+    _pg_bn(keys, p + "conv_branch.3", cout)
+    _pg_conv(keys, p + "conv_branch.5", 3, cout, cout)
+
+
+def _pg_ublock(keys, p, planes, reps):
+    for i in range(reps):
+        _pg_resblock(keys, f"{p}blocks.block{i}.", planes[0], planes[0])
+    if len(planes) > 1:
+        _pg_bn(keys, p + "conv.0", planes[0])
+        _pg_conv(keys, p + "conv.2", 2, planes[0], planes[1])
+        _pg_ublock(keys, p + "u.", planes[1:], reps)
+        _pg_bn(keys, p + "deconv.0", planes[1])
+        _pg_conv(keys, p + "deconv.2", 2, planes[1], planes[0])
+        for i in range(reps):
+            _pg_resblock(keys, f"{p}blocks_tail.block{i}.", planes[0] * (2 - i), planes[0])
+
+
+def pointgroup_keys(m, block_reps):
+    """The parameter and buffer names of PointGroup(m, block_reps) with residual blocks and use_coords, and their
+    shapes, in module order (num_batches_tracked left out).  The score branch's keys are included: the reference
+    loads strictly, although inference never runs that branch."""
+    keys = OrderedDict()
+    _pg_conv(keys, "input_conv.0", 3, PG_INPUT_C, m)
+    _pg_ublock(keys, "unet.", [m * (i + 1) for i in range(PG_LEVELS)], block_reps)
+    _pg_bn(keys, "output_layer.0", m)
+    keys["offset.0.weight"], keys["offset.0.bias"] = (m, m), (m,)
+    _pg_bn(keys, "offset.1", m)
+    keys["offset.3.weight"], keys["offset.3.bias"] = (3, m), (3,)
+    _pg_ublock(keys, "score_unet.", [m, 2 * m], 2)
+    _pg_bn(keys, "score_outputlayer.0", m)
+    keys["score_linear.weight"], keys["score_linear.bias"] = (1, m), (1,)
+    return keys
+
+
+def check_pointgroup_state_dict(sd, m, block_reps):
+    """Strict check of a PointGroup state_dict: raises RuntimeError naming the missing or unexpected keys, or
+    ValueError naming the first key whose shape is wrong."""
+    want = pointgroup_keys(m, block_reps)
+    have = [k for k in sd.keys() if not k.endswith("num_batches_tracked")]
+    missing, extra = [k for k in want if k not in sd], sorted(set(have) - set(want))
+    if missing or extra:
+        raise RuntimeError(f"checkpoint does not match PointGroup(m={m}, block_reps={block_reps}): "
+                           f"missing={missing[:8]} unexpected={extra[:8]}")
+    for k, shape in want.items():
+        got = tuple(sd[k].shape)
+        if got != shape:
+            raise ValueError(f"checkpoint key {k} has shape {got}, PointGroup(m={m}, block_reps={block_reps}) "
+                             f"expects {shape}")
+
+
+def _bn_affine(sd, p):
+    """Eval-mode BatchNorm1d as y = x * scale + shift, computed in float64 and narrowed to float32."""
+    g, beta = _np64(sd[p + ".weight"]), _np64(sd[p + ".bias"])
+    mu, var = _np64(sd[p + ".running_mean"]), _np64(sd[p + ".running_var"])
+    s = g / np.sqrt(var + BN_EPS)
+    return np.float32(s), np.float32(beta - mu * s)
+
+
+def _f32(sd, k, K=None):
+    a = _np64(sd[k]).astype(np.float32)
+    return np.ascontiguousarray(a if K is None else a.reshape(K, a.shape[-2], a.shape[-1]))
+
+
+def _pack_resblock(sd, p, cin, cout):
+    blk = {"bn1": _bn_affine(sd, p + "conv_branch.0"),
+           "W1": _f32(sd, p + "conv_branch.2.weight", 27), "b1": _f32(sd, p + "conv_branch.2.bias"),
+           "bn2": _bn_affine(sd, p + "conv_branch.3"),
+           "W2": _f32(sd, p + "conv_branch.5.weight", 27), "b2": _f32(sd, p + "conv_branch.5.bias"),
+           "Wi": None, "bi": None}
+    if cin != cout:
+        blk["Wi"], blk["bi"] = _f32(sd, p + "i_branch.0.weight", 1), _f32(sd, p + "i_branch.0.bias")
+    return blk
+
+
+def pack_pointgroup(sd, m, block_reps):
+    """The float32 arrays the device forward runs on, from a PointGroup state_dict (``module.`` prefixes and a
+    'state_dict' wrapper are stripped; the key set and shapes are checked strictly).  Returns a dict:
+      input: (W (27,6,m), b); levels: one dict per level l = 0..6 with C = (l+1) m and
+        blocks / tail: lists of residual blocks {bn1: (scale, shift), W1 (27,Cin,C), b1, bn2, W2 (27,C,C), b2,
+        Wi (1,Cin,C) or None, bi}, and for l < 6 down: (bn, W (8,C,C+m), b), up: (bn, W (8,C+m,C), b);
+      head: {bn: output_layer's (scale, shift), W1 (m,m) [in][out] and b1 with offset.1 folded in, W2 (m,3), b2}."""
+    if any(k.startswith("module.") for k in sd) or "state_dict" in sd:
+        sd = strip_module_prefix(sd)
+    check_pointgroup_state_dict(sd, m, block_reps)
+    out = {"input": (_f32(sd, "input_conv.0.weight", 27), _f32(sd, "input_conv.0.bias")), "levels": []}
+    p = "unet."
+    for lv in range(PG_LEVELS):
+        C = m * (lv + 1)
+        L = {"blocks": [_pack_resblock(sd, f"{p}blocks.block{i}.", C, C) for i in range(block_reps)]}
+        if lv < PG_LEVELS - 1:
+            L["down"] = (_bn_affine(sd, p + "conv.0"), _f32(sd, p + "conv.2.weight", 8), _f32(sd, p + "conv.2.bias"))
+            L["up"] = (_bn_affine(sd, p + "deconv.0"), _f32(sd, p + "deconv.2.weight", 8),
+                       _f32(sd, p + "deconv.2.bias"))
+            L["tail"] = [_pack_resblock(sd, f"{p}blocks_tail.block{i}.", C * (2 - i), C) for i in range(block_reps)]
+        out["levels"].append(L)
+        p += "u."
+    W1, b1 = _fold(sd, "offset.0", "offset.1")
+    W2, b2 = _fold(sd, "offset.3", None)
+    out["head"] = {"bn": _bn_affine(sd, "output_layer.0"), "W1": np.float32(W1), "b1": np.float32(b1),
+                   "W2": np.float32(W2), "b2": np.float32(b2)}
+    return out

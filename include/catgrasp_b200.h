@@ -458,6 +458,20 @@ int  cg_spconv_down_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *nvox, in
 int  cg_spconv_conv_dev(cg_ctx *ctx, const float *in, int Cin, const int32_t *nbr, int K, const int32_t *nout, int M,
                         const float *W, int Cout, const float *bn_scale, const float *bn_shift, const float *bias,
                         const float *residual, float *out);
+/* PointGroup's voxelisation, pointgroup_ops mode 4 (the mean): out (V,C) rows v < min(*nvox, V) = the mean of the
+ * rows of feats (N,C) whose p2v (N) is v, as voxelize_fp_cuda_ sums it: out = 0, then for each such point in
+ * ascending index out = fl(out + fl(fl(1 / n) * x)) in fp32, no FMA, so the result is deterministic.  A site with no
+ * point is 0; a point whose p2v is not a site below min(*nvox, V) is ignored.  Rows from min(*nvox, V) on are not
+ * written.                                                                                                        */
+int  cg_pointgroup_voxel_mean_dev(cg_ctx *ctx, const float *feats, int N, int C, const int32_t *p2v,
+                                  const int32_t *nvox, int V, float *out);
+/* PointGroup's output_layer and offset head, one site per warp: a = max(in * bn_scale + bn_shift, 0) (m channels),
+ * h = max(W1^T a + b1, 0) with the head's BN folded into W1 (m,m) [in][out] and b1 (m), out_site (V,3) rows
+ * v < min(*nvox, V) = W2^T h + b2 with W2 (m,3) [in][out]; each output one fp32 FMA chain over the inputs ascending,
+ * then the bias.  out (N,3) = out_site[p2v[i]], NaN for a point naming no site.  m in [1, 512].                 */
+int  cg_pointgroup_head_dev(cg_ctx *ctx, const float *in, int m, const int32_t *nvox, int V, const float *bn_scale,
+                            const float *bn_shift, const float *W1, const float *b1, const float *W2, const float *b2,
+                            const int32_t *p2v, int N, float *out_site, float *out);
 
 /* ---- PointNet++ primitives (device pointers) ---------------------------
  * Replace the free functions of pointnet2.py:14-149.  Indices are int32 on
