@@ -156,6 +156,8 @@ SIGNATURES = {
     "cg_spconv_conv_dev": (_i, [_vp, _D, _i, _D, _i, _D, _i, _D, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_pointgroup_voxel_mean_dev": (_i, [_vp, _D, _i, _i, _D, _D, _i, _D], TORCH),
     "cg_pointgroup_head_dev": (_i, [_vp, _D, _i, _D, _i, _D, _D, _D, _D, _D, _D, _D, _i, _D, _D], TORCH),
+    "cg_segment_table_dev": (_i, [_vp, _D, _i, _D, _i, _i, _i, _D, _D, _D, _D, _D, _D, _D, _D, _D], TORCH),
+    "cg_rank_grasps_dev": (_i, [_vp, _D, _i, _i, _i, _D, _D, _D, _D], TORCH),
     "cg_square_distance_dev": (_i, [_vp, _D, _D, _i, _i, _i, _D], TORCH),
     "cg_index_points_dev": (_i, [_vp, _D, _D, _i, _i, _i, _i, _D], TORCH),
     "cg_fps_dev": (_i, [_vp, _D, _i, _i, _i, _D, _D], TORCH),

@@ -145,43 +145,54 @@ def estimate_normals(pts, radius, max_nn, view_port=(0.0, 0.0, 0.0)):
 
 
 def prepare_object(ob_pts, ob_normals, scene_pts, gripper_diameter, octo_resolution=0.001, K=None):
-    """run_grasp_simulation.py:113-139 and :171-175 (compute_candidate_grasp_one_ob) in one call, numpy in and out.
+    """run_grasp_simulation.py:113-139 and :171-175 (compute_candidate_grasp_one_ob) in one call: numpy in, numpy out;
+    CUDA tensors in, CUDA tensors out.
 
     Returns None when fewer than 100 voxels survive the 0.5 mm down-sampling (:116-118); otherwise a dict with
     ``data`` ({'cloud_xyz', 'cloud_normal'}: each voxel mean snapped to its nearest object point, duplicates kept,
     :119-126), ``background_pts`` (the occupancy samples of the scene around the object, :130-139),
     ``points_for_sample`` and ``normals_for_sample`` (:171-175).  ``K`` is handed to makeOccupancyGridFromCloudScan,
-    which does not use it."""
+    which does not use it.  The object and scene points stay on the device either way; the occupancy grid is built
+    by the host entry of makeOccupancyGridFromCloudScan."""
     from .my_cpp import makeOccupancyGridFromCloudScan
-    ob_pts = np.asarray(ob_pts)
-    ob_normals = np.asarray(ob_normals)
-    scene_pts = np.asarray(scene_pts)
-    ob_index = CloudIndex(ob_pts, 0.0005)
-    down, _ = ob_index.voxel_means()                                                   # :113-115
-    if down.shape[0] < 100:                                                            # :116-118
+    like = ob_pts
+    ob_pts, ob_normals, scene_pts = (a if isinstance(a, torch.Tensor) else np.asarray(a)
+                                     for a in (ob_pts, ob_normals, scene_pts))
+    ctx, ob_pts, ob_normals, scene_pts = _lib.inputs(
+        ob_pts, ob_normals, scene_pts,
+        dtype=tuple(torch.float32 if str(a.dtype).endswith("float32") else torch.float64
+                    for a in (ob_pts, ob_normals, scene_pts)))
+    ob_pts, ob_normals, scene_pts = ob_pts.reshape(-1, 3), ob_normals.reshape(-1, 3), scene_pts.reshape(-1, 3)
+    dev = ctx.device
+    ob_index = CloudIndex(ob_pts, 0.0005, dev)
+    n_down = ob_index.n_cells                                                          # :113-115
+    if n_down < 100:                                                                   # :116-118
         return None
+    down, _ = ob_index.voxel_means()
     del ob_index
     # :119-122 snap: a voxel mean and its members share a voxel, so the nearest member is within the diagonal; the
     # bound is widened by 1e-9 relative so rounding at a voxel face cannot exclude it
     snap_bound = 0.0005 * np.sqrt(3.0) * (1 + 1e-9)
-    index = CloudIndex(ob_pts, snap_bound)
-    _, ids = index.nearest(down, snap_bound)
-    ids = ids.cpu().numpy().astype(np.int64)
-    if (ids < 0).any():
+    _, ids = CloudIndex(ob_pts, snap_bound, dev).nearest(down, snap_bound)
+    if bool((ids < 0).any()):
         raise _lib.CgError("prepare_object: a voxel mean has no object point within its voxel's diagonal")
-    data = {"cloud_xyz": ob_pts[ids].reshape(-1, 3), "cloud_normal": ob_normals[ids].reshape(-1, 3)}
+    ids = ids.to(torch.int64)
+    xyz, nrm = ob_pts[ids], ob_normals[ids]
     # :130-134 crop: scene points whose nearest object point is within gripper_diameter/2 (sqrt(d2) <= R)
     R = gripper_diameter / 2
-    crop_index = CloudIndex(ob_pts, _query_cell(ob_pts, R))
-    keep = torch.nonzero(crop_index.within(scene_pts, R, compare_sqrt=True)).reshape(-1).cpu().numpy()
-    background = scene_pts[keep]
+    keep = torch.nonzero(CloudIndex(ob_pts, _query_cell(ob_pts, R), dev).within(scene_pts, R, compare_sqrt=True))
+    background = scene_pts[keep.reshape(-1)]
     background, _ = cloudA_minus_cloudB(background, ob_pts, thres=0.005)               # :135
     if background.shape[0]:
-        background = voxel_down_sample(background, 0.001)                             # :136-137
+        background = voxel_down_sample(background, 0.001).cpu().numpy()              # :136-137
         background_pts = makeOccupancyGridFromCloudScan(background, np.eye(3) if K is None else K, octo_resolution)
     else:
         background_pts = np.zeros((0, 3), np.float32)
-    xyz = data["cloud_xyz"]
-    voxel_size = float(np.linalg.norm(xyz.max(axis=0) - xyz.min(axis=0)) / 10.0)       # :172, in the cloud's dtype
-    pfs, nfs = voxel_down_sample(xyz, voxel_size, normals=data["cloud_normal"])         # :171-175
-    return {"data": data, "background_pts": background_pts, "points_for_sample": pfs, "normals_for_sample": nfs}
+    # :172, in the cloud's dtype (the extent is exact; the norm is numpy's)
+    ext = (xyz.amax(0) - xyz.amin(0)).cpu().numpy()
+    voxel_size = float(np.linalg.norm(ext) / 10.0)
+    pfs, nfs = voxel_down_sample(xyz, voxel_size, normals=nrm)                         # :171-175
+    background_pts = torch.from_numpy(background_pts).to(xyz.device)
+    xyz, nrm, background_pts, pfs, nfs = _lib.returned(like, xyz, nrm, background_pts, pfs, nfs)
+    return {"data": {"cloud_xyz": xyz, "cloud_normal": nrm}, "background_pts": background_pts,
+            "points_for_sample": pfs, "normals_for_sample": nfs}

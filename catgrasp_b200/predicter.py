@@ -400,8 +400,8 @@ def slice_keep_mask(xyz):
 
 
 class PointGroupPredictor:
-    """predicter.py:206-338: the segmentation of a pile into instances.  The host front runs in numpy and on the
-    device's cloud kernels, the network (voxelisation, U-Net, offset head) on the device (catgrasp_b200.pointgroup),
+    """predicter.py:206-338: the segmentation of a pile into instances.  The front runs on the device's cloud kernels
+    (device_front), the network (voxelisation, U-Net, offset head) on the device (catgrasp_b200.pointgroup),
     the clustering after it in segment.pointgroup_labels.  Only the shipped structure is implemented: mode 4,
     use_coords, residual blocks, input_channel 3 and n_slice_per_side 1; any m and block_reps 1 or 2."""
 
@@ -436,48 +436,66 @@ class PointGroupPredictor:
         if int(c["block_reps"]) not in (1, 2):
             raise NotImplementedError(f"PointGroupPredictor: block_reps = {c['block_reps']}; only 1 and 2 build")
 
-    def host_front(self, data):
-        """predicter.py:234-300 with n_slice_per_side = 1: (xyz_original_all (N,3) float32, locs (N,3) int64,
-        feats (N,6) float32, spatial_shape (3 ints)), numpy."""
+    def device_front(self, data):
+        """predicter.py:234-300 with n_slice_per_side = 1, on the device for numpy or CUDA input: (xyz_original_all
+        (N,3) float32, locs (N,3) int64, feats (N,6) float32) CUDA tensors and spatial_shape (3 ints).  Every step is
+        in the input's dtype as the reference computes it: the keep mask, the 0.5 mm voxel means snapped to their
+        nearest point, and the sites trunc(fl(fl(x * scale) - min)), the scale first and each operation rounded on
+        its own."""
         import torch
         from .cloud import CloudIndex
         from . import _lib
         self._check_structure()
-        xyz, nrm = np.asarray(data["cloud_xyz"]), np.asarray(data["cloud_normal"])
-        keep = slice_keep_mask(xyz)
+        dev = self.model.ctx.device
+        ctx, xyz, nrm = _lib.inputs(data["cloud_xyz"], data["cloud_normal"], ctx=self.model.ctx,
+                                    dtype=tuple(_float_dtype(a) for a in (data["cloud_xyz"], data["cloud_normal"])))
+        keep = torch.nonzero(slice_keep_mask(xyz)).reshape(-1)
         xo, no = xyz[keep], nrm[keep]
         ds = float(self.cfg["downsample_size"])
-        dev = self.model.ctx.device
         down, _ = CloudIndex(xo, ds, dev).voxel_means()
         # the snap (cKDTree.query): a voxel mean and its members share a voxel, so the nearest member is within the
         # diagonal, widened by 1e-9 relative against rounding at a voxel face
         snap = ds * np.sqrt(3.0) * (1 + 1e-9)
         _, ids = CloudIndex(xo, snap, dev).nearest(down, snap)
-        ids = ids.cpu().numpy()
-        if (ids < 0).any():
+        if bool((ids < 0).any()):
             raise _lib.CgError("PointGroupPredictor: a voxel mean has no point within its voxel's diagonal")
+        ids = ids.to(torch.int64)
         xo, no = xo[ids], no[ids]
         s = xo * self.cfg_pg["scale"]
-        s -= s.min(0)
-        locs = torch.from_numpy(s).long().numpy()
-        shape = tuple(int(v) for v in np.maximum(locs.max(0) + 1, int(self.cfg_pg["full_scale"][0])))
-        feats = np.concatenate([no.astype(np.float32), xo.astype(np.float32)], 1)
-        return xo.astype(np.float32), locs, feats, shape
+        s = s - s.amin(0)
+        locs = s.to(torch.int64)                                         # truncation, as torch's .long() on the host
+        hi = (locs.amax(0) + 1).cpu().numpy()
+        shape = tuple(int(v) for v in np.maximum(hi, int(self.cfg_pg["full_scale"][0])))
+        feats = torch.cat([no.to(torch.float32), xo.to(torch.float32)], 1)
+        return xo.to(torch.float32), locs, feats, shape
+
+    def host_front(self, data):
+        """device_front with numpy results: (xyz_original_all (N,3) float32, locs (N,3) int64, feats (N,6) float32,
+        spatial_shape (3 ints))."""
+        xo, locs, feats, shape = self.device_front(data)
+        return xo.cpu().numpy(), locs.cpu().numpy(), feats.cpu().numpy(), shape
 
     def offsets(self, data):
-        """The host front and the network: (xyz_original_all (N,3) float32 numpy, pt_offsets (N,3) float32 CUDA)."""
-        import torch
+        """The front and the network: (xyz_original_all (N,3) float32, pt_offsets (N,3) float32), CUDA tensors."""
         from . import spconv
-        xo, locs, feats, shape = self.host_front(data)
-        dev = self.model.device
-        level, p2v = spconv.index(torch.from_numpy(locs).to(dev), shape)
-        return xo, self.model.offsets(level, p2v, torch.from_numpy(feats).to(dev))
+        xo, locs, feats, shape = self.device_front(data)
+        level, p2v = spconv.index(locs, shape)
+        return xo, self.model.offsets(level, p2v, feats)
 
     def predict(self, data):
-        """predicter.py:232-338: labels_all (M,) int64, one per point of data['cloud_xyz']; sets self.xyz_shifted."""
+        """predicter.py:232-338: labels_all (M,) int64, one per point of data['cloud_xyz'], and self.xyz_shifted; numpy
+        for numpy input, CUDA tensors for CUDA input."""
         from .segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
         xo, off = self.offsets(data)
-        labels_all, xyz_shifted = pointgroup_labels(xo, off.cpu().numpy(), data["cloud_xyz"],
-                                                    MEANSHIFT_BANDWIDTH[self.class_name])
+        labels_all, xyz_shifted = pointgroup_labels(xo, off, data["cloud_xyz"], MEANSHIFT_BANDWIDTH[self.class_name])
+        if not getattr(data["cloud_xyz"], "is_cuda", False):
+            labels_all, xyz_shifted = labels_all.cpu().numpy(), xyz_shifted.cpu().numpy()
         self.xyz_shifted = xyz_shifted
         return labels_all
+
+
+def _float_dtype(a):
+    """torch dtype of a float32 / float64 array or tensor (anything else is widened to float64)."""
+    import torch
+    name = str(a.dtype)
+    return torch.float32 if name.endswith("float32") else torch.float64

@@ -473,6 +473,32 @@ int  cg_pointgroup_head_dev(cg_ctx *ctx, const float *in, int m, const int32_t *
                             const float *bn_shift, const float *W1, const float *b1, const float *W2, const float *b2,
                             const int32_t *p2v, int N, float *out_site, float *out);
 
+/* ---- per-pick glue (csrc/cg_pick.cu; catgrasp_b200/pick.py) ---------------------------------------------------
+ * Device pointers, the context's stream, no synchronisation.
+ *
+ * cg_segment_table_dev: run_grasp_simulation.py:217-240 and :253-259 on labels (M) int32 or int64 (labels_is_i64)
+ * and points x (M,3) float32 or float64 (x_is_f64).  Labels are dense in [0, L): L is the segmenter's cluster count
+ * (MeanShift's number of centres, i.e. labels.max() + 1); a label outside [0, L) belongs to no segment.  Per label l:
+ * out_count[l], the exact per-axis out_min / out_max (L,3) float64 (0 for an empty label), and out_inlier[l] (uint8):
+ * count >= 500 and not n / ((q0 * q1) * q2) < 0.01, q = (max - min) / 0.001 rounded in the cloud's dtype, the division
+ * by the product in float64 (a zero extent gives inf: an inlier).  out_labels (M, the labels' dtype) = the label, or -1
+ * where it is no inlier (:240).  out_order (L): the inlier labels by count descending, ties in descending label order
+ * (reversed(sorted(..., key=count))), then -1; *out_n_kept their number.  out_offsets (L+1): out_offsets[0] = 0 and
+ * out_offsets[k+1] - out_offsets[k] = the count of out_order[k] (0 past the kept ones); out_index (M): the point
+ * indices of the k-th kept segment, ascending, at [out_offsets[k], out_offsets[k+1]); entries from
+ * out_offsets[*out_n_kept] on are not meaningful.  M >= 0, 1 <= L < 2^30.                                        */
+int  cg_segment_table_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64, int M, int L,
+                          void *out_labels, int32_t *out_count, double *out_min, double *out_max, uint8_t *out_inlier,
+                          int32_t *out_order, int32_t *out_n_kept, int32_t *out_offsets, int32_t *out_index);
+/* cg_rank_grasps_dev: run_grasp_simulation.py:311-328.  probs (G,C) float32, p_T_given_G (G) float64 ->
+ * out_p_G (G) = (pred * arange(C)).sum() / denom bit for bit with numpy (float64 products, numpy's pairwise summation
+ * order), denom = len(cfg_grasp['classes']) - 1 (:313; the shipped grasp-Q net has C = 10 outputs for 11 class edges,
+ * so denom = C); out_p_T_G (G) = p_T_given_G * p_G; out_perm (G) int32 = Python's stable sorted(key=-p_T_G):
+ * descending, equal keys (+0.0 and -0.0 included) in input order.  G >= 0, 1 <= C <= 128, denom >= 1; NaN keys are
+ * not ordered.                                                                                                     */
+int  cg_rank_grasps_dev(cg_ctx *ctx, const float *probs, int G, int C, int denom, const double *p_T_given_G,
+                        double *out_p_G, double *out_p_T_G, int32_t *out_perm);
+
 /* ---- PointNet++ primitives (device pointers) ---------------------------
  * Replace the free functions of pointnet2.py:14-149.  Indices are int32 on
  * the device (the Python mirror widens to int64 like the reference).        */
