@@ -53,21 +53,16 @@ def all_gather_records(local_rec, n_total, group=None):
 def sharded_predict_batch(predicter, data, grasp_poses, subsample=None, group=None):
     """``GraspPredicter.predict_batch(data, grasp_poses)`` (predicter.py:67-94) with the candidate list sharded over the
     ranks of ``group``: every rank calls this with the SAME arguments, scores its contiguous block
-    ``shard_range(B, rank, world)`` against the replicated cloud and weights, and one all-gather of the (B, 12) records
-    rebuilds the full, candidate-ordered result on every rank.  Same return value as predict_batch; with
+    (``predicter.score(..., shard=shard_range(B, rank, world))``) against the replicated cloud and weights, and one
+    all-gather of the (B, 12) records rebuilds the full, candidate-ordered result on every rank.  Same return value as predict_batch; with
     ``subsample="host"`` every rank consumes the global numpy generator exactly like the single-process call."""
-    import numpy as np
+    from .predicter import result_list
     B = len(grasp_poses)
     if B == 0:
         return []
     world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
     rank = dist.get_rank(group) if world > 1 else 0
-    lo, hi = shard_range(B, rank, world)
-    d_probs = predicter.predict_batch(data, grasp_poses, subsample=subsample, shard=(lo, hi))
-    rec = torch.zeros((hi - lo, RECORD_FLOATS), dtype=torch.float32, device=d_probs.device)
-    rec[:, : d_probs.shape[1]] = d_probs
-    full = all_gather_records(rec, B, group=group)
-    probs = full[:, : d_probs.shape[1]].cpu().numpy()
-    labels = probs.argmax(1)
-    conf = probs[np.arange(B), labels]
-    return [[l, c, p] for l, c, p in zip(labels, conf, probs)]
+    d_probs = predicter.score(data, grasp_poses, subsample=subsample, shard=shard_range(B, rank, world))
+    zero = torch.zeros((d_probs.shape[0],), device=d_probs.device)    # scoring has no status or offset: both columns 0
+    full = all_gather_records(pack_records(d_probs, zero, zero), B, group=group)
+    return result_list(unpack_records(full, d_probs.shape[1])[0].cpu().numpy())

@@ -148,8 +148,57 @@ class GraspPredicter:
             self._pin = torch.empty((need + need // 4,), dtype=torch.int32).pin_memory()
         return self._pin[:need].view(B, n_pts)
 
-    def predict_batch(self, data, grasp_poses, ids=None, subsample=None, shard=None):
-        """predicter.py:67-94.  Returns list of [label np.int64, confidence np.float32, probs (n_out,) f32].
+    def _given_ids(self, ids, lo, hi):
+        """Caller-given subsets: numpy's global generator is not touched.  Yields (first row, device ids) launches."""
+        import torch
+        if hi > lo:
+            yield 0, torch.from_numpy(np.ascontiguousarray(np.asarray(ids)[lo:hi], dtype=np.int32)).to(self.model.device)
+
+    def _device_draw(self, M, lo, hi):
+        """The counter-based draw on the GPU (cg_draw_ids_dev): consumes ONE value of numpy's global generator, the
+        seed, whatever the shard; a candidate's subset depends on the seed and its place in the whole list only."""
+        seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+        if hi > lo:
+            yield 0, self.model.draw_ids_dev(M, int(self.cfg["n_pts"]), hi - lo, seed=seed, first_candidate=lo)
+
+    def _host_draw(self, M, lo, hi, B_all):
+        """The reference's draw: walks numpy's global generator over the WHOLE list in C (skip the ``lo`` candidates
+        before the shard, draw the shard, skip the ``B_all - hi`` after it) and puts the advanced state back.  The
+        worker thread draws chunk k+1 into the pinned buffer while the GPU scores chunk k."""
+        import queue
+        import threading
+        import torch
+        B, n_pts = hi - lo, int(self.cfg["n_pts"])
+        h_ids = self._pinned_ids(B, n_pts)
+        d_ids = torch.empty((B, n_pts), dtype=torch.int32, device=self.model.device)
+        draw = _LegacyDraw()
+        q = queue.Queue()
+
+        def producer():
+            try:
+                draw.skip(M, n_pts, lo)
+                for c0 in range(0, B, self.chunk):
+                    c1 = min(B, c0 + self.chunk)
+                    draw.draw(M, n_pts, c1 - c0, out=h_ids[c0:c1])
+                    q.put((c0, c1))
+                draw.skip(M, n_pts, B_all - hi)
+                q.put(None)
+            except Exception as e:   # surfaces in the consumer
+                q.put(e)
+        t = threading.Thread(target=producer, daemon=True)
+        t.start()
+        while (item := q.get()) is not None:
+            if isinstance(item, Exception):
+                raise item
+            c0, c1 = item
+            d_ids[c0:c1].copy_(h_ids[c0:c1], non_blocking=True)
+            yield c0, d_ids[c0:c1]
+        t.join()
+        draw.commit()
+
+    def score(self, data, grasp_poses, ids=None, subsample=None, shard=None):
+        """The probabilities of candidates ``shard=(lo, hi)`` of the list (default: all of it) as a (hi-lo, n_out)
+        float32 CUDA tensor.
 
         ``data`` is not modified (the reference deep-copies it, :72).  ``ids`` (B,n_pts) overrides the draw.
         ``subsample`` (default ``self.subsample``):
@@ -159,18 +208,13 @@ class GraspPredicter:
           "device" -- a statistically equivalent counter-based draw on the GPU (cg_draw_ids_dev); consumes ONE value
                       of the global numpy generator (the seed) instead of one shuffle per candidate.  Not the
                       reference's numbers: use it when throughput matters more than replaying a reference run.
-        ``shard=(lo, hi)`` scores only candidates [lo, hi) of the list and returns their (hi-lo, n_out) probabilities
-        as a CUDA tensor -- the random stream is consumed for the WHOLE list (the other candidates' draws are skipped in
-        C), so every rank of a sharded call stays on the reference's stream (catgrasp_b200.dist.sharded_predict_batch).
+        The random stream is consumed for the WHOLE list whatever the shard, so every rank of a sharded call stays on
+        the reference's stream (catgrasp_b200.dist.sharded_predict_batch).
         """
         import torch
-        from . import _lib
         B_all = len(grasp_poses)
-        if B_all == 0:
-            return []
-        lo_s, hi_s = (0, B_all) if shard is None else (int(shard[0]), int(shard[1]))
-        assert 0 <= lo_s <= hi_s <= B_all
-        B = hi_s - lo_s
+        lo, hi = (0, B_all) if shard is None else (int(shard[0]), int(shard[1]))
+        assert 0 <= lo <= hi <= B_all
         mode = subsample or self.subsample
         assert mode in ("host", "device"), mode
         xyz = np.asarray(data["cloud_xyz"], dtype=np.float64)
@@ -178,105 +222,60 @@ class GraspPredicter:
         valid_mask = xyz[:, 2] >= 0.1                                   # dataset_grasp.py:64
         xyz = np.ascontiguousarray(xyz[valid_mask].reshape(-1, 3))
         nrm = np.ascontiguousarray(nrm[valid_mask].reshape(-1, 3))
-        M, n_pts = xyz.shape[0], int(self.cfg["n_pts"])
-        poses = np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).reshape(B_all, 4, 4)[lo_s:hi_s])
-        if ids is not None:
-            ids = np.asarray(ids)[lo_s:hi_s]
-        net, dev = self.model, self.model.device
-        ctx_engine = net.ctx.get_engine()
-        if ctx_engine != self.engine:       # the context (one per device) is shared: select this predicter's engine per call
-            net.ctx.set_engine(self.engine)
-        try:
-            return self._predict_batch(data, grasp_poses, ids, mode, shard, xyz, nrm, poses, M, n_pts, B, B_all, lo_s, hi_s)
-        finally:
-            if ctx_engine != self.engine:
-                net.ctx.set_engine(ctx_engine)
-
-    def _predict_batch(self, data, grasp_poses, ids, mode, shard, xyz, nrm, poses, M, n_pts, B, B_all, lo_s, hi_s):
-        import torch
-        net, dev = self.model, self.model.device
-        if B == 0:   # an empty shard still consumes the stream like everybody else
-            if ids is None and mode == "device":
-                np.random.randint(0, 2 ** 63 - 1, dtype=np.int64)
-            elif ids is None:
-                d = _LegacyDraw()
-                d.skip(M, n_pts, B_all)
-                d.commit()
-            import torch as _t
-            return _t.empty((0, net.n_out), dtype=_t.float32, device=dev)
+        M = xyz.shape[0]
+        poses = np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).reshape(B_all, 4, 4)[lo:hi])
+        net, dev, ctx = self.model, self.model.device, self.model.ctx
         with torch.cuda.device(dev):
             d_xyz, d_nrm = torch.from_numpy(xyz).to(dev), torch.from_numpy(nrm).to(dev)
             d_pose = torch.from_numpy(poses).to(dev)
             d_mean = torch.from_numpy(np.ascontiguousarray(self.cfg["mean"].reshape(-1))).to(dev) if "mean" in self.cfg else None
             d_std = torch.from_numpy(np.ascontiguousarray(self.cfg["std"].reshape(-1))).to(dev) if "std" in self.cfg else None
-            d_probs = torch.empty((B, net.n_out), dtype=torch.float32, device=dev)
-            d_label = torch.empty((B,), dtype=torch.int32, device=dev)
+            d_probs = torch.empty((hi - lo, net.n_out), dtype=torch.float32, device=dev)
+            d_label = torch.empty((hi - lo,), dtype=torch.int32, device=dev)
 
-            def run(engine_override=None):
-                if ids is not None or mode == "device":
-                    if ids is not None:
-                        d_ids = torch.from_numpy(np.ascontiguousarray(ids, dtype=np.int32)).to(dev)
-                    else:
-                        d_ids = net.draw_ids_dev(M, n_pts, B, seed=self._device_seed, first_candidate=lo_s)
-                    net.graspq_dev(d_xyz, d_nrm, d_pose, d_ids, d_mean, d_std, out=(d_probs, d_label))
-                    return
-                # bit-parity mode: C continuation of numpy's generator on a worker thread, chunk by chunk
-                import queue
-                import threading
-                h_ids = self._pinned_ids(B, n_pts)
-                draw = self._draw
-                bounds = [(lo, min(B, lo + self.chunk)) for lo in range(0, B, self.chunk)]
-                q = queue.Queue()
+            def forward(c0, d_ids):
+                c1 = c0 + d_ids.shape[0]
+                net.graspq_dev(d_xyz, d_nrm, d_pose[c0:c1], d_ids, d_mean, d_std, out=(d_probs[c0:c1], d_label[c0:c1]))
 
-                def producer():
-                    try:
-                        if not self._drawn and lo_s > 0:
-                            draw.skip(M, n_pts, lo_s)
-                        for lo, hi in bounds:
-                            if not self._drawn:
-                                draw.draw(M, n_pts, hi - lo, out=h_ids[lo:hi])
-                            q.put((lo, hi))
-                        if not self._drawn and hi_s < B_all:
-                            draw.skip(M, n_pts, B_all - hi_s)
-                    except Exception as e:   # surfaces in the consumer
-                        q.put(e)
-                t = threading.Thread(target=producer, daemon=True)
-                t.start()
-                d_ids = torch.empty((B, n_pts), dtype=torch.int32, device=dev)
-                for _ in bounds:
-                    item = q.get()
-                    if isinstance(item, Exception):
-                        raise item
-                    lo, hi = item
-                    d_ids[lo:hi].copy_(h_ids[lo:hi], non_blocking=True)
-                    net.graspq_dev(d_xyz, d_nrm, d_pose[lo:hi], d_ids[lo:hi], d_mean, d_std,
-                                   out=(d_probs[lo:hi], d_label[lo:hi]))
-                t.join()
-                self._drawn = True
+            if ids is not None:
+                launches = self._given_ids(ids, lo, hi)
+            elif mode == "device":
+                launches = self._device_draw(M, lo, hi)
+            else:
+                launches = self._host_draw(M, lo, hi, B_all)
+            ctx_engine = ctx.get_engine()
+            ctx.set_engine(self.engine)         # the context (one per device) is shared: this predicter's engine, per call
+            try:
+                done = []
+                for c0, d_ids in launches:
+                    forward(c0, d_ids)
+                    done.append((c0, d_ids))
+                if self.engine >= 2 and ctx.fp16_overflow():
+                    # the fast engines clamp the 128->1024 layer's inputs to the fp16 range: redo on the near-fp32
+                    # engine from the ids already on the device, launch for launch (a launch's batch size selects the
+                    # FC kernel, so the same cuts give the bits of a call made on engine 1)
+                    print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (wgmma bf16 hi/lo x3)")
+                    ctx.set_engine(1)
+                    for c0, d_ids in done:
+                        forward(c0, d_ids)
+            finally:
+                ctx.set_engine(ctx_engine)
+        return d_probs
 
-            if ids is None and mode == "device":
-                self._device_seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
-            if ids is None and mode == "host":
-                self._draw, self._drawn = _LegacyDraw(), False
-            run()
-            probs = None if shard is not None else d_probs.cpu().numpy()
-            if net.ctx.get_engine() >= 2 and net.ctx.fp16_overflow():
-                # the fast engines clamp the 128->1024 layer's inputs to the fp16 range: redo on the near-fp32 engine
-                print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (wgmma bf16 hi/lo x3)")
-                eng = net.ctx.get_engine()
-                net.ctx.set_engine(1)
-                try:
-                    run()
-                    probs = None if shard is not None else d_probs.cpu().numpy()
-                finally:
-                    net.ctx.set_engine(eng)
-            if ids is None and mode == "host":
-                self._draw.commit()
-        if shard is not None:
-            return d_probs
-        labels = probs.argmax(1)                                         # predicter.py:87-91
-        conf = probs[np.arange(B), labels]
-        return [[l, c, p] for l, c, p in zip(labels, conf, probs)]
+    def predict_batch(self, data, grasp_poses, ids=None, subsample=None):
+        """predicter.py:67-94.  Returns list of [label np.int64, confidence np.float32, probs (n_out,) f32]: ``score``
+        on the whole list (same ``ids`` and ``subsample``), copied to the host once."""
+        if len(grasp_poses) == 0:
+            return []
+        return result_list(self.score(data, grasp_poses, ids=ids, subsample=subsample).cpu().numpy())
+
+
+def result_list(probs):
+    """(B, n_out) host probabilities as the reference returns them (predicter.py:87-91): [label, confidence, probs]
+    per candidate."""
+    labels = probs.argmax(1)
+    conf = probs[np.arange(len(probs)), labels]
+    return [[l, c, p] for l, c, p in zip(labels, conf, probs)]
 
 
 class NunocsPredicter:

@@ -352,9 +352,10 @@ def _overflow_state_dict():
     return sd
 
 
-def test_fp16_activation_overflow_is_reported(cuda, tmp_path):
+def test_fp16_activation_overflow_is_reported(cuda, tmp_path, capsys):
     """Layer-2 outputs beyond 65504: engines 2 and 3 clamp them and must raise the overflow flag (engine 1 must not);
-    reading the flag clears it; GraspPredicter on engine 2 then re-runs on engine 1."""
+    reading the flag clears it; GraspPredicter on engine 2 or 3 then re-runs on engine 1: over several chunks, with
+    either draw or caller-given ids, without touching numpy's generator, and leaving the shared context as it was."""
     from catgrasp_b200.predicter import GraspPredicter
     from catgrasp_b200.synthetic import make_candidates, make_pile, write_artifacts
     sd = _overflow_state_dict()
@@ -373,10 +374,23 @@ def test_fp16_activation_overflow_is_reported(cuda, tmp_path):
     adir = write_artifacts(str(tmp_path / "artifacts-47"), "cls", n_pts=256, state_dict=sd)
     scene = make_pile(1500, n_objects=3, seed=9)
     data = {"cloud_xyz": scene["cloud_xyz"], "cloud_normal": scene["cloud_normal"]}
-    poses = list(make_candidates(scene["cloud_xyz"], scene["cloud_normal"], 12, seed=10))
-    out = {}
-    for e in (1, 2):
-        gp = GraspPredicter("nut", artifact_dir=adir, engine=e)
-        np.random.seed(3)
-        out[e] = np.stack([o[2] for o in gp.predict_batch(data, poses)])
-    assert np.array_equal(out[2].view(np.uint32), out[1].view(np.uint32))
+    poses = list(make_candidates(scene["cloud_xyz"], scene["cloud_normal"], 13, seed=10))
+    M = int((scene["cloud_xyz"][:, 2] >= 0.1).sum())
+    given = np.random.RandomState(11).randint(0, M, (13, 256)).astype(np.int32)
+    ctx = net.ctx
+    for tag, kw in (("host", {"subsample": "host"}), ("device", {"subsample": "device"}), ("ids", {"ids": given})):
+        out, nxt = {}, {}
+        for e in (1, 2, 3):
+            gp = GraspPredicter("nut", artifact_dir=adir, engine=e)
+            gp.chunk = 5                      # the host draw runs in chunks of 5, 5 and 3
+            for call in (0, 1):               # the second call: no state survives the first
+                capsys.readouterr()
+                np.random.seed(3)
+                probs = np.stack([o[2] for o in gp.predict_batch(data, poses, **kw)])
+                nxt[e] = np.random.rand(2)
+                assert ("re-running on engine 1" in capsys.readouterr().out) == (e >= 2), (tag, e, call)
+                assert ctx.get_engine() == 3 and ctx.fp16_overflow() is False, (tag, e, call)
+                assert np.array_equal(probs.view(np.uint32), out.setdefault(e, probs).view(np.uint32)), (tag, e, call)
+        for e in (2, 3):                      # the re-run: engine 1's bits, numpy's generator where engine 1 leaves it
+            assert np.array_equal(out[e].view(np.uint32), out[1].view(np.uint32)), (tag, e)
+            assert np.array_equal(nxt[e], nxt[1]), (tag, e)
