@@ -28,9 +28,11 @@
 //
 // CTA = 384 threads: two consumer warpgroups, one producer warp and three helper warps.  Warpgroup w builds the front
 // of the tile's points [w TILE / 2, (w + 1) TILE / 2) in 64-row blocks, and in L3 computes the channels 64w .. 64w+63
-// of every 128-channel chunk over all the tile's points.  The helpers keep per-candidate work off the consumers' path:
-// the next candidate's pose inverse, T3 and T64 operand image, and the global fold (bias, ReLU, atomicMax) of each
-// finished candidate's max.
+// of every 128-channel chunk over all the tile's points.  The helpers keep the input rows and per-candidate work off
+// the consumers' path: one tile ahead they gather the tile's cloud rows and apply the float64 pose transform,
+// normalisation and T3 into the shared input tile X0 [TILE][6], which the consumers read at the start of the tile's
+// 6 -> 64 layer; they also write each candidate's T64 operand image and do the global fold (bias, ReLU, atomicMax) of
+// each finished candidate's max.
 #include <limits.h>
 #include <stdlib.h>
 
@@ -75,29 +77,35 @@ struct Misc {
   float bias0[64];
   float bias1[64];
   float bias2[128];
-  double pinv[12];
-  double mean[6];
+  double mean[6];                            // input normalisation: (w - mean) * sden
   double sden[6];
-  float T3[12];
-  unsigned long long full_bar[NSLOT_MAX];    // producer -> consumers: W3 slot landed
+  unsigned long long full_bar[NSLOT_MAX];   // producer -> consumers: W3 slot landed
   unsigned long long empty_bar[NSLOT_MAX];   // consumers -> producer: every consumer warp is done reading the slot
   unsigned long long w_bar;                  // resident W1 / W2 landed
-  // Per-candidate hand-offs; k counts the candidates of the CTA's range.  pinv, T3 and the T64 image exist once: the
-  // helpers rewrite them for candidate k + 1 between the consumers' last front of candidate k and their first of k + 1.
-  unsigned long long cand_bar;               // helpers -> consumers: pinv / T3 / T64 image of candidate k written
-  unsigned long long front_bar;              // consumers -> helpers: every consumer is past the last front of k
+  // X0 exists once: the helpers write the rows of tile t + 1 once every consumer has read those of tile t.
+  unsigned long long x0_full;                // helpers -> consumers: X0 holds the current tile's rows
+  unsigned long long x0_empty;               // consumers -> helpers: every consumer is past the tile's last X0 read
+  // Per-candidate hand-offs; k counts the candidates of the CTA's range.  The T64 image exists once: the helpers
+  // rewrite it for candidate k + 1 between the consumers' last L1 of candidate k and their first of k + 1.
+  unsigned long long cand_bar;               // helpers -> consumers: T64 image of candidate k written
+  unsigned long long front_bar;              // consumers -> helpers: every consumer is past the last L1 of k
   unsigned long long keys_bar[2];            // consumers -> helpers: candidate k's max is in keys[k & 1]
 };
-
-constexpr size_t SMEM_BYTES = MISC_OFF + sizeof(Misc);
-static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_90");
+// the input tile X0: float [TILE][6], the 6 input values of each point; a 24-byte row stride is conflict-free for the
+// 8 rows of a fragment
+constexpr uint32_t X0_OFF = MISC_OFF + sizeof(Misc);
+__host__ __device__ constexpr size_t smem_bytes(int passes) { return X0_OFF + (size_t)tile_points(passes) * 6 * 4; }
+static_assert(smem_bytes(1) <= 232448 && smem_bytes(3) <= 232448, "exceeds the 227 KB per-CTA shared memory of sm_90");
 
 #ifdef CG_EXPERIMENTS
-// Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer warp of TL_CTAS sampled CTAs (spread over
-// the grid) sums clock64() cycles per phase over its tiles and writes one record of TL_REC words: the TL_NPHASE
-// sums, its tile count and its total cycles.  TL_L3_WAIT and TL_RING lie inside TL_L3.
+// Phase timeline (developer builds, CG_TRUNK_TIMELINE=1): every consumer and helper warp of TL_CTAS sampled CTAs
+// (spread over the grid) sums clock64() cycles per phase over its tiles and writes one record of TL_REC words: the
+// phase sums, its tile count and its total cycles.  Consumer phases TL_*: TL_L3_WAIT and TL_RING lie inside TL_L3.
+// Helper phases TH_*: building X0 (gather, transform, stores), waiting for the consumers to free X0, the T64
+// hand-off and the fold.  A CTA's records: its NCW consumer warps, then its 3 helper warps.
 enum { TL_START, TL_INPUT, TL_FRONT, TL_X3, TL_L3, TL_L3_WAIT, TL_RING, TL_NPHASE };
-constexpr int TL_CTAS = 8, TL_REC = TL_NPHASE + 2;
+enum { TH_BUILD, TH_EMPTY, TH_CAND, TH_FOLD, TH_NPHASE };
+constexpr int TL_CTAS = 8, TL_REC = TL_NPHASE + 2, TL_WARPS = NCW + 3;
 __host__ __device__ constexpr int TL_STRIDE(int B) { return B >= TL_CTAS ? B / TL_CTAS : 1; }
 #define TL_PARAM , unsigned long long *tl
 #define TL_ARG(p) , p
@@ -142,6 +150,10 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
   const uint32_t wbar_s = misc_s + (uint32_t)offsetof(Misc, w_bar);
   const uint32_t cand_s = misc_s + (uint32_t)offsetof(Misc, cand_bar), front_s = misc_s + (uint32_t)offsetof(Misc, front_bar);
   const uint32_t keys_s = misc_s + (uint32_t)offsetof(Misc, keys_bar);
+  const uint32_t x0f_s = misc_s + (uint32_t)offsetof(Misc, x0_full), x0e_s = misc_s + (uint32_t)offsetof(Misc, x0_empty);
+  float *x0 = reinterpret_cast<float *>(smem + X0_OFF);
+  // the T64 image is the only per-candidate operand the consumers read
+  const bool t64_handoff = a.stage1_mode == 2;
 
   // ---- one-time setup --------------------------------------------------------------------------------------
   for (int i = tid; i < 6 * 64; i += NTC) S.w0[i] = a.l0.Wt[i];
@@ -152,7 +164,7 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
   if (tid < 128) S.bias2[tid] = a.l2.b[tid];
   if (a.in.x_direct == nullptr && tid < 6) {
     S.mean[tid] = a.in.mean ? a.in.mean[tid] : 0.0;
-    S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: the hot loop multiplies
+    S.sden[tid] = a.in.stdv ? 1.0 / (a.in.stdv[tid] + 1e-15) : 1.0;   // reciprocal: every row multiplies
   }
   if (tid == 0) {
     for (int i = 0; i < NSLOT; i++) {
@@ -160,6 +172,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
       mbar_init(empty_s + 8u * i, NCW);
     }
     mbar_init(wbar_s, 1);
+    mbar_init(x0f_s, NHELP);
+    mbar_init(x0e_s, NCW * 32);
     mbar_init(cand_s, NHELP);
     mbar_init(front_s, NCW * 32);
     mbar_init(keys_s, NCW * 32);
@@ -167,6 +181,36 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
     mbar_init_fence();
   }
   __syncthreads();
+
+#ifdef CG_EXPERIMENTS
+  // phase timeline of the sampled CTAs (scripts/trunk_timeline.py): cycles per phase summed over this warp's tiles
+  const bool tl_on = tl != nullptr && blockIdx.x % TL_STRIDE(gridDim.x) == 0 &&
+                     (int)(blockIdx.x / TL_STRIDE(gridDim.x)) < TL_CTAS;
+  unsigned long long tl_sum[TL_NPHASE] = {}, tl_t0 = clock64(), tl_t = tl_t0, tl_s;
+#define TL_MARK(phase)                   \
+  do {                                   \
+    const unsigned long long _t = clock64(); \
+    tl_sum[phase] += _t - tl_t;          \
+    tl_t = _t;                           \
+  } while (0)
+#define TL_SPAN_BEGIN() (tl_s = clock64())
+#define TL_SPAN_END(phase) (tl_sum[phase] += clock64() - tl_s)
+  // record of this warp (record index rec) over its `tiles` tiles
+#define TL_WRITE(rec, tiles)                                                                              \
+  do {                                                                                                    \
+    if (tl_on && lane == 0) {                                                                             \
+      unsigned long long *o = tl + ((size_t)(blockIdx.x / TL_STRIDE(gridDim.x)) * TL_WARPS + (rec)) * TL_REC; \
+      for (int p = 0; p < TL_NPHASE; p++) o[p] = tl_sum[p];                                               \
+      o[TL_NPHASE] = (unsigned long long)(tiles);                                                         \
+      o[TL_NPHASE + 1] = clock64() - tl_t0;                                                               \
+    }                                                                                                     \
+  } while (0)
+#else
+#define TL_MARK(phase) ((void)0)
+#define TL_SPAN_BEGIN() ((void)0)
+#define TL_SPAN_END(phase) ((void)0)
+#define TL_WRITE(rec, tiles) ((void)0)
+#endif
 
   if (warp == PROD_WARP) {
     // ======================= producer: resident W2 (+ shared W1), then W3 slot by slot =======================
@@ -189,147 +233,173 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
   }
 
   if (warp >= HELP_WARP) {
-    // ======================= helpers: per-candidate constants and the global fold =======================
-    // Candidate k's inputs are loaded (and T64 converted) before waiting for the consumers to leave candidate k - 1,
-    // so that only the shared-memory stores sit between the consumers' last front of k - 1 and their first of k.
-    // The fold of candidate k - 1 follows the hand-over of k; the consumers cannot fill keys[(k - 1) & 1] again
-    // before the hand-over of k + 1, which comes after that fold.
+    // ======================= helpers: the input tile X0, the T64 image and the global fold =======================
+    // The helpers walk the CTA's tiles one ahead of the consumers.  For tile t they load and transform the rows into
+    // registers, wait until every consumer has read X0 of tile t - 1 (in tile t - 1's 6 -> 64 layer) and only then
+    // store; tile t - 1's L1, L2 and L3 cover the loads.  Row n >= N of candidate b duplicates a valid point of b: it
+    // cannot change a max.  At the first tile of candidate k the T64 image comes first, in the same way: loaded and
+    // converted, then stored once every consumer is past the last L1 of k - 1 (just after their last X0 read of k - 1).
+    // The fold of k - 1 comes after X0 of k's first tile, so a fold never delays an X0; the consumers cannot fill
+    // keys[(k - 1) & 1] again before X0 of k + 1's first tile, which comes after that fold.
     const int ht = tid - HELP_WARP * 32;
-    for (int k = 0; k <= ncand; k++) {
-      if (k < ncand) {
-        const int b = b_first + k;
+    constexpr int XR = (TILE + NHELP - 1) / NHELP;   // X0 rows of this thread: ht + NHELP i < TILE
+    const bool xd = a.in.x_direct != nullptr;
+    // the candidate's pose inverse and T3 (mean and sden are the call's, in shared memory)
+    double pinv[12];
+    float t3[9] = {};
+    // x_direct rows travel as exact float -> double
+    auto fetch_id = [&](int b, int n) -> int {
+      if (n >= N) n = N - 1;
+      return (!xd && a.in.ids) ? __ldg(a.in.ids + (size_t)b * N + n) : n;
+    };
+    auto fetch_row = [&](int b, int id, double *r) {
+      if (xd) {
+        const float *xr = a.in.x_direct + ((size_t)b * N + id) * 6;
+#pragma unroll
+        for (int k = 0; k < 6; k++) r[k] = __ldg(xr + k);
+      } else {
+        const double *px = a.in.cloud_xyz + (size_t)id * 3;
+        const double *pn = a.in.cloud_nrm + (size_t)id * 3;
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          r[k] = __ldg(px + k);
+          r[3 + k] = __ldg(pn + k);
+        }
+      }
+    };
+    // input row (6 floats after pose transform / normalisation / T3)
+    auto finish_row = [&](const double *r, float *v) {
+      if (xd) {
+#pragma unroll
+        for (int k = 0; k < 6; k++) v[k] = (float)r[k];
+      } else {
+        const double x = r[0], y = r[1], z = r[2];
+        const double nx = r[3], ny = r[4], nz = r[5];
+        const double *R = pinv;
+        double w[6];
+        w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
+        w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
+        w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
+        w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
+        w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
+        w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
+#pragma unroll
+        for (int k = 0; k < 6; k++) v[k] = (float)((w[k] - S.mean[k]) * S.sden[k]);
+      }
+      if (a.T3) {  // xyz @ T3 (pointnet2.py:248), normals pass through (:245-250)
+        const float x = v[0], y = v[1], z = v[2];
+        v[0] = fmaf(z, t3[6], fmaf(y, t3[3], x * t3[0]));
+        v[1] = fmaf(z, t3[7], fmaf(y, t3[4], x * t3[1]));
+        v[2] = fmaf(z, t3[8], fmaf(y, t3[5], x * t3[2]));
+      }
+    };
+    // candidate kp of the range: bias and ReLU commute with the max (both are monotone), so they follow it.  Every
+    // one of the 1024 keys was stored by its channel's owner before the consumers arrived on keys_bar.
+    auto fold = [&](int kp) {
+      mbar_wait(keys_s + 8u * (kp & 1), ((uint32_t)kp >> 1) & 1u);
+      const uint32_t *kb = keys + (kp & 1) * 1024;
+      uint32_t *g = a.gmax_keys + (size_t)(b_first + kp) * 1024;
+      for (int ch = ht; ch < 1024; ch += NHELP) {
+        float m = cg_key2f(kb[ch]) + __ldg(&a.l3.b[ch]);
+        if (a.relu3) m = fmaxf(m, 0.f);
+        atomicMax(&g[ch], cg_f2key(m));
+      }
+    };
+    // the ids of this thread's rows of a tile are loaded one iteration ahead, so that a tile's build waits only for the
+    // dependent cloud rows
+    int ids[XR];
+    auto load_ids = [&](int t) {
+      const int b = t / ntiles, j = t - b * ntiles;
+#pragma unroll
+      for (int i = 0; i < XR; i++)
+        if (ht + NHELP * i < TILE) ids[i] = fetch_id(b, j * TILE + ht + NHELP * i);
+    };
+    load_ids(t_begin);
+#pragma unroll 1
+    for (int it = 0; it < my_tiles; it++) {
+      const int b = (t_begin + it) / ntiles, j = t_begin + it - b * ntiles, ci = b - b_first;
+      const bool cand_first = it == 0 || j == 0;
+      // the T64 image comes before the candidate's pinv / T3, so that those are not live beside it
+      if (cand_first && t64_handoff) {
         // T64 as the B operand of L1:  B[j][kk] = T64[kk][j]  (pointnet2.py:257).  Unit u = (row j, 8-wide K chunk
         // kc) is one 16-byte chunk of the hi and of the lo image; a warp's 32 rows read 32 consecutive floats.
         constexpr int TU = (64 * 8 + NHELP - 1) / NHELP;
         uint32_t t64h[TU][4], t64l[TU][4];
-        if (a.stage1_mode == 2) {
-          const float *Tb = a.T64 + (size_t)b * 4096;
+        const float *Tb = a.T64 + (size_t)b * 4096;
 #pragma unroll
-          for (int i = 0; i < TU; i++) {
-            const int u = ht + NHELP * i;
-            if (u < 512) {
-              float v[8];
+        for (int i = 0; i < TU; i++) {
+          const int u = ht + NHELP * i;
+          if (u < 512) {
+            float tv[8];
 #pragma unroll
-              for (int e = 0; e < 8; e++) v[e] = __ldg(Tb + (8 * (u >> 6) + e) * 64 + (u & 63));
+            for (int e = 0; e < 8; e++) tv[e] = __ldg(Tb + (8 * (u >> 6) + e) * 64 + (u & 63));
 #pragma unroll
-              for (int e = 0; e < 4; e++) split_bf16x2(v[2 * e], v[2 * e + 1], t64h[i][e], t64l[i][e]);
-            }
+            for (int e = 0; e < 4; e++) split_bf16x2(tv[2 * e], tv[2 * e + 1], t64h[i][e], t64l[i][e]);
           }
         }
-        double pinv[12];
-        const bool do_pinv = a.in.x_direct == nullptr && ht == 0;
-        if (do_pinv) pose_inverse(a.in.poses + (size_t)b * 16, pinv);
-        const float t3 = (a.T3 && ht < 9) ? a.T3[b * 9 + ht] : 0.f;
-        if (k > 0) mbar_wait(front_s, (uint32_t)(k - 1) & 1u);
-        if (a.stage1_mode == 2) {
+        if (ci > 0) mbar_wait(front_s, (uint32_t)(ci - 1) & 1u);
 #pragma unroll
-          for (int i = 0; i < TU; i++) {
-            const int u = ht + NHELP * i;
-            if (u < 512) {
-              const uint32_t off = row_chunk_off(u & 63, u >> 6);
-              *reinterpret_cast<uint4 *>(smem + W1_OFF + off) =
-                  make_uint4(t64h[i][0], t64h[i][1], t64h[i][2], t64h[i][3]);
-              *reinterpret_cast<uint4 *>(smem + W1_OFF + 8192 + off) =
-                  make_uint4(t64l[i][0], t64l[i][1], t64l[i][2], t64l[i][3]);
-            }
+        for (int i = 0; i < TU; i++) {
+          const int u = ht + NHELP * i;
+          if (u < 512) {
+            const uint32_t off = row_chunk_off(u & 63, u >> 6);
+            *reinterpret_cast<uint4 *>(smem + W1_OFF + off) =
+                make_uint4(t64h[i][0], t64h[i][1], t64h[i][2], t64h[i][3]);
+            *reinterpret_cast<uint4 *>(smem + W1_OFF + 8192 + off) =
+                make_uint4(t64l[i][0], t64l[i][1], t64l[i][2], t64l[i][3]);
           }
-          fence_proxy_async();
         }
-        if (do_pinv) {
-#pragma unroll
-          for (int i = 0; i < 12; i++) S.pinv[i] = pinv[i];
-        }
-        if (ht < 9) S.T3[ht] = t3;
+        fence_proxy_async();
         mbar_arrive(cand_s);
+        TL_MARK(TH_CAND);
       }
-      if (k > 0) {
-        // candidate k - 1: bias and ReLU commute with the max (both are monotone), so they follow it.  Every one of
-        // the 1024 keys was stored by its channel's owner before the consumers arrived on keys_bar.
-        const int kp = k - 1;
-        mbar_wait(keys_s + 8u * (kp & 1), ((uint32_t)kp >> 1) & 1u);
-        const uint32_t *kb = keys + (kp & 1) * 1024;
-        uint32_t *g = a.gmax_keys + (size_t)(b_first + kp) * 1024;
-        for (int ch = ht; ch < 1024; ch += NHELP) {
-          float m = cg_key2f(kb[ch]) + __ldg(&a.l3.b[ch]);
-          if (a.relu3) m = fmaxf(m, 0.f);
-          atomicMax(&g[ch], cg_f2key(m));
+      if (cand_first) {
+        if (!xd) pose_inverse(a.in.poses + (size_t)b * 16, pinv);
+        if (a.T3) {
+#pragma unroll
+          for (int e = 0; e < 9; e++) t3[e] = a.T3[b * 9 + e];
         }
+      }
+      // ---- X0 of tile it ----
+      float v[XR][6];
+      {
+        double r[XR][6];
+#pragma unroll
+        for (int i = 0; i < XR; i++)
+          if (ht + NHELP * i < TILE) fetch_row(b, ids[i], r[i]);
+#pragma unroll
+        for (int i = 0; i < XR; i++)
+          if (ht + NHELP * i < TILE) finish_row(r[i], v[i]);
+      }
+      TL_MARK(TH_BUILD);
+      if (it > 0) mbar_wait(x0e_s, (uint32_t)(it - 1) & 1u);
+      TL_MARK(TH_EMPTY);
+#pragma unroll
+      for (int i = 0; i < XR; i++)
+        if (ht + NHELP * i < TILE) {
+          float2 *dst = reinterpret_cast<float2 *>(x0 + (ht + NHELP * i) * 6);
+          dst[0] = make_float2(v[i][0], v[i][1]);
+          dst[1] = make_float2(v[i][2], v[i][3]);
+          dst[2] = make_float2(v[i][4], v[i][5]);
+        }
+      mbar_arrive(x0f_s);
+      if (it + 1 < my_tiles) load_ids(t_begin + it + 1);
+      TL_MARK(TH_BUILD);
+      if (cand_first && ci > 0) {
+        fold(ci - 1);
+        TL_MARK(TH_FOLD);
       }
     }
+    fold(ncand - 1);
+    TL_MARK(TH_FOLD);
+    TL_WRITE(NCW + warp - HELP_WARP, my_tiles);
     return;
   }
 
   // ======================= consumer warpgroups =======================
   const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, q = lane & 3;
   float vmax = 0.f;   // largest 128->1024 input seen by this thread (post-ReLU, fp16 engines): reported if beyond the fp16 range
-#ifdef CG_EXPERIMENTS
-  // phase timeline of the sampled CTAs (scripts/trunk_timeline.py): cycles per phase summed over this warp's tiles
-  const bool tl_on = tl != nullptr && blockIdx.x % TL_STRIDE(gridDim.x) == 0 &&
-                     (int)(blockIdx.x / TL_STRIDE(gridDim.x)) < TL_CTAS;
-  unsigned long long tl_sum[TL_NPHASE] = {}, tl_t0 = clock64(), tl_t = tl_t0, tl_s;
-#define TL_MARK(phase)                   \
-  do {                                   \
-    const unsigned long long _t = clock64(); \
-    tl_sum[phase] += _t - tl_t;          \
-    tl_t = _t;                           \
-  } while (0)
-#define TL_SPAN_BEGIN() (tl_s = clock64())
-#define TL_SPAN_END(phase) (tl_sum[phase] += clock64() - tl_s)
-#else
-#define TL_MARK(phase) ((void)0)
-#define TL_SPAN_BEGIN() ((void)0)
-#define TL_SPAN_END(phase) ((void)0)
-#endif
   mbar_wait(wbar_s, 0u);
-
-  // The ids of a tile's point rows are fetched one tile ahead (during the previous tile's L3) and the dependent
-  // cloud rows at the start of each 64-row block (the rows of both blocks do not fit beside the front's registers).  Row n >= N of candidate b duplicates a valid point of b: it cannot change a max.
-  // x_direct rows travel as exact float -> double.
-  auto fetch_id = [&](int b, int n) -> int {
-    if (n >= N) n = N - 1;
-    return (a.in.x_direct == nullptr && a.in.ids) ? __ldg(a.in.ids + (size_t)b * N + n) : n;
-  };
-  auto fetch_row = [&](int b, int id, double *r) {
-    if (a.in.x_direct) {
-      const float *xr = a.in.x_direct + ((size_t)b * N + id) * 6;
-#pragma unroll
-      for (int k = 0; k < 6; k++) r[k] = __ldg(xr + k);
-    } else {
-      const double *px = a.in.cloud_xyz + (size_t)id * 3;
-      const double *pn = a.in.cloud_nrm + (size_t)id * 3;
-#pragma unroll
-      for (int k = 0; k < 3; k++) {
-        r[k] = __ldg(px + k);
-        r[3 + k] = __ldg(pn + k);
-      }
-    }
-  };
-  // input row (6 floats after pose transform / normalisation / T3)
-  auto finish_row = [&](const double *r, float *v) {
-    if (a.in.x_direct) {
-#pragma unroll
-      for (int k = 0; k < 6; k++) v[k] = (float)r[k];
-    } else {
-      const double x = r[0], y = r[1], z = r[2];
-      const double nx = r[3], ny = r[4], nz = r[5];
-      const double *R = S.pinv;
-      double w[6];
-      w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
-      w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
-      w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
-      w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
-      w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
-      w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
-#pragma unroll
-      for (int k = 0; k < 6; k++) v[k] = (float)((w[k] - S.mean[k]) * S.sden[k]);
-    }
-    if (a.T3) {  // xyz @ T3 (pointnet2.py:248), normals pass through (:245-250)
-      const float x = v[0], y = v[1], z = v[2];
-      v[0] = fmaf(z, S.T3[6], fmaf(y, S.T3[3], x * S.T3[0]));
-      v[1] = fmaf(z, S.T3[7], fmaf(y, S.T3[4], x * S.T3[1]));
-      v[2] = fmaf(z, S.T3[8], fmaf(y, S.T3[5], x * S.T3[2]));
-    }
-  };
 
   // W3 ring slot and mbarrier phase of K-block kb of chunk c of the current tile
   uint32_t gslot = 0;   // W3 slots consumed before the current tile
@@ -338,32 +408,29 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
 
   // this thread's front rows of a tile: prow(blk) and prow(blk) + 8 of each 64-row block blk
   auto prow = [&](int blk) { return wg * (TILE / 2) + blk * 64 + w4 * 16 + g; };
-  int ids[NBLK][2];
-  {
-    const int j = t_begin - b_first * ntiles;
-#pragma unroll
-    for (int blk = 0; blk < NBLK; blk++)
-#pragma unroll
-      for (int r = 0; r < 2; r++) ids[blk][r] = fetch_id(b_first, j * TILE + prow(blk) + 8 * r);
-  }
   TL_MARK(TL_START);
   for (int it = 0; it < my_tiles; it++) {
     // tile j of candidate b, candidate ci of the range; the candidate's first / last tile in this range
     const int b = (t_begin + it) / ntiles, j = t_begin + it - b * ntiles, ci = b - b_first;
     const bool cand_first = it == 0 || j == 0, cand_last = it + 1 == my_tiles || j + 1 == ntiles;
-    if (cand_first) mbar_wait(cand_s, (uint32_t)ci & 1u);   // pinv / T3 / T64 image of candidate b
+    if (cand_first && t64_handoff) mbar_wait(cand_s, (uint32_t)ci & 1u);   // T64 image of candidate b
+    mbar_wait(x0f_s, (uint32_t)it & 1u);   // X0 holds this tile's input rows
 #pragma unroll 1
     for (int blk = 0; blk < NBLK; blk++) {
       const int p0 = j * TILE + prow(blk);   // this thread's rows: points p0 and p0 + 8
       // ---- 6 -> 64 (+bias, ReLU) straight into the D-fragment layout of a 64-column tile ----
       float d64[32];
       {
-        double r0[6], r1[6];
-        fetch_row(b, blk == 0 ? ids[0][0] : ids[NBLK - 1][0], r0);   // constant indices: ids stays in registers
-        fetch_row(b, blk == 0 ? ids[0][1] : ids[NBLK - 1][1], r1);
         float v0[6], v1[6];
-        finish_row(r0, v0);
-        finish_row(r1, v1);
+        const float2 *x0r = reinterpret_cast<const float2 *>(x0 + prow(blk) * 6);
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          const float2 u0 = x0r[k], u1 = x0r[24 + k];   // rows prow and prow + 8
+          v0[2 * k] = u0.x;
+          v0[2 * k + 1] = u0.y;
+          v1[2 * k] = u1.x;
+          v1[2 * k + 1] = u1.y;
+        }
         TL_MARK(TL_INPUT);
 #pragma unroll
         for (int m = 0; m < 8; m++)
@@ -381,6 +448,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
             d64[4 * m + 2 + e] = fmaxf(o1, 0.f);
           }
       }
+      // this thread's last X0 read of the tile is done: the helpers may store the next tile's rows
+      if (blk == NBLK - 1) mbar_arrive(x0e_s);
       uint32_t xh[4][4], xl[4][4];   // A fragments of the layer input (K = 64), bf16 hi + lo
       // ---- L1: 64 -> 64 (STNkd shared conv, or the per-candidate T64 feature transform) ----
       if (has_l1) {
@@ -418,8 +487,8 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
           }
         }
       }
-      // the last read of candidate b's pinv / T3 / T64 image in this range is done: the helpers may replace them
-      if (cand_last && blk == NBLK - 1) mbar_arrive(front_s);
+      // the last read of candidate b's T64 image in this range is done: the helpers may replace it
+      if (t64_handoff && cand_last && blk == NBLK - 1) mbar_arrive(front_s);
       // ---- L2: 64 -> 128 ----
       float acc[64];
       d_to_a<4, false>(d64, xh, xl);
@@ -552,15 +621,6 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
         }
       }
     };
-    // the next tile's ids are loaded while nothing depends on them (a last tile re-reads its own)
-    {
-      const int nt = t_begin + it + (it + 1 < my_tiles ? 1 : 0);
-      const int nb = nt / ntiles, pn = (nt - nb * ntiles) * TILE;
-#pragma unroll
-      for (int blk = 0; blk < NBLK; blk++)
-#pragma unroll
-        for (int r = 0; r < 2; r++) ids[blk][r] = fetch_id(nb, pn + prow(blk) + 8 * r);
-    }
 #pragma unroll 1
     for (int u0 = 0; u0 < NU; u0 += GROUP) {
       float acc3[2][64];   // even / odd units
@@ -587,18 +647,11 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
     TL_MARK(TL_L3);
   }
   if (F16 && vmax > 65504.f && a.ovf_flag) atomicOr(a.ovf_flag, 1u);
-#ifdef CG_EXPERIMENTS
-  if (tl_on && lane == 0) {
-    unsigned long long *o = tl + ((size_t)(blockIdx.x / TL_STRIDE(gridDim.x)) * NCW + warp) * TL_REC;
-#pragma unroll
-    for (int p = 0; p < TL_NPHASE; p++) o[p] = tl_sum[p];
-    o[TL_NPHASE] = (unsigned long long)my_tiles;
-    o[TL_NPHASE + 1] = clock64() - tl_t0;
-  }
-#endif
+  TL_WRITE(warp, my_tiles);
 #undef TL_MARK
 #undef TL_SPAN_BEGIN
 #undef TL_SPAN_END
+#undef TL_WRITE
 }
 
 }  // namespace
@@ -606,9 +659,9 @@ __global__ void __launch_bounds__(NTC, 1) trunk_tc_kernel(const cg_trunk_args a 
 size_t cg_tc_image_bytes() { return (size_t)IMG_W3H_OFF + IMG_W3H; }
 
 int cg_tc_prepare(cg_ctx *ctx, const float *Wt3, const float *Wt2, const float *Wt1, void *dst_dev, int *f16_ok) {
-  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(3)));
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(2)));
+  CG_CUDA(ctx, cudaFuncSetAttribute(trunk_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes(1)));
   float wmax = 0.f;
   for (size_t i = 0; i < (size_t)128 * 1024; i++) wmax = fmaxf(wmax, fabsf(Wt3[i]));
   *f16_ok = (wmax < 65504.f) ? 1 : 0;   // otherwise the fp16 image would hold infinities
@@ -649,15 +702,16 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
 #ifdef CG_EXPERIMENTS
   static const bool timeline = getenv("CG_TRUNK_TIMELINE") && atoi(getenv("CG_TRUNK_TIMELINE")) != 0;
   unsigned long long *tl = nullptr;
-  const size_t tl_words = (size_t)TL_CTAS * NCW * TL_REC;
+  const size_t tl_words = (size_t)TL_CTAS * TL_WARPS * TL_REC;
   if (timeline) {
     CG_CUDA(ctx, cudaMallocAsync(&tl, tl_words * 8, ctx->stream));
     CG_CUDA(ctx, cudaMemsetAsync(tl, 0, tl_words * 8, ctx->stream));
   }
 #endif
-  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
-  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
-  else trunk_tc_kernel<1><<<grid, NTC, SMEM_BYTES, ctx->stream>>>(a TL_ARG(tl));
+  const size_t smem = smem_bytes(passes);
+  if (passes == 3) trunk_tc_kernel<3><<<grid, NTC, smem, ctx->stream>>>(a TL_ARG(tl));
+  else if (passes == 2) trunk_tc_kernel<2><<<grid, NTC, smem, ctx->stream>>>(a TL_ARG(tl));
+  else trunk_tc_kernel<1><<<grid, NTC, smem, ctx->stream>>>(a TL_ARG(tl));
   CG_LAUNCH_CHECK(ctx);
 #ifdef CG_EXPERIMENTS
   if (timeline) {
@@ -665,31 +719,38 @@ int cg_trunk_launch_tc(cg_ctx *ctx, const cg_trunk_args &a) {
     CG_CUDA(ctx, cudaMemcpyAsync(h.data(), tl, tl_words * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CG_CUDA(ctx, cudaFreeAsync(tl, ctx->stream));
     CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    // cycles of one warp, averaged over the consumer warps of the sampled CTAs; the warps of a CTA run
+    // cycles of one warp, averaged over the consumer (helper) warps of the sampled CTAs; the warps of a CTA run
     // concurrently, so "total" is also the CTA's cycles
-    double sum[TL_NPHASE + 1] = {}, tiles = 0;
+    double sum[TL_NPHASE + 1] = {}, tiles = 0, hsum[TH_NPHASE + 1] = {}, htiles = 0;
     int recs = 0;
-    for (int r = 0; r < TL_CTAS * NCW; r++) {
+    for (int r = 0; r < TL_CTAS * TL_WARPS; r++) {
       const unsigned long long *o = &h[(size_t)r * TL_REC];
       if (o[TL_NPHASE] == 0) continue;
-      for (int p = 0; p < TL_NPHASE; p++) sum[p] += (double)o[p];
-      sum[TL_NPHASE] += (double)o[TL_NPHASE + 1];
-      tiles += (double)o[TL_NPHASE];
-      recs++;
+      if (r % TL_WARPS < NCW) {
+        for (int p = 0; p < TL_NPHASE; p++) sum[p] += (double)o[p];
+        sum[TL_NPHASE] += (double)o[TL_NPHASE + 1];
+        tiles += (double)o[TL_NPHASE];
+        recs++;
+      } else {
+        for (int p = 0; p < TH_NPHASE; p++) hsum[p] += (double)o[p];
+        hsum[TH_NPHASE] += (double)o[TL_NPHASE + 1];
+        htiles += (double)o[TL_NPHASE];
+      }
     }
     if (recs > 0) {
       // per 128 points, so that tiles of 128 and 256 points compare directly; tensor-pipe cycles of 128 points at
       // 2048 dense fp16 / bf16 MAC per clock per SM
-      const double p128 = tiles * (tp / 128);
+      const double p128 = tiles * (tp / 128), h128 = htiles * (tp / 128);
       const double l3 = 128.0 * 128 * 1024 / 2048 * passes, l12 = 128.0 * 64 * (128 + (a.stage1_mode ? 64 : 0)) * 3 / 2048;
       const double tot = sum[TL_NPHASE] / p128;
       fprintf(stderr,
               "[trunk-timeline] passes=%d B=%d N=%d stage1=%d tile=%d tiles/CTA=%.0f warps=%d  clk/128 pts: start %.0f  "
               "input %.0f  front %.0f  x3 %.0f  l3 %.0f (wgmma-wait %.0f, ring-wait %.0f)  total %.0f  | tensor work "
-              "%.0f clk/128 pts -> busy %.1f%%\n",
+              "%.0f clk/128 pts -> busy %.1f%%  | helpers: x0 build %.0f  x0-empty wait %.0f  t64 %.0f  fold %.0f\n",
               passes, a.B, a.N, a.stage1_mode, tp, tiles / recs, recs, sum[TL_START] / p128, sum[TL_INPUT] / p128,
               sum[TL_FRONT] / p128, sum[TL_X3] / p128, sum[TL_L3] / p128, sum[TL_L3_WAIT] / p128, sum[TL_RING] / p128,
-              tot, l3 + l12, 100.0 * (l3 + l12) / tot);
+              tot, l3 + l12, 100.0 * (l3 + l12) / tot, hsum[TH_BUILD] / h128, hsum[TH_EMPTY] / h128,
+              hsum[TH_CAND] / h128, hsum[TH_FOLD] / h128);
     }
   }
 #endif

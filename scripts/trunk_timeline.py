@@ -6,12 +6,18 @@ engine with CG_TRUNK_TIMELINE=1.  Every trunk launch prints one line to stderr: 
 per 128 points (engine 3 runs 256-point tiles, engines 1 and 2 128-point tiles), averaged over the warps of 8 sampled
 CTAs, split into
   start   W2 landed (once per CTA, spread over its tiles)
-  input   the cloud-row loads and the float64 input transform of the rows
+  input   waiting for the helpers to fill the input tile X0, and reading this warp's rows from it
   front   6->64 FMA, L1, L2
   x3      waiting for the other warpgroup to leave the previous tile's L3, storing X3, and the barrier after it
   l3      128->1024 and the max; of which wgmma-wait = waiting for a wgmma group, ring-wait = waiting for W3 slots
 and the tensor-busy estimate: the tensor work of 128 points at 2048 dense fp16 / bf16 MAC per clock per SM over their
-cycles.
+cycles.  The same line gives the helper warps' cycles per 128 points, averaged over the helper warps of the sampled
+CTAs:
+  x0 build       gathering the cloud rows, the float64 transform, and storing them into X0
+  x0-empty wait  waiting for the consumers to finish reading the previous tile's X0
+  t64            converting and storing each candidate's T64 operand image (encoder trunk), with its wait
+  fold           the global fold of each finished candidate's max, with its wait
+The helpers keep up when x0-empty wait is large beside x0 build and the consumers' input stays small.
 
     python scripts/trunk_timeline.py [--engines 3,1] [-B 4096] [-N 1024]
 """
