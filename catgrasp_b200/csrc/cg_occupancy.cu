@@ -11,7 +11,7 @@
 // are recomputed from the integer cell index at every step (no accumulation); a hit counts when |cell centre| <=
 // |sample|.  The oracle is compiled with -ffp-contract=off; nvcc contracts a*b + c into an FMA by default, so every
 // floating-point operation of the cast kernel is written as an explicit round-to-nearest intrinsic, which nvcc never
-// fuses (tests/test_bitexact_codegen.py checks the PTX for FMAs).  An exact rational statement of the rule, without
+// fuses (tests/test_codegen.py checks the PTX for FMAs).  An exact rational statement of the rule, without
 // the kernel's arithmetic or its early exit, is oracle/occupancy_exact.py.
 // The reference's own function, compiled against a restatement of the octomap calls it makes (oracle/build_ref.py,
 // oracle/ref_shim/octomap/octomap.h), returns exactly the same samples (tests/test_mycpp_golden.py); parity with the

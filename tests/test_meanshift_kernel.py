@@ -4,7 +4,7 @@ PointGroupPredictor.predict (tests/golden/segment.npz).
 
 Seeded mutations and the test that catches each:
   - membership `d2 < bw2` for `<=`                   test_dyadic_lattice_on_the_boundary (neighbours at d2 == bw^2)
-  - FMA contraction in the ascent's distance        test_meanshift_codegen.py::test_no_fused_multiply_add
+  - FMA contraction in the ascent's distance        test_codegen.py::test_entry_contract (ascent_kernel's no_fma)
   - a float64 sum in place of the int64 sum         test_piles, test_numpy_and_tensor_input_agree (centres move)
   - suppression without the (count, x, y, z) order  test_chain_of_equal_count_modes (the greedy order decides)
   - centres collapsed by bit pattern, not value     test_signed_zeros_and_duplicates

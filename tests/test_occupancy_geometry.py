@@ -25,7 +25,7 @@ occupancy_ref.c, which shares the kernel's control flow (the mutants are not bui
 - the step of a negative axis started at k + 1 (``step > 0 ? 1 : 0`` read as 1 for both signs), in both:
   test_exact_reference_agrees_with_occupancy_ref[straddle];
 - the origin cell not tested first: test_exact_reference_agrees_with_occupancy_ref[at_camera];
-- contraction re-enabled in the cast kernel: tests/test_bitexact_codegen.py (this file cannot see a 1-ulp change).
+- contraction re-enabled in the cast kernel: tests/test_codegen.py (this file cannot see a 1-ulp change).
 
 No case can tell the final ``cdist <= dist_q`` (common.cpp:388-393) from ``<``: they differ only when the float64
 centre distance equals the sample's float32 norm, and a cell centre's distance is never a float32.  Its square is
