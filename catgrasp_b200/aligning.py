@@ -4,6 +4,9 @@ hypotheses scored on the GPU (csrc/cg_ransac.cu; SURVEY.md 8f F1).
 The host keeps exactly the reference's RNG consumption -- one ``np.random.choice(len(source), 4, replace=False)`` per
 iteration, all drawn up front (aligning.py:91-97) -- and the reference's selection rule (first maximum of the inlier
 ratio over the hypotheses that survive the gates, aligning.py:105-117).
+
+``ransac9d_pose`` is the device-side form used by NunocsPredicter.predict: both thresholds scored, selected and
+checked in one launch on CUDA tensors (cg_ransac9d_pose_dev), with the subsets given by the caller.
 """
 import numpy as np
 
@@ -39,3 +42,36 @@ def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree
     errs = np.linalg.norm((best_transform @ np.c_[source, np.ones(N)].T).T[:, :3] - target, axis=-1)
     inliers = np.where(errs <= PassThreshold)[0]
     return best_transform, inliers
+
+
+REC_PER_THR = 19     # include/catgrasp_b200.h, cg_ransac9d_pose_dev's record
+
+
+def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 99]), min_scale=np.array([0, 0, 0]),
+                  max_dimensions=None, ratio_threshold=0.003):
+    """The NUNOCS pose search on the device, for CUDA tensors ``source`` / ``target`` (N,3) float64 and ``ids``
+    (T*H,4) int32 (rows t*H .. t*H+H-1 are threshold t's subsets), T = len(thresholds) in {1, 2}.  One launch, no
+    synchronisation.  Returns a dict of CUDA tensors (views of the launch's record):
+      per threshold: 'winner' (T,) the first maximum among valid hypotheses or -1, 'count' (T,) its inlier count,
+      'T' (T,4,4) its transform (bit for bit estimate9DTransform's on the same subsets), 'count_ratio' (T,) its
+      count of residuals <= ratio_threshold;
+      overall: 'chosen' () the threshold predict would pick or -1, 'pose' (4,4), 'best_ratio' ()."""
+    import torch
+    from . import _lib
+    ctx, source, target = _lib.inputs(source, target, dtype=torch.float64)
+    _, ids = _lib.inputs(ids, dtype=torch.int32, ctx=ctx)
+    thr = np.ascontiguousarray(np.asarray(thresholds, dtype=np.float64).reshape(-1))
+    T = thr.size
+    assert T in (1, 2) and ids.shape[0] % T == 0 and ids.shape[1] == 4, (thr, tuple(ids.shape))
+    H = ids.shape[0] // T
+    mins = np.ascontiguousarray(np.asarray(min_scale, dtype=np.float64).reshape(3))
+    maxs = np.ascontiguousarray(np.asarray(max_scale, dtype=np.float64).reshape(3))
+    mdim = None if max_dimensions is None else np.ascontiguousarray(np.asarray(max_dimensions, dtype=np.float64).reshape(3))
+    rec = torch.empty((T * REC_PER_THR + 18,), dtype=torch.float64, device=source.device)
+    ctx.call("cg_ransac9d_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs, mdim,
+             float(ratio_threshold), rec)
+    per = rec[:T * REC_PER_THR].view(T, REC_PER_THR)
+    tail = rec[T * REC_PER_THR:]
+    return {"winner": per[:, 0].to(torch.int64), "count": per[:, 1].to(torch.int64), "T": per[:, 2:18].view(T, 4, 4),
+            "count_ratio": per[:, 18].to(torch.int64), "chosen": tail[0].to(torch.int64), "pose": tail[1:17].view(4, 4),
+            "best_ratio": tail[17], "record": rec}

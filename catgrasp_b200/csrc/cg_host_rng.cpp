@@ -104,6 +104,36 @@ int upper_scalar(const uint32_t *w, int avail, uint32_t &i_io, uint32_t &mask_io
   return k;
 }
 
+// The scan with the accepted words kept: step i's j goes to js[top - i] (top = M - 1), so js lists the shuffle's
+// swap partners from i = M-1 down.  A rejected word's store lands in the slot the next accepted word overwrites.
+int record_scalar(const uint32_t *w, int avail, uint32_t &i_io, uint32_t &mask_io, uint32_t *js, uint32_t top) {
+  uint32_t i = i_io, mask = mask_io;
+  int k = 0;
+  while (k < avail && i >= 1) {
+    const uint32_t lim = mask >> 1, m = mask;
+    while (k < avail && i > lim) {
+      const uint32_t j = w[k] & m;
+      js[top - i] = j;
+      i -= (j <= i) ? 1u : 0u;
+      k++;
+    }
+    if (i <= lim) mask >>= 1;
+  }
+  i_io = i;
+  mask_io = mask;
+  return k;
+}
+
+// Backward pass over the steps i = i0 .. M-1 (js[M-1-i] = j_i) for output slots that sit below every remaining i: the
+// swap at step i moves a slot's element only if the slot tracks position j_i, and then it came from position i.
+void follow_scalar(const uint32_t *js, uint32_t M, uint32_t i, uint32_t *pos, int n) {
+  for (; i < M; i++) {
+    const uint32_t j = js[M - 1 - i];
+    for (int k = 0; k < n; k++)
+      if (pos[k] == j) { pos[k] = i; break; }
+  }
+}
+
 #if CG_X86
 // ---- AVX2 ---------------------------------------------------------------------------------------------------------
 #define CG_AVX2 __attribute__((target("avx2,popcnt")))
@@ -247,6 +277,60 @@ CG_AVX512 int upper_avx512(const uint32_t *w, int avail, uint32_t &i_io, uint32_
   return k;
 }
 
+CG_AVX512 int record_avx512(const uint32_t *w, int avail, uint32_t &i_io, uint32_t &mask_io, uint32_t *js, uint32_t top) {
+  uint32_t i = i_io, mask = mask_io;
+  int k = 0;
+  const __m512i lane = _mm512_setr_epi32(0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15);
+  while (k < avail && i >= 1) {
+    const uint32_t lim = mask >> 1, m = mask;
+    const __m512i vm = _mm512_set1_epi32((int)m);
+    while (k + 16 <= avail && i > lim + 16) {
+      const __m512i v = _mm512_and_si512(_mm512_loadu_si512(w + k), vm);
+      const __mmask16 rej = _mm512_cmpgt_epu32_mask(v, _mm512_set1_epi32((int)i));
+      const __mmask16 nacc = _mm512_cmpgt_epu32_mask(v, _mm512_sub_epi32(_mm512_set1_epi32((int)i), lane));
+      if (rej != nacc) break;
+      // accepted j's in step order; the full 16-wide store writes past them into slots later steps overwrite
+      _mm512_storeu_si512(js + (top - i), _mm512_maskz_compress_epi32((__mmask16)~nacc, v));
+      i -= 16u - (uint32_t)__builtin_popcount((unsigned)nacc);
+      k += 16;
+    }
+    for (int n = 0; n < 16 && k < avail && i > lim; n++, k++) {
+      const uint32_t j = w[k] & m;
+      js[top - i] = j;
+      i -= (j <= i) ? 1u : 0u;
+    }
+    if (i <= lim) mask >>= 1;
+  }
+  i_io = i;
+  mask_io = mask;
+  return k;
+}
+
+CG_AVX512 void follow_avx512(const uint32_t *js, uint32_t M, uint32_t i, uint32_t *pos, int n) {
+  __m512i P[16];   // the tracked positions, broadcast
+  for (int k = 0; k < n; k++) P[k] = _mm512_set1_epi32((int)pos[k]);
+  // 32 steps at a time: steps i .. i+15 are lanes 15 .. 0 of js[M-16-i ..], steps i+16 .. i+31 lanes 15 .. 0 of
+  // js[M-32-i ..]; the earliest hit is the highest set lane, and the scan resumes right after it
+  while (i + 32 <= M) {
+    const __m512i lo = _mm512_loadu_si512(js + (M - 16 - i)), hi = _mm512_loadu_si512(js + (M - 32 - i));
+    __mmask16 hlo = 0, hhi = 0;
+    for (int k = 0; k < n; k++) {
+      hlo |= _mm512_cmpeq_epu32_mask(lo, P[k]);
+      hhi |= _mm512_cmpeq_epu32_mask(hi, P[k]);
+    }
+    if (!(hlo | hhi)) {
+      i += 32;
+      continue;
+    }
+    const uint32_t step = hlo ? i + (uint32_t)__builtin_clz((unsigned)hlo) - 16u : i + (uint32_t)__builtin_clz((unsigned)hhi);
+    const uint32_t j = js[M - 1 - step];
+    for (int k = 0; k < n; k++)
+      if (pos[k] == j) { pos[k] = step; P[k] = _mm512_set1_epi32((int)step); break; }
+    i = step + 1;
+  }
+  follow_scalar(js, M, i, pos, n);
+}
+
 #endif   // CG_X86
 
 struct Isa {
@@ -254,6 +338,8 @@ struct Isa {
   void (*temper)(const uint32_t *, uint32_t *, int);
   int (*scan)(const uint32_t *, int, uint32_t &, uint32_t &);
   int (*upper)(const uint32_t *, int, uint32_t &, uint32_t &, uint32_t, int32_t *, uint32_t);
+  int (*record)(const uint32_t *, int, uint32_t &, uint32_t &, uint32_t *, uint32_t);
+  void (*follow)(const uint32_t *, uint32_t, uint32_t, uint32_t *, int);
   int level;
 };
 Isa pick_isa(int force) {
@@ -261,12 +347,12 @@ Isa pick_isa(int force) {
   __builtin_cpu_init();
   int level = __builtin_cpu_supports("avx512f") ? 2 : (__builtin_cpu_supports("avx2") ? 1 : 0);
   if (force >= 0 && force < level) level = force;
-  if (level == 2) return {refill_avx512, temper_avx512, scan_avx512, upper_avx512, 2};
-  if (level == 1) return {refill_avx2, temper_avx2, scan_avx2, upper_scalar, 1};
+  if (level == 2) return {refill_avx512, temper_avx512, scan_avx512, upper_avx512, record_avx512, follow_avx512, 2};
+  if (level == 1) return {refill_avx2, temper_avx2, scan_avx2, upper_scalar, record_scalar, follow_scalar, 1};
 #else
   (void)force;
 #endif
-  return {refill_scalar, temper_scalar, scan_scalar, upper_scalar, 0};
+  return {refill_scalar, temper_scalar, scan_scalar, upper_scalar, record_scalar, follow_scalar, 0};
 }
 Isa g_isa = pick_isa(-1);
 
@@ -330,6 +416,41 @@ void shuffle_skip(Mt &g, int64_t M) {
   }
 }
 
+// Small subsets (n_pts <= SLOT_MAX): follow the n_pts output slots instead of replaying the shuffle.  The walk keeps
+// every step's j (js needs M - 1 + 16 entries); the element that ends in slot k is found by undoing the swaps from the
+// last step (i = 1) up: a slot's position changes at step i only if it is i or j_i.  Above the slots (i >= n_pts) a
+// tracked position is always below i, so only j_i == position matters, and that is rare: the backward pass is n_pts
+// compares per step, a fraction of the walk's cost.
+constexpr int SLOT_MAX = 16;
+
+void shuffle_slots(Mt &g, int64_t M, int32_t n_pts, uint32_t *js, int32_t *out) {
+  const uint32_t top = (uint32_t)(M - 1);
+  uint32_t mask = mask_of(top);
+  uint32_t i = top;
+  uint32_t tmp[MT_N];
+  while (i >= 1) {
+    if (g.pos == MT_N) {
+      g_isa.refill(g.key);
+      g.pos = 0;
+    }
+    const int avail = MT_N - g.pos;
+    g_isa.temper(g.key + g.pos, tmp, avail);
+    g.pos += g_isa.record(tmp, avail, i, mask, js, top);
+  }
+  uint32_t pos[SLOT_MAX];
+  for (int k = 0; k < n_pts; k++) pos[k] = (uint32_t)k;
+  uint32_t s = 1;
+  for (; s < (uint32_t)n_pts && s < (uint32_t)M; s++) {   // the steps among the slots: the full swap
+    const uint32_t j = js[top - s];
+    for (int k = 0; k < n_pts; k++) {
+      if (pos[k] == s) pos[k] = j;
+      else if (pos[k] == j) pos[k] = s;
+    }
+  }
+  g_isa.follow(js, (uint32_t)M, s, pos, n_pts);
+  for (int k = 0; k < n_pts; k++) out[k] = (int32_t)pos[k];
+}
+
 inline void backoff(int &spins) {
   if (++spins < 4096) {
 #if CG_X86
@@ -380,6 +501,12 @@ extern "C" int cg_host_legacy_choice(uint32_t *key, int32_t *pos, int64_t M, int
     return CG_OK;
   }
   // replace=False: permutation(M)[:n_pts]: shuffle arange(M) from the top, j = random_interval(i)
+  if (n_pts <= SLOT_MAX) {   // one thread: the walk is the whole cost, workers would only wait for it
+    std::vector<uint32_t> js((size_t)M + 16);
+    for (int64_t c = 0; c < count; c++) shuffle_slots(g, M, n_pts, js.data(), out + c * (int64_t)n_pts);
+    *pos = g.pos;
+    return CG_OK;
+  }
   if (nthreads <= 0) {
     // the walk is ~6x faster than one replay: a dozen workers keep up with it, more only add wake-up traffic
     nthreads = (int32_t)std::thread::hardware_concurrency();

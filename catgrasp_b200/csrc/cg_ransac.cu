@@ -7,7 +7,12 @@
 //   -> R := U V^T, det > 0 (:51-53) -> T = [R diag(scales) | t] (:55)
 //   -> extent of inv(T) target <= max_dimensions (:58-62) -> inlier ratio |T src - tgt| <= threshold (:64-67).
 // One CTA per hypothesis: thread 0 does the 4x4 solve / 3x3 polar step in float64, all threads stream the N points.
-// The 4-subsets are drawn on the host with the reference's numpy RNG calls (aligning.py:91-97).
+// The 4-subsets come from the host (the reference's numpy RNG calls, aligning.py:91-97) or from cg_draw_ids_dev.
+//
+// cg_ransac9d_pose_dev runs the same kernel over one or two thresholds (one set of H subsets each) and also does what
+// the host did with the scores: the first maximum among valid hypotheses per threshold (aligning.py:115) through a
+// 64-bit atomicMax key, then, in the last CTA to finish (fence + counter), predict's choice between the thresholds
+// (predicter.py:152-172: det test, inlier ratio at 3 mm, strict `>`).  Nothing comes back to the host.
 #include "cg_common.cuh"
 
 namespace {
@@ -121,22 +126,42 @@ __device__ void jacobi3(double A[3][3], double V[3][3], double w[3]) {
   for (int i = 0; i < 3; i++) w[i] = A[i][i];
 }
 
+// Gates of one launch, by value: the scale gates, the optional extent gate and up to two thresholds.
+struct Gates {
+  double thr[2];
+  double min_scale[3], max_scale[3], max_dims[3];
+  int has_max_dims;
+};
+
+// The fused selection (cg_ransac9d_pose_dev); keys == nullptr switches it off (cg_ransac9d_host).
+//   keys[t]: per-threshold atomicMax of (count << 32) | (0xFFFFFFFF - h) over valid hypotheses (0: none valid);
+//   keys[n_thr]: the completion counter.  record: see include/catgrasp_b200.h.
+struct Fuse {
+  unsigned long long *keys;
+  double *record;
+  double ratio_thr;
+  int n_thr;
+};
+
+constexpr int REC_PER_THR = 19;   // winner, count, T (16), count at ratio_thr
+
 __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__ src, const double *__restrict__ tgt, int N,
-                                                      const int32_t *__restrict__ ids, int H, double thr,
-                                                      const double *__restrict__ min_scale,
-                                                      const double *__restrict__ max_scale,
-                                                      const double *__restrict__ max_dims, double *__restrict__ out_ratio,
-                                                      double *__restrict__ out_T, unsigned char *__restrict__ out_valid) {
+                                                      const int32_t *__restrict__ ids, int H, const Gates g,
+                                                      double *__restrict__ out_ratio, double *__restrict__ out_T,
+                                                      unsigned char *__restrict__ out_valid, const Fuse f) {
   __shared__ double T[12], Ti[12];
   __shared__ int ok;
   __shared__ double red[RT / 32][6];
   __shared__ int redc[RT / 32];
-  const int h = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  __shared__ int last;
+  // one CTA per (threshold, hypothesis): CTA b scores hypothesis b % H of threshold b / H with the subset ids[b]
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const double thr = b < H ? g.thr[0] : g.thr[1];   // no run-time index into the parameter block
   if (tid == 0) {
     ok = 0;
     double M[4][4], B[4][3], X[4][3], M0[4][4], B0[4][3];
     for (int i = 0; i < 4; i++) {
-      const int id = ids[h * 4 + i];
+      const int id = ids[(size_t)b * 4 + i];
       // cv2.estimateAffine3D (aligning.py:27) narrows its inputs to CV_32F before the double-precision solve:
       // the four sample points go through float, the residual pass below keeps the caller's float64.
       for (int k = 0; k < 3; k++) {
@@ -157,7 +182,7 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
       }
       for (int j = 0; j < 3; j++) {   // scales = column norms (aligning.py:41)
         sc[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
-        if (sc[j] > max_scale[j] || sc[j] < min_scale[j]) good = false;
+        if (sc[j] > g.max_scale[j] || sc[j] < g.min_scale[j]) good = false;
       }
     }
     if (good) {
@@ -205,55 +230,119 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
     }
   }
   __syncthreads();
-  if (!ok) {
-    if (tid == 0) { out_valid[h] = 0; out_ratio[h] = 0.0; }
-    return;
-  }
-  double mn[3] = {1e300, 1e300, 1e300}, mx[3] = {-1e300, -1e300, -1e300};
-  int cnt = 0;
-  for (int i = tid; i < N; i += RT) {
-    const double sx = src[(size_t)i * 3], sy = src[(size_t)i * 3 + 1], sz = src[(size_t)i * 3 + 2];
-    const double tx = tgt[(size_t)i * 3], ty = tgt[(size_t)i * 3 + 1], tz = tgt[(size_t)i * 3 + 2];
-    const double ex = T[0] * sx + T[1] * sy + T[2] * sz + T[3] - tx;
-    const double ey = T[4] * sx + T[5] * sy + T[6] * sz + T[7] - ty;
-    const double ez = T[8] * sx + T[9] * sy + T[10] * sz + T[11] - tz;
-    if (sqrt(ex * ex + ey * ey + ez * ez) <= thr) cnt++;
-    if (max_dims) {
-      for (int k = 0; k < 3; k++) {
-        const double c = Ti[k * 4] * tx + Ti[k * 4 + 1] * ty + Ti[k * 4 + 2] * tz + Ti[k * 4 + 3];
-        mn[k] = fmin(mn[k], c); mx[k] = fmax(mx[k], c);
+  if (ok) {
+    double mn[3] = {1e300, 1e300, 1e300}, mx[3] = {-1e300, -1e300, -1e300};
+    int cnt = 0;
+    for (int i = tid; i < N; i += RT) {
+      const double sx = src[(size_t)i * 3], sy = src[(size_t)i * 3 + 1], sz = src[(size_t)i * 3 + 2];
+      const double tx = tgt[(size_t)i * 3], ty = tgt[(size_t)i * 3 + 1], tz = tgt[(size_t)i * 3 + 2];
+      const double ex = T[0] * sx + T[1] * sy + T[2] * sz + T[3] - tx;
+      const double ey = T[4] * sx + T[5] * sy + T[6] * sz + T[7] - ty;
+      const double ez = T[8] * sx + T[9] * sy + T[10] * sz + T[11] - tz;
+      if (sqrt(ex * ex + ey * ey + ez * ez) <= thr) cnt++;
+      if (g.has_max_dims) {
+        for (int k = 0; k < 3; k++) {
+          const double c = Ti[k * 4] * tx + Ti[k * 4 + 1] * ty + Ti[k * 4 + 2] * tz + Ti[k * 4 + 3];
+          mn[k] = fmin(mn[k], c); mx[k] = fmax(mx[k], c);
+        }
       }
     }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    for (int k = 0; k < 3; k++) {
-      mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
-      mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+    for (int o = 16; o > 0; o >>= 1) {
+      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+      for (int k = 0; k < 3; k++) {
+        mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
+        mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+      }
     }
+    if (lane == 0) {
+      redc[wid] = cnt;
+      for (int k = 0; k < 3; k++) { red[wid][k] = mn[k]; red[wid][3 + k] = mx[k]; }
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int c = 0;
+      for (int w2 = 0; w2 < RT / 32; w2++) {
+        c += redc[w2];
+        for (int k = 0; k < 3; k++) { mn[k] = fmin(mn[k], red[w2][k]); mx[k] = fmax(mx[k], red[w2][3 + k]); }
+      }
+      bool good = true;
+      if (g.has_max_dims)
+        for (int k = 0; k < 3; k++)
+          if (mx[k] - mn[k] > g.max_dims[k]) good = false;
+      if (out_valid) {
+        out_valid[b] = good ? 1 : 0;
+        out_ratio[b] = good ? (double)c / (double)N : 0.0;
+      }
+      if (good) {
+        for (int k = 0; k < 12; k++) out_T[(size_t)b * 16 + k] = T[k];
+        out_T[(size_t)b * 16 + 12] = 0.0; out_T[(size_t)b * 16 + 13] = 0.0; out_T[(size_t)b * 16 + 14] = 0.0;
+        out_T[(size_t)b * 16 + 15] = 1.0;
+        // count / N is monotone in count, so the largest key is the host's first maximum among valid hypotheses
+        if (f.keys)
+          atomicMax(&f.keys[b / H], ((unsigned long long)c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(b % H)));
+      }
+    }
+  } else if (tid == 0 && out_valid) {
+    out_valid[b] = 0; out_ratio[b] = 0.0;
   }
-  if (lane == 0) {
-    redc[wid] = cnt;
-    for (int k = 0; k < 3; k++) { red[wid][k] = mn[k]; red[wid][3 + k] = mx[k]; }
+  if (!f.keys) return;
+
+  // ---- the last CTA to finish reads the winners and picks the pose (predicter.py:152-172's loop over thresholds)
+  if (tid == 0) {
+    __threadfence();   // this CTA's T and key before its count
+    last = atomicAdd(&f.keys[f.n_thr], 1ull) == (unsigned long long)gridDim.x - 1;
   }
   __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double *rec = f.record;
+  double best_ratio = 0.0;
+  int chosen = -1;
+  for (int t = 0; t < f.n_thr; t++) {
+    if (tid == 0) {
+      const unsigned long long key = atomicAdd(&f.keys[t], 0ull);
+      ok = key ? (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)) : -1;
+    }
+    __syncthreads();
+    const int w = ok;
+    if (w >= 0 && tid < 12) T[tid] = __ldcg(&out_T[((size_t)t * H + w) * 16 + tid]);   // the scoring pass's T, not a recompute
+    __syncthreads();
+    int cnt = 0;
+    if (w >= 0)
+      for (int i = tid; i < N; i += RT) {
+        const double sx = src[(size_t)i * 3], sy = src[(size_t)i * 3 + 1], sz = src[(size_t)i * 3 + 2];
+        const double ex = T[0] * sx + T[1] * sy + T[2] * sz + T[3] - tgt[(size_t)i * 3];
+        const double ey = T[4] * sx + T[5] * sy + T[6] * sz + T[7] - tgt[(size_t)i * 3 + 1];
+        const double ez = T[8] * sx + T[9] * sy + T[10] * sz + T[11] - tgt[(size_t)i * 3 + 2];
+        if (sqrt(ex * ex + ey * ey + ez * ez) <= f.ratio_thr) cnt++;
+      }
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) redc[wid] = cnt;
+    __syncthreads();
+    if (tid == 0) {
+      double *r = rec + (size_t)t * REC_PER_THR;
+      int c3 = 0;
+      for (int w2 = 0; w2 < RT / 32; w2++) c3 += redc[w2];
+      r[0] = (double)w;
+      r[1] = w >= 0 ? (double)(int)(__ldcg(&f.keys[t]) >> 32) : 0.0;
+      for (int k = 0; k < 16; k++) r[2 + k] = w >= 0 ? __ldcg(&out_T[((size_t)t * H + w) * 16 + k]) : 0.0;
+      r[18] = (double)c3;
+      if (w >= 0) {
+        // predict's checks on the winner: det(T[:3,:3]) >= 0, then ratio > best_ratio (the first threshold wins a tie;
+        // a winner with no point within ratio_thr is not a pose)
+        const double det = T[0] * (T[5] * T[10] - T[6] * T[9]) - T[1] * (T[4] * T[10] - T[6] * T[8]) +
+                           T[2] * (T[4] * T[9] - T[5] * T[8]);
+        const double ratio = (double)c3 / (double)N;
+        if (!(det < 0) && ratio > best_ratio) { best_ratio = ratio; chosen = t; }
+      }
+    }
+    __syncthreads();
+  }
   if (tid == 0) {
-    int c = 0;
-    for (int w2 = 0; w2 < RT / 32; w2++) {
-      c += redc[w2];
-      for (int k = 0; k < 3; k++) { mn[k] = fmin(mn[k], red[w2][k]); mx[k] = fmax(mx[k], red[w2][3 + k]); }
-    }
-    bool good = true;
-    if (max_dims)
-      for (int k = 0; k < 3; k++)
-        if (mx[k] - mn[k] > max_dims[k]) good = false;
-    out_valid[h] = good ? 1 : 0;
-    out_ratio[h] = good ? (double)c / (double)N : 0.0;
-    if (good) {
-      for (int k = 0; k < 12; k++) out_T[(size_t)h * 16 + k] = T[k];
-      out_T[(size_t)h * 16 + 12] = 0.0; out_T[(size_t)h * 16 + 13] = 0.0; out_T[(size_t)h * 16 + 14] = 0.0;
-      out_T[(size_t)h * 16 + 15] = 1.0;
-    }
+    double *r = rec + (size_t)f.n_thr * REC_PER_THR;
+    r[0] = (double)chosen;
+    for (int k = 0; k < 16; k++) r[1 + k] = chosen >= 0 ? rec[(size_t)chosen * REC_PER_THR + 2 + k] : 0.0;
+    r[17] = best_ratio;
   }
 }
 
@@ -266,31 +355,57 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
   CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && min_scale && max_scale, "ransac9d: bad arguments");
   CG_REQUIRE(ctx, out_ratio && out_T && out_valid, "ransac9d: outputs");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  double *d_src, *d_tgt, *d_par, *d_ratio, *d_T; int32_t *d_ids; unsigned char *d_valid;
+  double *d_src, *d_tgt, *d_ratio, *d_T; int32_t *d_ids; unsigned char *d_valid;
   int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
     d_src = ar.take<double>((size_t)N * 3);
     d_tgt = ar.take<double>((size_t)N * 3);
     d_ids = ar.take<int32_t>((size_t)H * 4);
-    d_par = ar.take<double>(9);
     d_ratio = ar.take<double>(H);
     d_T = ar.take<double>((size_t)H * 16);
     d_valid = ar.take<unsigned char>(H);
   });
   if (rc) return rc;
-  double par[9];
-  for (int k = 0; k < 3; k++) { par[k] = min_scale[k]; par[3 + k] = max_scale[k]; par[6 + k] = max_dims ? max_dims[k] : 0.0; }
+  Gates g{};
+  g.thr[0] = g.thr[1] = pass_threshold;
+  for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
+  g.has_max_dims = max_dims != nullptr;
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemcpyAsync(d_src, source, (size_t)N * 24, cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemcpyAsync(d_tgt, target, (size_t)N * 24, cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemcpyAsync(d_ids, ids, (size_t)H * 16, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_par, par, sizeof(par), cudaMemcpyHostToDevice, st));
   CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, st));
-  ransac9d_kernel<<<H, RT, 0, st>>>(d_src, d_tgt, N, d_ids, H, pass_threshold, d_par, d_par + 3, max_dims ? d_par + 6 : nullptr,
-                                    d_ratio, d_T, d_valid);
+  ransac9d_kernel<<<H, RT, 0, st>>>(d_src, d_tgt, N, d_ids, H, g, d_ratio, d_T, d_valid, Fuse{nullptr, nullptr, 0.0, 0});
   CG_LAUNCH_CHECK(ctx);
   CG_CUDA(ctx, cudaMemcpyAsync(out_ratio, d_ratio, (size_t)H * 8, cudaMemcpyDeviceToHost, st));
   CG_CUDA(ctx, cudaMemcpyAsync(out_T, d_T, (size_t)H * 128, cudaMemcpyDeviceToHost, st));
   CG_CUDA(ctx, cudaMemcpyAsync(out_valid, d_valid, (size_t)H, cudaMemcpyDeviceToHost, st));
   CG_CUDA(ctx, cudaStreamSynchronize(st));
+  return CG_OK;
+}
+
+extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
+                                    int H, const double *thresholds, int n_thr, const double min_scale[3],
+                                    const double max_scale[3], const double *max_dims, double ratio_threshold,
+                                    double *out_record) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && thresholds && (n_thr == 1 || n_thr == 2) && min_scale &&
+                      max_scale && out_record, "ransac9d_pose: bad arguments");
+  CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_pose: too many hypotheses");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  double *d_T; unsigned long long *d_keys;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    d_T = ar.take<double>((size_t)n_thr * H * 16);        // every valid hypothesis's T, read back by the last CTA
+    d_keys = ar.take<unsigned long long>((size_t)n_thr + 1);   // per-threshold keys, then the completion counter
+  });
+  if (rc) return rc;
+  Gates g{};
+  for (int t = 0; t < 2; t++) g.thr[t] = thresholds[t < n_thr ? t : 0];
+  for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
+  g.has_max_dims = max_dims != nullptr;
+  cudaStream_t st = ctx->stream;
+  CG_CUDA(ctx, cudaMemsetAsync(d_keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
+  ransac9d_kernel<<<n_thr * H, RT, 0, st>>>(source, target, N, ids, H, g, nullptr, d_T, nullptr,
+                                            Fuse{d_keys, out_record, ratio_threshold, n_thr});
+  CG_LAUNCH_CHECK(ctx);
   return CG_OK;
 }

@@ -35,6 +35,12 @@ class _Net:
     def _empty(self, *shape, dtype=torch.float32):
         return torch.empty(shape, dtype=dtype, device=self.device)
 
+    def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0):
+        """Counter-based subset draw on the device (cg_draw_ids_dev): (count, n_pts) int32 cuda tensor."""
+        ids = self._empty(count, n_pts, dtype=torch.int32)
+        self.ctx.call("cg_draw_ids_dev", self.ctx.h, int(M), int(n_pts), int(count), int(seed), int(first_candidate), ids)
+        return ids
+
 
 class PointNetCls(_Net):
     """forward(x:(B,N,6)) -> logits (B,n_out); mirrors pointnet2.py:289-299 (first return value)."""
@@ -50,12 +56,6 @@ class PointNetCls(_Net):
         return (logits, probs) if return_probs else logits
 
     __call__ = forward
-
-    def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0):
-        """Counter-based subset draw on the device (cg_draw_ids_dev): (count, n_pts) int32 cuda tensor."""
-        ids = self._empty(count, n_pts, dtype=torch.int32)
-        self.ctx.call("cg_draw_ids_dev", self.ctx.h, int(M), int(n_pts), int(count), int(seed), int(first_candidate), ids)
-        return ids
 
     def graspq_dev(self, cloud_xyz, cloud_nrm, poses, ids, mean=None, std=None, out=None):
         """Fused transform + forward + softmax on device tensors; returns (probs (B,n_out) f32, label (B,) i32)."""

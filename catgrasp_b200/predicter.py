@@ -4,9 +4,10 @@ Host side (numpy, identical RNG consumption to the reference):
   * z >= 0.1 mask and the per-candidate ``np.random.choice`` subset (dataset_grasp.py:64,72-73;
     dataset_nunocs.py:40-44) -- only the *indices* are drawn on the host;
   * NUNOCS min/max-extent normalisation (augmentations.py:70-75);
-  * the 9-DoF RANSAC (aligning.py:83-119) stays a host stage (SURVEY.md 8f F1).
+  * the 9-DoF RANSAC's 4-subsets (aligning.py:91-97), drawn in C on numpy's generator.
 Device side (libcatgrasp_b200.so): per-candidate rigid transform + normalisation + PointNet forward
-+ softmax / argmax post-processing.
++ softmax / argmax post-processing; the 9-DoF RANSAC's scoring and selection at both thresholds (one launch).
+``subsample = "device"`` on either predicter moves the draws (and NUNOCS's transform) to the GPU as well.
 """
 import copy
 import os
@@ -300,6 +301,14 @@ class NunocsPredicter:
         self.model = PointNetSeg(sd, device=device)
         assert self.model.n_out == 3 * self.cfg["ce_loss_bins"]
         self.ransac_max_iter = 10000
+        # "host": the reference's numpy draws, bit for bit (the transform's subset, then 2 x ransac_max_iter RANSAC
+        # subsets drawn in C); "device": counter-based draws on the GPU from one numpy value, not the reference's
+        # numbers, and no host walk of the generator
+        self.subsample = "host"
+
+    THRESHOLDS = (0.003, 0.005)           # predicter.py:154, the RANSAC pass thresholds in the order predict tries them
+    ERR_THRES = 0.003                     # predicter.py:163, the ratio predict compares between them
+    MAX_DIMENSIONS = np.array([1.2, 1.2, 1.2])
 
     def transform(self, data, ids=None):
         """NunocsIsolatedDataset.transform in 'test' phase (dataset_nunocs.py:38-65)."""
@@ -340,41 +349,121 @@ class NunocsPredicter:
         return coords, conf_z
 
     def predict(self, data, ids=None):
-        """predicter.py:135-203: (nocs_cloud, transform) or (None, None)."""
-        from .aligning import estimate9DTransform
+        """predicter.py:135-203: (nocs_cloud, transform) or (None, None); numpy for numpy input, CUDA tensors for
+        CUDA input.  Sets data_transformed, confidence_z, pred_bins and, with a pose, best_ratio and nocs_pose.
+        ``ids`` (n_pts,) overrides the cloud subset; ``self.subsample`` picks the random numbers ("host" / "device")."""
+        assert self.subsample in ("host", "device"), self.subsample
+        if self.subsample == "device":
+            return self._predict_device(data, ids)
+        if getattr(data["cloud_xyz"], "is_cuda", False):
+            data = {k: (v.cpu().numpy() if hasattr(v, "is_cuda") else v) for k, v in data.items()}
+            nocs, tf = self._predict_host(data, ids)
+            return (None, None) if tf is None else self._on(self.model.device, nocs, tf)
+        return self._predict_host(data, ids)
+
+    def _on(self, dev, *arrays):
+        import torch
+        return tuple(torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in arrays)
+
+    def _ransac(self, source, target, ids):
+        from .aligning import ransac9d_pose
+        return ransac9d_pose(source, target, ids, self.THRESHOLDS, max_scale=self.max_scale, min_scale=self.min_scale,
+                             max_dimensions=self.MAX_DIMENSIONS, ratio_threshold=self.ERR_THRES)
+
+    def _predict_host(self, data, ids):
+        """The reference's numbers: the transform's subset from np.random.choice, then both thresholds' subsets in
+        one C draw that continues numpy's stream where the reference's two loops would (aligning.py:91-97), one
+        fused launch on them, and predict's post-processing in numpy on the two winners' T (predicter.py:152-172)."""
         nocs_cloud, _ = self.predict_nocs(data, ids=ids)
         ori_cloud = self.data_transformed["cloud_xyz_original"]
-        nocs_cloud_down = copy.deepcopy(nocs_cloud)
-        ori_cloud_down = copy.deepcopy(ori_cloud)
+        symmetry_tf = np.eye(4)
+        source = np.ascontiguousarray((symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3], dtype=np.float64)
+        target = np.ascontiguousarray(ori_cloud, dtype=np.float64)
+        N, H = len(source), int(self.ransac_max_iter)
+        if N < 4:
+            raise ValueError("Cannot take a larger sample than population when 'replace=False'")   # as np.random.choice
+        draw = _LegacyDraw()
+        hyp = draw.draw(N, 4, len(self.THRESHOLDS) * H)
+        draw.commit()
+        dev = self.model.device
+        rec = self._ransac(*self._on(dev, source, target, hyp))["record"].cpu().numpy()
         best_ratio = 0
         best_transform = None
-        best_symmetry_tf = None
-        for symmetry_tf in [np.eye(4)]:
-            tmp_nocs_cloud_down = (symmetry_tf @ to_homo(nocs_cloud_down).T).T[:, :3]
-            for thres in [0.003, 0.005]:
-                transform, inliers = estimate9DTransform(
-                    source=tmp_nocs_cloud_down, target=ori_cloud_down, PassThreshold=thres,
-                    max_iter=self.ransac_max_iter, max_scale=self.max_scale, min_scale=self.min_scale,
-                    max_dimensions=np.array([1.2, 1.2, 1.2]))
-                if transform is None:
-                    continue
-                if np.linalg.det(transform[:3, :3]) < 0:
-                    continue
-                transformed = (transform @ to_homo(tmp_nocs_cloud_down).T).T[:, :3]
-                err_thres = 0.003
-                errs = np.linalg.norm(transformed - ori_cloud_down, axis=1)
-                ratio = np.sum(errs <= err_thres) / len(errs)
-                if ratio > best_ratio:
-                    best_ratio = ratio
-                    best_symmetry_tf = symmetry_tf
-                    best_transform = transform.copy()
+        for t in range(len(self.THRESHOLDS)):
+            r = rec[t * 19:(t + 1) * 19]
+            if r[0] < 0:                                                  # estimate9DTransform returned None
+                continue
+            transform = r[2:18].reshape(4, 4).copy()
+            if np.linalg.det(transform[:3, :3]) < 0:
+                continue
+            transformed = (transform @ to_homo(source).T).T[:, :3]
+            errs = np.linalg.norm(transformed - target, axis=1)
+            ratio = np.sum(errs <= self.ERR_THRES) / len(errs)
+            if ratio > best_ratio:
+                best_ratio = ratio
+                best_transform = transform.copy()
         if best_transform is None:
             return None, None
         self.best_ratio = best_ratio
-        transform = best_transform
-        self.nocs_pose = transform.copy()
-        nocs_cloud = (best_symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
-        return nocs_cloud, transform
+        self.nocs_pose = best_transform.copy()
+        nocs_cloud = (symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
+        return nocs_cloud, best_transform
+
+    def device_transform(self, data, ids=None, seed=None):
+        """transform() on the device in float64 for numpy or CUDA input: the z >= 0.1 mask, the subset (``ids``, else
+        candidate 0 of cg_draw_ids_dev with ``seed``), the min/extent normalisation and the mean/std scaling.  With
+        the same ids, 'input' equals transform()'s bit for bit.  Returns a dict of CUDA tensors ('cloud_xyz',
+        'cloud_normal', 'cloud_xyz_original', 'keep_ids', 'input').  With CUDA input the masked point count is read
+        on the host (one synchronisation): it sizes the draw."""
+        import torch
+        from . import _lib
+        n_pts = int(self.cfg["n_pts"])
+        ctx, xyz, nrm = _lib.inputs(data["cloud_xyz"], data["cloud_normal"], dtype=torch.float64, ctx=self.model.ctx)
+        if getattr(data["cloud_xyz"], "is_cuda", False):
+            keep_ids = torch.nonzero(data["cloud_xyz"][:, 2] >= 0.1).reshape(-1).to(xyz.device)   # in the input's dtype
+        else:
+            keep_ids = torch.from_numpy(np.nonzero(np.asarray(data["cloud_xyz"])[:, 2] >= 0.1)[0]).to(xyz.device)
+        if ids is None:
+            sub = self.model.draw_ids_dev(keep_ids.numel(), n_pts, 1, seed, first_candidate=0)[0].long()
+        else:
+            sub = torch.as_tensor(np.asarray(ids) if not hasattr(ids, "is_cuda") else ids).to(xyz.device).long()
+        keep_ids = keep_ids[sub]
+        x0, nr = xyz[keep_ids], nrm[keep_ids]
+        mn = x0.amin(0)
+        scale = (x0.amax(0) - mn).max()
+        xn = (x0 - mn) / (scale + 1e-15)
+        inp = torch.cat([xn, nr], 1)
+        if "mean" in self.cfg:
+            mean, std = self._on(xyz.device, self.cfg["mean"].reshape(1, -1), self.cfg["std"].reshape(1, -1))
+            inp = (inp - mean) / (std + 1e-15)
+        return {"cloud_xyz": xn, "cloud_normal": nr, "cloud_xyz_original": x0, "keep_ids": keep_ids, "input": inp}
+
+    def _predict_device(self, data, ids):
+        """Device mode: consumes ONE value of numpy's global generator (the seed, np.random.randint as
+        GraspPredicter's device draw does).  Candidate 0 of cg_draw_ids_dev(seed) is the cloud subset, candidates
+        1 .. H the first threshold's subsets and H+1 .. 2H the second's; the forward, the RANSAC and predict's
+        choice between thresholds run on the device.  The host waits for the masked point count with CUDA input,
+        and for the record (whether there is a pose, best_ratio) and, with numpy input, the copy of the results."""
+        import torch
+        seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+        cuda_in = getattr(data["cloud_xyz"], "is_cuda", False)
+        H, n_thr = int(self.ransac_max_iter), len(self.THRESHOLDS)
+        dt = self.device_transform(data, ids=ids, seed=seed)
+        coords, conf_z, bins = self.model.nunocs_dev(dt["input"].to(torch.float32), int(self.cfg["ce_loss_bins"]))
+        source = coords.to(torch.float64)
+        hyp = self.model.draw_ids_dev(source.shape[0], 4, n_thr * H, seed, first_candidate=1)
+        res = self._ransac(source, dt["cloud_xyz_original"], hyp)
+        rec = res["record"].cpu().numpy()
+        host = (lambda t: t.cpu().numpy()) if not cuda_in else (lambda t: t)
+        self.data_transformed = {k: host(v) for k, v in dt.items()}
+        self.confidence_z, self.pred_bins = host(conf_z), host(bins)
+        tail = rec[n_thr * 19:]
+        if tail[0] < 0:
+            return None, None
+        self.best_ratio = float(tail[17])
+        pose = host(res["pose"].clone())
+        self.nocs_pose = pose.copy() if not cuda_in else pose.clone()
+        return host(source), pose
 
 
 def flatten_config(cfg, out=None):

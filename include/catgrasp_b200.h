@@ -2,7 +2,9 @@
  * catgrasp_b200.h -- C ABI of libcatgrasp_b200.so (sm_90a, H100).
  *
  * This is the drop-in boundary for CaTGrasp's per-scene grasp-scoring hot
- * path.  Every entry point is `extern "C"`, takes plain pointers and sizes,
+ * path and the per-pick stages around it (segmentation, NUNOCS and its 9-DoF
+ * pose search, the grasp samplers and filters, affordance transfer, ranking).
+ * Every entry point is `extern "C"`, takes plain pointers and sizes,
  * returns an int status (0 = ok, negative = CG_E*), and never calls exit().
  * Each entry cites the reference interface (file:line under the reference
  * checkout) that it replaces.
@@ -339,6 +341,22 @@ int cg_occupancy_from_scan_host(cg_ctx *ctx, const float *pts_host, int P, float
 int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids, int H,
                      double pass_threshold, const double min_scale[3], const double max_scale[3],
                      const double *max_dims, double *out_ratio, double *out_T, unsigned char *out_valid);
+/* The whole NUNOCS pose search in one launch on device buffers (replaces aligning.py:83-119 twice and
+ * predicter.py:152-172): the same scoring as cg_ransac9d_host for n_thr (1 or 2) thresholds, each with its own H
+ * subsets (ids (n_thr*H,4): rows t*H .. t*H+H-1 belong to thresholds[t]), then the selection on the device:
+ *   per threshold, the winner = the first maximum of the inlier count among valid hypotheses (the host's
+ *   keep[argmax(ratio[keep])]); its T is the scoring pass's, bit for bit cg_ransac9d_host's T[winner];
+ *   the pose = the first threshold whose winner has det(T[:3,:3]) >= 0 and the largest ratio
+ *   count(|T src - tgt| <= ratio_threshold) / N, strictly above the previous best (starting at 0).
+ * out_record (n_thr*19 + 18 float64, integers stored exactly):
+ *   per threshold t at t*19: [winner h or -1, its count at thresholds[t], T (4x4, zeros if none),
+ *                             its count at ratio_threshold]
+ *   then [chosen threshold or -1, pose (4x4, zeros if none), best_ratio].
+ * Runs on the context stream and does not synchronise.                                                         */
+int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids, int H,
+                         const double *thresholds /* host */, int n_thr, const double min_scale[3] /* host */,
+                         const double max_scale[3] /* host */, const double *max_dims /* host */,
+                         double ratio_threshold, double *out_record);
 
 /* ---- Cone pose enumeration (device pointers, float64 like the reference's numpy) ----------
  * Replaces: dexnet/grasping/grasp_sampler.py:266-286 (PointConeGraspSampler.sample_one_surface_point: the

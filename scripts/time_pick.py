@@ -2,7 +2,9 @@
 stages once, per-object stages summed over the objects) on the 16-object full-resolution render_depth pile (the
 reference K, 1544 x 2064), with synthetic weights: the renderer's id map stands in for the segmentation.  Each stage time ends in a device synchronise.
 
-    python scripts/time_pick.py [--reps 3]
+    python scripts/time_pick.py [--reps 3] [--subsample host|device]
+
+--subsample device runs NUNOCS and grasp-Q on their device draws (no host walk of numpy's generator).
 """
 import argparse
 import os
@@ -34,6 +36,7 @@ class IdSegmenter:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--subsample", choices=("host", "device"), default="host")
     a = ap.parse_args()
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip()
@@ -47,6 +50,8 @@ def main():
     npd = NunocsPredicter("nut", artifact_dir=synthetic.write_artifacts(
         f"{tmp}/seg", "seg", 2048, with_normalizer=False, state_dict=synthetic.make_lattice_seg_state_dict(seed=5)),
         device=0)
+    npd.subsample = gp.subsample = a.subsample
+    print("subsample:", a.subsample)
     seg = IdSegmenter(torch.from_numpy(ids[~bg].astype(np.int64)).to(dev))
     g = synthetic.make_gripper_proxy()
     box = [0.0, 0.045, -0.010, 0.010]
