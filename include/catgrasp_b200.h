@@ -365,12 +365,14 @@ int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target
  *   surface_pts (S,3), R0 (S,9 row-major: columns approach / major / minor, computed on the host, :262),
  *   R_sphere (NS,9), R_inplane (NI,9), depths (ND) = np.arange(0, hand_depth, approach_step)
  *   out_poses64 (P,16) row-major 4x4, P = S * (1 + NS*NI) * ND, ordered (surface point, rotation, depth) like the
- *   reference's list; out_poses32 (P,16) or NULL = the same poses narrowed to float32 for cg_filter_grasp_pose_dev.   */
+ *   reference's list; out_poses32 (P,16) or NULL = the same poses narrowed to float32 for cg_filter_grasp_pose_dev.
+ *   CG_EINVAL, before any launch: P >= 2^31, or NS, NI > 0 with R_sphere or R_inplane NULL.                         */
 int cg_cone_poses_dev(cg_ctx *ctx, const double *surface_pts, const double *R0, int S, const double *R_sphere, int NS,
                       const double *R_inplane, int NI, const double *depths, int ND, double init_bite,
                       double *out_poses64, float *out_poses32);
 /* grasp_sampler.py:191-203: shift every pose along its y axis to the middle of the object's extent (pts (M,3) float64,
- * camera frame) in the grasp frame; poses are updated in place (poses32 may be NULL).                                */
+ * camera frame) in the grasp frame; poses are updated in place (poses32 may be NULL).  M = 0 is CG_EINVAL; P = 0
+ * returns CG_OK without work.                                                                                        */
 int cg_center_grasps_dev(cg_ctx *ctx, double *poses64, float *poses32, int P, const double *pts, int M);
 
 /* ---- Affordance transfer per grasp (device pointers, float64) --------------------------------
