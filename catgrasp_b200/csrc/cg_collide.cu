@@ -426,31 +426,22 @@ extern "C" int cg_filter_grasp_pose_host(cg_ctx *ctx, const cg_filter_params *pr
                                          int P1, cg_sdf *sdf_enclosed, const float *enclosed_pts, int P2,
                                          uint8_t *out_status, int8_t *out_offset, float *out_poses) {
   if (!ctx) return CG_EINVAL;
-  CG_REQUIRE(ctx, prm && grasp_poses && symmetry_tfs && G > 0 && S > 0, "filter_host: poses");
+  CG_REQUIRE(ctx, grasp_poses && symmetry_tfs && G > 0 && S > 0, "filter_host: poses");
   CG_REQUIRE(ctx, out_status && out_offset && out_poses, "filter_host: outputs");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t Q = (size_t)G * S;
-  float *d_g, *d_s, *d_p1, *d_p2, *d_po; uint8_t *d_st; int8_t *d_of;
-  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
-    d_g = ar.take<float>((size_t)G * 16);
-    d_s = ar.take<float>((size_t)S * 16);
-    d_p1 = ar.take<float>((size_t)P1 * 3 + 1);
-    d_p2 = ar.take<float>((size_t)P2 * 3 + 1);
-    d_st = ar.take<uint8_t>(Q);
-    d_of = ar.take<int8_t>(Q);
-    d_po = ar.take<float>(Q * 16);
+  // a point set stages as (P,3) floats; a negative count stages nothing and is cg_filter_grasp_pose_dev's to judge
+  const size_t n1 = P1 > 0 ? (size_t)P1 * 3 : 0, n2 = P2 > 0 ? (size_t)P2 * 3 : 0;
+  const float *d_g, *d_s, *d_p1, *d_p2; uint8_t *d_st; int8_t *d_of; float *d_po;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_g = io.in(grasp_poses, (size_t)G * 16);
+    d_s = io.in(symmetry_tfs, (size_t)S * 16);
+    d_p1 = io.in(open_pts, n1);
+    d_p2 = io.in(enclosed_pts, n2);
+    d_st = io.out(out_status, Q);
+    d_of = io.out(out_offset, Q);
+    d_po = io.out(out_poses, Q * 16);
+  }, [&] {
+    return cg_filter_grasp_pose_dev(ctx, prm, d_g, G, d_s, S, sdf_open, d_p1, P1, sdf_enclosed, d_p2, P2, d_st, d_of,
+                                    d_po);
   });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemcpyAsync(d_g, grasp_poses, (size_t)G * 64, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_s, symmetry_tfs, (size_t)S * 64, cudaMemcpyHostToDevice, st));
-  if (P1 > 0) CG_CUDA(ctx, cudaMemcpyAsync(d_p1, open_pts, (size_t)P1 * 12, cudaMemcpyHostToDevice, st));
-  if (P2 > 0) CG_CUDA(ctx, cudaMemcpyAsync(d_p2, enclosed_pts, (size_t)P2 * 12, cudaMemcpyHostToDevice, st));
-  rc = cg_filter_grasp_pose_dev(ctx, prm, d_g, G, d_s, S, sdf_open, d_p1, P1, sdf_enclosed, d_p2, P2, d_st, d_of, d_po);
-  if (rc) return rc;
-  CG_CUDA(ctx, cudaMemcpyAsync(out_status, d_st, Q, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(out_offset, d_of, Q, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(out_poses, d_po, Q * 64, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaStreamSynchronize(st));
-  return CG_OK;
 }

@@ -35,9 +35,10 @@ struct cg_ctx {
   // grow-only device workspace, carved per call
   void *ws = nullptr;
   size_t ws_bytes = 0;
-  // second device arena for *_host entry points' device copies of I/O
+  // second device arena for *_host entry points' device copies of I/O (carved only by cg_io_stage)
   void *io = nullptr;
   size_t io_bytes = 0;
+  bool io_held = false;   // a cg_io_stage compute step is running: its pieces of io must stay where they are
 };
 
 #define CG_CUDA(ctx, call)                                                        \
@@ -86,7 +87,7 @@ struct cg_sdf {
 // border_nonneg / border_min of a host copy of the grid (decides the filter's out-of-box shortcut)
 void cg_sdf_border_stats(cg_sdf *s, const float *grid_host);
 
-int cg_ws_reserve(cg_ctx *ctx, size_t bytes);   // grow-only (cg_api.cu); call sites use cg_ws_carve / cg_io_carve
+int cg_ws_reserve(cg_ctx *ctx, size_t bytes);   // grow-only (cg_api.cu); call sites use cg_ws_carve / cg_io_stage
 int cg_io_reserve(cg_ctx *ctx, size_t bytes);
 
 // Bump allocator over an arena: each piece starts at the next multiple of 256 bytes from the base.  An arena over
@@ -105,11 +106,15 @@ struct cg_arena {
 };
 
 // cg_ws_carve / cg_io_carve(ctx, layout): layout(cg_arena &) makes one call's take()s and stores the pointers.  It runs
-// over a measuring arena, the context's ws (*_dev internals) or io (*_host staging) arena grows to the bytes measured,
-// and it runs again over that arena.  Growing frees the arena: code that holds pieces of a carve must not call anything
-// that carves the same arena (a *_host call holds its io pieces across the *_dev call it wraps, which carves ws only).
+// over a measuring arena, the context's ws (*_dev internals) or io (cg_io_stage) arena grows to the bytes measured, and
+// it runs again over that arena.  Growing frees the arena: code that holds pieces of a carve must not call anything
+// that carves the same arena.  An io carve while a cg_io_stage compute step holds io is refused.
 template <typename Layout>
 int cg_carve(cg_ctx *ctx, bool io, Layout &layout) {
+  if (io && ctx->io_held) {
+    ctx->err = "internal error: the compute step of a *_host call carved the io arena that holds its pieces";
+    return CG_EINVAL;
+  }
   cg_arena measure(nullptr);
   layout(measure);
   const int rc = io ? cg_io_reserve(ctx, measure.off) : cg_ws_reserve(ctx, measure.off);
@@ -122,6 +127,46 @@ int cg_carve(cg_ctx *ctx, bool io, Layout &layout) {
 }
 template <typename Layout> int cg_ws_carve(cg_ctx *ctx, Layout &&layout) { return cg_carve(ctx, false, layout); }
 template <typename Layout> int cg_io_carve(cg_ctx *ctx, Layout &&layout) { return cg_carve(ctx, true, layout); }
+
+// The io pieces of a *_host call, in declaration order: in(host, n) is copied from the host before the compute step,
+// out(host, n) back to the host after it unless host is null, take<T>(n) is scratch.  0-element pieces copy nothing.
+struct cg_io_pieces {
+  struct Copy { void *dst; const void *src; size_t bytes; };
+  cg_arena *ar = nullptr;
+  std::vector<Copy> h2d, d2h;
+  template <typename T> T *take(size_t n) { return ar->take<T>(n); }
+  template <typename T> T *in(const T *host, size_t n) {
+    T *d = take<T>(n);
+    h2d.push_back({d, host, n * sizeof(T)});
+    return d;
+  }
+  template <typename T> T *out(T *host, size_t n) {
+    T *d = take<T>(n);
+    if (host) d2h.push_back({host, d, n * sizeof(T)});
+    return d;
+  }
+};
+
+// cg_io_stage(ctx, layout, compute), what every *_host entry point does: carve layout(cg_io_pieces &) over io, enqueue
+// the inputs' copies on ctx->stream, compute(), the outputs' copies, and synchronise.  A failing compute()'s status is
+// returned with nothing copied back.  compute() may carve ws but not io, which holds its pieces: that is refused.
+template <typename Layout, typename Compute>
+int cg_io_stage(cg_ctx *ctx, Layout &&layout, Compute &&compute) {
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  cg_io_pieces io;
+  int rc = cg_io_carve(ctx, [&](cg_arena &ar) { io = cg_io_pieces{&ar, {}, {}}; layout(io); });
+  if (rc) return rc;
+  for (const auto &c : io.h2d)
+    if (c.bytes) CG_CUDA(ctx, cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->io_held = true;
+  rc = compute();
+  ctx->io_held = false;
+  if (rc) return rc;
+  for (const auto &c : io.d2h)
+    if (c.bytes) CG_CUDA(ctx, cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return CG_OK;
+}
 
 // one owning device allocation: freed when it goes out of scope unless release() hands it on
 struct DevBuf {

@@ -277,48 +277,30 @@ extern "C" int cg_graspq_forward_host(cg_net *net, const double *cloud_xyz, cons
   cg_ctx *ctx = net->ctx;
   CG_REQUIRE(ctx, cloud_xyz && cloud_nrm && poses && ids && out_probs, "graspq_host: null argument");
   CG_REQUIRE(ctx, M > 0 && B > 0 && N > 0, "graspq_host: bad shape");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int n_out = net->n_out;
-  double *d_xyz, *d_nrm, *d_pose, *d_mean, *d_std; int32_t *d_ids, *d_label; float *d_probs;
-  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
-    d_xyz = ar.take<double>((size_t)M * 3);
-    d_nrm = ar.take<double>((size_t)M * 3);
-    d_pose = ar.take<double>((size_t)B * 16);
-    d_ids = ar.take<int32_t>((size_t)B * N);
-    d_mean = ar.take<double>(6);
-    d_std = ar.take<double>(6);
-    d_probs = ar.take<float>((size_t)B * n_out);
-    d_label = ar.take<int32_t>(B);
-  });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemcpyAsync(d_xyz, cloud_xyz, (size_t)M * 24, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_nrm, cloud_nrm, (size_t)M * 24, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_pose, poses, (size_t)B * 128, cudaMemcpyHostToDevice, st));
   // The subset indices are the bulk of the input (4 B x N per candidate; 16.8 MB for 4096 x 1024).  When the caller's
   // buffer is pinned (page-locked, mapped under UVA) the trunk kernels read it in place: every index is fetched exactly
   // once per trunk launch, two tiles ahead of its use, so the PCIe / C2C transfer hides under the kernels instead of
-  // sitting in front of them.  Pageable memory takes the staged copy.
-  const int32_t *ids_dev = d_ids;
-  {
-    cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, ids) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer != nullptr)
-      ids_dev = static_cast<const int32_t *>(at.devicePointer);
-    else
-      cudaGetLastError();   // an unregistered pointer is not an error here
-  }
-  if (ids_dev == d_ids) CG_CUDA(ctx, cudaMemcpyAsync(d_ids, ids, (size_t)B * N * 4, cudaMemcpyHostToDevice, st));
-  if (mean && stdv) {
-    CG_CUDA(ctx, cudaMemcpyAsync(d_mean, mean, 48, cudaMemcpyHostToDevice, st));
-    CG_CUDA(ctx, cudaMemcpyAsync(d_std, stdv, 48, cudaMemcpyHostToDevice, st));
-  }
-  rc = cg_graspq_forward_dev(net, d_xyz, d_nrm, M, d_pose, B, ids_dev, N, mean ? d_mean : nullptr,
-                             stdv ? d_std : nullptr, d_probs, d_label);
-  if (rc) return rc;
-  CG_CUDA(ctx, cudaMemcpyAsync(out_probs, d_probs, (size_t)B * n_out * 4, cudaMemcpyDeviceToHost, st));
-  if (out_label) CG_CUDA(ctx, cudaMemcpyAsync(out_label, d_label, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaStreamSynchronize(st));
-  return CG_OK;
+  // sitting in front of them.  Pageable memory takes the staged copy.  The mapped address is the current device's.
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int32_t *ids_mapped = nullptr;
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, ids) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer != nullptr)
+    ids_mapped = static_cast<const int32_t *>(at.devicePointer);
+  else
+    cudaGetLastError();   // an unregistered pointer is not an error here
+  const double *d_xyz, *d_nrm, *d_pose, *d_mean, *d_std; const int32_t *d_ids; int32_t *d_label; float *d_probs;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_xyz = io.in(cloud_xyz, (size_t)M * 3);
+    d_nrm = io.in(cloud_nrm, (size_t)M * 3);
+    d_pose = io.in(poses, (size_t)B * 16);
+    d_ids = ids_mapped ? ids_mapped : io.in(ids, (size_t)B * N);
+    d_mean = mean ? io.in(mean, 6) : nullptr;
+    d_std = stdv ? io.in(stdv, 6) : nullptr;
+    d_probs = io.out(out_probs, (size_t)B * net->n_out);
+    d_label = io.out(out_label, B);
+  }, [&] {
+    return cg_graspq_forward_dev(net, d_xyz, d_nrm, M, d_pose, B, d_ids, N, d_mean, d_std, d_probs, d_label);
+  });
 }
 
 extern "C" int cg_cls_forward_dev(cg_net *net, const float *x, int B, int N, float *out_logits, float *out_probs) {
@@ -376,22 +358,11 @@ extern "C" int cg_nunocs_forward_host(cg_net *net, const float *x_host, int N, i
   if (!net) return CG_EINVAL;
   cg_ctx *ctx = net->ctx;
   CG_REQUIRE(ctx, x_host && N > 0 && out_coords, "nunocs_host: bad arguments");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  float *d_x, *d_c, *d_z; int32_t *d_b;
-  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
-    d_x = ar.take<float>((size_t)N * 6);
-    d_c = ar.take<float>((size_t)N * 3);
-    d_b = ar.take<int32_t>((size_t)N * 3);
-    d_z = ar.take<float>(N);
-  });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemcpyAsync(d_x, x_host, (size_t)N * 24, cudaMemcpyHostToDevice, st));
-  rc = cg_nunocs_forward_dev(net, d_x, N, bins, d_c, d_z, d_b);
-  if (rc) return rc;
-  CG_CUDA(ctx, cudaMemcpyAsync(out_coords, d_c, (size_t)N * 12, cudaMemcpyDeviceToHost, st));
-  if (out_conf_z) CG_CUDA(ctx, cudaMemcpyAsync(out_conf_z, d_z, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
-  if (out_bins) CG_CUDA(ctx, cudaMemcpyAsync(out_bins, d_b, (size_t)N * 12, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaStreamSynchronize(st));
-  return CG_OK;
+  const float *d_x; float *d_c, *d_z; int32_t *d_b;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_x = io.in(x_host, (size_t)N * 6);
+    d_c = io.out(out_coords, (size_t)N * 3);
+    d_z = io.out(out_conf_z, N);
+    d_b = io.out(out_bins, (size_t)N * 3);
+  }, [&] { return cg_nunocs_forward_dev(net, d_x, N, bins, d_c, d_z, d_b); });
 }

@@ -132,22 +132,17 @@ extern "C" int cg_occupancy_from_scan_host(cg_ctx *ctx, const float *pts_host, i
   const size_t bits = (size_t)g.dx * g.dy * g.dz;
   CG_REQUIRE(ctx, bits < (size_t(1) << 33), "occupancy: occupied-cell bounding box too large");
   const size_t words = (bits + 31) / 32;
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  float *d_pts; unsigned *d_mask; unsigned char *d_flags;
-  rc = cg_io_carve(ctx, [&](cg_arena &ar) {
-    d_pts = ar.take<float>((size_t)P * 3);
-    d_mask = ar.take<unsigned>(words);
-    d_flags = ar.take<unsigned char>((size_t)total);
+  const float *d_pts; unsigned *d_mask; unsigned char *d_flags;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_pts = io.in(pts_host, (size_t)P * 3);
+    d_mask = io.take<unsigned>(words);
+    d_flags = io.out(out_flags_host, (size_t)total);
+  }, [&] {
+    CG_CUDA(ctx, cudaMemsetAsync(d_mask, 0, words * 4, ctx->stream));
+    occ_mark_kernel<<<(P + 255) / 256, 256, 0, ctx->stream>>>(d_pts, P, g, d_mask);
+    CG_LAUNCH_CHECK(ctx);
+    occ_cast_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(g, d_mask, d_flags);
+    CG_LAUNCH_CHECK(ctx);
+    return CG_OK;
   });
-  if (rc) return rc;
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemcpyAsync(d_pts, pts_host, (size_t)P * 12, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemsetAsync(d_mask, 0, words * 4, st));
-  occ_mark_kernel<<<(P + 255) / 256, 256, 0, st>>>(d_pts, P, g, d_mask);
-  CG_LAUNCH_CHECK(ctx);
-  occ_cast_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, d_mask, d_flags);
-  CG_LAUNCH_CHECK(ctx);
-  CG_CUDA(ctx, cudaMemcpyAsync(out_flags_host, d_flags, (size_t)total, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaStreamSynchronize(st));
-  return CG_OK;
 }

@@ -354,33 +354,25 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
   if (!ctx) return CG_EINVAL;
   CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && min_scale && max_scale, "ransac9d: bad arguments");
   CG_REQUIRE(ctx, out_ratio && out_T && out_valid, "ransac9d: outputs");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  double *d_src, *d_tgt, *d_ratio, *d_T; int32_t *d_ids; unsigned char *d_valid;
-  int rc = cg_io_carve(ctx, [&](cg_arena &ar) {
-    d_src = ar.take<double>((size_t)N * 3);
-    d_tgt = ar.take<double>((size_t)N * 3);
-    d_ids = ar.take<int32_t>((size_t)H * 4);
-    d_ratio = ar.take<double>(H);
-    d_T = ar.take<double>((size_t)H * 16);
-    d_valid = ar.take<unsigned char>(H);
-  });
-  if (rc) return rc;
   Gates g{};
   g.thr[0] = g.thr[1] = pass_threshold;
   for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
   g.has_max_dims = max_dims != nullptr;
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemcpyAsync(d_src, source, (size_t)N * 24, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_tgt, target, (size_t)N * 24, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(d_ids, ids, (size_t)H * 16, cudaMemcpyHostToDevice, st));
-  CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, st));
-  ransac9d_kernel<<<H, RT, 0, st>>>(d_src, d_tgt, N, d_ids, H, g, d_ratio, d_T, d_valid, Fuse{nullptr, nullptr, 0.0, 0});
-  CG_LAUNCH_CHECK(ctx);
-  CG_CUDA(ctx, cudaMemcpyAsync(out_ratio, d_ratio, (size_t)H * 8, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(out_T, d_T, (size_t)H * 128, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaMemcpyAsync(out_valid, d_valid, (size_t)H, cudaMemcpyDeviceToHost, st));
-  CG_CUDA(ctx, cudaStreamSynchronize(st));
-  return CG_OK;
+  const double *d_src, *d_tgt; const int32_t *d_ids; double *d_ratio, *d_T; unsigned char *d_valid;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_src = io.in(source, (size_t)N * 3);
+    d_tgt = io.in(target, (size_t)N * 3);
+    d_ids = io.in(ids, (size_t)H * 4);
+    d_ratio = io.out(out_ratio, H);
+    d_T = io.out(out_T, (size_t)H * 16);
+    d_valid = io.out(out_valid, H);
+  }, [&] {
+    CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, ctx->stream));
+    ransac9d_kernel<<<H, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, g, d_ratio, d_T, d_valid,
+                                               Fuse{nullptr, nullptr, 0.0, 0});
+    CG_LAUNCH_CHECK(ctx);
+    return CG_OK;
+  });
 }
 
 extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
