@@ -5,7 +5,9 @@ Restates, independently of catgrasp_b200/pointgroup.py and csrc/cg_spconv.cu:
     ``voxelization`` mode 4 (out = 0; for each point out = fl(out + fl(fl(1/n) * x)), float32, no FMA);
   * the host front of PointGroupPredictor.predict (predicter.py:234-300) with n_slice_per_side = 1;
   * the network up to ``pt_offsets`` (PointGroup/model/pointgroup/pointgroup.py: input_conv, UBlock of
-    [m, ..., 7m], output_layer, offset head), composed from oracle/spconv_ref.conv.
+    [m, ..., 7m], output_layer, offset head), composed from oracle/spconv_ref.conv;
+  * the same U-Net as an explicit plan of layers (``plan``), one layer at a time (``layer``), so a test can hold each
+    device layer to a one-layer bound on the device's own inputs and check its wiring exactly.
 
 Bound (the rule of spconv_ref.py, per value): every activation carries |device - exact| <= e, where the device works in
 fp32 on BN scale / shift and folded head weights that were narrowed from float64.  A BN + ReLU in front of a conv is
@@ -15,6 +17,8 @@ The head's first Linear runs on float32 weights rounded from the folded float64 
 The bound is rigorous and grows by the weights' absolute row sums at every layer, so after the U-Net's ~60 layers in
 series it is loose by many orders of magnitude; tests pair it with a relative check against the float64 values.
 """
+from collections import namedtuple
+
 import numpy as np
 
 from . import spconv_ref as S
@@ -188,6 +192,98 @@ def forward(sd, m, block_reps, vox, shape, vfeats, p2v):
     y, ey = _conv(sd, "input_conv.0", x, np.zeros_like(x), levels[0][1], 27)
     y, ey = _ublock(sd, "unet.", y, ey, levels, 0, m, block_reps)
     o, eo = head(sd, y, ey)
+    o, eo = o[rank], eo[rank]
+    p2v = np.asarray(p2v, dtype=np.int64)
+    return o[p2v], eo[p2v], o, eo
+
+
+# ---------------------------------------------------------------- the same network as an explicit layer plan
+INPUT_C = 6              # normals + coordinates
+VFEATS = "vfeats"        # the source name of the voxel features
+KERNEL = {"subm3": 27, "subm1": 1, "down": 8, "up": 8}
+
+Layer = namedtuple("Layer", "name kind level K cin cout bn src res")
+Layer.__doc__ = """One convolution of the U-Net: ``name`` its state-dict prefix (also the name of its output), ``kind``
+subm3 / subm1 (the identity branch) / down / up, ``level`` the level of its output rows, K, cin, cout, ``bn`` the
+prefix of the BN + ReLU in front of it or None, ``src`` the names whose outputs are concatenated (in order) into its
+input, ``res`` the names that make its residual, or None."""
+
+
+def plan(m, block_reps):
+    """The U-Net's convolutions in forward order, as ``Layer`` records, wired as ``forward`` wires them."""
+    out = []
+
+    def conv(name, kind, level, cin, cout, src, bn=None, res=None):
+        out.append(Layer(name, kind, level, KERNEL[kind], cin, cout, bn, tuple(src), res))
+        return (name,)
+
+    def block(p, level, src, cin, cout):
+        res = conv(p + "i_branch.0", "subm1", level, cin, cout, src) if cin != cout else src
+        h = conv(p + "conv_branch.2", "subm3", level, cin, cout, src, bn=p + "conv_branch.0")
+        return conv(p + "conv_branch.5", "subm3", level, cout, cout, h, bn=p + "conv_branch.3", res=res)
+
+    def ublock(p, i, src):
+        C = m * (i + 1)
+        for j in range(block_reps):
+            src = block(f"{p}blocks.block{j}.", i, src, C, C)
+        if i == LEVELS - 1:
+            return src
+        y = conv(p + "conv.2", "down", i + 1, C, C + m, src, bn=p + "conv.0")
+        y = ublock(p + "u.", i + 1, y)
+        src = src + conv(p + "deconv.2", "up", i, C + m, C, y, bn=p + "deconv.0")
+        for j in range(block_reps):
+            src = block(f"{p}blocks_tail.block{j}.", i, src, C * (2 - j), C)
+        return src
+
+    ublock("unet.", 0, conv("input_conv.0", "subm3", 0, INPUT_C, m, (VFEATS,)))
+    return out
+
+
+def table(rec, levels):
+    """The gather table ``rec`` runs on, from ``levels_of``: None for the identity branch."""
+    if rec.kind == "subm3":
+        return levels[rec.level][1]
+    if rec.kind == "down":
+        return levels[rec.level - 1][2]
+    if rec.kind == "up":
+        return levels[rec.level][3]
+    return None
+
+
+def _layer(sd, rec, x, ex, res, eres, levels, rows=None):
+    if rec.bn is not None:
+        x, ex = _bn_act(sd, rec.bn, x, ex)
+    W = _np(sd, rec.name + ".weight").reshape(rec.K, rec.cin, rec.cout)
+    return S.conv(x, table(rec, levels), W, bias=_np(sd, rec.name + ".bias"), residual=res, ex=ex, eres=eres,
+                  rows=rows)
+
+
+def layer(sd, rec, x, residual, levels, rows=None):
+    """One layer's float64 output and bound on ``rows`` (default all) for the input x and residual taken as exact."""
+    x = np.asarray(x, dtype=np.float64)
+    return _layer(sd, rec, x, np.zeros_like(x), residual, None, levels, rows)
+
+
+def _gather(outs, names):
+    if len(names) == 1:
+        return outs[names[0]]
+    return tuple(np.concatenate([outs[n][i] for n in names], 1) for i in (0, 1))
+
+
+def forward_by_plan(sd, m, block_reps, vox, shape, vfeats, p2v):
+    """``forward`` computed by walking ``plan``: the same values and bounds, bit for bit."""
+    vox = np.asarray(vox, dtype=np.int64)
+    order = np.argsort(S.pack(vox), kind="stable")
+    rank = np.empty_like(order)
+    rank[order] = np.arange(len(order))
+    levels = levels_of(vox[order], tuple(int(s) for s in shape))
+    x = np.asarray(vfeats, dtype=np.float64)[order]
+    outs = {VFEATS: (x, np.zeros_like(x))}
+    for rec in plan(m, block_reps):
+        x, ex = _gather(outs, rec.src)
+        res, eres = (None, None) if rec.res is None else _gather(outs, rec.res)
+        outs[rec.name] = _layer(sd, rec, x, ex, res, eres, levels)
+    o, eo = head(sd, *outs[rec.name])
     o, eo = o[rank], eo[rank]
     p2v = np.asarray(p2v, dtype=np.int64)
     return o[p2v], eo[p2v], o, eo

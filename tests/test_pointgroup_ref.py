@@ -44,6 +44,48 @@ def test_oracle_forward_matches_golden(cls):
     assert np.array_equal(bound, G[f"{cls}_bound"])
 
 
+def _same(a, b):
+    return all(np.array_equal(np.asarray(x).view(np.uint64), np.asarray(y).view(np.uint64)) for x, y in zip(a, b))
+
+
+@pytest.mark.parametrize("cls", CLASSES)
+def test_plan_matches_forward_golden(cls):
+    args = (golden_state_dict(), M, REPS, G[f"{cls}_sites"], G[f"{cls}_spatial_shape"], G[f"{cls}_vfeats"],
+            G[f"{cls}_p2v"])
+    assert _same(PR.forward_by_plan(*args), PR.forward(*args))
+
+
+@pytest.mark.parametrize("m,reps,seed", [(32, 2, 41), (8, 1, 42)])
+def test_plan_matches_forward_synthetic(m, reps, seed):
+    sd = PR.synthetic_state_dict(list(weights.pointgroup_keys(m, reps).items()), seed)
+    rng = np.random.RandomState(seed)
+    vox = np.unique(rng.randint(0, 16, (2000, 3)), axis=0)
+    vox = vox[rng.permutation(len(vox))]                  # forward takes the sites in any order
+    p2v = rng.randint(0, len(vox), 3000)
+    args = (sd, m, reps, vox, (128, 128, 128), rng.randn(len(vox), PR.INPUT_C).astype(np.float32), p2v)
+    assert _same(PR.forward_by_plan(*args), PR.forward(*args))
+
+
+@pytest.mark.parametrize("m,reps", [(16, 2), (12, 1)])
+def test_plan_covers_every_convolution(m, reps):
+    recs = PR.plan(m, reps)
+    keys = weights.pointgroup_keys(m, reps)
+    convs = [k[:-len(".weight")] for k, s in keys.items() if len(s) == 5 and k.startswith(("input_conv.", "unet."))]
+    assert sorted(r.name for r in recs) == sorted(convs)
+    for r in recs:
+        k = round(r.K ** (1 / 3))
+        assert keys[r.name + ".weight"] == (k, k, k, r.cin, r.cout)
+        if r.bn is not None:
+            assert keys[r.bn + ".weight"] == (r.cin,)
+    # every source is an earlier layer (or the voxel features) and the widths add up
+    width = {PR.VFEATS: PR.INPUT_C}
+    for r in recs:
+        assert sum(width[s] for s in r.src) == r.cin
+        assert r.res is None or sum(width[s] for s in r.res) == r.cout
+        width[r.name] = r.cout
+    assert recs[-1].level == 0 and recs[-1].cout == m
+
+
 def test_keep_mask_drops_float32_xmax():
     # in float32, xmin + (xmax - xmin) rounds below xmax here, so the reference drops the point at xmax
     xmin, xmax = np.float32(-0.07290356), np.float32(0.19376823)
