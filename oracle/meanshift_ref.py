@@ -8,7 +8,14 @@ q = rint(ldexp(p - origin, 41 - E)), origin = min_bound - bw/2, E = ceil(log2(ma
 is dtype(ldexp(sum) / n + origin) in X's dtype.  The post-processing is sklearn's own (_mean_shift.py, fit): a dict of
 centres keyed by value, sorted by (count, centre) descending, greedy suppression within bw, nearest kept centre with
 ties to the smaller index.
+
+step_bruteforce and modes_bruteforce restate one ascent step and the post-processing with no tree at all: every
+(centre, point) and every (mode, mode) pair is compared.  They pin the tree-based ascent / modes above, and they let a
+test feed the kernel's own intermediate results (a run stopped at max_iter k, the kernel's seed centres) through one
+more step or through the post-processing.
 """
+import math
+
 import numpy as np
 from scipy.spatial import cKDTree
 
@@ -120,6 +127,93 @@ def modes(centres, counts, bw):
         if unique[i]:
             unique[nbr[i]] = False
     return sc[unique]
+
+
+def frame(X, bw):
+    """(origin, E) of the kernel's fixed point (cg_meanshift.cu's header): origin = min_bound - bw/2 per axis, the
+    origin of the cell index over X, and E the smallest integer with 2^E >= max(p - origin) + bw."""
+    X64 = np.asarray(X, np.float64)
+    origin = X64.min(axis=0) - bw * 0.5
+    umax = max(float(X64[:, a].max()) - float(origin[a]) for a in range(3))
+    m, e = math.frexp(umax + bw)
+    return origin, e - 1 if m == 0.5 else e
+
+
+def step_bruteforce(X, bw, M, chunk=1 << 22):
+    """One ascent step from every centre of M (rows in X's dtype) over all points of X, pair by pair:
+    (new centre in X's dtype, set size, the set's mean in float64 as sklearn defines it).
+
+    Membership is d2 = (dx*dx + dy*dy) + dz*dz <= bw*bw, each operation rounded on its own; the new centre is
+    dtype(float(sum q) * 2^(E-41) / n + origin) with q the int64 fixed-point image of each point.  The mean is summed
+    in extended precision, so it is within an ulp of the exact mean of the set.  A centre with an empty set keeps its
+    value, count 0 and a NaN mean.  Works through chunks of about `chunk` pairs."""
+    X = np.asarray(X)
+    T = X.dtype.type
+    X64 = X.astype(np.float64)
+    M = np.asarray(M, T).reshape(-1, 3)
+    M64 = M.astype(np.float64)
+    origin, E = frame(X64, bw)
+    q = np.rint((X64 - origin) * math.ldexp(1.0, QBITS - E)).astype(np.int64)
+    bw2 = bw * bw
+    new = M.copy()
+    n = np.zeros(len(M), np.int64)
+    mean = np.full((len(M), 3), np.nan)
+    rows = max(1, chunk // len(X))
+    for s in range(0, len(M), rows):
+        m = M64[s:s + rows]
+        dx = m[:, None, 0] - X64[None, :, 0]
+        dy = m[:, None, 1] - X64[None, :, 1]
+        dz = m[:, None, 2] - X64[None, :, 2]
+        r, c = np.nonzero((dx * dx + dy * dy) + dz * dz <= bw2)
+        if not len(r):
+            continue
+        cnt = np.bincount(r, minlength=len(m))
+        full = np.flatnonzero(cnt)
+        starts = np.concatenate([[0], np.cumsum(cnt)[:-1]])[full]
+        sums = np.add.reduceat(q[c], starts, axis=0)                           # int64: below 2^62 for P <= 2^21
+        ext = np.add.reduceat(X64[c].astype(np.longdouble), starts, axis=0)
+        n[s + full] = cnt[full]
+        mean[s + full] = (ext / cnt[full, None].astype(np.longdouble)).astype(np.float64)
+        for i, k in enumerate(full.tolist()):
+            for a in range(3):
+                v = float(int(sums[i, a])) * math.ldexp(1.0, E - QBITS) / float(cnt[k]) + float(origin[a])
+                new[s + k, a] = T(v)
+    return new, n, mean
+
+
+def bound_ratio(centre, mean, E):
+    """|centre - mean| over its bound, per entry, for a centre from the fixed-point step and its set's mean (NaN rows,
+    empty sets, give 0).  Each q is within half a quantum 2^(E-41) of fl(p - origin), itself within 2^(E-53) of
+    p - origin; the int64 -> double conversion and the division add 2^(E-53) each; adding the origin rounds by half
+    an ulp of the centre in float64, narrowing by half an ulp in the centre's dtype; the mean is good to an ulp."""
+    c = np.asarray(centre)
+    c64 = c.astype(np.float64)
+    bound = (0.5 * math.ldexp(1.0, E - QBITS) + 3 * math.ldexp(1.0, E - 53) + np.spacing(np.abs(c64)) / 2
+             + np.spacing(np.abs(c)).astype(np.float64) / 2 + np.spacing(np.abs(np.nan_to_num(mean))))
+    return np.nan_to_num(np.abs(c64 - mean) / bound)
+
+
+def modes_bruteforce(seed_centres, seed_counts, bw):
+    """sklearn's post-processing with no tree: seeds with a non-empty set in a dict keyed by centre value (-0.0 ==
+    0.0; the first key, the last count), sorted by (count, x, y, z) descending, then greedy suppression in that order
+    over all later pairs with d2 = (dx*dx + dy*dy) + dz*dz <= bw*bw.  The kept centres in the seeds' dtype."""
+    c = np.asarray(seed_centres)
+    T = c.dtype.type
+    d = {}
+    for key, k in zip(c.astype(np.float64).tolist(), np.asarray(seed_counts).tolist()):
+        if k:
+            d[tuple(key)] = k
+    ranked = sorted(d.items(), key=lambda t: (t[1], t[0][0], t[0][1], t[0][2]), reverse=True)
+    sc = np.array([t[0] for t in ranked], np.float64).reshape(-1, 3)
+    keep = np.ones(len(sc), bool)
+    bw2 = bw * bw
+    for i in range(len(sc)):
+        if keep[i]:
+            dx = sc[i, 0] - sc[i + 1:, 0]
+            dy = sc[i, 1] - sc[i + 1:, 1]
+            dz = sc[i, 2] - sc[i + 1:, 2]
+            keep[i + 1:] &= ~((dx * dx + dy * dy) + dz * dz <= bw2)
+    return sc[keep].astype(T)
 
 
 def fit(X, bw, max_iter=300):

@@ -61,6 +61,51 @@ def test_max_iter_zero_and_empty_sets_follow_sklearn():
         assert np.array_equal(o["labels"], sk.labels_)
 
 
+@pytest.mark.parametrize("dtype", [np.float32, np.float64])
+def test_step_bruteforce_is_one_step_of_the_ascent(dtype):
+    """The ascent at max_iter k, seed by seed: a seed still moving after run k - 1 (X itself before run 0) takes one
+    step_bruteforce step from its centre there, and stops at k when that step is empty or shorter than 1e-3 bw; every
+    other seed keeps run k - 1's result.  Each step lands within the fixed point's bound of its set's mean."""
+    bw = 0.007
+    X = shifted_pile(1500, 8, seed=1, pull=0.3).astype(dtype)
+    origin, E = meanshift_ref.frame(X, bw)
+    o, e, _ = meanshift_ref.quantise(X.astype(np.float64), bw)
+    assert E == e and origin.tobytes() == o.tobytes()
+    c_prev, n_prev, it_prev = X, np.zeros(len(X), np.int64), np.zeros(len(X), np.int64)
+    moving = np.ones(len(X), bool)
+    for k in range(5):
+        c, n, it = meanshift_ref.ascent(X, bw, max_iter=k)
+        assert c[~moving].tobytes() == c_prev[~moving].tobytes()
+        assert np.array_equal(n[~moving], n_prev[~moving]) and np.array_equal(it[~moving], it_prev[~moving])
+        new, cnt, mean = meanshift_ref.step_bruteforce(X, bw, c_prev[moving])
+        assert new.tobytes() == c[moving].tobytes() and np.array_equal(cnt, n[moving]) and (it[moving] == k).all()
+        assert (meanshift_ref.bound_ratio(new, mean, E) <= 1.0).all()
+        d = (new - c_prev[moving]).astype(np.float64)
+        step = np.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
+        moving[np.flatnonzero(moving)[(cnt == 0) | (step <= 1e-3 * bw)]] = False
+        c_prev, n_prev, it_prev = c, n, it
+    assert moving.any() and not moving.all()
+
+
+@pytest.mark.parametrize("max_iter", [0, 300])
+@pytest.mark.parametrize("dtype", [np.float32, np.float64])
+@pytest.mark.parametrize("bw", [0.005, 0.007, 0.009])
+def test_modes_bruteforce_equals_modes(bw, dtype, max_iter):
+    X = shifted_pile(1500, 8, seed=1, pull=0.0).astype(dtype)
+    c, n, _ = meanshift_ref.ascent(X, bw, max_iter=max_iter)
+    got = meanshift_ref.modes_bruteforce(c, n, bw)
+    assert got.dtype == X.dtype and got.tobytes() == meanshift_ref.modes(c, n, bw).tobytes()
+
+
+def test_modes_bruteforce_dict_rule():
+    """Equal centres (+0.0 and -0.0 among them) collapse to the first seed's value with the last seed's count."""
+    c = np.array([[-0.0, 1.0, 2.0], [5.0, 5.0, 5.0], [0.0, 1.0, 2.0], [9.0, 9.0, 9.0]])
+    assert meanshift_ref.modes_bruteforce(c, [1, 2, 3, 0], 0.5).tobytes() == np.array(
+        [[-0.0, 1.0, 2.0], [5.0, 5.0, 5.0]]).tobytes()
+    assert meanshift_ref.modes_bruteforce(c, [3, 2, 1, 0], 0.5).tobytes() == np.array(
+        [[5.0, 5.0, 5.0], [-0.0, 1.0, 2.0]]).tobytes()
+
+
 X_OK = np.zeros((4, 3), np.float32) + np.arange(4, dtype=np.float32)[:, None] * 0.01
 
 
