@@ -8,6 +8,7 @@ the card's name and power limit, for several ring depths.
 
     python scripts/l2_stream_probe.py [--reps 400]
 """
+import _harness
 import argparse
 import os
 import subprocess
@@ -99,9 +100,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=400, help="passes over the 256 KB image per CTA")
     args = ap.parse_args()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print(f"card: {gpu}")
+    print("card:", _harness.card())
     with tempfile.TemporaryDirectory(prefix="cg_l2probe_") as td:
         src, exe = os.path.join(td, "probe.cu"), os.path.join(td, "probe")
         with open(src, "w") as f:
@@ -110,9 +109,7 @@ def main():
         subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-o", exe, src])
         out = subprocess.run([exe, str(args.reps)], capture_output=True, text=True)
         print(out.stdout, end="")
-        clk = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True).stdout.strip()
-        print(f"SM clock after the run: {clk}")
+        print(f"SM clock after the run: {_harness.smi('clocks.sm')}")
         if out.returncode != 0:
             raise SystemExit(out.returncode)
 

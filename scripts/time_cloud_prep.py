@@ -8,52 +8,25 @@ numpy back-projection).  open3d's voxel_down_sample and estimate_normals are not
 
     python scripts/time_cloud_prep.py [--objects 8] [--reps 5] [--out results/time_cloud_prep.json]
 """
+import _harness
 import argparse
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from catgrasp_b200 import cloud, synthetic
 
-from catgrasp_b200 import cloud, synthetic   # noqa: E402
-
-K = np.array([2257.7500557850776, 0, 1032, 0, 2257.4882391629421, 772, 0, 0, 1], np.float64).reshape(3, 3)
-
-
-def card():
-    try:
-        return subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                                       text=True).strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f"unknown ({e})"
+K = _harness.REFERENCE_K
 
 
 def gpu_ms(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    out = []
-    for _ in range(reps):
-        s.record()
-        fn()
-        e.record()
-        e.synchronize()
-        out.append(s.elapsed_time(e))
-    return float(np.median(out))
+    return float(np.median(_harness.synced_ms(fn, reps, 1)))
 
 
 def host_ms(fn, reps):
-    out = []
-    for _ in range(reps):
-        t = time.perf_counter()
-        fn()
-        out.append(1e3 * (time.perf_counter() - t))
-    return float(np.median(out))
+    return float(np.median(_harness.wall_ms(fn, reps, 0)))
 
 
 def main():
@@ -62,10 +35,10 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
-    depth, ids = synthetic.render_depth(K, 1544, 2064, n_objects=a.objects, seed=0, bin_size=0.2)
+    res = {"card": _harness.card(), "frame": list(_harness.REFERENCE_HW)}
+    print("card:", res["card"])
+    depth, ids = synthetic.render_depth(K, *_harness.REFERENCE_HW, n_objects=a.objects, seed=0, bin_size=0.2)
     d_dev = torch.from_numpy(depth).cuda()
-    res = {"card": card(), "frame": [1544, 2064]}
 
     xyz_dev = cloud.depth2xyzmap(d_dev, K)
     xyz = xyz_dev.cpu().numpy()

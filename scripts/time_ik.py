@@ -6,17 +6,15 @@ Prints the card name and power limit read in the same run, then one line per mea
 
     python scripts/time_ik.py
 """
+import _harness
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden"))
 
 from catgrasp_b200 import my_cpp  # noqa: E402
 from catgrasp_b200.ik import iiwa14_fk, iiwa14_ik  # noqa: E402
@@ -25,32 +23,13 @@ from catgrasp_b200.synthetic import make_filter_case  # noqa: E402
 from make_golden_mycpp import IK_LOWER, IK_UPPER, ik_frames  # noqa: E402
 
 
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:      # noqa: BLE001
-        q = f"nvidia-smi unavailable ({e})"
-    return f"{torch.cuda.get_device_name(0)} | {q}"
-
-
-def timed(fn, reps=20, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ts = []
-    for _ in range(reps):
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b))
+def timed(fn, reps=20):
+    ts = _harness.synced_ms(fn, reps, 3)
     return float(np.median(ts)), float(np.min(ts))
 
 
 def main():
-    print("device:", card())
+    print("card:", _harness.card())
     rng = np.random.RandomState(0)
     Q = 1 << 20
     q = rng.uniform(-2.5, 2.5, (Q, 7))

@@ -4,17 +4,15 @@ sklearn's MeanShift on the host cores for comparison.  Prints the card and its p
 
     python scripts/time_meanshift.py [--reps 5] [--no-sklearn]
 """
+import _harness
 import argparse
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-from catgrasp_b200 import segment, synthetic   # noqa: E402
+from catgrasp_b200 import segment, synthetic
 
 
 def scene(n_points, n_objects, seed, pull=0.6, noise=0.001):
@@ -27,17 +25,8 @@ def scene(n_points, n_objects, seed, pull=0.6, noise=0.001):
 
 
 def cuda_ms(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    out = []
-    for _ in range(reps):
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        out.append(a.elapsed_time(b))
-    return np.median(out), min(out), max(out)
+    ts = _harness.synced_ms(fn, reps, 1)
+    return np.median(ts), min(ts), max(ts)
 
 
 def main():
@@ -45,9 +34,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--no-sklearn", action="store_true")
     args = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    print("card:", q.stdout.strip() or torch.cuda.get_device_name(0), "| host cores:", os.cpu_count())
+    print("card:", _harness.card(), "| host cores:", os.cpu_count())
     bw = segment.MEANSHIFT_BANDWIDTH["nut"]
     for n_points, n_objects, seed in ((8000, 16, 1), (40000, 40, 2), (160000, 160, 3)):
         xyz, off = scene(n_points, n_objects, seed)

@@ -9,40 +9,31 @@ against cg_host_legacy_skip over the same stream.
 
     python scripts/time_nunocs.py [--reps 5]
 """
+import _harness
 import argparse
 import copy
 import os
-import subprocess
 import sys
 import tempfile
-import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
 
 from catgrasp_b200 import cloud, synthetic   # noqa: E402
 from catgrasp_b200.predicter import NunocsPredicter, _LegacyDraw   # noqa: E402
 
-K = np.array([2257.7500557850776, 0, 1032, 0, 2257.4882391629421, 772, 0, 0, 1], np.float64).reshape(3, 3)
-
-
-def spread(ts):
-    ts = np.asarray(ts)
-    return f"median {np.median(ts):9.2f} ms  min {ts.min():9.2f}  max {ts.max():9.2f}  (n={len(ts)})"
+K = _harness.REFERENCE_K
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     a = ap.parse_args()
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip()
-    print("GPU:", smi)
+    print("card:", _harness.card())
     from test_ransac_pose import old_predict
-    depth, ids = synthetic.render_depth(K, 1544, 2064, n_objects=16, seed=1)
+    depth, ids = synthetic.render_depth(K, *_harness.REFERENCE_HW, n_objects=16, seed=1)
     xyz = cloud.depth2xyzmap(depth, K)
     lab = ids[ids >= 0]
     pts = xyz[ids >= 0].reshape(-1, 3)
@@ -55,30 +46,27 @@ def main():
         device=0)
     print(f"object: {len(ob)} points, n_pts {npd.cfg['n_pts']}, H = {npd.ransac_max_iter} per threshold")
 
+    times, poses = {"old": [], "host": [], "device": []}, {}
+
     def run(mode):
-        np.random.seed(0)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
         if mode == "old":
-            out = old_predict(npd, copy.deepcopy(data))[1]
+            poses[mode] = old_predict(npd, copy.deepcopy(data))[1]
         else:
             npd.subsample = mode
-            out = npd.predict(copy.deepcopy(data))[1]
-        torch.cuda.synchronize()
-        return (time.perf_counter() - t0) * 1e3, out
+            poses[mode] = npd.predict(copy.deepcopy(data))[1]
 
-    times, poses = {"old": [], "host": [], "device": []}, {}
-    for m in times:
-        run(m)                                                # warm-up
+    for m in times:                                           # warm-up
+        np.random.seed(0)
+        run(m)
     for _ in range(a.reps):
         for m in times:
-            t, poses[m] = run(m)
-            times[m].append(t)
+            np.random.seed(0)
+            times[m] += _harness.wall_ms(lambda: run(m), 1, 0)
     same = (poses["old"] is None and poses["host"] is None) or \
         (poses["old"] is not None and poses["host"] is not None and poses["old"].tobytes() == poses["host"].tobytes())
     print(f"host pose == old pose bit for bit: {same}")
     for m in ("old", "host", "device"):
-        print(f"predict {m:7s} {spread(times[m])}")
+        print(f"predict {m:7s} {_harness.summary(times[m])}")
 
     # the fused launch alone
     from catgrasp_b200.aligning import ransac9d_pose
@@ -90,33 +78,20 @@ def main():
     tgt = torch.from_numpy(npd.data_transformed["cloud_xyz_original"]).to(dev)
     hyp = npd.model.draw_ids_dev(src.shape[0], 4, 2 * npd.ransac_max_iter, 1, first_candidate=1)
     kw = dict(max_scale=npd.max_scale, min_scale=npd.min_scale, max_dimensions=npd.MAX_DIMENSIONS)
-    for _ in range(3):
-        ransac9d_pose(src, tgt, hyp, npd.THRESHOLDS, **kw)
-    ev = []
-    for _ in range(20):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        ransac9d_pose(src, tgt, hyp, npd.THRESHOLDS, **kw)
-        e1.record()
-        ev.append((e0, e1))
-    torch.cuda.synchronize()
-    print(f"fused launch (N = {src.shape[0]}, 2 x {npd.ransac_max_iter}) {spread([x.elapsed_time(y) for x, y in ev])}")
+    ts = _harness.queued_ms(lambda: ransac9d_pose(src, tgt, hyp, npd.THRESHOLDS, **kw), 20, 3)
+    print(f"fused launch (N = {src.shape[0]}, 2 x {npd.ransac_max_iter}) {_harness.summary(ts)}")
 
     # the host draw against the walk alone
     td, ts = [], []
     for _ in range(a.reps):
         np.random.seed(1)
         d = _LegacyDraw()
-        t0 = time.perf_counter()
-        d.draw(8192, 4, 20000)
-        td.append((time.perf_counter() - t0) * 1e3)
+        td += _harness.wall_ms(lambda: d.draw(8192, 4, 20000), 1, 0)
         np.random.seed(1)
         d = _LegacyDraw()
-        t0 = time.perf_counter()
-        d.skip(8192, 4, 20000)
-        ts.append((time.perf_counter() - t0) * 1e3)
-    print(f"host draw 20000 x (4 of 8192)      {spread(td)}")
-    print(f"cg_host_legacy_skip, same stream   {spread(ts)}")
+        ts += _harness.wall_ms(lambda: d.skip(8192, 4, 20000), 1, 0)
+    print(f"host draw 20000 x (4 of 8192)      {_harness.summary(td)}")
+    print(f"cg_host_legacy_skip, same stream   {_harness.summary(ts)}")
     print(f"draw / skip (medians) {np.median(td) / np.median(ts):.2f}")
 
 

@@ -6,21 +6,17 @@ reference K, 1544 x 2064), with synthetic weights: the renderer's id map stands 
 
 --subsample device runs NUNOCS and grasp-Q on their device draws (no host walk of numpy's generator).
 """
+import _harness
 import argparse
-import os
-import subprocess
-import sys
 import tempfile
 import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from catgrasp_b200 import pick, synthetic
 
-from catgrasp_b200 import pick, synthetic   # noqa: E402
-
-K = np.array([2257.7500557850776, 0, 1032, 0, 2257.4882391629421, 772, 0, 0, 1], np.float64).reshape(3, 3)
+K = _harness.REFERENCE_K
 CFG_RUN = {"nocs_grasp_sampler_score_larger_than": 0.95, "nocs_grasp_sampler_max_n_grasp": 10000,
            "cone_grasp_smapler_n_sphere_dir": 30, "cone_grasp_smapler_approach_step": 0.002}
 
@@ -38,10 +34,8 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--subsample", choices=("host", "device"), default="host")
     a = ap.parse_args()
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip()
-    print("GPU:", smi)
-    depth, ids = synthetic.render_depth(K, 1544, 2064, n_objects=16, seed=1)
+    print("card:", _harness.card())
+    depth, ids = synthetic.render_depth(K, *_harness.REFERENCE_HW, n_objects=16, seed=1)
     bg = ids < 0
     dev = torch.device("cuda", 0)
     from catgrasp_b200.predicter import GraspPredicter, NunocsPredicter

@@ -7,10 +7,9 @@ the camera (no stage's time depends on their values).  Median of 5 after 2 warm-
 
     python scripts/time_pointgroup.py [--objects 16] [--m 16 32]
 """
+import _harness
 import argparse
 import os
-import subprocess
-import sys
 import tempfile
 import time
 
@@ -18,17 +17,12 @@ import numpy as np
 import torch
 import yaml
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from catgrasp_b200 import pointgroup, spconv, synthetic, weights     # noqa: E402
-from catgrasp_b200.predicter import PointGroupPredictor               # noqa: E402
-from catgrasp_b200.segment import MEANSHIFT_BANDWIDTH, pointgroup_labels   # noqa: E402
-from oracle.pointgroup_ref import synthetic_state_dict                # noqa: E402
+from catgrasp_b200 import pointgroup, spconv, synthetic, weights
+from catgrasp_b200.predicter import PointGroupPredictor
+from catgrasp_b200.segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
+from oracle.pointgroup_ref import synthetic_state_dict
 
-K = np.array([2257.7500557850776, 0, 1032, 0, 2257.4882391629421, 772, 0, 0, 1], np.float64).reshape(3, 3)
-
-
-def _med(xs):
-    return float(np.median(xs))
+K = _harness.REFERENCE_K
 
 
 def _predictor(m, tmp):
@@ -79,10 +73,8 @@ def main():
     ap.add_argument("--objects", type=int, default=16)
     ap.add_argument("--m", type=int, nargs="+", default=[16, 32])
     args = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                          capture_output=True, text=True).stdout.strip().splitlines()[0]
-    print(f"card: {card}")
-    depth, _ = synthetic.render_depth(K, 1544, 2064, n_objects=args.objects, seed=0, bin_size=0.2)
+    print("card:", _harness.card())
+    depth, _ = synthetic.render_depth(K, *_harness.REFERENCE_HW, n_objects=args.objects, seed=0, bin_size=0.2)
     v, u = np.nonzero(depth >= 0.1)
     z = depth[v, u].astype(np.float64)
     xyz = np.stack([(u - K[0, 2]) * z / K[0, 0], (v - K[1, 2]) * z / K[1, 1], z], 1).astype(np.float32)
@@ -99,7 +91,7 @@ def main():
                   f"levels {r0['levels']}")
             for k in ("host front", "voxelisation", "forward (GPU)", "forward enqueue (host)", "head (GPU)",
                       "pointgroup_labels", "total"):
-                print(f"  {k:24s} {_med([r[k] for r in runs]):9.3f} ms")
+                print(f"  {k:24s} {_harness.summary([r[k] for r in runs])}")
 
 
 if __name__ == "__main__":

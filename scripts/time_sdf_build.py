@@ -5,20 +5,17 @@ One build = the blocking cg_sdf_from_mesh call (host-side Morton sort and snappi
 download of the grid for its boundary statistics), bracketed by CUDA events on the stream it runs on; median of
 repeats after warm-up.  The brute-force oracle's host time for the same grid is extrapolated from a sample of nodes, as
 context.  With culling, going from 12 k to 200 k triangles of the same geometry should cost far less than 16x."""
+import _harness
 import argparse
 import ctypes as C
-import os
-import subprocess
-import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import numpy as np
+import torch
 
-from catgrasp_b200 import _lib  # noqa: E402
-from catgrasp_b200.synthetic import make_gripper_proxy, make_hex_nut_mesh, tessellated_box_mesh  # noqa: E402
-from oracle.sdf_mesh_ref import grid_geometry, node_positions, sdf_mesh_ref  # noqa: E402
+from catgrasp_b200 import _lib
+from catgrasp_b200.synthetic import make_gripper_proxy, make_hex_nut_mesh, tessellated_box_mesh
+from oracle.sdf_mesh_ref import grid_geometry, node_positions, sdf_mesh_ref
 
 
 def tessellated_proxy(m):
@@ -36,14 +33,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--oracle-sample", type=int, default=256)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
     torch.cuda.set_device(0)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    print(f"card: {q[0] if q else torch.cuda.get_device_name(0)}")
+    print("card:", _harness.card())
     ctx = _lib.Context.get(0)
     ctx.use_torch_stream()
-    stream = torch.cuda.current_stream()
     g = make_gripper_proxy()["open"]
     meshes = [("proxy", g["V"], g["F"]), ("proxy_tess12k", *tessellated_proxy(18)),
               ("proxy_tess200k", *tessellated_proxy(75)), ("hex_nut", *make_hex_nut_mesh(n_seg=480))]
@@ -57,15 +50,11 @@ def main():
             ms = []
             for it in range(a.warmup + a.repeats):
                 h = C.c_void_p()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(stream)
-                ctx.check(ctx.lib.cg_sdf_from_mesh(ctx.h, _lib.ptr(V), V.shape[0], _lib.ptr(F), F.shape[0],
-                                                   C.c_float(res), 5, C.byref(h)))
-                e1.record(stream)
-                torch.cuda.synchronize()
-                ctx.lib.cg_sdf_destroy(h)
+                t = _harness.synced_ms(lambda: ctx.check(ctx.lib.cg_sdf_from_mesh(
+                    ctx.h, _lib.ptr(V), V.shape[0], _lib.ptr(F), F.shape[0], C.c_float(res), 5, C.byref(h))), 1, 0)
+                ctx.lib.cg_sdf_destroy(h)          # outside the timed build
                 if it >= a.warmup:
-                    ms.append(e0.elapsed_time(e1))
+                    ms += t
             dims, origin, r32 = grid_geometry(V, res, 5)
             ncell = int(np.prod(dims))
             idx = np.stack([rng.randint(0, d, a.oracle_sample) for d in dims], 1)

@@ -7,30 +7,19 @@ runs.  Prints the card, its power limit, per-level site counts and the FLOPs of 
 
     python scripts/time_spconv.py [--objects 16] [--m 16]
 """
+import _harness
 import argparse
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from catgrasp_b200 import _lib, spconv, synthetic   # noqa: E402
+from catgrasp_b200 import _lib, spconv, synthetic
 
-K = np.array([2257.7500557850776, 0, 1032, 0, 2257.4882391629421, 772, 0, 0, 1], np.float64).reshape(3, 3)
+K = _harness.REFERENCE_K
 
 
-def _time(fn, reps=20, warm=5):
-    for _ in range(warm):
-        fn()
-    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
-    for a, b in ev:
-        a.record()
-        fn()
-        b.record()
-    torch.cuda.synchronize()
-    return float(np.median([a.elapsed_time(b) for a, b in ev]))
+def _time(fn):
+    return float(np.median(_harness.queued_ms(fn, 20, 5)))
 
 
 def main():
@@ -38,10 +27,8 @@ def main():
     ap.add_argument("--objects", type=int, default=16)
     ap.add_argument("--m", type=int, default=16)
     args = ap.parse_args()
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                          capture_output=True, text=True).stdout.strip().splitlines()[0]
-    print(f"card: {card}")
-    depth, _ = synthetic.render_depth(K, 1544, 2064, n_objects=args.objects, seed=0, bin_size=0.2)
+    print("card:", _harness.card())
+    depth, _ = synthetic.render_depth(K, *_harness.REFERENCE_HW, n_objects=args.objects, seed=0, bin_size=0.2)
     v, u = np.nonzero(depth >= 0.1)
     z = depth[v, u].astype(np.float64)
     xyz = np.stack([(u - K[0, 2]) * z / K[0, 0], (v - K[1, 2]) * z / K[1, 1], z], 1)
