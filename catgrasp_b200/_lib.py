@@ -140,6 +140,8 @@ SIGNATURES = {
     "cg_occupancy_from_scan_host": (_i, [_vp, _H, _i, _f, _H], OWN),
     "cg_ransac9d_host": (_i, [_vp, _H, _H, _i, _H, _i, _d, _H, _H, _H, _H, _H, _H], OWN),
     "cg_ransac9d_pose_dev": (_i, [_vp, _D, _D, _i, _D, _i, _H, _i, _H, _H, _H, _d, _D], TORCH),
+    "cg_ransac9d_kdtree_host": (_i, [_vp, _H, _H, _i, _H, _i, _d, _H, _H, _H, _d, _H, _H, _H], OWN),
+    "cg_ransac9d_kdtree_pose_dev": (_i, [_vp, _D, _D, _i, _D, _i, _H, _i, _H, _H, _H, _d, _d, _D], TORCH),
     "cg_cone_poses_dev": (_i, [_vp, _D, _D, _i, _D, _i, _D, _i, _D, _i, _d, _D, _D], TORCH),
     "cg_center_grasps_dev": (_i, [_vp, _D, _D, _i, _D, _i], TORCH),
     "cg_grasp_affordance_dev": (_i, [_vp, _D, _i, _D, _D, _D, _i, _H, _H, _i, _d, _D, _D], TORCH),

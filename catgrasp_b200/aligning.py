@@ -7,18 +7,55 @@ ratio over the hypotheses that survive the gates, aligning.py:105-117).
 
 ``ransac9d_pose`` is the device-side form used by NunocsPredicter.predict: both thresholds scored, selected and
 checked in one launch on CUDA tensors (cg_ransac9d_pose_dev), with the subsets given by the caller.
+
+Both take the reference's kd-tree evaluation (aligning.py:68-79): each hypothesis is scored by the two-way
+nearest-neighbour test between the transformed source and the target, each thinned to voxel means of size
+``kdtree_eval_resolution``, out of 2N (cg_ransac9d_kdtree_host / cg_ransac9d_kdtree_pose_dev).
 """
+import math
+
 import numpy as np
 
 from . import _lib
 
 
+def _resolution(r):
+    """The kd-tree evaluation's voxel size as a float; ValueError when it is missing, not positive or not finite."""
+    try:
+        v = float(r)
+    except (TypeError, ValueError):
+        raise ValueError(f"kdtree_eval_resolution must be a positive finite number, got {r!r}") from None
+    if not (math.isfinite(v) and v > 0.0):
+        raise ValueError(f"kdtree_eval_resolution must be a positive finite number, got {r!r}")
+    return v
+
+
+def transform_points(T, pts):
+    """src_t = T [pts, 1] in the kd-tree kernel's operation order, ((T00 x + T01 y) + T02 z) + T03 per row, each
+    operation rounded on its own."""
+    p = np.asarray(pts, np.float64)
+    return np.stack([((T[a, 0] * p[:, 0] + T[a, 1] * p[:, 1]) + T[a, 2] * p[:, 2]) + T[a, 3] for a in range(3)], 1)
+
+
+def kdtree_inliers(T, source, target, PassThreshold, kdtree_eval_resolution):
+    """aligning.py:79 for the hypothesis T: the source points whose transform lies within PassThreshold of a voxel
+    mean of the target (voxel size kdtree_eval_resolution), with the kernel's src_t and distances."""
+    from .cloud import CloudIndex, _query_cell
+    import torch
+    src_t = transform_points(T, source)
+    down = CloudIndex(np.ascontiguousarray(target, np.float64), kdtree_eval_resolution).voxel_means()[0]
+    mask = CloudIndex(down, _query_cell(down, PassThreshold), device=down.device.index).within(
+        torch.from_numpy(np.ascontiguousarray(src_t)).to(down.device), PassThreshold, compare_sqrt=True)
+    return np.nonzero(mask.cpu().numpy())[0]
+
+
 def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree_for_eval=False,
                         kdtree_eval_resolution=None, max_scale=np.array([99, 99, 99]),
                         min_scale=np.array([0, 0, 0]), max_dimensions=None):
-    """Returns (best_transform (4,4) float64, inliers) or (None, None), like aligning.py:83-119."""
-    if use_kdtree_for_eval:
-        raise NotImplementedError("kd-tree evaluation (aligning.py:68-79) is never enabled by the predicter")
+    """Returns (best_transform (4,4) float64, inliers) or (None, None), like aligning.py:83-119.  With
+    use_kdtree_for_eval the ratio is the kd-tree evaluation's and the inliers are the winner's source points within
+    PassThreshold of the target's voxel means (aligning.py:68-79); at most CG_RANSAC_KD_MAX_N = 65536 points."""
+    r = _resolution(kdtree_eval_resolution) if use_kdtree_for_eval else None
     source = np.ascontiguousarray(source, dtype=np.float64)
     target = np.ascontiguousarray(target, dtype=np.float64)
     N = source.shape[0]
@@ -32,13 +69,19 @@ def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree
     ratio = np.empty(max_iter, np.float64)
     T = np.empty((max_iter, 4, 4), np.float64)
     valid = np.empty(max_iter, np.uint8)
-    ctx.call("cg_ransac9d_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs, mdim, ratio,
-             T, valid)
+    if r is None:
+        ctx.call("cg_ransac9d_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs, mdim,
+                 ratio, T, valid)
+    else:
+        ctx.call("cg_ransac9d_kdtree_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs,
+                 mdim, r, ratio, T, valid)
     keep = np.nonzero(valid)[0]
     if keep.size == 0:
         return None, None
     best = keep[np.argmax(ratio[keep])]                         # first maximum among the survivors (aligning.py:115)
     best_transform = T[best].copy()
+    if r is not None:
+        return best_transform, kdtree_inliers(best_transform, source, target, PassThreshold, r)
     errs = np.linalg.norm((best_transform @ np.c_[source, np.ones(N)].T).T[:, :3] - target, axis=-1)
     inliers = np.where(errs <= PassThreshold)[0]
     return best_transform, inliers
@@ -48,16 +91,19 @@ REC_PER_THR = 19     # include/catgrasp_b200.h, cg_ransac9d_pose_dev's record
 
 
 def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 99]), min_scale=np.array([0, 0, 0]),
-                  max_dimensions=None, ratio_threshold=0.003):
+                  max_dimensions=None, ratio_threshold=0.003, kdtree_eval_resolution=None):
     """The NUNOCS pose search on the device, for CUDA tensors ``source`` / ``target`` (N,3) float64 and ``ids``
     (T*H,4) int32 (rows t*H .. t*H+H-1 are threshold t's subsets), T = len(thresholds) in {1, 2}.  One launch, no
     synchronisation.  Returns a dict of CUDA tensors (views of the launch's record):
       per threshold: 'winner' (T,) the first maximum among valid hypotheses or -1, 'count' (T,) its inlier count,
       'T' (T,4,4) its transform (bit for bit estimate9DTransform's on the same subsets), 'count_ratio' (T,) its
       count of residuals <= ratio_threshold;
-      overall: 'chosen' () the threshold predict would pick or -1, 'pose' (4,4), 'best_ratio' ()."""
+      overall: 'chosen' () the threshold predict would pick or -1, 'pose' (4,4), 'best_ratio' ().
+    With ``kdtree_eval_resolution`` the hypotheses are scored by the kd-tree evaluation (each 'count' out of 2N; the
+    launch then synchronises, see cg_ransac9d_kdtree_pose_dev)."""
     import torch
     from . import _lib
+    r = None if kdtree_eval_resolution is None else _resolution(kdtree_eval_resolution)
     ctx, source, target = _lib.inputs(source, target, dtype=torch.float64)
     _, ids = _lib.inputs(ids, dtype=torch.int32, ctx=ctx)
     thr = np.ascontiguousarray(np.asarray(thresholds, dtype=np.float64).reshape(-1))
@@ -68,8 +114,12 @@ def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 9
     maxs = np.ascontiguousarray(np.asarray(max_scale, dtype=np.float64).reshape(3))
     mdim = None if max_dimensions is None else np.ascontiguousarray(np.asarray(max_dimensions, dtype=np.float64).reshape(3))
     rec = torch.empty((T * REC_PER_THR + 18,), dtype=torch.float64, device=source.device)
-    ctx.call("cg_ransac9d_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs, mdim,
-             float(ratio_threshold), rec)
+    if r is None:
+        ctx.call("cg_ransac9d_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs, mdim,
+                 float(ratio_threshold), rec)
+    else:
+        ctx.call("cg_ransac9d_kdtree_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs,
+                 mdim, float(ratio_threshold), r, rec)
     per = rec[:T * REC_PER_THR].view(T, REC_PER_THR)
     tail = rec[T * REC_PER_THR:]
     return {"winner": per[:, 0].to(torch.int64), "count": per[:, 1].to(torch.int64), "T": per[:, 2:18].view(T, 4, 4),

@@ -66,10 +66,7 @@ __global__ void key_kernel(const double *__restrict__ pts, int P, double ox, dou
                            uint64_t *__restrict__ keys, int32_t *__restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= P) return;
-  const int64_t x = (int64_t)floor(__ddiv_rn(__dsub_rn(pts[3 * (size_t)i], ox), cell));
-  const int64_t y = (int64_t)floor(__ddiv_rn(__dsub_rn(pts[3 * (size_t)i + 1], oy), cell));
-  const int64_t z = (int64_t)floor(__ddiv_rn(__dsub_rn(pts[3 * (size_t)i + 2], oz), cell));
-  keys[i] = pack(x, y, z, bits);
+  keys[i] = cell_key(pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2], ox, oy, oz, cell, bits);
   vals[i] = i;
 }
 

@@ -1,5 +1,5 @@
 // cg_cloud_index.cuh -- the uniform-grid point index of cg_cloud.cu and the device helpers that query it, shared by
-// every source that searches a cloud (cg_cloud.cu, cg_meanshift.cu).  See cg_cloud.cu for the index's layout.
+// every source that searches a cloud (cg_cloud.cu, cg_meanshift.cu, cg_ransac.cu).  See cg_cloud.cu for the index's layout.
 #pragma once
 #include <cmath>
 #include "cg_common.cuh"
@@ -47,6 +47,16 @@ __device__ __forceinline__ uint64_t pack(int64_t x, int64_t y, int64_t z, int b)
   return ((uint64_t)x << (2 * b)) | ((uint64_t)y << b) | (uint64_t)z;
 }
 
+// a point's cell key: floor((p - origin) / cell) per axis, each operation rounded on its own, packed x major.  The
+// caller guarantees every coordinate lies in [0, 2^bits).
+__device__ __forceinline__ uint64_t cell_key(double px, double py, double pz, double ox, double oy, double oz, double cell,
+                                             int bits) {
+  const int64_t x = (int64_t)floor(__ddiv_rn(__dsub_rn(px, ox), cell));
+  const int64_t y = (int64_t)floor(__ddiv_rn(__dsub_rn(py, oy), cell));
+  const int64_t z = (int64_t)floor(__ddiv_rn(__dsub_rn(pz, oz), cell));
+  return pack(x, y, z, bits);
+}
+
 // cells [lo, hi] on one axis that can hold a point within R of q; false when none of them is occupied
 __device__ __forceinline__ bool axis_range(double q, double o, double R, double cell, int64_t maxc, int64_t &lo, int64_t &hi) {
   const double d = __dsub_rn(q, o);
@@ -82,9 +92,14 @@ struct Columns {
     any = axis_range(qx, V.ox, R, V.cell, V.mx, x0, x1) && axis_range(qy, V.oy, R, V.cell, V.my, y0, y1) &&
           axis_range(qz, V.oz, R, V.cell, V.mz, z0, z1);
   }
+  // the occupied cells [a, b) of column (cx, cy), as positions in the cell table
+  __device__ __forceinline__ void cells(const IndexView &V, int64_t cx, int64_t cy, int &a, int &b) const {
+    a = lower_bound(V.ukey, 0, V.U, pack(cx, cy, z0, V.bits));
+    b = upper_bound(V.ukey, a, V.U, pack(cx, cy, z1, V.bits));
+  }
   __device__ __forceinline__ void run(const IndexView &V, int64_t cx, int64_t cy, int &s, int &e) const {
-    const int a = lower_bound(V.ukey, 0, V.U, pack(cx, cy, z0, V.bits));
-    const int b = upper_bound(V.ukey, a, V.U, pack(cx, cy, z1, V.bits));
+    int a, b;
+    cells(V, cx, cy, a, b);
     s = V.start[a];
     e = V.start[b];
   }

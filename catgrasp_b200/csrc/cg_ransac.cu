@@ -13,7 +13,19 @@
 // the host did with the scores: the first maximum among valid hypotheses per threshold (aligning.py:115) through a
 // 64-bit atomicMax key, then, in the last CTA to finish (fence + counter), predict's choice between the thresholds
 // (predicter.py:152-172: det test, inlier ratio at 3 mm, strict `>`).  Nothing comes back to the host.
-#include "cg_common.cuh"
+//
+// With a KdEval the same kernel scores by aligning.py:68-79 instead (use_kdtree_for_eval): for src_t = T [source, 1],
+//   count = #{i : some voxel mean of the target is within thr of src_t[i]} + #{j : some voxel mean of src_t is within
+//   thr of target[j]},   ratio = count / 2N.
+// cKDTree's `nearest distance <= thr` is an existence test, so neither side needs a tree.  The target's voxel means
+// come from a cg_cloud_index of the target (cell = resolution), built once per call; each CTA bins its own src_t into
+// an open-addressing hash table of cells in a workspace of its own, sums each voxel in ascending point index (one
+// warp per quarter of the table, so no sum depends on arrival order) and divides by the count, as voxel_kernel does.
+// All of it is float64 without FMA: src_t = ((T00 x + T01 y) + T02 z) + T03, cells floor((p - origin) / r) with
+// origin = min_bound - r * 0.5, distances cg_cloud_index.cuh's dist2 and a correctly rounded sqrt.  In this mode the
+// grid is persistent (one workspace per CTA, CTAs loop over the hypotheses).
+#include <algorithm>
+#include "cg_cloud_index.cuh"
 
 namespace {
 
@@ -145,17 +157,204 @@ struct Fuse {
 
 constexpr int REC_PER_THR = 19;   // winner, count, T (16), count at ratio_thr
 
-__global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__ src, const double *__restrict__ tgt, int N,
-                                                      const int32_t *__restrict__ ids, int H, const Gates g,
-                                                      double *__restrict__ out_ratio, double *__restrict__ out_T,
-                                                      unsigned char *__restrict__ out_valid, const Fuse f) {
+// The kd-tree evaluation (ws == nullptr switches it off).  Each CTA owns ws + blockIdx.x * stride: src_t (N,3), each
+// point's hash slot (N), then the table of 2^cap_log2 >= 2N cells: keys, counts, sums (later means).
+struct KdEval {
+  IndexView tv;            // the target's index (cell = r); the mean of cell table entry u is tmean[u]
+  const double *tmean;
+  double r;
+  char *ws;
+  size_t stride;
+  int cap_log2;
+  int *err;                // set to 1 when a transformed source is not finite or spans 2^KD_BITS voxels on an axis
+};
+
+constexpr int KD_BITS = MAX_AXIS_BITS;                    // bits per axis of a source voxel key
+constexpr uint64_t KD_EMPTY = ~0ull;                      // no key has all 63 + 1 bits set
+constexpr int KD_PARTS = RT / 32;                         // warps, each summing the voxels of one quarter of the table
+// The per-CTA workspaces of one call stay under 1 GiB (about 100 N bytes each) unless that leaves fewer CTAs than
+// SMs; below that the grid is the kernel's resident CTAs.
+constexpr size_t KD_WS_BYTES = size_t(1) << 30;
+
+__host__ __device__ inline size_t kd_src_bytes(int N) { return ((size_t)N * 3 * sizeof(double) + 255) & ~size_t(255); }
+__host__ __device__ inline size_t kd_slot_bytes(int N) { return ((size_t)N * sizeof(int32_t) + 255) & ~size_t(255); }
+__host__ inline size_t kd_stride(int N, int cap_log2) {
+  const size_t cap = size_t(1) << cap_log2;
+  return kd_src_bytes(N) + kd_slot_bytes(N) + cap * (sizeof(uint64_t) + sizeof(int32_t) + 3 * sizeof(double));
+}
+
+__device__ __forceinline__ unsigned kd_hash(uint64_t key, int cap_log2) {
+  return (unsigned)((key * 0x9E3779B97F4A7C15ull) >> (64 - cap_log2));
+}
+
+// some point of pts[a, b) has sqrt(dist2(q, p)) <= thr
+__device__ __forceinline__ bool any_within(const double *pts, int a, int b, double qx, double qy, double qz, double thr) {
+  for (int u = a; u < b; u++)
+    if (sqrt(dist2(qx, qy, qz, pts[3 * (size_t)u], pts[3 * (size_t)u + 1], pts[3 * (size_t)u + 2])) <= thr) return true;
+  return false;
+}
+
+// aligning.py:68-79 for the hypothesis T (shared, 12 doubles) at threshold thr: the two-way count, in thread 0, or -1
+// when the transformed source cannot be binned (k.err is then set).  Called by all RT threads.
+__device__ int kd_count(const KdEval &k, const double *__restrict__ src, const double *__restrict__ tgt, int N,
+                        const double *T, double thr, double (*red)[6], int *redc) {
+  __shared__ double so[3];
+  __shared__ int64_t smaxc[3];
+  __shared__ int sbad;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  char *base = k.ws + (size_t)blockIdx.x * k.stride;
+  double *P = reinterpret_cast<double *>(base);
+  int32_t *pslot = reinterpret_cast<int32_t *>(base + kd_src_bytes(N));
+  const unsigned cap = 1u << k.cap_log2, cmask = cap - 1u;
+  uint64_t *hkey = reinterpret_cast<uint64_t *>(base + kd_src_bytes(N) + kd_slot_bytes(N));
+  int32_t *hcnt = reinterpret_cast<int32_t *>(hkey + cap);
+  double *hsum = reinterpret_cast<double *>(hcnt + cap);   // cap * 4 bytes keeps it 8-byte aligned (cap >= 8)
+
+  // src_t, its bounds, and an empty table
+  double mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+  int bad = 0;
+  for (int i = tid; i < N; i += RT) {
+    const double x = src[(size_t)i * 3], y = src[(size_t)i * 3 + 1], z = src[(size_t)i * 3 + 2];
+    for (int a = 0; a < 3; a++) {
+      const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[a * 4], x), __dmul_rn(T[a * 4 + 1], y)),
+                                           __dmul_rn(T[a * 4 + 2], z)), T[a * 4 + 3]);
+      P[(size_t)i * 3 + a] = v;
+      if (!isfinite(v)) bad = 1;
+      mn[a] = fmin(mn[a], v); mx[a] = fmax(mx[a], v);
+    }
+  }
+  for (unsigned j = tid; j < cap; j += RT) {
+    hkey[j] = KD_EMPTY; hcnt[j] = 0;
+    hsum[3 * (size_t)j] = 0.0; hsum[3 * (size_t)j + 1] = 0.0; hsum[3 * (size_t)j + 2] = 0.0;
+  }
+  for (int o = 16; o > 0; o >>= 1)
+    for (int a = 0; a < 3; a++) {
+      mn[a] = fmin(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+      mx[a] = fmax(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+    }
+  if (lane == 0)
+    for (int a = 0; a < 3; a++) { red[wid][a] = mn[a]; red[wid][3 + a] = mx[a]; }
+  bad = __syncthreads_or(bad);
+  if (tid == 0) {
+    for (int w = 1; w < RT / 32; w++)
+      for (int a = 0; a < 3; a++) { mn[a] = fmin(mn[a], red[w][a]); mx[a] = fmax(mx[a], red[w][3 + a]); }
+    for (int a = 0; a < 3; a++) {
+      so[a] = __dsub_rn(mn[a], __dmul_rn(k.r, 0.5));                     // open3d: min_bound - voxel_size * 0.5
+      const double top = floor(__ddiv_rn(__dsub_rn(mx[a], so[a]), k.r));  // the largest point's cell (floor is monotone)
+      if (!(top < (double)(1 << KD_BITS))) bad = 1;
+      smaxc[a] = bad ? 0 : (int64_t)top;
+    }
+    sbad = bad;
+    if (bad) atomicExch(k.err, 1);
+  }
+  __syncthreads();
+  if (sbad) return -1;
+  const double ox = so[0], oy = so[1], oz = so[2];
+
+  // cells of the table; a cell's slot depends on arrival order, nothing computed from it does
+  for (int i = tid; i < N; i += RT) {
+    const uint64_t key = cell_key(P[(size_t)i * 3], P[(size_t)i * 3 + 1], P[(size_t)i * 3 + 2], ox, oy, oz, k.r, KD_BITS);
+    unsigned h = kd_hash(key, k.cap_log2);
+    for (;;) {
+      const uint64_t prev = atomicCAS((unsigned long long *)&hkey[h], (unsigned long long)KD_EMPTY, (unsigned long long)key);
+      if (prev == KD_EMPTY || prev == key) break;
+      h = (h + 1) & cmask;
+    }
+    pslot[i] = (int32_t)h;
+  }
+  __syncthreads();
+
+  // voxel sums in ascending point index: warp w owns the slots h % KD_PARTS == w and walks the points in order; the
+  // lowest lane of each group of equal slots adds the group's points one by one
+  for (int b0 = 0; b0 < N; b0 += 32) {
+    const int i = b0 + lane;
+    const int h = i < N ? pslot[i] : -1;
+    const bool mine = h >= 0 && (h % KD_PARTS) == wid;
+    const unsigned act = __ballot_sync(0xffffffffu, mine);
+    if (mine) {
+      const unsigned grp = __match_any_sync(act, h);
+      if (lane == __ffs(grp) - 1) {
+        double sx = hsum[3 * (size_t)h], sy = hsum[3 * (size_t)h + 1], sz = hsum[3 * (size_t)h + 2];
+        for (unsigned m = grp; m; m &= m - 1) {
+          const size_t o = 3 * (size_t)(b0 + __ffs(m) - 1);
+          sx = __dadd_rn(sx, P[o]); sy = __dadd_rn(sy, P[o + 1]); sz = __dadd_rn(sz, P[o + 2]);
+        }
+        hsum[3 * (size_t)h] = sx; hsum[3 * (size_t)h + 1] = sy; hsum[3 * (size_t)h + 2] = sz;
+        hcnt[h] += __popc(grp);
+      }
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+  for (unsigned j = tid; j < cap; j += RT) {
+    const int c = hcnt[j];
+    if (c == 0) continue;
+    const double dc = (double)c;
+    hsum[3 * (size_t)j] = __ddiv_rn(hsum[3 * (size_t)j], dc);
+    hsum[3 * (size_t)j + 1] = __ddiv_rn(hsum[3 * (size_t)j + 1], dc);
+    hsum[3 * (size_t)j + 2] = __ddiv_rn(hsum[3 * (size_t)j + 2], dc);
+  }
+  __syncthreads();
+
+  int cnt = 0;
+  // dists1 <= thr: src_t against the target's voxel means, through the target's cell table
+  for (int i = tid; i < N; i += RT) {
+    const double qx = P[(size_t)i * 3], qy = P[(size_t)i * 3 + 1], qz = P[(size_t)i * 3 + 2];
+    const Columns C(k.tv, qx, qy, qz, thr);
+    bool hit = false;
+    if (C.any)
+      for (int64_t cx = C.x0; cx <= C.x1 && !hit; cx++)
+        for (int64_t cy = C.y0; cy <= C.y1 && !hit; cy++) {
+          int a, b;
+          C.cells(k.tv, cx, cy, a, b);
+          hit = any_within(k.tmean, a, b, qx, qy, qz, thr);
+        }
+    cnt += hit ? 1 : 0;
+  }
+  // dists2 <= thr: the target against src_t's voxel means, cell by cell through the table.  The cell range is
+  // axis_range's, widened by RANGE_SLACK cells: a rounded mean may lie an ulp outside its voxel.
+  for (int j = tid; j < N; j += RT) {
+    const double qx = tgt[(size_t)j * 3], qy = tgt[(size_t)j * 3 + 1], qz = tgt[(size_t)j * 3 + 2];
+    int64_t x0, x1, y0, y1, z0, z1;
+    bool hit = false;
+    if (axis_range(qx, ox, thr, k.r, smaxc[0], x0, x1) && axis_range(qy, oy, thr, k.r, smaxc[1], y0, y1) &&
+        axis_range(qz, oz, thr, k.r, smaxc[2], z0, z1))
+      for (int64_t cx = x0; cx <= x1 && !hit; cx++)
+        for (int64_t cy = y0; cy <= y1 && !hit; cy++)
+          for (int64_t cz = z0; cz <= z1 && !hit; cz++) {
+            const uint64_t key = pack(cx, cy, cz, KD_BITS);
+            for (unsigned h = kd_hash(key, k.cap_log2);; h = (h + 1) & cmask) {
+              const uint64_t kh = hkey[h];
+              if (kh == KD_EMPTY) break;
+              if (kh == key) { hit = any_within(hsum, (int)h, (int)h + 1, qx, qy, qz, thr); break; }
+            }
+          }
+    cnt += hit ? 1 : 0;
+  }
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) redc[wid] = cnt;
+  __syncthreads();
+  int c = 0;
+  if (tid == 0)
+    for (int w = 0; w < RT / 32; w++) c += redc[w];
+  return c;
+}
+
+// Launched with RT threads.  __maxnreg__ rather than __launch_bounds__(RT): with the kd-tree path inlined, the launch
+// bound lets ptxas settle on 128 registers and spill the scoring loop; 168 keeps 3 CTAs per SM, as before that path.
+__global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src, const double *__restrict__ tgt, int N,
+                                                 const int32_t *__restrict__ ids, int H, int NB, const Gates g,
+                                                 double *__restrict__ out_ratio, double *__restrict__ out_T,
+                                                 unsigned char *__restrict__ out_valid, const Fuse f, const KdEval kd) {
   __shared__ double T[12], Ti[12];
   __shared__ int ok;
   __shared__ double red[RT / 32][6];
   __shared__ int redc[RT / 32];
   __shared__ int last;
-  // one CTA per (threshold, hypothesis): CTA b scores hypothesis b % H of threshold b / H with the subset ids[b]
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  // NB = (threshold, hypothesis) pairs: pair b scores hypothesis b % H of threshold b / H with the subset ids[b].  One
+  // CTA per pair (gridDim.x == NB), or, with the kd-tree evaluation, fewer CTAs that each take every gridDim.x-th pair.
+  for (int b = blockIdx.x; b < NB; b += gridDim.x) {
   const double thr = b < H ? g.thr[0] : g.thr[1];   // no run-time index into the parameter block
   if (tid == 0) {
     ok = 0;
@@ -259,19 +458,28 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
       for (int k = 0; k < 3; k++) { red[wid][k] = mn[k]; red[wid][3 + k] = mx[k]; }
     }
     __syncthreads();
+    int c = 0;
+    bool good = true;
     if (tid == 0) {
-      int c = 0;
       for (int w2 = 0; w2 < RT / 32; w2++) {
         c += redc[w2];
         for (int k = 0; k < 3; k++) { mn[k] = fmin(mn[k], red[w2][k]); mx[k] = fmax(mx[k], red[w2][3 + k]); }
       }
-      bool good = true;
       if (g.has_max_dims)
         for (int k = 0; k < 3; k++)
           if (mx[k] - mn[k] > g.max_dims[k]) good = false;
+    }
+    const int den = kd.ws ? 2 * N : N;
+    if (kd.ws) {                            // the gates above decide first; the kd-tree count replaces the residual count
+      if (tid == 0) ok = good;
+      __syncthreads();
+      if (ok) c = kd_count(kd, src, tgt, N, T, thr, red, redc);
+      if (c < 0) good = false;
+    }
+    if (tid == 0) {
       if (out_valid) {
         out_valid[b] = good ? 1 : 0;
-        out_ratio[b] = good ? (double)c / (double)N : 0.0;
+        out_ratio[b] = good ? (double)c / (double)den : 0.0;
       }
       if (good) {
         for (int k = 0; k < 12; k++) out_T[(size_t)b * 16 + k] = T[k];
@@ -284,6 +492,8 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
     }
   } else if (tid == 0 && out_valid) {
     out_valid[b] = 0; out_ratio[b] = 0.0;
+  }
+  __syncthreads();                         // T, Ti, ok, red and redc are the next pair's
   }
   if (!f.keys) return;
 
@@ -346,6 +556,62 @@ __global__ void __launch_bounds__(RT) ransac9d_kernel(const double *__restrict__
   }
 }
 
+// The target side of the kd-tree evaluation and the per-CTA workspaces: cg_cloud_index_create (which synchronises the
+// stream twice: the target's bounds, then its cell count), its voxel means, and the grid the workspaces allow.
+struct KdTarget {
+  cg_cloud_index *ix = nullptr;
+  int grid = 0, cap_log2 = 0;
+  size_t stride = 0;
+  ~KdTarget() { cg_cloud_index_destroy(ix); }   // synchronises the stream
+  int build(cg_ctx *ctx, const double *d_tgt, int N, double r, int nb) {
+    int rc = cg_cloud_index_create(ctx, d_tgt, N, r, &ix);
+    if (rc) return rc;
+    cap_log2 = 3;
+    while ((size_t(1) << cap_log2) < 2 * (size_t)N) cap_log2++;
+    stride = kd_stride(N, cap_log2);
+    int per_sm = 0;
+    CG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ransac9d_kernel, RT, 0));
+    const long long resident = (long long)std::max(per_sm, 1) * ctx->num_sms;
+    const long long budget = std::max<long long>(ctx->num_sms, (long long)(KD_WS_BYTES / stride));
+    grid = (int)std::min<long long>({(long long)nb, resident, budget});
+    return CG_OK;
+  }
+  // the call's workspace pieces: the target's voxel means, the error word, then one workspace per CTA
+  void take(cg_arena &ar, double *&tmean, int *&err, char *&ws) const {
+    tmean = ar.take<double>((size_t)ix->U * 3);
+    err = ar.take<int>(1);
+    ws = ar.take<char>(stride * (size_t)grid);
+  }
+  int launch_prep(cg_ctx *ctx, double *tmean, int *err) const {
+    int rc = cg_voxel_down_sample_dev(ix, nullptr, tmean, nullptr);
+    if (rc) return rc;
+    CG_CUDA(ctx, cudaMemsetAsync(err, 0, sizeof(int), ctx->stream));
+    return CG_OK;
+  }
+  KdEval eval(double r, const double *tmean, char *ws, int *err) const {
+    return KdEval{view_of(ix), tmean, r, ws, stride, cap_log2, err};
+  }
+  // the kernel's error word, after a synchronisation
+  int check(cg_ctx *ctx, const int *err) const {
+    int h = 0;
+    CG_CUDA(ctx, cudaMemcpyAsync(&h, err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    CG_REQUIRE(ctx, h == 0, "ransac9d_kdtree: a transformed source is not finite or spans 2^21 or more voxels on an axis");
+    return CG_OK;
+  }
+};
+
+Gates make_gates(const double *thresholds, int n_thr, const double min_scale[3], const double max_scale[3],
+                 const double *max_dims) {
+  Gates g{};
+  for (int t = 0; t < 2; t++) g.thr[t] = thresholds[t < n_thr ? t : 0];
+  for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
+  g.has_max_dims = max_dims != nullptr;
+  return g;
+}
+
+bool good_resolution(double r) { return std::isfinite(r) && r > 0.0; }
+
 }  // namespace
 
 extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids, int H,
@@ -354,10 +620,7 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
   if (!ctx) return CG_EINVAL;
   CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && min_scale && max_scale, "ransac9d: bad arguments");
   CG_REQUIRE(ctx, out_ratio && out_T && out_valid, "ransac9d: outputs");
-  Gates g{};
-  g.thr[0] = g.thr[1] = pass_threshold;
-  for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
-  g.has_max_dims = max_dims != nullptr;
+  const Gates g = make_gates(&pass_threshold, 1, min_scale, max_scale, max_dims);
   const double *d_src, *d_tgt; const int32_t *d_ids; double *d_ratio, *d_T; unsigned char *d_valid;
   return cg_io_stage(ctx, [&](cg_io_pieces &io) {
     d_src = io.in(source, (size_t)N * 3);
@@ -368,10 +631,43 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
     d_valid = io.out(out_valid, H);
   }, [&] {
     CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, ctx->stream));
-    ransac9d_kernel<<<H, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, g, d_ratio, d_T, d_valid,
-                                               Fuse{nullptr, nullptr, 0.0, 0});
+    ransac9d_kernel<<<H, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, H, g, d_ratio, d_T, d_valid,
+                                               Fuse{nullptr, nullptr, 0.0, 0}, KdEval{});
     CG_LAUNCH_CHECK(ctx);
     return CG_OK;
+  });
+}
+
+extern "C" int cg_ransac9d_kdtree_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
+                                       int H, double pass_threshold, const double min_scale[3], const double max_scale[3],
+                                       const double *max_dims, double resolution, double *out_ratio, double *out_T,
+                                       unsigned char *out_valid) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && min_scale && max_scale, "ransac9d_kdtree: bad arguments");
+  CG_REQUIRE(ctx, N <= CG_RANSAC_KD_MAX_N, "ransac9d_kdtree: N > CG_RANSAC_KD_MAX_N");
+  CG_REQUIRE(ctx, good_resolution(resolution), "ransac9d_kdtree: resolution must be positive and finite");
+  CG_REQUIRE(ctx, out_ratio && out_T && out_valid, "ransac9d_kdtree: outputs");
+  const Gates g = make_gates(&pass_threshold, 1, min_scale, max_scale, max_dims);
+  const double *d_src, *d_tgt; const int32_t *d_ids; double *d_ratio, *d_T; unsigned char *d_valid;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_src = io.in(source, (size_t)N * 3);
+    d_tgt = io.in(target, (size_t)N * 3);
+    d_ids = io.in(ids, (size_t)H * 4);
+    d_ratio = io.out(out_ratio, H);
+    d_T = io.out(out_T, (size_t)H * 16);
+    d_valid = io.out(out_valid, H);
+  }, [&] {
+    KdTarget kt;
+    int rc = kt.build(ctx, d_tgt, N, resolution, H);
+    if (rc) return rc;
+    double *tmean; int *err; char *ws;
+    if ((rc = cg_ws_carve(ctx, [&](cg_arena &ar) { kt.take(ar, tmean, err, ws); }))) return rc;
+    if ((rc = kt.launch_prep(ctx, tmean, err))) return rc;
+    CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, ctx->stream));
+    ransac9d_kernel<<<kt.grid, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, H, g, d_ratio, d_T, d_valid,
+                                                     Fuse{nullptr, nullptr, 0.0, 0}, kt.eval(resolution, tmean, ws, err));
+    CG_LAUNCH_CHECK(ctx);
+    return kt.check(ctx, err);
   });
 }
 
@@ -390,14 +686,43 @@ extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const dou
     d_keys = ar.take<unsigned long long>((size_t)n_thr + 1);   // per-threshold keys, then the completion counter
   });
   if (rc) return rc;
-  Gates g{};
-  for (int t = 0; t < 2; t++) g.thr[t] = thresholds[t < n_thr ? t : 0];
-  for (int k = 0; k < 3; k++) { g.min_scale[k] = min_scale[k]; g.max_scale[k] = max_scale[k]; g.max_dims[k] = max_dims ? max_dims[k] : 0.0; }
-  g.has_max_dims = max_dims != nullptr;
+  const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
   cudaStream_t st = ctx->stream;
   CG_CUDA(ctx, cudaMemsetAsync(d_keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
-  ransac9d_kernel<<<n_thr * H, RT, 0, st>>>(source, target, N, ids, H, g, nullptr, d_T, nullptr,
-                                            Fuse{d_keys, out_record, ratio_threshold, n_thr});
+  ransac9d_kernel<<<n_thr * H, RT, 0, st>>>(source, target, N, ids, H, n_thr * H, g, nullptr, d_T, nullptr,
+                                            Fuse{d_keys, out_record, ratio_threshold, n_thr}, KdEval{});
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
+}
+
+extern "C" int cg_ransac9d_kdtree_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N,
+                                           const int32_t *ids, int H, const double *thresholds, int n_thr,
+                                           const double min_scale[3], const double max_scale[3], const double *max_dims,
+                                           double ratio_threshold, double resolution, double *out_record) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && thresholds && (n_thr == 1 || n_thr == 2) && min_scale &&
+                      max_scale && out_record, "ransac9d_kdtree_pose: bad arguments");
+  CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_kdtree_pose: too many hypotheses");
+  CG_REQUIRE(ctx, N <= CG_RANSAC_KD_MAX_N, "ransac9d_kdtree_pose: N > CG_RANSAC_KD_MAX_N");
+  CG_REQUIRE(ctx, good_resolution(resolution), "ransac9d_kdtree_pose: resolution must be positive and finite");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  KdTarget kt;
+  int rc = kt.build(ctx, target, N, resolution, n_thr * H);
+  if (rc) return rc;
+  double *d_T, *tmean; unsigned long long *d_keys; int *err; char *ws;
+  rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    d_T = ar.take<double>((size_t)n_thr * H * 16);
+    d_keys = ar.take<unsigned long long>((size_t)n_thr + 1);
+    kt.take(ar, tmean, err, ws);
+  });
+  if (rc) return rc;
+  if ((rc = kt.launch_prep(ctx, tmean, err))) return rc;
+  const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
+  cudaStream_t st = ctx->stream;
+  CG_CUDA(ctx, cudaMemsetAsync(d_keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
+  ransac9d_kernel<<<kt.grid, RT, 0, st>>>(source, target, N, ids, H, n_thr * H, g, nullptr, d_T, nullptr,
+                                          Fuse{d_keys, out_record, ratio_threshold, n_thr},
+                                          kt.eval(resolution, tmean, ws, err));
+  CG_LAUNCH_CHECK(ctx);
+  return kt.check(ctx, err);
 }

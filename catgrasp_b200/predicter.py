@@ -305,6 +305,10 @@ class NunocsPredicter:
         # subsets drawn in C); "device": counter-based draws on the GPU from one numpy value, not the reference's
         # numbers, and no host walk of the generator
         self.subsample = "host"
+        # predicter.py:162-163's locals: score the RANSAC hypotheses by the kd-tree evaluation (aligning.py:68-79) at
+        # this voxel size, in either subsample mode; predict's 3 mm ratio between thresholds stays the residual one
+        self.use_kdtree_for_eval = False
+        self.kdtree_eval_resolution = 0.003
 
     THRESHOLDS = (0.003, 0.005)           # predicter.py:154, the RANSAC pass thresholds in the order predict tries them
     ERR_THRES = 0.003                     # predicter.py:163, the ratio predict compares between them
@@ -353,6 +357,7 @@ class NunocsPredicter:
         CUDA input.  Sets data_transformed, confidence_z, pred_bins and, with a pose, best_ratio and nocs_pose.
         ``ids`` (n_pts,) overrides the cloud subset; ``self.subsample`` picks the random numbers ("host" / "device")."""
         assert self.subsample in ("host", "device"), self.subsample
+        self._kd_resolution()
         if self.subsample == "device":
             return self._predict_device(data, ids)
         if getattr(data["cloud_xyz"], "is_cuda", False):
@@ -365,10 +370,16 @@ class NunocsPredicter:
         import torch
         return tuple(torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in arrays)
 
+    def _kd_resolution(self):
+        """The kd-tree evaluation's voxel size when it is on, else None; ValueError for a bad size."""
+        from .aligning import _resolution
+        return _resolution(self.kdtree_eval_resolution) if self.use_kdtree_for_eval else None
+
     def _ransac(self, source, target, ids):
         from .aligning import ransac9d_pose
         return ransac9d_pose(source, target, ids, self.THRESHOLDS, max_scale=self.max_scale, min_scale=self.min_scale,
-                             max_dimensions=self.MAX_DIMENSIONS, ratio_threshold=self.ERR_THRES)
+                             max_dimensions=self.MAX_DIMENSIONS, ratio_threshold=self.ERR_THRES,
+                             kdtree_eval_resolution=self._kd_resolution())
 
     def _predict_host(self, data, ids):
         """The reference's numbers: the transform's subset from np.random.choice, then both thresholds' subsets in

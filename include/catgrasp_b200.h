@@ -358,6 +358,32 @@ int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target
                          const double max_scale[3] /* host */, const double *max_dims /* host */,
                          double ratio_threshold, double *out_record);
 
+/* The same two entries with aligning.py:68-79's evaluation (use_kdtree_for_eval=True, kdtree_eval_resolution =
+ * resolution) in place of the residual count; the gates and the selection rules are unchanged.  For a hypothesis
+ * that passes the gates, with src_t = T [source, 1] and thr its threshold:
+ *   count = #{i : some voxel mean of target lies within thr of src_t[i]} + #{j : some voxel mean of src_t lies within
+ *           thr of target[j]}   (cKDTree's `distance <= thr` on both voxel-thinned clouds),
+ *   out_ratio = count / (2N); in the record of the pose entry, each winner's count is out of 2N (its count at
+ *   ratio_threshold is still the residual count out of N, as in predict).
+ * Voxels are cg_voxel_down_sample_dev's: cell floor((p - (min_bound - r*0.5)) / r), the mean of its points summed in
+ * ascending index.  src_t = ((T00 x + T01 y) + T02 z) + T03 per row and distances (dx*dx + dy*dy) + dz*dz, then
+ * sqrt, all float64 without FMA, so the counts are a function of T and the inputs alone.
+ * CG_EINVAL before any launch: N > CG_RANSAC_KD_MAX_N, or resolution not positive and finite.  CG_EINVAL after the
+ * launch: the target, or a transformed source, spans 2^21 or more voxels on an axis or is not finite.
+ * Synchronisation: both entries synchronise the stream three times -- building the target's cg_cloud_index (its
+ * bounds, then its cell count) and reading the kernel's error word at the end.  The device workspace holds about
+ * 100 N bytes per CTA of the launch (at most 1 GiB in all, or one CTA per SM if that is larger).                   */
+#define CG_RANSAC_KD_MAX_N 65536
+int cg_ransac9d_kdtree_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids, int H,
+                            double pass_threshold, const double min_scale[3], const double max_scale[3],
+                            const double *max_dims, double resolution, double *out_ratio, double *out_T,
+                            unsigned char *out_valid);
+int cg_ransac9d_kdtree_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
+                                int H, const double *thresholds /* host */, int n_thr,
+                                const double min_scale[3] /* host */, const double max_scale[3] /* host */,
+                                const double *max_dims /* host */, double ratio_threshold, double resolution,
+                                double *out_record);
+
 /* ---- Cone pose enumeration (device pointers, float64 like the reference's numpy) ----------
  * Replaces: dexnet/grasping/grasp_sampler.py:266-286 (PointConeGraspSampler.sample_one_surface_point: the
  *   R0 / R0 @ R_sphere @ R_inplane x approach-depth loops, Utils.py:172-179 normalizeRotation) and :191-203
