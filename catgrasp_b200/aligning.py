@@ -30,6 +30,23 @@ def _resolution(r):
     return v
 
 
+def _gates(min_scale, max_scale, max_dimensions):
+    """The scale gates and the optional extent gate as the entry points take them: (3,) float64 arrays, None for no
+    max_dimensions."""
+    def vec3(a):
+        return np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(3))
+    return vec3(min_scale), vec3(max_scale), None if max_dimensions is None else vec3(max_dimensions)
+
+
+def _ransac9d(ctx, mode, args, r, outputs):
+    """Calls cg_ransac9d_<mode> on ``args`` and ``outputs``, or with a kd-tree resolution ``r``
+    cg_ransac9d_kdtree_<mode>, which takes r between them."""
+    if r is None:
+        ctx.call(f"cg_ransac9d_{mode}", ctx.h, *args, *outputs)
+    else:
+        ctx.call(f"cg_ransac9d_kdtree_{mode}", ctx.h, *args, r, *outputs)
+
+
 def transform_points(T, pts):
     """src_t = T [pts, 1] in the kd-tree kernel's operation order, ((T00 x + T01 y) + T02 z) + T03 per row, each
     operation rounded on its own."""
@@ -62,19 +79,11 @@ def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree
     ids = np.empty((max_iter, 4), dtype=np.int32)
     for i in range(max_iter):                                   # aligning.py:91-97
         ids[i] = np.random.choice(len(source), size=4, replace=False)
-    ctx = _lib.Context.get()
-    mins = np.ascontiguousarray(np.asarray(min_scale, dtype=np.float64).reshape(3))
-    maxs = np.ascontiguousarray(np.asarray(max_scale, dtype=np.float64).reshape(3))
-    mdim = None if max_dimensions is None else np.ascontiguousarray(np.asarray(max_dimensions, dtype=np.float64).reshape(3))
     ratio = np.empty(max_iter, np.float64)
     T = np.empty((max_iter, 4, 4), np.float64)
     valid = np.empty(max_iter, np.uint8)
-    if r is None:
-        ctx.call("cg_ransac9d_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs, mdim,
-                 ratio, T, valid)
-    else:
-        ctx.call("cg_ransac9d_kdtree_host", ctx.h, source, target, N, ids, max_iter, float(PassThreshold), mins, maxs,
-                 mdim, r, ratio, T, valid)
+    _ransac9d(_lib.Context.get(), "host", (source, target, N, ids, max_iter, float(PassThreshold),
+                                          *_gates(min_scale, max_scale, max_dimensions)), r, (ratio, T, valid))
     keep = np.nonzero(valid)[0]
     if keep.size == 0:
         return None, None
@@ -87,7 +96,16 @@ def estimate9DTransform(source, target, PassThreshold, max_iter=1000, use_kdtree
     return best_transform, inliers
 
 
-REC_PER_THR = 19     # include/catgrasp_b200.h, cg_ransac9d_pose_dev's record
+REC_PER_THR = 19     # include/catgrasp_b200.h, cg_ransac9d_pose_dev's record: 19 doubles per threshold, then 18
+
+
+def read_record(rec, n_thr):
+    """cg_ransac9d_pose_dev's record of n_thr thresholds, as views of ``rec`` (a CUDA tensor or its host copy):
+    per threshold 'winner' (n_thr,), 'count' (n_thr,), 'T' (n_thr,4,4) and 'count_ratio' (n_thr,); overall 'chosen',
+    'pose' (4,4) and 'best_ratio'.  Every value is float64; the integers are stored exactly."""
+    per, tail = rec[:n_thr * REC_PER_THR].reshape(n_thr, REC_PER_THR), rec[n_thr * REC_PER_THR:]
+    return {"winner": per[:, 0], "count": per[:, 1], "T": per[:, 2:18].reshape(n_thr, 4, 4), "count_ratio": per[:, 18],
+            "chosen": tail[0], "pose": tail[1:17].reshape(4, 4), "best_ratio": tail[17]}
 
 
 def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 99]), min_scale=np.array([0, 0, 0]),
@@ -102,7 +120,6 @@ def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 9
     With ``kdtree_eval_resolution`` the hypotheses are scored by the kd-tree evaluation (each 'count' out of 2N; the
     launch then synchronises, see cg_ransac9d_kdtree_pose_dev)."""
     import torch
-    from . import _lib
     r = None if kdtree_eval_resolution is None else _resolution(kdtree_eval_resolution)
     ctx, source, target = _lib.inputs(source, target, dtype=torch.float64)
     _, ids = _lib.inputs(ids, dtype=torch.int32, ctx=ctx)
@@ -110,18 +127,10 @@ def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 9
     T = thr.size
     assert T in (1, 2) and ids.shape[0] % T == 0 and ids.shape[1] == 4, (thr, tuple(ids.shape))
     H = ids.shape[0] // T
-    mins = np.ascontiguousarray(np.asarray(min_scale, dtype=np.float64).reshape(3))
-    maxs = np.ascontiguousarray(np.asarray(max_scale, dtype=np.float64).reshape(3))
-    mdim = None if max_dimensions is None else np.ascontiguousarray(np.asarray(max_dimensions, dtype=np.float64).reshape(3))
     rec = torch.empty((T * REC_PER_THR + 18,), dtype=torch.float64, device=source.device)
-    if r is None:
-        ctx.call("cg_ransac9d_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs, mdim,
-                 float(ratio_threshold), rec)
-    else:
-        ctx.call("cg_ransac9d_kdtree_pose_dev", ctx.h, source, target, source.shape[0], ids, H, thr, T, mins, maxs,
-                 mdim, float(ratio_threshold), r, rec)
-    per = rec[:T * REC_PER_THR].view(T, REC_PER_THR)
-    tail = rec[T * REC_PER_THR:]
-    return {"winner": per[:, 0].to(torch.int64), "count": per[:, 1].to(torch.int64), "T": per[:, 2:18].view(T, 4, 4),
-            "count_ratio": per[:, 18].to(torch.int64), "chosen": tail[0].to(torch.int64), "pose": tail[1:17].view(4, 4),
-            "best_ratio": tail[17], "record": rec}
+    _ransac9d(ctx, "pose_dev", (source, target, source.shape[0], ids, H, thr, T,
+                                *_gates(min_scale, max_scale, max_dimensions), float(ratio_threshold)), r, (rec,))
+    out = read_record(rec, T)
+    for k in ("winner", "count", "count_ratio", "chosen"):
+        out[k] = out[k].to(torch.int64)
+    return {**out, "record": rec}

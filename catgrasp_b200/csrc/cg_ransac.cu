@@ -25,6 +25,7 @@
 // origin = min_bound - r * 0.5, distances cg_cloud_index.cuh's dist2 and a correctly rounded sqrt.  In this mode the
 // grid is persistent (one workspace per CTA, CTAs loop over the hypotheses).
 #include <algorithm>
+#include <memory>
 #include "cg_cloud_index.cuh"
 
 namespace {
@@ -340,164 +341,13 @@ __device__ int kd_count(const KdEval &k, const double *__restrict__ src, const d
   return c;
 }
 
-// Launched with RT threads.  __maxnreg__ rather than __launch_bounds__(RT): with the kd-tree path inlined, the launch
-// bound lets ptxas settle on 128 registers and spill the scoring loop; 168 keeps 3 CTAs per SM, as before that path.
-__global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src, const double *__restrict__ tgt, int N,
-                                                 const int32_t *__restrict__ ids, int H, int NB, const Gates g,
-                                                 double *__restrict__ out_ratio, double *__restrict__ out_T,
-                                                 unsigned char *__restrict__ out_valid, const Fuse f, const KdEval kd) {
-  __shared__ double T[12], Ti[12];
-  __shared__ int ok;
-  __shared__ double red[RT / 32][6];
-  __shared__ int redc[RT / 32];
+// The fused selection after the CTA's last pair: the last CTA to finish (fence + counter) reads each threshold's winner
+// and its T, counts the winner's residuals <= f.ratio_thr and makes predict's choice between the thresholds
+// (predicter.py:152-172's loop), into f.record.  Called by all RT threads; T and win are shared scratch.
+__device__ void select_pose(const Fuse &f, const double *src, const double *tgt, int N, int H, const double *out_T,
+                            double *T, int *redc, int &win) {
   __shared__ int last;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  // NB = (threshold, hypothesis) pairs: pair b scores hypothesis b % H of threshold b / H with the subset ids[b].  One
-  // CTA per pair (gridDim.x == NB), or, with the kd-tree evaluation, fewer CTAs that each take every gridDim.x-th pair.
-  for (int b = blockIdx.x; b < NB; b += gridDim.x) {
-  const double thr = b < H ? g.thr[0] : g.thr[1];   // no run-time index into the parameter block
-  if (tid == 0) {
-    ok = 0;
-    double M[4][4], B[4][3], X[4][3], M0[4][4], B0[4][3];
-    for (int i = 0; i < 4; i++) {
-      const int id = ids[(size_t)b * 4 + i];
-      // cv2.estimateAffine3D (aligning.py:27) narrows its inputs to CV_32F before the double-precision solve:
-      // the four sample points go through float, the residual pass below keeps the caller's float64.
-      for (int k = 0; k < 3; k++) {
-        M[i][k] = M0[i][k] = (double)(float)src[(size_t)id * 3 + k];
-        B[i][k] = B0[i][k] = (double)(float)tgt[(size_t)id * 3 + k];
-      }
-      M[i][3] = M0[i][3] = 1.0;
-    }
-    // X[j][k]: dst_k = sum_j X[j][k] * [src,1]_j  -> A[k][j] = X[j][k].  A pivot below 1e-12 (duplicate, coplanar or
-    // nearly so) sends the subset to the minimum-norm solve; it is as rare as such subsets are.
-    if (!solve4(M, B, X)) minnorm4(M0, B0, X);
-    bool good = true;
-    double A[3][3], t[3], sc[3];
-    {
-      for (int k = 0; k < 3; k++) {
-        for (int j = 0; j < 3; j++) A[k][j] = X[j][k];
-        t[k] = X[3][k];
-      }
-      for (int j = 0; j < 3; j++) {   // scales = column norms (aligning.py:41)
-        sc[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
-        if (sc[j] > g.max_scale[j] || sc[j] < g.min_scale[j]) good = false;
-      }
-    }
-    if (good) {
-      double R[3][3], G[3][3], V[3][3], w[3];
-      for (int i = 0; i < 3; i++)
-        for (int j = 0; j < 3; j++) R[i][j] = A[i][j] / sc[j];
-      for (int i = 0; i < 3; i++)
-        for (int j = 0; j < 3; j++) G[i][j] = R[0][i] * R[0][j] + R[1][i] * R[1][j] + R[2][i] * R[2][j];
-      jacobi3(G, V, w);             // R^T R = V diag(w) V^T, singular values = sqrt(w)
-      double smin = 1e300, smax = 0.0;
-      for (int i = 0; i < 3; i++) {
-        const double s = sqrt(fmax(w[i], 0.0));
-        smin = fmin(smin, s); smax = fmax(smax, s);
-      }
-      if (smin < 0.8 || smax > 1.2) good = false;
-      if (good) {
-        // U V^T = R V diag(1/s) V^T
-        double Q[3][3];
-        for (int i = 0; i < 3; i++)
-          for (int j = 0; j < 3; j++) {
-            double acc = 0.0;
-            for (int k = 0; k < 3; k++) acc += V[i][k] * V[j][k] / sqrt(w[k]);
-            Q[i][j] = acc;
-          }
-        double Ro[3][3];
-        for (int i = 0; i < 3; i++)
-          for (int j = 0; j < 3; j++) Ro[i][j] = R[i][0] * Q[0][j] + R[i][1] * Q[1][j] + R[i][2] * Q[2][j];
-        const double det = Ro[0][0] * (Ro[1][1] * Ro[2][2] - Ro[1][2] * Ro[2][1]) -
-                           Ro[0][1] * (Ro[1][0] * Ro[2][2] - Ro[1][2] * Ro[2][0]) +
-                           Ro[0][2] * (Ro[1][0] * Ro[2][1] - Ro[1][1] * Ro[2][0]);
-        if (det < 0) good = false;
-        if (good) {
-          for (int i = 0; i < 3; i++) {
-            for (int j = 0; j < 3; j++) T[i * 4 + j] = Ro[i][j] * sc[j];
-            T[i * 4 + 3] = t[i];
-          }
-          // inverse: (Ro S)^-1 = S^-1 Ro^T
-          for (int i = 0; i < 3; i++) {
-            for (int j = 0; j < 3; j++) Ti[i * 4 + j] = Ro[j][i] / sc[i];
-            Ti[i * 4 + 3] = -(Ti[i * 4 + 0] * t[0] + Ti[i * 4 + 1] * t[1] + Ti[i * 4 + 2] * t[2]);
-          }
-          ok = 1;
-        }
-      }
-    }
-  }
-  __syncthreads();
-  if (ok) {
-    double mn[3] = {1e300, 1e300, 1e300}, mx[3] = {-1e300, -1e300, -1e300};
-    int cnt = 0;
-    for (int i = tid; i < N; i += RT) {
-      const double sx = src[(size_t)i * 3], sy = src[(size_t)i * 3 + 1], sz = src[(size_t)i * 3 + 2];
-      const double tx = tgt[(size_t)i * 3], ty = tgt[(size_t)i * 3 + 1], tz = tgt[(size_t)i * 3 + 2];
-      const double ex = T[0] * sx + T[1] * sy + T[2] * sz + T[3] - tx;
-      const double ey = T[4] * sx + T[5] * sy + T[6] * sz + T[7] - ty;
-      const double ez = T[8] * sx + T[9] * sy + T[10] * sz + T[11] - tz;
-      if (sqrt(ex * ex + ey * ey + ez * ez) <= thr) cnt++;
-      if (g.has_max_dims) {
-        for (int k = 0; k < 3; k++) {
-          const double c = Ti[k * 4] * tx + Ti[k * 4 + 1] * ty + Ti[k * 4 + 2] * tz + Ti[k * 4 + 3];
-          mn[k] = fmin(mn[k], c); mx[k] = fmax(mx[k], c);
-        }
-      }
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-      for (int k = 0; k < 3; k++) {
-        mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
-        mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
-      }
-    }
-    if (lane == 0) {
-      redc[wid] = cnt;
-      for (int k = 0; k < 3; k++) { red[wid][k] = mn[k]; red[wid][3 + k] = mx[k]; }
-    }
-    __syncthreads();
-    int c = 0;
-    bool good = true;
-    if (tid == 0) {
-      for (int w2 = 0; w2 < RT / 32; w2++) {
-        c += redc[w2];
-        for (int k = 0; k < 3; k++) { mn[k] = fmin(mn[k], red[w2][k]); mx[k] = fmax(mx[k], red[w2][3 + k]); }
-      }
-      if (g.has_max_dims)
-        for (int k = 0; k < 3; k++)
-          if (mx[k] - mn[k] > g.max_dims[k]) good = false;
-    }
-    const int den = kd.ws ? 2 * N : N;
-    if (kd.ws) {                            // the gates above decide first; the kd-tree count replaces the residual count
-      if (tid == 0) ok = good;
-      __syncthreads();
-      if (ok) c = kd_count(kd, src, tgt, N, T, thr, red, redc);
-      if (c < 0) good = false;
-    }
-    if (tid == 0) {
-      if (out_valid) {
-        out_valid[b] = good ? 1 : 0;
-        out_ratio[b] = good ? (double)c / (double)den : 0.0;
-      }
-      if (good) {
-        for (int k = 0; k < 12; k++) out_T[(size_t)b * 16 + k] = T[k];
-        out_T[(size_t)b * 16 + 12] = 0.0; out_T[(size_t)b * 16 + 13] = 0.0; out_T[(size_t)b * 16 + 14] = 0.0;
-        out_T[(size_t)b * 16 + 15] = 1.0;
-        // count / N is monotone in count, so the largest key is the host's first maximum among valid hypotheses
-        if (f.keys)
-          atomicMax(&f.keys[b / H], ((unsigned long long)c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(b % H)));
-      }
-    }
-  } else if (tid == 0 && out_valid) {
-    out_valid[b] = 0; out_ratio[b] = 0.0;
-  }
-  __syncthreads();                         // T, Ti, ok, red and redc are the next pair's
-  }
-  if (!f.keys) return;
-
-  // ---- the last CTA to finish reads the winners and picks the pose (predicter.py:152-172's loop over thresholds)
   if (tid == 0) {
     __threadfence();   // this CTA's T and key before its count
     last = atomicAdd(&f.keys[f.n_thr], 1ull) == (unsigned long long)gridDim.x - 1;
@@ -511,10 +361,10 @@ __global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src,
   for (int t = 0; t < f.n_thr; t++) {
     if (tid == 0) {
       const unsigned long long key = atomicAdd(&f.keys[t], 0ull);
-      ok = key ? (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)) : -1;
+      win = key ? (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)) : -1;
     }
     __syncthreads();
-    const int w = ok;
+    const int w = win;
     if (w >= 0 && tid < 12) T[tid] = __ldcg(&out_T[((size_t)t * H + w) * 16 + tid]);   // the scoring pass's T, not a recompute
     __syncthreads();
     int cnt = 0;
@@ -556,50 +406,164 @@ __global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src,
   }
 }
 
-// The target side of the kd-tree evaluation and the per-CTA workspaces: cg_cloud_index_create (which synchronises the
-// stream twice: the target's bounds, then its cell count), its voxel means, and the grid the workspaces allow.
-struct KdTarget {
-  cg_cloud_index *ix = nullptr;
-  int grid = 0, cap_log2 = 0;
-  size_t stride = 0;
-  ~KdTarget() { cg_cloud_index_destroy(ix); }   // synchronises the stream
-  int build(cg_ctx *ctx, const double *d_tgt, int N, double r, int nb) {
-    int rc = cg_cloud_index_create(ctx, d_tgt, N, r, &ix);
-    if (rc) return rc;
-    cap_log2 = 3;
-    while ((size_t(1) << cap_log2) < 2 * (size_t)N) cap_log2++;
-    stride = kd_stride(N, cap_log2);
-    int per_sm = 0;
-    CG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ransac9d_kernel, RT, 0));
-    const long long resident = (long long)std::max(per_sm, 1) * ctx->num_sms;
-    const long long budget = std::max<long long>(ctx->num_sms, (long long)(KD_WS_BYTES / stride));
-    grid = (int)std::min<long long>({(long long)nb, resident, budget});
-    return CG_OK;
+// Launched with RT threads.  __maxnreg__ rather than __launch_bounds__(RT): with the kd-tree path inlined, the launch
+// bound lets ptxas settle on 128 registers and spill the scoring loop; 168 keeps 3 CTAs per SM, as before that path.
+// Thread 0's hypothesis and the residual count stay in the kernel body: moved into __device__ functions, even verbatim,
+// they change ptxas's register allocation and cost 0.2-0.7 % of the residual launch (H100 80GB HBM3, 700 W).
+__global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src, const double *__restrict__ tgt, int N,
+                                                 const int32_t *__restrict__ ids, int H, int NB, const Gates g,
+                                                 double *__restrict__ out_ratio, double *__restrict__ out_T,
+                                                 unsigned char *__restrict__ out_valid, const Fuse f, const KdEval kd) {
+  __shared__ double T[12], Ti[12];
+  __shared__ int ok;
+  __shared__ double red[RT / 32][6];
+  __shared__ int redc[RT / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  // NB = (threshold, hypothesis) pairs: pair b scores hypothesis b % H of threshold b / H with the subset ids[b].  One
+  // CTA per pair (gridDim.x == NB), or, with the kd-tree evaluation, fewer CTAs that each take every gridDim.x-th pair.
+  for (int b = blockIdx.x; b < NB; b += gridDim.x) {
+    const double thr = b < H ? g.thr[0] : g.thr[1];   // no run-time index into the parameter block
+    if (tid == 0) {
+      ok = 0;
+      double M[4][4], B[4][3], X[4][3], M0[4][4], B0[4][3];
+      for (int i = 0; i < 4; i++) {
+        const int id = ids[(size_t)b * 4 + i];
+        // cv2.estimateAffine3D (aligning.py:27) narrows its inputs to CV_32F before the double-precision solve:
+        // the four sample points go through float, the residual pass below keeps the caller's float64.
+        for (int k = 0; k < 3; k++) {
+          M[i][k] = M0[i][k] = (double)(float)src[(size_t)id * 3 + k];
+          B[i][k] = B0[i][k] = (double)(float)tgt[(size_t)id * 3 + k];
+        }
+        M[i][3] = M0[i][3] = 1.0;
+      }
+      // X[j][k]: dst_k = sum_j X[j][k] * [src,1]_j  -> A[k][j] = X[j][k].  A pivot below 1e-12 (duplicate, coplanar or
+      // nearly so) sends the subset to the minimum-norm solve; it is as rare as such subsets are.
+      if (!solve4(M, B, X)) minnorm4(M0, B0, X);
+      bool good = true;
+      double A[3][3], t[3], sc[3];
+      {
+        for (int k = 0; k < 3; k++) {
+          for (int j = 0; j < 3; j++) A[k][j] = X[j][k];
+          t[k] = X[3][k];
+        }
+        for (int j = 0; j < 3; j++) {   // scales = column norms (aligning.py:41)
+          sc[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
+          if (sc[j] > g.max_scale[j] || sc[j] < g.min_scale[j]) good = false;
+        }
+      }
+      if (good) {
+        double R[3][3], G[3][3], V[3][3], w[3];
+        for (int i = 0; i < 3; i++)
+          for (int j = 0; j < 3; j++) R[i][j] = A[i][j] / sc[j];
+        for (int i = 0; i < 3; i++)
+          for (int j = 0; j < 3; j++) G[i][j] = R[0][i] * R[0][j] + R[1][i] * R[1][j] + R[2][i] * R[2][j];
+        jacobi3(G, V, w);             // R^T R = V diag(w) V^T, singular values = sqrt(w)
+        double smin = 1e300, smax = 0.0;
+        for (int i = 0; i < 3; i++) {
+          const double s = sqrt(fmax(w[i], 0.0));
+          smin = fmin(smin, s); smax = fmax(smax, s);
+        }
+        if (smin < 0.8 || smax > 1.2) good = false;
+        if (good) {
+          // U V^T = R V diag(1/s) V^T
+          double Q[3][3];
+          for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) {
+              double acc = 0.0;
+              for (int k = 0; k < 3; k++) acc += V[i][k] * V[j][k] / sqrt(w[k]);
+              Q[i][j] = acc;
+            }
+          double Ro[3][3];
+          for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) Ro[i][j] = R[i][0] * Q[0][j] + R[i][1] * Q[1][j] + R[i][2] * Q[2][j];
+          const double det = Ro[0][0] * (Ro[1][1] * Ro[2][2] - Ro[1][2] * Ro[2][1]) -
+                             Ro[0][1] * (Ro[1][0] * Ro[2][2] - Ro[1][2] * Ro[2][0]) +
+                             Ro[0][2] * (Ro[1][0] * Ro[2][1] - Ro[1][1] * Ro[2][0]);
+          if (det < 0) good = false;
+          if (good) {
+            for (int i = 0; i < 3; i++) {
+              for (int j = 0; j < 3; j++) T[i * 4 + j] = Ro[i][j] * sc[j];
+              T[i * 4 + 3] = t[i];
+            }
+            // inverse: (Ro S)^-1 = S^-1 Ro^T
+            for (int i = 0; i < 3; i++) {
+              for (int j = 0; j < 3; j++) Ti[i * 4 + j] = Ro[j][i] / sc[i];
+              Ti[i * 4 + 3] = -(Ti[i * 4 + 0] * t[0] + Ti[i * 4 + 1] * t[1] + Ti[i * 4 + 2] * t[2]);
+            }
+            ok = 1;
+          }
+        }
+      }
+    }
+    __syncthreads();
+    if (ok) {
+      double mn[3] = {1e300, 1e300, 1e300}, mx[3] = {-1e300, -1e300, -1e300};
+      int cnt = 0;
+      for (int i = tid; i < N; i += RT) {
+        const double sx = src[(size_t)i * 3], sy = src[(size_t)i * 3 + 1], sz = src[(size_t)i * 3 + 2];
+        const double tx = tgt[(size_t)i * 3], ty = tgt[(size_t)i * 3 + 1], tz = tgt[(size_t)i * 3 + 2];
+        const double ex = T[0] * sx + T[1] * sy + T[2] * sz + T[3] - tx;
+        const double ey = T[4] * sx + T[5] * sy + T[6] * sz + T[7] - ty;
+        const double ez = T[8] * sx + T[9] * sy + T[10] * sz + T[11] - tz;
+        if (sqrt(ex * ex + ey * ey + ez * ez) <= thr) cnt++;
+        if (g.has_max_dims) {
+          for (int k = 0; k < 3; k++) {
+            const double c = Ti[k * 4] * tx + Ti[k * 4 + 1] * ty + Ti[k * 4 + 2] * tz + Ti[k * 4 + 3];
+            mn[k] = fmin(mn[k], c); mx[k] = fmax(mx[k], c);
+          }
+        }
+      }
+      for (int o = 16; o > 0; o >>= 1) {
+        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        for (int k = 0; k < 3; k++) {
+          mn[k] = fmin(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
+          mx[k] = fmax(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+        }
+      }
+      if (lane == 0) {
+        redc[wid] = cnt;
+        for (int k = 0; k < 3; k++) { red[wid][k] = mn[k]; red[wid][3 + k] = mx[k]; }
+      }
+      __syncthreads();
+      int c = 0;
+      bool good = true;
+      if (tid == 0) {
+        for (int w2 = 0; w2 < RT / 32; w2++) {
+          c += redc[w2];
+          for (int k = 0; k < 3; k++) { mn[k] = fmin(mn[k], red[w2][k]); mx[k] = fmax(mx[k], red[w2][3 + k]); }
+        }
+        if (g.has_max_dims)
+          for (int k = 0; k < 3; k++)
+            if (mx[k] - mn[k] > g.max_dims[k]) good = false;
+      }
+      const int den = kd.ws ? 2 * N : N;
+      if (kd.ws) {                            // the gates above decide first; the kd-tree count replaces the residual count
+        if (tid == 0) ok = good;
+        __syncthreads();
+        if (ok) c = kd_count(kd, src, tgt, N, T, thr, red, redc);
+        if (c < 0) good = false;
+      }
+      if (tid == 0) {
+        if (out_valid) {
+          out_valid[b] = good ? 1 : 0;
+          out_ratio[b] = good ? (double)c / (double)den : 0.0;
+        }
+        if (good) {
+          for (int k = 0; k < 12; k++) out_T[(size_t)b * 16 + k] = T[k];
+          out_T[(size_t)b * 16 + 12] = 0.0; out_T[(size_t)b * 16 + 13] = 0.0; out_T[(size_t)b * 16 + 14] = 0.0;
+          out_T[(size_t)b * 16 + 15] = 1.0;
+          // count / N is monotone in count, so the largest key is the host's first maximum among valid hypotheses
+          if (f.keys)
+            atomicMax(&f.keys[b / H], ((unsigned long long)c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(b % H)));
+        }
+      }
+    } else if (tid == 0 && out_valid) {
+      out_valid[b] = 0; out_ratio[b] = 0.0;
+    }
+    __syncthreads();                         // T, Ti, ok, red and redc are the next pair's
   }
-  // the call's workspace pieces: the target's voxel means, the error word, then one workspace per CTA
-  void take(cg_arena &ar, double *&tmean, int *&err, char *&ws) const {
-    tmean = ar.take<double>((size_t)ix->U * 3);
-    err = ar.take<int>(1);
-    ws = ar.take<char>(stride * (size_t)grid);
-  }
-  int launch_prep(cg_ctx *ctx, double *tmean, int *err) const {
-    int rc = cg_voxel_down_sample_dev(ix, nullptr, tmean, nullptr);
-    if (rc) return rc;
-    CG_CUDA(ctx, cudaMemsetAsync(err, 0, sizeof(int), ctx->stream));
-    return CG_OK;
-  }
-  KdEval eval(double r, const double *tmean, char *ws, int *err) const {
-    return KdEval{view_of(ix), tmean, r, ws, stride, cap_log2, err};
-  }
-  // the kernel's error word, after a synchronisation
-  int check(cg_ctx *ctx, const int *err) const {
-    int h = 0;
-    CG_CUDA(ctx, cudaMemcpyAsync(&h, err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    CG_REQUIRE(ctx, h == 0, "ransac9d_kdtree: a transformed source is not finite or spans 2^21 or more voxels on an axis");
-    return CG_OK;
-  }
-};
+  if (f.keys) select_pose(f, src, tgt, N, H, out_T, T, redc, ok);
+}
 
 Gates make_gates(const double *thresholds, int n_thr, const double min_scale[3], const double max_scale[3],
                  const double *max_dims) {
@@ -611,6 +575,71 @@ Gates make_gates(const double *thresholds, int n_thr, const double min_scale[3],
 }
 
 bool good_resolution(double r) { return std::isfinite(r) && r > 0.0; }
+
+// Every launch of ransac9d_kernel: H hypotheses for each of n_thr thresholds on device inputs.  Without a record it
+// writes cg_ransac9d_host's per-hypothesis out_ratio, out_T (zeroed first) and out_valid; with one, the fused selection
+// writes cg_ransac9d_pose_dev's record and every T goes to the workspace.  kd_r > 0 scores by the kd-tree evaluation
+// at that resolution: the target's index and voxel means, a persistent grid with one workspace per CTA, and the
+// kernel's error word read back.  That synchronises the stream twice in cg_cloud_index_create, once for the error word
+// and once more when the index is destroyed.
+int ransac9d(cg_ctx *ctx, const double *src, const double *tgt, int N, const int32_t *ids, int H, int n_thr,
+             const Gates &g, double kd_r, double *out_ratio, double *out_T, unsigned char *out_valid, double *record,
+             double ratio_thr) {
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int nb = n_thr * H;
+  const bool kd = kd_r > 0.0;
+  std::unique_ptr<cg_cloud_index, void (*)(cg_cloud_index *)> ix(nullptr, cg_cloud_index_destroy);
+  int grid = nb, cap_log2 = 3;
+  size_t stride = 0;
+  if (kd) {
+    cg_cloud_index *p = nullptr;
+    int rc = cg_cloud_index_create(ctx, tgt, N, kd_r, &p);
+    ix.reset(p);
+    if (rc) return rc;
+    while ((size_t(1) << cap_log2) < 2 * (size_t)N) cap_log2++;
+    stride = kd_stride(N, cap_log2);
+    int per_sm = 0;
+    CG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ransac9d_kernel, RT, 0));
+    const long long resident = (long long)std::max(per_sm, 1) * ctx->num_sms;
+    const long long budget = std::max<long long>(ctx->num_sms, (long long)(KD_WS_BYTES / stride));
+    grid = (int)std::min<long long>({(long long)nb, resident, budget});
+  }
+  unsigned long long *keys = nullptr;   // per-threshold keys, then the completion counter
+  double *tmean = nullptr;              // the target's voxel means
+  int *err = nullptr;
+  char *ws = nullptr;                   // one workspace per CTA
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    if (record) {
+      out_T = ar.take<double>((size_t)nb * 16);   // every valid hypothesis's T, read back by the last CTA
+      keys = ar.take<unsigned long long>((size_t)n_thr + 1);
+    }
+    if (kd) {
+      tmean = ar.take<double>((size_t)ix->U * 3);
+      err = ar.take<int>(1);
+      ws = ar.take<char>(stride * (size_t)grid);
+    }
+  });
+  if (rc) return rc;
+  cudaStream_t st = ctx->stream;
+  if (kd) {
+    if ((rc = cg_voxel_down_sample_dev(ix.get(), nullptr, tmean, nullptr))) return rc;
+    CG_CUDA(ctx, cudaMemsetAsync(err, 0, sizeof(int), st));
+  }
+  if (record)
+    CG_CUDA(ctx, cudaMemsetAsync(keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
+  else
+    CG_CUDA(ctx, cudaMemsetAsync(out_T, 0, (size_t)H * 128, st));
+  const Fuse f = record ? Fuse{keys, record, ratio_thr, n_thr} : Fuse{};
+  const KdEval k = kd ? KdEval{view_of(ix.get()), tmean, kd_r, ws, stride, cap_log2, err} : KdEval{};
+  ransac9d_kernel<<<grid, RT, 0, st>>>(src, tgt, N, ids, H, nb, g, out_ratio, out_T, out_valid, f, k);
+  CG_LAUNCH_CHECK(ctx);
+  if (!kd) return CG_OK;
+  int h = 0;
+  CG_CUDA(ctx, cudaMemcpyAsync(&h, err, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CG_CUDA(ctx, cudaStreamSynchronize(st));
+  CG_REQUIRE(ctx, h == 0, "ransac9d_kdtree: a transformed source is not finite or spans 2^21 or more voxels on an axis");
+  return CG_OK;
+}
 
 }  // namespace
 
@@ -629,13 +658,7 @@ extern "C" int cg_ransac9d_host(cg_ctx *ctx, const double *source, const double 
     d_ratio = io.out(out_ratio, H);
     d_T = io.out(out_T, (size_t)H * 16);
     d_valid = io.out(out_valid, H);
-  }, [&] {
-    CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, ctx->stream));
-    ransac9d_kernel<<<H, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, H, g, d_ratio, d_T, d_valid,
-                                               Fuse{nullptr, nullptr, 0.0, 0}, KdEval{});
-    CG_LAUNCH_CHECK(ctx);
-    return CG_OK;
-  });
+  }, [&] { return ransac9d(ctx, d_src, d_tgt, N, d_ids, H, 1, g, 0.0, d_ratio, d_T, d_valid, nullptr, 0.0); });
 }
 
 extern "C" int cg_ransac9d_kdtree_host(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
@@ -656,19 +679,7 @@ extern "C" int cg_ransac9d_kdtree_host(cg_ctx *ctx, const double *source, const 
     d_ratio = io.out(out_ratio, H);
     d_T = io.out(out_T, (size_t)H * 16);
     d_valid = io.out(out_valid, H);
-  }, [&] {
-    KdTarget kt;
-    int rc = kt.build(ctx, d_tgt, N, resolution, H);
-    if (rc) return rc;
-    double *tmean; int *err; char *ws;
-    if ((rc = cg_ws_carve(ctx, [&](cg_arena &ar) { kt.take(ar, tmean, err, ws); }))) return rc;
-    if ((rc = kt.launch_prep(ctx, tmean, err))) return rc;
-    CG_CUDA(ctx, cudaMemsetAsync(d_T, 0, (size_t)H * 128, ctx->stream));
-    ransac9d_kernel<<<kt.grid, RT, 0, ctx->stream>>>(d_src, d_tgt, N, d_ids, H, H, g, d_ratio, d_T, d_valid,
-                                                     Fuse{nullptr, nullptr, 0.0, 0}, kt.eval(resolution, tmean, ws, err));
-    CG_LAUNCH_CHECK(ctx);
-    return kt.check(ctx, err);
-  });
+  }, [&] { return ransac9d(ctx, d_src, d_tgt, N, d_ids, H, 1, g, resolution, d_ratio, d_T, d_valid, nullptr, 0.0); });
 }
 
 extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N, const int32_t *ids,
@@ -679,20 +690,8 @@ extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const dou
   CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && thresholds && (n_thr == 1 || n_thr == 2) && min_scale &&
                       max_scale && out_record, "ransac9d_pose: bad arguments");
   CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_pose: too many hypotheses");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  double *d_T; unsigned long long *d_keys;
-  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
-    d_T = ar.take<double>((size_t)n_thr * H * 16);        // every valid hypothesis's T, read back by the last CTA
-    d_keys = ar.take<unsigned long long>((size_t)n_thr + 1);   // per-threshold keys, then the completion counter
-  });
-  if (rc) return rc;
   const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemsetAsync(d_keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
-  ransac9d_kernel<<<n_thr * H, RT, 0, st>>>(source, target, N, ids, H, n_thr * H, g, nullptr, d_T, nullptr,
-                                            Fuse{d_keys, out_record, ratio_threshold, n_thr}, KdEval{});
-  CG_LAUNCH_CHECK(ctx);
-  return CG_OK;
+  return ransac9d(ctx, source, target, N, ids, H, n_thr, g, 0.0, nullptr, nullptr, nullptr, out_record, ratio_threshold);
 }
 
 extern "C" int cg_ransac9d_kdtree_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N,
@@ -705,24 +704,7 @@ extern "C" int cg_ransac9d_kdtree_pose_dev(cg_ctx *ctx, const double *source, co
   CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_kdtree_pose: too many hypotheses");
   CG_REQUIRE(ctx, N <= CG_RANSAC_KD_MAX_N, "ransac9d_kdtree_pose: N > CG_RANSAC_KD_MAX_N");
   CG_REQUIRE(ctx, good_resolution(resolution), "ransac9d_kdtree_pose: resolution must be positive and finite");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  KdTarget kt;
-  int rc = kt.build(ctx, target, N, resolution, n_thr * H);
-  if (rc) return rc;
-  double *d_T, *tmean; unsigned long long *d_keys; int *err; char *ws;
-  rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
-    d_T = ar.take<double>((size_t)n_thr * H * 16);
-    d_keys = ar.take<unsigned long long>((size_t)n_thr + 1);
-    kt.take(ar, tmean, err, ws);
-  });
-  if (rc) return rc;
-  if ((rc = kt.launch_prep(ctx, tmean, err))) return rc;
   const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
-  cudaStream_t st = ctx->stream;
-  CG_CUDA(ctx, cudaMemsetAsync(d_keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
-  ransac9d_kernel<<<kt.grid, RT, 0, st>>>(source, target, N, ids, H, n_thr * H, g, nullptr, d_T, nullptr,
-                                          Fuse{d_keys, out_record, ratio_threshold, n_thr},
-                                          kt.eval(resolution, tmean, ws, err));
-  CG_LAUNCH_CHECK(ctx);
-  return kt.check(ctx, err);
+  return ransac9d(ctx, source, target, N, ids, H, n_thr, g, resolution, nullptr, nullptr, nullptr, out_record,
+                  ratio_threshold);
 }

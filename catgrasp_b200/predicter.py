@@ -385,6 +385,7 @@ class NunocsPredicter:
         """The reference's numbers: the transform's subset from np.random.choice, then both thresholds' subsets in
         one C draw that continues numpy's stream where the reference's two loops would (aligning.py:91-97), one
         fused launch on them, and predict's post-processing in numpy on the two winners' T (predicter.py:152-172)."""
+        from .aligning import read_record
         nocs_cloud, _ = self.predict_nocs(data, ids=ids)
         ori_cloud = self.data_transformed["cloud_xyz_original"]
         symmetry_tf = np.eye(4)
@@ -397,14 +398,14 @@ class NunocsPredicter:
         hyp = draw.draw(N, 4, len(self.THRESHOLDS) * H)
         draw.commit()
         dev = self.model.device
-        rec = self._ransac(*self._on(dev, source, target, hyp))["record"].cpu().numpy()
+        res = self._ransac(*self._on(dev, source, target, hyp))
+        found = read_record(res["record"].cpu().numpy(), len(self.THRESHOLDS))
         best_ratio = 0
         best_transform = None
         for t in range(len(self.THRESHOLDS)):
-            r = rec[t * 19:(t + 1) * 19]
-            if r[0] < 0:                                                  # estimate9DTransform returned None
+            if found["winner"][t] < 0:                                    # estimate9DTransform returned None
                 continue
-            transform = r[2:18].reshape(4, 4).copy()
+            transform = found["T"][t].copy()
             if np.linalg.det(transform[:3, :3]) < 0:
                 continue
             transformed = (transform @ to_homo(source).T).T[:, :3]
@@ -456,6 +457,7 @@ class NunocsPredicter:
         choice between thresholds run on the device.  The host waits for the masked point count with CUDA input,
         and for the record (whether there is a pose, best_ratio) and, with numpy input, the copy of the results."""
         import torch
+        from .aligning import read_record
         seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
         cuda_in = getattr(data["cloud_xyz"], "is_cuda", False)
         H, n_thr = int(self.ransac_max_iter), len(self.THRESHOLDS)
@@ -464,14 +466,13 @@ class NunocsPredicter:
         source = coords.to(torch.float64)
         hyp = self.model.draw_ids_dev(source.shape[0], 4, n_thr * H, seed, first_candidate=1)
         res = self._ransac(source, dt["cloud_xyz_original"], hyp)
-        rec = res["record"].cpu().numpy()
+        found = read_record(res["record"].cpu().numpy(), n_thr)
         host = (lambda t: t.cpu().numpy()) if not cuda_in else (lambda t: t)
         self.data_transformed = {k: host(v) for k, v in dt.items()}
         self.confidence_z, self.pred_bins = host(conf_z), host(bins)
-        tail = rec[n_thr * 19:]
-        if tail[0] < 0:
+        if found["chosen"] < 0:
             return None, None
-        self.best_ratio = float(tail[17])
+        self.best_ratio = float(found["best_ratio"])
         pose = host(res["pose"].clone())
         self.nocs_pose = pose.copy() if not cuda_in else pose.clone()
         return host(source), pose
