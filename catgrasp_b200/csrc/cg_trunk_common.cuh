@@ -1,6 +1,6 @@
 // cg_trunk_common.cuh -- device helpers shared by the fp32-SIMT trunk (engine 0) and the
 // tensor-core trunk (engines 1-3): register-tiled fp32 layers over k-major shared-memory tiles, the
-// float64 pose inverse and cp.async wrappers.
+// float64 pose inverse and transform of an input row, its T3 product, and cp.async wrappers.
 #pragma once
 #include "cg_net.cuh"
 
@@ -71,6 +71,28 @@ static __device__ void pose_inverse(const double *P, double *out) {
   out[9] = -(out[0] * tx + out[1] * ty + out[2] * tz);
   out[10] = -(out[3] * tx + out[4] * ty + out[5] * tz);
   out[11] = -(out[6] * tx + out[7] * ty + out[8] * tz);
+}
+
+// One cloud row (x, y, z, nx, ny, nz) into the candidate's frame in float64: w[0..2] = Rinv xyz + tinv,
+// w[3..5] = Rinv nrm, with R = pose_inverse's output.  Both trunks then normalise w and narrow it to float, but not
+// in the same way: engine 0 divides by (std + 1e-15), engines 1-3 multiply by its reciprocal, so engine 0's input
+// rows can differ from the other engines' in the last bit.
+__device__ __forceinline__ void pose_transform(const double *R, double x, double y, double z, double nx, double ny,
+                                               double nz, double *w) {
+  w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
+  w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
+  w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
+  w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
+  w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
+  w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
+}
+
+// xyz @ T3 (pointnet2.py:248) of one input row v[6]; the normals pass through (:245-250)
+__device__ __forceinline__ void apply_t3(const float *t3, float *v) {
+  const float x = v[0], y = v[1], z = v[2];
+  v[0] = fmaf(z, t3[6], fmaf(y, t3[3], x * t3[0]));
+  v[1] = fmaf(z, t3[7], fmaf(y, t3[4], x * t3[1]));
+  v[2] = fmaf(z, t3[8], fmaf(y, t3[5], x * t3[2]));
 }
 
 

@@ -116,23 +116,12 @@ __global__ void __launch_bounds__(NT, 1) trunk_simt_kernel(const cg_trunk_args a
         const double *pn = a.in.cloud_nrm + (size_t)id * 3;
         const double x = px[0], y = px[1], z = px[2];
         const double nx = pn[0], ny = pn[1], nz = pn[2];
-        const double *R = S.pinv;
         double w[6];
-        w[0] = R[0] * x + R[1] * y + R[2] * z + R[9];
-        w[1] = R[3] * x + R[4] * y + R[5] * z + R[10];
-        w[2] = R[6] * x + R[7] * y + R[8] * z + R[11];
-        w[3] = R[0] * nx + R[1] * ny + R[2] * nz;
-        w[4] = R[3] * nx + R[4] * ny + R[5] * nz;
-        w[5] = R[6] * nx + R[7] * ny + R[8] * nz;
+        pose_transform(S.pinv, x, y, z, nx, ny, nz, w);
 #pragma unroll
         for (int k = 0; k < 6; k++) v[k] = (float)((w[k] - S.mean[k]) / S.sden[k]);
       }
-      if (a.T3) {  // xyz @ T3 (pointnet2.py:248), normals pass through (:245-250)
-        const float x = v[0], y = v[1], z = v[2];
-        v[0] = fmaf(z, S.T3[6], fmaf(y, S.T3[3], x * S.T3[0]));
-        v[1] = fmaf(z, S.T3[7], fmaf(y, S.T3[4], x * S.T3[1]));
-        v[2] = fmaf(z, S.T3[8], fmaf(y, S.T3[5], x * S.T3[2]));
-      }
+      if (a.T3) apply_t3(S.T3, v);
 #pragma unroll
       for (int k = 0; k < 6; k++) S.in_s[k * TP + tid] = v[k];
     }
