@@ -126,6 +126,8 @@ SIGNATURES = {
     "cg_encoder_probe_dev": (_i, [_vp, _D, _D, _D, _i, _D, _D, _D, _D, _i, _i, _D, _D, _D, _D], TORCH),
     "cg_nunocs_forward_host": (_i, [_vp, _H, _i, _i, _H, _H, _H], OWN),
     "cg_nunocs_forward_dev": (_i, [_vp, _D, _i, _i, _D, _D, _D], TORCH),
+    "cg_nunocs_forward_many_host": (_i, [_vp, _H, _i, _i, _i, _H, _H, _H], OWN),
+    "cg_nunocs_forward_many_dev": (_i, [_vp, _D, _i, _i, _i, _D, _D, _D], TORCH),
     "cg_sdf_create": (_i, [_vp, _H, _i, _i, _i, _H, _f, _H], OWN),
     "cg_sdf_destroy": (None, [_vp], None),
     "cg_sdf_lookup_dev": (_i, [_vp, _D, _i, _i, _D], TORCH),
@@ -140,6 +142,7 @@ SIGNATURES = {
     "cg_occupancy_from_scan_host": (_i, [_vp, _H, _i, _f, _H], OWN),
     "cg_ransac9d_host": (_i, [_vp, _H, _H, _i, _H, _i, _d, _H, _H, _H, _H, _H, _H], OWN),
     "cg_ransac9d_pose_dev": (_i, [_vp, _D, _D, _i, _D, _i, _H, _i, _H, _H, _H, _d, _D], TORCH),
+    "cg_ransac9d_pose_many_dev": (_i, [_vp, _D, _D, _i, _i, _D, _i, _H, _i, _H, _H, _H, _d, _D], TORCH),
     "cg_ransac9d_kdtree_host": (_i, [_vp, _H, _H, _i, _H, _i, _d, _H, _H, _H, _d, _H, _H, _H], OWN),
     "cg_ransac9d_kdtree_pose_dev": (_i, [_vp, _D, _D, _i, _D, _i, _H, _i, _H, _H, _H, _d, _d, _D], TORCH),
     "cg_cone_poses_dev": (_i, [_vp, _D, _D, _i, _D, _i, _D, _i, _D, _i, _d, _D, _D], TORCH),

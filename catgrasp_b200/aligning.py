@@ -134,3 +134,24 @@ def ransac9d_pose(source, target, ids, thresholds, max_scale=np.array([99, 99, 9
     for k in ("winner", "count", "count_ratio", "chosen"):
         out[k] = out[k].to(torch.int64)
     return {**out, "record": rec}
+
+
+def ransac9d_pose_many(source, target, ids, thresholds, max_scale=np.array([99, 99, 99]),
+                       min_scale=np.array([0, 0, 0]), max_dimensions=None, ratio_threshold=0.003):
+    """ransac9d_pose (residual evaluation) for B objects at once: ``source`` / ``target`` (B,N,3) float64 and ``ids``
+    (B,T*H,4) int32 CUDA tensors.  Returns the (B, T*19 + 18) float64 CUDA tensor of records, row b being
+    ransac9d_pose's 'record' for source[b], target[b], ids[b] bit for bit (cg_ransac9d_pose_many_dev); read a row
+    with read_record.  No synchronisation."""
+    import torch
+    ctx, source, target = _lib.inputs(source, target, dtype=torch.float64)
+    _, ids = _lib.inputs(ids, dtype=torch.int32, ctx=ctx)
+    thr = np.ascontiguousarray(np.asarray(thresholds, dtype=np.float64).reshape(-1))
+    T = thr.size
+    B, N = source.shape[0], source.shape[1]
+    assert T in (1, 2) and source.shape == (B, N, 3) and target.shape == (B, N, 3), (thr, tuple(source.shape))
+    assert ids.dim() == 3 and ids.shape[0] == B and ids.shape[1] % T == 0 and ids.shape[2] == 4, tuple(ids.shape)
+    H = ids.shape[1] // T
+    rec = torch.empty((B, T * REC_PER_THR + 18), dtype=torch.float64, device=source.device)
+    ctx.call("cg_ransac9d_pose_many_dev", ctx.h, source, target, B, N, ids, H, thr, T,
+             *_gates(min_scale, max_scale, max_dimensions), float(ratio_threshold), rec)
+    return rec

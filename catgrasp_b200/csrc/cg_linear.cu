@@ -187,7 +187,7 @@ __global__ void __launch_bounds__(256) linear_wide_kernel(const float *__restric
 // Few-row variant (M <= 8: the per-scene NUNOCS heads, B = 1): 16 output columns per CTA, K split over 64 thread
 // groups whose partial sums meet in shared memory -- latency-bound GEMV work that the tiled kernels serialise badly
 // (a 1024->512 layer is 32 CTAs of 16 dependent loop steps; with 64 columns x 16 slices it was 8 CTAs of 64 steps).
-constexpr int RM = 8;
+constexpr int RM = CG_FC_FEW_ROWS;
 constexpr int RQ = 4;     // column quads per CTA
 constexpr int RS = 64;    // k-slices per CTA
 constexpr int RC = RQ * 4;

@@ -138,20 +138,28 @@ void encoder_ws_carve(cg_arena &ar, int B, EncoderWs &w) {
 }
 
 // The FC chain after a trunk (STN3d, STNkd, cls head): layers L[l], L[l+1], L[l+2] =
-// 1024 -> 512 (ReLU, from the max-pool keys in w.gmax) -> 256 (ReLU) -> out (no ReLU)
-int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, float *out) {
-  int rc;
-  if ((rc = cg_linear_launch(ctx, L[l], reinterpret_cast<const float *>(w.gmax), B, w.f1, CG_FC_RELU | CG_FC_KEYS)))
-    return rc;
-  if ((rc = cg_linear_launch(ctx, L[l + 1], w.f1, B, w.f2, CG_FC_RELU))) return rc;
-  return cg_linear_launch(ctx, L[l + 2], w.f2, B, out, 0);
+// 1024 -> 512 (ReLU, from the max-pool keys in w.gmax) -> 256 (ReLU) -> out (no ReLU).
+// rows > 0 launches it on groups of at most `rows` clouds (0: all B in one launch per layer).
+int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, float *out, int rows = 0) {
+  const int g = rows > 0 ? rows : B;
+  for (int r0 = 0; r0 < B; r0 += g) {
+    const int m = B - r0 < g ? B - r0 : g;
+    int rc;
+    if ((rc = cg_linear_launch(ctx, L[l], reinterpret_cast<const float *>(w.gmax + (size_t)r0 * 1024), m,
+                               w.f1 + (size_t)r0 * 512, CG_FC_RELU | CG_FC_KEYS)))
+      return rc;
+    if ((rc = cg_linear_launch(ctx, L[l + 1], w.f1 + (size_t)r0 * 512, m, w.f2 + (size_t)r0 * 256, CG_FC_RELU)))
+      return rc;
+    if ((rc = cg_linear_launch(ctx, L[l + 2], w.f2 + (size_t)r0 * 256, m, out + (size_t)r0 * L[l + 2].C, 0))) return rc;
+  }
+  return CG_OK;
 }
 
 // Runs the PointNetEncoder (pointnet2.py:241-271) for B clouds; on return w.gmax holds the
 // (B,1024) global feature as order-preserving keys; pf_out (optional) the 64-ch point feature.
-// keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.
+// keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.  fc_rows: fc_chain's rows.
 int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs &w, float *pf_out,
-                    uint32_t *keys_out = nullptr) {
+                    uint32_t *keys_out = nullptr, int fc_rows = 0) {
   cg_ctx *ctx = net->ctx;
   const cg_layer *L = net->L;
   int rc;
@@ -164,14 +172,14 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   a.l2 = L[L_S3_C2]; a.l3 = L[L_S3_C3]; a.tc_img = net->tc_img[0]; a.tc_f16_ok = net->tc_f16_ok[0]; a.relu3 = 1; a.gmax_keys = w.gmax; a.pf_out = nullptr;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = fc_chain(ctx, L, L_S3_F1, B, w, w.T3))) return rc;
+  if ((rc = fc_chain(ctx, L, L_S3_F1, B, w, w.T3, fc_rows))) return rc;
   // --- trunk B: encoder conv1 + STNkd convs + max (pointnet2.py:252, :208-213)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.T3 = w.T3; a.l0 = L[L_E_C1]; a.stage1_mode = 1; a.l1 = L[L_SK_C1];
   a.l2 = L[L_SK_C2]; a.l3 = L[L_SK_C3]; a.tc_img = net->tc_img[1]; a.tc_f16_ok = net->tc_f16_ok[1]; a.relu3 = 1;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out + (size_t)B * 1024, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = fc_chain(ctx, L, L_SK_F1, B, w, w.T64))) return rc;
+  if ((rc = fc_chain(ctx, L, L_SK_F1, B, w, w.T64, fc_rows))) return rc;
   // --- trunk C: conv1, @T64, conv2, conv3(+BN, no ReLU), max (pointnet2.py:252-265)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.stage1_mode = 2; a.T64 = w.T64; a.l1 = cg_layer{nullptr, nullptr, 64, 64};
@@ -214,8 +222,9 @@ int cls_forward_impl(cg_net *net, const cg_input_src &in_all, int B_all, int N, 
   return CG_OK;
 }
 
+// fc_rows > 0: the per-cloud FC layers run on groups of at most fc_rows clouds (encoder_forward)
 int seg_forward_impl(cg_net *net, const float *x, int B, int N, float *out_logits, int bins, float *out_coords,
-                     float *out_conf, int32_t *out_bins) {
+                     float *out_conf, int32_t *out_bins, int fc_rows = 0) {
   cg_ctx *ctx = net->ctx;
   CG_REQUIRE(ctx, net->kind == CG_NET_SEG, "net is not a PointNetSeg");
   CG_REQUIRE(ctx, B > 0 && N > 0 && x, "seg: bad arguments");
@@ -238,10 +247,14 @@ int seg_forward_impl(cg_net *net, const float *x, int B, int N, float *out_logit
   cg_input_src in;
   memset(&in, 0, sizeof(in));
   in.x_direct = x;
-  if ((rc = encoder_forward(net, in, B, N, w, pf))) return rc;
+  if ((rc = encoder_forward(net, in, B, N, w, pf, nullptr, fc_rows))) return rc;
   const cg_layer *L = net->L;
   // global half of conv1 (pointnet2.py:270-271 tiles the global feature over N; it is constant per cloud)
-  if ((rc = cg_linear_launch(ctx, L[L_HEAD0], reinterpret_cast<const float *>(w.gmax), B, biasg, CG_FC_KEYS))) return rc;
+  const int g = fc_rows > 0 ? fc_rows : B;
+  for (int r0 = 0; r0 < B; r0 += g)
+    if ((rc = cg_linear_launch(ctx, L[L_HEAD0], reinterpret_cast<const float *>(w.gmax + (size_t)r0 * 1024),
+                               B - r0 < g ? B - r0 : g, biasg + (size_t)r0 * 512, CG_FC_KEYS)))
+      return rc;
   if ((rc = cg_linear_launch(ctx, L[L_HEAD1], pf, (int)P, y1, CG_FC_RELU, biasg, N))) return rc;
   if ((rc = cg_linear_launch(ctx, L[L_HEAD2], y1, (int)P, y2, CG_FC_RELU))) return rc;
   if ((rc = cg_linear_launch(ctx, L[L_HEAD3], y2, (int)P, y3, CG_FC_RELU))) return rc;
@@ -365,4 +378,49 @@ extern "C" int cg_nunocs_forward_host(cg_net *net, const float *x_host, int N, i
     d_z = io.out(out_conf_z, N);
     d_b = io.out(out_bins, (size_t)N * 3);
   }, [&] { return cg_nunocs_forward_dev(net, d_x, N, bins, d_c, d_z, d_b); });
+}
+
+// Objects per pass of the batched NUNOCS forward: whole objects up to CG_NUNOCS_MANY_PASS_POINTS points.  Below 64
+// points a cloud's point-wise layers take another kernel at B = 1 than in a batch (cg_linear_launch), so one object.
+static int nunocs_pass_objects(int B, int N) {
+  if (N < 64) return 1;
+  long long p = CG_NUNOCS_MANY_PASS_POINTS / N;
+  if (p > CHUNK_B) p = CHUNK_B;
+  if (p > B) p = B;
+  return p < 1 ? 1 : (int)p;
+}
+
+extern "C" int cg_nunocs_forward_many_dev(cg_net *net, const float *x, int B, int N, int bins, float *out_coords,
+                                          float *out_conf_z, int32_t *out_bins) {
+  if (!net) return CG_EINVAL;
+  cg_ctx *ctx = net->ctx;
+  CG_REQUIRE(ctx, x && N > 0 && out_coords, "nunocs_many: bad arguments");
+  CG_REQUIRE(ctx, B >= 1 && B <= CG_NUNOCS_MANY_MAX_B, "nunocs_many: 1 <= B <= CG_NUNOCS_MANY_MAX_B");
+  CG_REQUIRE(ctx, net->kind == CG_NET_SEG && bins > 0 && bins * 3 == net->n_out, "nunocs_many: n_out != 3*bins");
+  const int per = nunocs_pass_objects(B, N);
+  for (int b0 = 0; b0 < B; b0 += per) {
+    const int nb = B - b0 < per ? B - b0 : per;
+    const size_t p0 = (size_t)b0 * N;
+    int rc = seg_forward_impl(net, x + p0 * 6, nb, N, nullptr, bins, out_coords + p0 * 3,
+                              out_conf_z ? out_conf_z + p0 : nullptr, out_bins ? out_bins + p0 * 3 : nullptr,
+                              CG_FC_FEW_ROWS);   // the kernel and the sums a single cloud gets
+    if (rc) return rc;
+  }
+  return CG_OK;
+}
+
+extern "C" int cg_nunocs_forward_many_host(cg_net *net, const float *x_host, int B, int N, int bins, float *out_coords,
+                                           float *out_conf_z, int32_t *out_bins) {
+  if (!net) return CG_EINVAL;
+  cg_ctx *ctx = net->ctx;
+  CG_REQUIRE(ctx, x_host && N > 0 && out_coords, "nunocs_many_host: bad arguments");
+  CG_REQUIRE(ctx, B >= 1 && B <= CG_NUNOCS_MANY_MAX_B, "nunocs_many_host: 1 <= B <= CG_NUNOCS_MANY_MAX_B");
+  const size_t P = (size_t)B * N;
+  const float *d_x; float *d_c, *d_z; int32_t *d_b;
+  return cg_io_stage(ctx, [&](cg_io_pieces &io) {
+    d_x = io.in(x_host, P * 6);
+    d_c = io.out(out_coords, P * 3);
+    d_z = io.out(out_conf_z, P);
+    d_b = io.out(out_bins, P * 3);
+  }, [&] { return cg_nunocs_forward_many_dev(net, d_x, B, N, bins, d_c, d_z, d_b); });
 }

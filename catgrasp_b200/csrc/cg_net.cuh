@@ -89,6 +89,9 @@ enum : unsigned {
   CG_FC_RELU = 1u,   // ReLU after the bias
   CG_FC_KEYS = 2u,   // X holds order-preserving uint keys (a trunk's max-pool output), decoded on load
 };
+// cg_linear_launch runs M <= CG_FC_FEW_ROWS rows on its few-row kernel (below the tensor-core kernel's 64), whose
+// sums for a row do not depend on M
+constexpr int CG_FC_FEW_ROWS = 8;
 int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, float *Y, unsigned flags,
                      const float *row_bias = nullptr, int rows_per_bias = 0);
 // tensor-core FC path (cg_linear_tc.cu).  The image builder returns nullptr in *img for shapes the kernel does not take

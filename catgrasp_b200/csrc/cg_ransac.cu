@@ -419,6 +419,16 @@ __global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src,
   __shared__ double red[RT / 32][6];
   __shared__ int redc[RT / 32];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  // Object blockIdx.y of a batched pose search (cg_ransac9d_pose_many_dev): its source, target, subsets, T workspace,
+  // keys and record.  Every other launch has gridDim.y == 1.
+  const size_t obj = blockIdx.y;
+  src += obj * N * 3;
+  tgt += obj * N * 3;
+  ids += obj * NB * 4;
+  out_T += obj * NB * 16;
+  Fuse fo = f;
+  fo.keys += obj * (f.n_thr + 1);
+  fo.record += obj * (f.n_thr * REC_PER_THR + 18);
   // NB = (threshold, hypothesis) pairs: pair b scores hypothesis b % H of threshold b / H with the subset ids[b].  One
   // CTA per pair (gridDim.x == NB), or, with the kd-tree evaluation, fewer CTAs that each take every gridDim.x-th pair.
   for (int b = blockIdx.x; b < NB; b += gridDim.x) {
@@ -553,8 +563,8 @@ __global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src,
           out_T[(size_t)b * 16 + 12] = 0.0; out_T[(size_t)b * 16 + 13] = 0.0; out_T[(size_t)b * 16 + 14] = 0.0;
           out_T[(size_t)b * 16 + 15] = 1.0;
           // count / N is monotone in count, so the largest key is the host's first maximum among valid hypotheses
-          if (f.keys)
-            atomicMax(&f.keys[b / H], ((unsigned long long)c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(b % H)));
+          if (fo.keys)
+            atomicMax(&fo.keys[b / H], ((unsigned long long)c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(b % H)));
         }
       }
     } else if (tid == 0 && out_valid) {
@@ -562,7 +572,7 @@ __global__ void __maxnreg__(168) ransac9d_kernel(const double *__restrict__ src,
     }
     __syncthreads();                         // T, Ti, ok, red and redc are the next pair's
   }
-  if (f.keys) select_pose(f, src, tgt, N, H, out_T, T, redc, ok);
+  if (fo.keys) select_pose(fo, src, tgt, N, H, out_T, T, redc, ok);
 }
 
 Gates make_gates(const double *thresholds, int n_thr, const double min_scale[3], const double max_scale[3],
@@ -582,12 +592,17 @@ bool good_resolution(double r) { return std::isfinite(r) && r > 0.0; }
 // at that resolution: the target's index and voxel means, a persistent grid with one workspace per CTA, and the
 // kernel's error word read back.  That synchronises the stream twice in cg_cloud_index_create, once for the error word
 // and once more when the index is destroyed.
+// With a record, B objects (B > 1 only without kd_r): src / tgt (B,N,3), ids (B,nb,4), record B records; the grid's y
+// is the object, CG_RANSAC_MANY_PASS_PAIRS / nb objects per launch at most, the launches in object order over one
+// workspace.
 int ransac9d(cg_ctx *ctx, const double *src, const double *tgt, int N, const int32_t *ids, int H, int n_thr,
              const Gates &g, double kd_r, double *out_ratio, double *out_T, unsigned char *out_valid, double *record,
-             double ratio_thr) {
+             double ratio_thr, int B = 1) {
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const int nb = n_thr * H;
   const bool kd = kd_r > 0.0;
+  CG_REQUIRE(ctx, B == 1 || (record && !kd), "ransac9d: several objects need the fused selection without kd_r");
+  const int per_launch = (int)std::min<long long>(B, std::max<long long>(1, CG_RANSAC_MANY_PASS_PAIRS / nb));
   std::unique_ptr<cg_cloud_index, void (*)(cg_cloud_index *)> ix(nullptr, cg_cloud_index_destroy);
   int grid = nb, cap_log2 = 3;
   size_t stride = 0;
@@ -609,9 +624,9 @@ int ransac9d(cg_ctx *ctx, const double *src, const double *tgt, int N, const int
   int *err = nullptr;
   char *ws = nullptr;                   // one workspace per CTA
   int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
-    if (record) {
-      out_T = ar.take<double>((size_t)nb * 16);   // every valid hypothesis's T, read back by the last CTA
-      keys = ar.take<unsigned long long>((size_t)n_thr + 1);
+    if (record) {   // per object: every valid hypothesis's T, read back by the last CTA; keys and counter
+      out_T = ar.take<double>((size_t)per_launch * nb * 16);
+      keys = ar.take<unsigned long long>((size_t)per_launch * (n_thr + 1));
     }
     if (kd) {
       tmean = ar.take<double>((size_t)ix->U * 3);
@@ -625,14 +640,19 @@ int ransac9d(cg_ctx *ctx, const double *src, const double *tgt, int N, const int
     if ((rc = cg_voxel_down_sample_dev(ix.get(), nullptr, tmean, nullptr))) return rc;
     CG_CUDA(ctx, cudaMemsetAsync(err, 0, sizeof(int), st));
   }
-  if (record)
-    CG_CUDA(ctx, cudaMemsetAsync(keys, 0, ((size_t)n_thr + 1) * sizeof(unsigned long long), st));
-  else
-    CG_CUDA(ctx, cudaMemsetAsync(out_T, 0, (size_t)H * 128, st));
-  const Fuse f = record ? Fuse{keys, record, ratio_thr, n_thr} : Fuse{};
+  if (!record) CG_CUDA(ctx, cudaMemsetAsync(out_T, 0, (size_t)H * 128, st));
   const KdEval k = kd ? KdEval{view_of(ix.get()), tmean, kd_r, ws, stride, cap_log2, err} : KdEval{};
-  ransac9d_kernel<<<grid, RT, 0, st>>>(src, tgt, N, ids, H, nb, g, out_ratio, out_T, out_valid, f, k);
-  CG_LAUNCH_CHECK(ctx);
+  const size_t rec_len = (size_t)n_thr * REC_PER_THR + 18;
+  for (int b0 = 0; b0 < B; b0 += per_launch) {
+    const int nob = std::min(per_launch, B - b0);
+    if (record)
+      CG_CUDA(ctx, cudaMemsetAsync(keys, 0, (size_t)nob * (n_thr + 1) * sizeof(unsigned long long), st));
+    const Fuse f = record ? Fuse{keys, record + (size_t)b0 * rec_len, ratio_thr, n_thr} : Fuse{};
+    const size_t o = (size_t)b0 * N * 3;
+    ransac9d_kernel<<<dim3(grid, nob), RT, 0, st>>>(src + o, tgt + o, N, ids + (size_t)b0 * nb * 4, H, nb, g, out_ratio,
+                                                   out_T, out_valid, f, k);
+    CG_LAUNCH_CHECK(ctx);
+  }
   if (!kd) return CG_OK;
   int h = 0;
   CG_CUDA(ctx, cudaMemcpyAsync(&h, err, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -692,6 +712,20 @@ extern "C" int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const dou
   CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_pose: too many hypotheses");
   const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
   return ransac9d(ctx, source, target, N, ids, H, n_thr, g, 0.0, nullptr, nullptr, nullptr, out_record, ratio_threshold);
+}
+
+extern "C" int cg_ransac9d_pose_many_dev(cg_ctx *ctx, const double *source, const double *target, int B, int N,
+                                         const int32_t *ids, int H, const double *thresholds, int n_thr,
+                                         const double min_scale[3], const double max_scale[3], const double *max_dims,
+                                         double ratio_threshold, double *out_records) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, source && target && ids && N >= 4 && H > 0 && thresholds && (n_thr == 1 || n_thr == 2) && min_scale &&
+                      max_scale && out_records, "ransac9d_pose_many: bad arguments");
+  CG_REQUIRE(ctx, B >= 1 && B <= CG_NUNOCS_MANY_MAX_B, "ransac9d_pose_many: 1 <= B <= CG_NUNOCS_MANY_MAX_B");
+  CG_REQUIRE(ctx, (long long)H * n_thr <= 0x7FFFFFFFll, "ransac9d_pose_many: too many hypotheses");
+  const Gates g = make_gates(thresholds, n_thr, min_scale, max_scale, max_dims);
+  return ransac9d(ctx, source, target, N, ids, H, n_thr, g, 0.0, nullptr, nullptr, nullptr, out_records,
+                  ratio_threshold, B);
 }
 
 extern "C" int cg_ransac9d_kdtree_pose_dev(cg_ctx *ctx, const double *source, const double *target, int N,

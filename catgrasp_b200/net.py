@@ -35,9 +35,10 @@ class _Net:
     def _empty(self, *shape, dtype=torch.float32):
         return torch.empty(shape, dtype=dtype, device=self.device)
 
-    def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0):
-        """Counter-based subset draw on the device (cg_draw_ids_dev): (count, n_pts) int32 cuda tensor."""
-        ids = self._empty(count, n_pts, dtype=torch.int32)
+    def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0, out=None):
+        """Counter-based subset draw on the device (cg_draw_ids_dev): (count, n_pts) int32 cuda tensor (``out`` if
+        given)."""
+        ids = self._empty(count, n_pts, dtype=torch.int32) if out is None else out
         self.ctx.call("cg_draw_ids_dev", self.ctx.h, int(M), int(n_pts), int(count), int(seed), int(first_candidate), ids)
         return ids
 
@@ -111,4 +112,25 @@ class PointNetSeg(_Net):
         conf = self._empty(N)
         b = self._empty(N, 3, dtype=torch.int32)
         self.ctx.call("cg_nunocs_forward_dev", self.h, x, N, int(bins), coords, conf, b)
+        return coords, conf, b
+
+    def nunocs_many_host(self, x, bins):
+        """x (B,N,6) float32 host -> (coords (B,N,3) f32, conf_z (B,N) f32, bins (B,N,3) i32): nunocs_host on each
+        x[b], bit for bit, in one batched forward (cg_nunocs_forward_many_host)."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        B, N, _ = x.shape
+        coords = np.empty((B, N, 3), np.float32)
+        conf = np.empty((B, N), np.float32)
+        b = np.empty((B, N, 3), np.int32)
+        self.ctx.call("cg_nunocs_forward_many_host", self.h, x, B, N, int(bins), coords, conf, b)
+        return coords, conf, b
+
+    def nunocs_many_dev(self, x, bins):
+        """nunocs_many_host on the device: CUDA tensors in and out, no synchronisation."""
+        _, x = _lib.inputs(x, dtype=torch.float32, ctx=self.ctx)
+        B, N, _ = x.shape
+        coords = self._empty(B, N, 3)
+        conf = self._empty(B, N)
+        b = self._empty(B, N, 3, dtype=torch.int32)
+        self.ctx.call("cg_nunocs_forward_many_dev", self.h, x, B, N, int(bins), coords, conf, b)
         return coords, conf, b

@@ -94,6 +94,23 @@ def draw_subsample_ids(M, n_pts, count=None):
     return out
 
 
+def draw_nunocs_many(Ms, n_pts, n_hyp, given=None):
+    """The host-mode random numbers of a loop of NunocsPredicter.predict calls, in the loop's order, in one walk of
+    numpy's GLOBAL generator (cg_host_legacy_choice): for each object b, its cloud subset
+    ``np.random.choice(np.arange(Ms[b]), n_pts, replace=Ms[b] < n_pts)`` (not drawn where ``given[b]`` is not None),
+    then its ``n_hyp`` RANSAC 4-subsets of n_pts points (aligning.py:91-97).  Returns (list of (n_pts,) int32 subsets
+    or None, (B, n_hyp, 4) int32); the generator's state is put back once, at the end."""
+    B = len(Ms)
+    hyp = np.empty((B, n_hyp, 4), dtype=np.int32)
+    subs = []
+    d = _LegacyDraw()
+    for b, M in enumerate(Ms):
+        subs.append(d.draw(int(M), n_pts, 1)[0] if given is None or given[b] is None else None)
+        d.draw(n_pts, 4, n_hyp, out=hyp[b])
+    d.commit()
+    return subs, hyp
+
+
 class GraspPredicter:
     """predicter.py:39-94."""
 
@@ -385,7 +402,6 @@ class NunocsPredicter:
         """The reference's numbers: the transform's subset from np.random.choice, then both thresholds' subsets in
         one C draw that continues numpy's stream where the reference's two loops would (aligning.py:91-97), one
         fused launch on them, and predict's post-processing in numpy on the two winners' T (predicter.py:152-172)."""
-        from .aligning import read_record
         nocs_cloud, _ = self.predict_nocs(data, ids=ids)
         ori_cloud = self.data_transformed["cloud_xyz_original"]
         symmetry_tf = np.eye(4)
@@ -399,7 +415,19 @@ class NunocsPredicter:
         draw.commit()
         dev = self.model.device
         res = self._ransac(*self._on(dev, source, target, hyp))
-        found = read_record(res["record"].cpu().numpy(), len(self.THRESHOLDS))
+        best_ratio, best_transform = self._choose_host(res["record"].cpu().numpy(), source, target)
+        if best_transform is None:
+            return None, None
+        self.best_ratio = best_ratio
+        self.nocs_pose = best_transform.copy()
+        nocs_cloud = (symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
+        return nocs_cloud, best_transform
+
+    def _choose_host(self, record, source, target):
+        """predict's choice between the thresholds in numpy (predicter.py:152-172) from a pose search's host record:
+        (best_ratio, best_transform), best_transform None when no threshold gives a pose."""
+        from .aligning import read_record
+        found = read_record(record, len(self.THRESHOLDS))
         best_ratio = 0
         best_transform = None
         for t in range(len(self.THRESHOLDS)):
@@ -414,12 +442,7 @@ class NunocsPredicter:
             if ratio > best_ratio:
                 best_ratio = ratio
                 best_transform = transform.copy()
-        if best_transform is None:
-            return None, None
-        self.best_ratio = best_ratio
-        self.nocs_pose = best_transform.copy()
-        nocs_cloud = (symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
-        return nocs_cloud, best_transform
+        return best_ratio, best_transform
 
     def device_transform(self, data, ids=None, seed=None):
         """transform() on the device in float64 for numpy or CUDA input: the z >= 0.1 mask, the subset (``ids``, else
@@ -476,6 +499,212 @@ class NunocsPredicter:
         pose = host(res["pose"].clone())
         self.nocs_pose = pose.copy() if not cuda_in else pose.clone()
         return host(source), pose
+
+    def predict_many(self, datas, ids=None):
+        """predict for a list of objects: ``[self.predict(d) for d in datas]`` (with ``ids[b]`` for object b), bit for
+        bit, from the same state of numpy's global generator, which it leaves where the loop would; the attributes
+        data_transformed, confidence_z, pred_bins, best_ratio and nocs_pose are left as the loop leaves them.
+        ``datas`` are all numpy or all CUDA-tensor dicts with 'cloud_xyz' and 'cloud_normal' (M_b,3); they are not
+        modified.  ``ids`` (optional) is a list of B subsets of n_pts indices into the masked cloud, or None entries.
+        Returns one (nocs_cloud, pose) per object, (None, None) for an object with no pose.
+
+        The random numbers are drawn first, in the loop's order (host mode: object b's cloud subset, then its
+        2 x ransac_max_iter RANSAC subsets, in one walk of the generator; device mode: one seed per object), then
+        the forward runs on all objects in one batched pass (cg_nunocs_forward_many_*) and the residual pose search
+        in one launch over (object, threshold, hypothesis) (cg_ransac9d_pose_many_dev).  With use_kdtree_for_eval
+        the pose search runs one object at a time after the batched forward, as each builds its own target index.
+
+        The whole list is checked before any random number is drawn or any device work starts: a masked cloud that
+        is empty (where predict's draw raises) gives predict's ValueError, and mixed or malformed inputs a
+        ValueError.  So on error numpy's generator is left untouched, where the loop would have drawn for the
+        objects before the failing one."""
+        assert self.subsample in ("host", "device"), self.subsample
+        self._kd_resolution()
+        datas = list(datas)
+        B = len(datas)
+        ids = [None] * B if ids is None else [i if i is None or hasattr(i, "is_cuda") else np.asarray(i) for i in ids]
+        cuda_in, counts = self._check_many(datas, ids)
+        if B == 0:
+            return []
+        if self.subsample == "device":
+            return self._predict_many_device(datas, ids, counts, cuda_in)
+        if cuda_in:
+            datas = [{k: (v.cpu().numpy() if hasattr(v, "is_cuda") else v) for k, v in d.items()} for d in datas]
+            ids = [i if i is None or not hasattr(i, "is_cuda") else i.cpu().numpy() for i in ids]
+            return [(None, None) if tf is None else self._on(self.model.device, nocs, tf)
+                    for nocs, tf in self._predict_many_host(datas, ids, counts)]
+        return self._predict_many_host(datas, ids, counts)
+
+    def _check_many(self, datas, ids):
+        """predict_many's checks, before any draw: (whether the inputs are CUDA tensors, masked point counts)."""
+        import torch
+        n_pts = int(self.cfg["n_pts"])
+        if len(ids) != len(datas):
+            raise ValueError(f"predict_many: {len(ids)} id subsets for {len(datas)} objects")
+        if n_pts < 4:
+            raise ValueError("Cannot take a larger sample than population when 'replace=False'")   # as predict
+        kinds = set()
+        for b, d in enumerate(datas):
+            if not hasattr(d, "keys") or "cloud_xyz" not in d or "cloud_normal" not in d:
+                raise ValueError(f"predict_many: object {b} is not a dict with 'cloud_xyz' and 'cloud_normal'")
+            xyz, nrm = d["cloud_xyz"], d["cloud_normal"]
+            for a in (xyz, nrm):
+                kinds.add("cuda" if isinstance(a, torch.Tensor) and a.is_cuda else
+                          "numpy" if isinstance(a, np.ndarray) else type(a).__name__)
+            if len(kinds) > 1 or not kinds <= {"cuda", "numpy"}:
+                raise ValueError(f"predict_many: the clouds must be all numpy arrays or all CUDA tensors, got "
+                                 f"{sorted(kinds)}")
+            if len(xyz.shape) != 2 or xyz.shape[1] != 3 or tuple(nrm.shape) != tuple(xyz.shape):
+                raise ValueError(f"predict_many: object {b} has cloud_xyz {tuple(xyz.shape)} and cloud_normal "
+                                 f"{tuple(nrm.shape)}; both must be (M,3)")
+            if ids[b] is not None and tuple(ids[b].shape) != (n_pts,):
+                raise ValueError(f"predict_many: ids[{b}] has shape {tuple(ids[b].shape)}, not ({n_pts},)")
+        cuda_in = kinds == {"cuda"}
+        if cuda_in:
+            dev = self.model.device
+            vals = [(d["cloud_xyz"][:, 2] >= 0.1).sum().to(dev) for d in datas]   # the mask in the input's dtype
+            for i in ids:
+                if i is not None:
+                    i = torch.as_tensor(i).to(dev)
+                    vals += [i.min(), i.max()]
+            vals = torch.stack([v.to(torch.int64) for v in vals]).cpu().numpy()   # one synchronisation
+            counts, lims = vals[:len(datas)], vals[len(datas):].reshape(-1, 2)
+        else:
+            counts = np.array([np.count_nonzero(np.asarray(d["cloud_xyz"])[:, 2] >= 0.1) for d in datas], np.int64)
+            host_ids = [np.asarray(i.cpu() if hasattr(i, "is_cuda") else i) for i in ids if i is not None]
+            lims = np.array([(i.min(), i.max()) for i in host_ids], np.int64).reshape(-1, 2)
+        k = 0
+        for b, M in enumerate(counts):
+            if ids[b] is None:
+                if M == 0:
+                    raise ValueError("'a' cannot be empty unless no samples are taken")   # predict's np.random.choice
+                continue
+            if lims[k, 0] < 0 or lims[k, 1] >= M:
+                raise ValueError(f"predict_many: ids[{b}] indexes outside the {M} points with z >= 0.1")
+            k += 1
+        return cuda_in, [int(M) for M in counts]
+
+    def _predict_many_host(self, datas, ids, counts):
+        """predict_many on numpy input in host mode: the draws in one walk, transform() per object, one forward, one
+        pose search (or one per object with the kd-tree evaluation), one copy of the records, _choose_host."""
+        import torch
+        n_pts, H, B = int(self.cfg["n_pts"]), int(self.ransac_max_iter), len(datas)
+        subs, hyp = draw_nunocs_many(counts, n_pts, len(self.THRESHOLDS) * H, given=ids)
+        dts, xs = [], np.empty((B, n_pts, 6), dtype=np.float32)
+        for b, data in enumerate(datas):
+            d = dict(data)                                                  # predict_nocs, without writing to data
+            d["cloud_nocs"] = np.zeros(d["cloud_xyz"].shape)
+            d["cloud_rgb"] = np.zeros(d["cloud_xyz"].shape)
+            dts.append(self.transform(copy.deepcopy(d), ids=subs[b] if ids[b] is None else ids[b]))
+            xs[b] = np.ascontiguousarray(dts[b]["input"], dtype=np.float64).astype(np.float32)
+        coords, conf_z, bins = self.model.nunocs_many_host(xs, int(self.cfg["ce_loss_bins"]))
+        symmetry_tf = np.eye(4)
+        source = [np.ascontiguousarray((symmetry_tf @ to_homo(coords[b]).T).T[:, :3], dtype=np.float64)
+                  for b in range(B)]
+        target = [np.ascontiguousarray(dt["cloud_xyz_original"], dtype=np.float64) for dt in dts]
+        dev = self.model.device
+        if self.use_kdtree_for_eval:
+            recs = [self._ransac(*self._on(dev, source[b], target[b], hyp[b]))["record"] for b in range(B)]
+            recs = torch.stack(recs)
+        else:
+            recs = self._ransac_many(*self._on(dev, np.stack(source), np.stack(target), hyp))
+        recs = recs.cpu().numpy()
+        out = []
+        for b in range(B):                                                  # the attributes in the loop's order
+            self.data_transformed, self.confidence_z, self.pred_bins = dts[b], conf_z[b], bins[b]
+            best_ratio, best_transform = self._choose_host(recs[b], source[b], target[b])
+            if best_transform is None:
+                out.append((None, None))
+                continue
+            self.best_ratio = best_ratio
+            self.nocs_pose = best_transform.copy()
+            out.append((source[b], best_transform))
+        return out
+
+    def _ransac_many(self, source, target, ids):
+        from .aligning import ransac9d_pose_many
+        return ransac9d_pose_many(source, target, ids, self.THRESHOLDS, max_scale=self.max_scale,
+                                  min_scale=self.min_scale, max_dimensions=self.MAX_DIMENSIONS,
+                                  ratio_threshold=self.ERR_THRES)
+
+    def _device_transform_many(self, datas, ids, seeds, counts):
+        """device_transform for every object: (B,n_pts,*) CUDA tensors 'cloud_xyz', 'cloud_normal',
+        'cloud_xyz_original', 'keep_ids' and 'input', row b bit for bit device_transform(datas[b], ids[b],
+        seeds[b]).  The subsets are drawn per object (each has its own point count and seed); the gathers,
+        normalisation and scaling run on all objects at once.  No synchronisation."""
+        import torch
+        from . import _lib
+        n_pts, B = int(self.cfg["n_pts"]), len(datas)
+        ctx = self.model.ctx
+        xyz_all, nrm_all, keep, glob = [], [], [], []
+        off = 0
+        for b, d in enumerate(datas):
+            _, xyz, nrm = _lib.inputs(d["cloud_xyz"], d["cloud_normal"], dtype=torch.float64, ctx=ctx)
+            if getattr(d["cloud_xyz"], "is_cuda", False):
+                k = torch.nonzero_static(d["cloud_xyz"][:, 2] >= 0.1, size=counts[b]).reshape(-1).to(xyz.device)
+            else:
+                k = torch.from_numpy(np.nonzero(np.asarray(d["cloud_xyz"])[:, 2] >= 0.1)[0]).to(xyz.device)
+            if ids[b] is None:
+                sub = self.model.draw_ids_dev(counts[b], n_pts, 1, seeds[b], first_candidate=0)[0].long()
+            else:
+                sub = torch.as_tensor(np.asarray(ids[b]) if not hasattr(ids[b], "is_cuda") else ids[b]).to(
+                    xyz.device).long()
+            keep.append(k[sub])
+            glob.append(keep[-1] + off)
+            off += xyz.shape[0]
+            xyz_all.append(xyz)
+            nrm_all.append(nrm)
+        g = torch.cat(glob)
+        x0 = torch.cat(xyz_all)[g].reshape(B, n_pts, 3)
+        nr = torch.cat(nrm_all)[g].reshape(B, n_pts, 3)
+        mn = x0.amin(1, keepdim=True)
+        scale = (x0.amax(1, keepdim=True) - mn).amax(2, keepdim=True)
+        xn = (x0 - mn) / (scale + 1e-15)
+        inp = torch.cat([xn, nr], 2)
+        if "mean" in self.cfg:
+            mean, std = self._on(x0.device, self.cfg["mean"].reshape(1, 1, -1), self.cfg["std"].reshape(1, 1, -1))
+            inp = (inp - mean) / (std + 1e-15)
+        return {"cloud_xyz": xn, "cloud_normal": nr, "cloud_xyz_original": x0, "keep_ids": torch.stack(keep),
+                "input": inp}
+
+    def _predict_many_device(self, datas, ids, counts, cuda_in):
+        """predict_many in device mode: B seeds (np.random.randint, in the loop's order), the batched transform and
+        forward, each object's RANSAC subsets as candidates 1 .. 2H of cg_draw_ids_dev under its seed, one pose
+        search, one copy of the records (and, with numpy input, one of the results)."""
+        import torch
+        from .aligning import REC_PER_THR
+        n_thr, H, B = len(self.THRESHOLDS), int(self.ransac_max_iter), len(datas)
+        seeds = [int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64)) for _ in range(B)]
+        dt = self._device_transform_many(datas, ids, seeds, counts)
+        coords, conf_z, bins = self.model.nunocs_many_dev(dt["input"].to(torch.float32), int(self.cfg["ce_loss_bins"]))
+        source = coords.to(torch.float64)
+        N = source.shape[1]
+        hyp = torch.empty((B, n_thr * H, 4), dtype=torch.int32, device=source.device)
+        for b in range(B):
+            self.model.draw_ids_dev(N, 4, n_thr * H, seeds[b], first_candidate=1, out=hyp[b])
+        if self.use_kdtree_for_eval:
+            recs = torch.stack([self._ransac(source[b], dt["cloud_xyz_original"][b], hyp[b])["record"]
+                                for b in range(B)])
+        else:
+            recs = self._ransac_many(source, dt["cloud_xyz_original"], hyp)
+        rec_host = recs.cpu().numpy()
+        if not cuda_in:
+            dt = {k: v.cpu().numpy() for k, v in dt.items()}
+            source, conf_z, bins = source.cpu().numpy(), conf_z.cpu().numpy(), bins.cpu().numpy()
+        tail = n_thr * REC_PER_THR                                          # [chosen, pose (16), best_ratio]
+        out = []
+        for b in range(B):                                                  # the attributes in the loop's order
+            self.data_transformed = {k: v[b] for k, v in dt.items()}
+            self.confidence_z, self.pred_bins = conf_z[b], bins[b]
+            if rec_host[b, tail] < 0:
+                out.append((None, None))
+                continue
+            self.best_ratio = float(rec_host[b, tail + 17])
+            pose = recs[b, tail + 1:tail + 17].reshape(4, 4).clone() if cuda_in else \
+                rec_host[b, tail + 1:tail + 17].reshape(4, 4).copy()
+            self.nocs_pose = pose.copy() if not cuda_in else pose.clone()
+            out.append((source[b], pose))
+        return out
 
 
 def flatten_config(cfg, out=None):

@@ -183,6 +183,18 @@ int cg_nunocs_forward_host(cg_net *net, const float *x_host, int N, int bins,
                            float *out_coords, float *out_conf_z, int32_t *out_bins);
 int cg_nunocs_forward_dev(cg_net *net, const float *x, int N, int bins,
                           float *out_coords, float *out_conf_z, int32_t *out_bins);
+/* The same for B objects of N points each (replaces predicter.py:136-150 once per object of a list):
+ * x (B,N,6) -> coords (B,N,3), conf_z (B,N), bins (B,N,3).  Object b's outputs are those of
+ * cg_nunocs_forward_dev on x[b], bit for bit, on every engine: the per-cloud FC layers run in groups of at
+ * most 8 clouds (the few-row kernel a single cloud takes), and N < 64 runs one object per pass.  The forward
+ * runs in passes of at most CG_NUNOCS_MANY_PASS_POINTS points (whole objects); CG_EINVAL before any launch
+ * unless 1 <= B <= CG_NUNOCS_MANY_MAX_B and N > 0.  _dev runs on the context stream and does not synchronise. */
+#define CG_NUNOCS_MANY_MAX_B 65535
+#define CG_NUNOCS_MANY_PASS_POINTS (1 << 18)
+int cg_nunocs_forward_many_host(cg_net *net, const float *x_host, int B, int N, int bins,
+                                float *out_coords, float *out_conf_z, int32_t *out_bins);
+int cg_nunocs_forward_many_dev(cg_net *net, const float *x, int B, int N, int bins,
+                               float *out_coords, float *out_conf_z, int32_t *out_bins);
 
 /* ---- SDF grid ----------------------------------------------------------
  * Replaces: meshpy/meshpy/sdf.py:217-289 (Sdf3D), sdf_file.py:59-87.
@@ -357,6 +369,18 @@ int cg_ransac9d_pose_dev(cg_ctx *ctx, const double *source, const double *target
                          const double *thresholds /* host */, int n_thr, const double min_scale[3] /* host */,
                          const double max_scale[3] /* host */, const double *max_dims /* host */,
                          double ratio_threshold, double *out_record);
+/* cg_ransac9d_pose_dev for B objects of N correspondences each (predicter.py:152-172 once per object of a list):
+ * source, target (B,N,3), ids (B, n_thr*H, 4) -- object b's rows as cg_ransac9d_pose_dev's ids --, out_records
+ * (B, n_thr*19 + 18): object b's record as cg_ransac9d_pose_dev writes it for source[b], target[b], ids[b], bit
+ * for bit.  One CTA per (object, threshold, hypothesis); the winner keys, the completion counter and the last
+ * CTA's choice are per object.  At most CG_RANSAC_MANY_PASS_PAIRS CTAs per launch (whole objects; one object
+ * when n_thr*H is larger), the launches in object order.  CG_EINVAL before any launch unless
+ * 1 <= B <= CG_NUNOCS_MANY_MAX_B.  Runs on the context stream and does not synchronise.                        */
+#define CG_RANSAC_MANY_PASS_PAIRS (1 << 20)
+int cg_ransac9d_pose_many_dev(cg_ctx *ctx, const double *source, const double *target, int B, int N,
+                              const int32_t *ids, int H, const double *thresholds /* host */, int n_thr,
+                              const double min_scale[3] /* host */, const double max_scale[3] /* host */,
+                              const double *max_dims /* host */, double ratio_threshold, double *out_records);
 
 /* The same two entries with aligning.py:68-79's evaluation (use_kdtree_for_eval=True, kdtree_eval_resolution =
  * resolution) in place of the residual count; the gates and the selection rules are unchanged.  For a hypothesis
