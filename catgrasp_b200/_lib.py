@@ -112,10 +112,12 @@ SIGNATURES = {
     "cg_net_blob_floats": (_sz, [_i, _i], None),
     "cg_graspq_forward_host": (_i, [_vp, _H, _H, _i, _H, _i, _H, _i, _H, _H, _H, _H], OWN),
     "cg_graspq_forward_dev": (_i, [_vp, _D, _D, _i, _D, _i, _D, _i, _D, _D, _D, _D], TORCH),
+    "cg_graspq_forward_many_dev": (_i, [_vp, _D, _D, _i, _D, _i, _D, _i, _D, _D, _H, _i, _D, _D], TORCH),
     "cg_host_legacy_choice": (_i, [_H, _H, C.c_int64, C.c_int32, C.c_int32, _H, C.c_int32], None),
     "cg_host_legacy_skip": (_i, [_H, _H, C.c_int64, C.c_int32, C.c_int32], None),
     "cg_host_rng_isa": (_i, [_i], None),
     "cg_draw_ids_dev": (_i, [_vp, _i, _i, _i, C.c_uint64, C.c_int64, _D], TORCH),
+    "cg_draw_ids_many_dev": (_i, [_vp, _i, _D, _D, _D, _D, _i, _i, _D], TORCH),
     "cg_mlp_create": (_i, [_vp, _i, _H, _H, _H, _H], OWN),
     "cg_mlp_destroy": (None, [_vp], None),
     "cg_shared_mlp_dev": (_i, [_vp, _D, C.c_int64, _D], TORCH),

@@ -192,12 +192,22 @@ constexpr int RQ = 4;     // column quads per CTA
 constexpr int RS = 64;    // k-slices per CTA
 constexpr int RC = RQ * 4;
 
+// With groups.n > 0 one launch runs groups.n independent row groups, blockIdx.y picking one: group g is rows
+// (groups.g[g] >> 4) .. + (groups.g[g] & 15) - 1 of X and Y, and each of its rows gets the sums a launch on that group
+// alone gives (row m of a group uses bias row m / bias_row_div counted from the group's first row).
 __global__ void __launch_bounds__(256) linear_rows_kernel(const float *__restrict__ X, int M, int K,
                                                            const float *__restrict__ Wt,
                                                            const float *__restrict__ bias, int N, int relu,
                                                            int bias_row_div, int x_is_keys,
-                                                           float *__restrict__ Y) {
+                                                           float *__restrict__ Y,
+                                                           const __grid_constant__ cg_fc_row_groups groups) {
   __shared__ float red[RS][RM][RC + 1];
+  if (groups.n > 0) {
+    const int32_t g = groups.g[blockIdx.y];
+    X += (size_t)(g >> 4) * K;
+    Y += (size_t)(g >> 4) * N;
+    M = g & 15;
+  }
   const int tid = threadIdx.x;
   const int nq = tid % RQ, ks = tid / RQ;          // RQ column quads x RS k-slices
   const int n = blockIdx.x * RC + nq * 4;
@@ -324,7 +334,10 @@ int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, floa
   if (ctx->engine >= 1 && L.tc && M >= 64)
     return cg_linear_tc_launch(ctx, X, M, K, L.tc, bias, N, relu, bias_row_div, x_is_keys, Y);
   if (M <= RM) {
-    linear_rows_kernel<<<(N + RC - 1) / RC, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
+    cg_fc_row_groups one;
+    one.n = 0;
+    linear_rows_kernel<<<(N + RC - 1) / RC, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y,
+                                                                   one);
     CG_LAUNCH_CHECK(ctx);
     return CG_OK;
   }
@@ -339,6 +352,40 @@ int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, floa
   linear_kernel<<<grid, 256, 0, ctx->stream>>>(X, M, K, Wt, bias, N, relu, bias_row_div, x_is_keys, Y);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
+}
+
+int cg_linear_launch_groups(cg_ctx *ctx, const cg_layer &L, const float *X, const int32_t *rows, int n_groups, float *Y,
+                            unsigned flags) {
+  const int K = L.K, N = L.C;
+  CG_REQUIRE(ctx, K > 0 && N > 0 && n_groups > 0, "linear_groups: bad shape");
+  const int relu = (flags & CG_FC_RELU) != 0, x_is_keys = (flags & CG_FC_KEYS) != 0;
+  cg_fc_row_groups few;
+  few.n = 0;
+  auto flush = [&]() -> int {
+    if (few.n == 0) return CG_OK;
+    linear_rows_kernel<<<dim3((N + RC - 1) / RC, few.n), 256, 0, ctx->stream>>>(X, 0, K, L.Wt, L.b, N, relu, 0,
+                                                                              x_is_keys, Y, few);
+    CG_LAUNCH_CHECK(ctx);
+    few.n = 0;
+    return CG_OK;
+  };
+  long long total = 0;
+  for (int i = 0; i < n_groups; i++) {
+    CG_REQUIRE(ctx, rows[i] > 0, "linear_groups: empty group");
+    total += rows[i];
+  }
+  CG_REQUIRE(ctx, total < (1 << 27), "linear_groups: 2^27 rows or more");
+  int r0 = 0, rc;
+  for (int i = 0; i < n_groups; r0 += rows[i++]) {
+    const int m = rows[i];
+    if (m <= RM) {   // the kernel cg_linear_launch takes for m rows, m <= 8 (it never takes tensor cores below 64)
+      few.g[few.n++] = (r0 << 4) | m;
+      if (few.n == CG_FC_GROUPS_PER_LAUNCH && (rc = flush())) return rc;
+    } else if ((rc = cg_linear_launch(ctx, L, X + (size_t)r0 * K, m, Y + (size_t)r0 * N, flags))) {
+      return rc;
+    }
+  }
+  return flush();
 }
 
 int cg_softmax_launch(cg_ctx *ctx, const float *logits, int B, int C, float *probs, int32_t *label) {

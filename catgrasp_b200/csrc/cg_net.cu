@@ -33,7 +33,7 @@ void layer_dims(int kind, int n_out, LayerDim d[L_COUNT]) {
 
 inline size_t pad64(size_t n) { return (n + 63) & ~size_t(63); }
 
-constexpr int CHUNK_B = 16384;  // candidates per internal pass (bounds the T64 workspace to 256 MB)
+constexpr int CHUNK_B = CG_GRASPQ_CHUNK_B;  // candidates per internal pass (bounds the T64 workspace to 256 MB)
 
 }  // namespace
 
@@ -140,7 +140,17 @@ void encoder_ws_carve(cg_arena &ar, int B, EncoderWs &w) {
 // The FC chain after a trunk (STN3d, STNkd, cls head): layers L[l], L[l+1], L[l+2] =
 // 1024 -> 512 (ReLU, from the max-pool keys in w.gmax) -> 256 (ReLU) -> out (no ReLU).
 // rows > 0 launches it on groups of at most `rows` clouds (0: all B in one launch per layer).
-int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, float *out, int rows = 0) {
+// groups (host, n_groups entries summing to B): launch each layer on these row groups instead (cg_linear_launch_groups).
+int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, float *out, int rows = 0,
+             const int32_t *groups = nullptr, int n_groups = 0) {
+  if (groups) {
+    int rc;
+    if ((rc = cg_linear_launch_groups(ctx, L[l], reinterpret_cast<const float *>(w.gmax), groups, n_groups, w.f1,
+                                      CG_FC_RELU | CG_FC_KEYS)))
+      return rc;
+    if ((rc = cg_linear_launch_groups(ctx, L[l + 1], w.f1, groups, n_groups, w.f2, CG_FC_RELU))) return rc;
+    return cg_linear_launch_groups(ctx, L[l + 2], w.f2, groups, n_groups, out, 0);
+  }
   const int g = rows > 0 ? rows : B;
   for (int r0 = 0; r0 < B; r0 += g) {
     const int m = B - r0 < g ? B - r0 : g;
@@ -157,9 +167,11 @@ int fc_chain(cg_ctx *ctx, const cg_layer *L, int l, int B, const EncoderWs &w, f
 
 // Runs the PointNetEncoder (pointnet2.py:241-271) for B clouds; on return w.gmax holds the
 // (B,1024) global feature as order-preserving keys; pf_out (optional) the 64-ch point feature.
-// keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.  fc_rows: fc_chain's rows.
+// keys_out (optional, test hook): (3,B,1024) copies of the three trunks' max-pool keys.  fc_rows, fc_groups,
+// n_fc_groups: fc_chain's rows, groups and n_groups.
 int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs &w, float *pf_out,
-                    uint32_t *keys_out = nullptr, int fc_rows = 0) {
+                    uint32_t *keys_out = nullptr, int fc_rows = 0, const int32_t *fc_groups = nullptr,
+                    int n_fc_groups = 0) {
   cg_ctx *ctx = net->ctx;
   const cg_layer *L = net->L;
   int rc;
@@ -172,14 +184,14 @@ int encoder_forward(cg_net *net, const cg_input_src &in, int B, int N, EncoderWs
   a.l2 = L[L_S3_C2]; a.l3 = L[L_S3_C3]; a.tc_img = net->tc_img[0]; a.tc_f16_ok = net->tc_f16_ok[0]; a.relu3 = 1; a.gmax_keys = w.gmax; a.pf_out = nullptr;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = fc_chain(ctx, L, L_S3_F1, B, w, w.T3, fc_rows))) return rc;
+  if ((rc = fc_chain(ctx, L, L_S3_F1, B, w, w.T3, fc_rows, fc_groups, n_fc_groups))) return rc;
   // --- trunk B: encoder conv1 + STNkd convs + max (pointnet2.py:252, :208-213)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.T3 = w.T3; a.l0 = L[L_E_C1]; a.stage1_mode = 1; a.l1 = L[L_SK_C1];
   a.l2 = L[L_SK_C2]; a.l3 = L[L_SK_C3]; a.tc_img = net->tc_img[1]; a.tc_f16_ok = net->tc_f16_ok[1]; a.relu3 = 1;
   if ((rc = trunk_launch(ctx, a))) return rc;
   if (keys_out) CG_CUDA(ctx, cudaMemcpyAsync(keys_out + (size_t)B * 1024, w.gmax, kb, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = fc_chain(ctx, L, L_SK_F1, B, w, w.T64, fc_rows))) return rc;
+  if ((rc = fc_chain(ctx, L, L_SK_F1, B, w, w.T64, fc_rows, fc_groups, n_fc_groups))) return rc;
   // --- trunk C: conv1, @T64, conv2, conv3(+BN, no ReLU), max (pointnet2.py:252-265)
   CG_CUDA(ctx, cudaMemsetAsync(w.gmax, 0, (size_t)B * 1024 * 4, ctx->stream));
   a.stage1_mode = 2; a.T64 = w.T64; a.l1 = cg_layer{nullptr, nullptr, 64, 64};
@@ -281,6 +293,53 @@ extern "C" int cg_graspq_forward_dev(cg_net *net, const double *cloud_xyz, const
   in.cloud_xyz = cloud_xyz; in.cloud_nrm = cloud_nrm; in.poses = poses; in.ids = ids;
   in.mean = mean; in.stdv = stdv; in.M = M;
   return cls_forward_impl(net, in, B, N, nullptr, out_probs, out_label);
+}
+
+extern "C" int cg_graspq_forward_many_dev(cg_net *net, const double *cloud_xyz, const double *cloud_nrm, int M_total,
+                                          const double *poses, int B_total, const int32_t *ids, int N,
+                                          const double *mean, const double *stdv, const int32_t *fc_groups,
+                                          int n_groups, float *out_probs, int32_t *out_label) {
+  if (!net) return CG_EINVAL;
+  cg_ctx *ctx = net->ctx;
+  CG_REQUIRE(ctx, net->kind == CG_NET_CLS, "graspq_many: net is not a PointNetCls");
+  CG_REQUIRE(ctx, cloud_xyz && cloud_nrm && poses && ids && fc_groups && out_probs, "graspq_many: null argument");
+  CG_REQUIRE(ctx, M_total > 0 && B_total > 0 && N > 0 && n_groups > 0, "graspq_many: bad shape");
+  CG_REQUIRE(ctx, (mean == nullptr) == (stdv == nullptr), "graspq_many: mean/std must come together");
+  long long sum = 0;
+  for (int i = 0; i < n_groups; i++) {
+    CG_REQUIRE(ctx, fc_groups[i] >= 1 && fc_groups[i] <= CG_GRASPQ_CHUNK_B, "graspq_many: a group of 1 .. CHUNK_B rows");
+    sum += fc_groups[i];
+  }
+  CG_REQUIRE(ctx, sum == B_total, "graspq_many: the groups do not add up to B_total");
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int n_out = net->n_out;
+  const int Bc_max = B_total < CHUNK_B ? B_total : CHUNK_B;
+  EncoderWs w;
+  float *logits;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    encoder_ws_carve(ar, Bc_max, w);
+    logits = ar.take<float>((size_t)Bc_max * n_out);
+  });
+  if (rc) return rc;
+  cg_input_src in;
+  memset(&in, 0, sizeof(in));
+  in.cloud_xyz = cloud_xyz; in.cloud_nrm = cloud_nrm; in.mean = mean; in.stdv = stdv; in.M = M_total;
+  // passes of whole groups, at most CHUNK_B candidates each: a candidate's trunk keys do not depend on the pass, and
+  // each group's FC layers get the launch (and so the bits) the group's own call gets
+  for (int g0 = 0, b0 = 0; g0 < n_groups;) {
+    int g1 = g0, B = 0;
+    while (g1 < n_groups && B + fc_groups[g1] <= CHUNK_B) B += fc_groups[g1++];
+    in.poses = poses + (size_t)b0 * 16;
+    in.ids = ids + (size_t)b0 * N;
+    if ((rc = encoder_forward(net, in, B, N, w, nullptr, nullptr, 0, fc_groups + g0, g1 - g0))) return rc;
+    if ((rc = fc_chain(ctx, net->L, L_HEAD0, B, w, logits, 0, fc_groups + g0, g1 - g0))) return rc;
+    if ((rc = cg_softmax_launch(ctx, logits, B, n_out, out_probs + (size_t)b0 * n_out,
+                                out_label ? out_label + b0 : nullptr)))
+      return rc;
+    g0 = g1;
+    b0 += B;
+  }
+  return CG_OK;
 }
 
 extern "C" int cg_graspq_forward_host(cg_net *net, const double *cloud_xyz, const double *cloud_nrm, int M,

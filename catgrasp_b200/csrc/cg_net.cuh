@@ -94,6 +94,18 @@ enum : unsigned {
 constexpr int CG_FC_FEW_ROWS = 8;
 int cg_linear_launch(cg_ctx *ctx, const cg_layer &L, const float *X, int M, float *Y, unsigned flags,
                      const float *row_bias = nullptr, int rows_per_bias = 0);
+// Row groups of the few-row kernel for one launch: g[i] = first row << 4 | rows (1 .. CG_FC_FEW_ROWS); n = 0 is a
+// plain launch on M rows.
+constexpr int CG_FC_GROUPS_PER_LAUNCH = 128;
+struct cg_fc_row_groups {
+  int n;
+  int32_t g[CG_FC_GROUPS_PER_LAUNCH];
+};
+// cg_linear_launch on each of n_groups consecutive row groups of X / Y (rows[i] rows each, host array), with each
+// group's bits: the groups of at most CG_FC_FEW_ROWS rows share few-row launches (CG_FC_GROUPS_PER_LAUNCH per launch),
+// every other group is a cg_linear_launch of its own.  Layer bias only; fewer than 2^27 rows in all.
+int cg_linear_launch_groups(cg_ctx *ctx, const cg_layer &L, const float *X, const int32_t *rows, int n_groups, float *Y,
+                            unsigned flags);
 // tensor-core FC path (cg_linear_tc.cu).  The image builder returns nullptr in *img for shapes the kernel does not take
 // (K % 64 != 0 or N < 64); otherwise a device image the caller frees with cudaFree.  It also sets the kernel's
 // shared-memory limit on the current device.

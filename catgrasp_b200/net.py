@@ -42,6 +42,21 @@ class _Net:
         self.ctx.call("cg_draw_ids_dev", self.ctx.h, int(M), int(n_pts), int(count), int(seed), int(first_candidate), ids)
         return ids
 
+    def draw_ids_many_dev(self, Ms, n_pts, counts, seeds, bases, out=None):
+        """cg_draw_ids_dev for several objects in one launch (cg_draw_ids_many_dev): a (sum(counts), n_pts) int32 CUDA
+        tensor whose rows of object o are ``draw_ids_dev(Ms[o], n_pts, counts[o], seeds[o]) + bases[o]``."""
+        n_obj = len(Ms)
+        rows = np.zeros(n_obj + 1, np.int64)
+        rows[1:] = np.cumsum(np.asarray(counts, np.int64))
+        ids = self._empty(int(rows[-1]), n_pts, dtype=torch.int32) if out is None else out
+        if n_obj == 0 or rows[-1] == 0:
+            return ids
+        _, m, s, r, b = _lib.inputs(np.asarray(Ms, np.int32), np.asarray(seeds, np.uint64).view(np.int64), rows,
+                                    np.asarray(bases, np.int32), dtype=(torch.int32, torch.int64, torch.int64,
+                                                                        torch.int32), ctx=self.ctx)
+        self.ctx.call("cg_draw_ids_many_dev", self.ctx.h, n_obj, m, s, r, b, int(n_pts), int(rows[-1]), ids)
+        return ids
+
 
 class PointNetCls(_Net):
     """forward(x:(B,N,6)) -> logits (B,n_out); mirrors pointnet2.py:289-299 (first return value)."""
@@ -65,6 +80,18 @@ class PointNetCls(_Net):
         N = ids.shape[1]
         probs, label = out if out is not None else (self._empty(B, self.n_out), self._empty(B, dtype=torch.int32))
         self.ctx.call("cg_graspq_forward_dev", self.h, cloud_xyz, cloud_nrm, M, poses, B, ids, N, mean, std, probs, label)
+        return probs, label
+
+    def graspq_many_dev(self, cloud_xyz, cloud_nrm, poses, ids, groups, mean=None, std=None, out=None):
+        """graspq_dev over the candidates of several objects (cg_graspq_forward_many_dev): the clouds concatenated,
+        ``ids`` rebased to their rows, ``groups`` the row counts of the graspq_dev launches to reproduce (their FC
+        kernels, and so their bits).  Returns (probs (B,n_out) f32, label (B,) i32 or None); ``out`` = (probs, label
+        or None)."""
+        M, B, N = cloud_xyz.shape[0], poses.shape[0], ids.shape[1]
+        groups = np.ascontiguousarray(groups, dtype=np.int32)
+        probs, label = out if out is not None else (self._empty(B, self.n_out), self._empty(B, dtype=torch.int32))
+        self.ctx.call("cg_graspq_forward_many_dev", self.h, cloud_xyz, cloud_nrm, M, poses, B, ids, N, mean, std,
+                      groups, len(groups), probs, label)
         return probs, label
 
     def graspq_host(self, cloud_xyz, cloud_nrm, poses, ids, mean=None, std=None, out_probs=None, out_label=None):

@@ -111,6 +111,105 @@ def draw_nunocs_many(Ms, n_pts, n_hyp, given=None):
     return subs, hyp
 
 
+GRASPQ_CHUNK_B = 16384   # candidates per internal pass of cg_graspq_forward_*_dev (CG_GRASPQ_CHUNK_B)
+
+
+def graspq_fc_groups(counts, launch=None):
+    """The FC row groups of a loop of GraspPredicter.score calls, one per object with counts[o] candidates: each
+    call's graspq_dev launches cover ``launch`` candidates (host-drawn subsets: GraspPredicter.chunk) or the whole
+    list (None: device-drawn or given subsets), and cg_graspq_forward_dev cuts each launch at GRASPQ_CHUNK_B.
+    Returns (groups (G,) int32 row counts in row order, spans (O,2) int64: object o's groups are
+    groups[spans[o,0]:spans[o,1]])."""
+    groups, spans = [], np.zeros((len(counts), 2), np.int64)
+    for o, B in enumerate(counts):
+        spans[o, 0] = len(groups)
+        step = B if launch is None else int(launch)
+        for c0 in range(0, B, max(step, 1)):
+            L = min(step, B - c0)
+            groups += [min(GRASPQ_CHUNK_B, L - k) for k in range(0, L, GRASPQ_CHUNK_B)]
+        spans[o, 1] = len(groups)
+    return np.asarray(groups, np.int32), spans
+
+
+def host_draw_stages(groups, chunk):
+    """Stages of the host-drawn pipeline: consecutive groups packed into row ranges of at most ``chunk`` rows (one
+    group per stage where a group is larger).  Returns a list of (first row, end row, first group, end group)."""
+    stages, r0, g0, rows = [], 0, 0, 0
+    for g, m in enumerate(groups):
+        if rows and rows + int(m) > chunk:
+            stages.append((r0, r0 + rows, g0, g))
+            r0, g0, rows = r0 + rows, g, 0
+        rows += int(m)
+    if rows:
+        stages.append((r0, r0 + rows, g0, len(groups)))
+    return stages
+
+
+def walk_grasp_many(Ms, counts, n_pts, stages, out):
+    """The host-mode draws of a loop of GraspPredicter.predict_batch calls in ONE walk of numpy's global generator
+    (cg_host_legacy_choice): object o's counts[o] subsets of n_pts points out of Ms[o] (replace = Ms[o] < n_pts), in
+    object order, into the rows of ``out`` (sum(counts), n_pts) int32.  A generator: it draws stage by stage (row
+    ranges from host_draw_stages, cut anywhere) and yields each stage as it is drawn; the generator's state is put
+    back once, after the last stage."""
+    draw = _LegacyDraw()
+    first = np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64))])
+    for stage in stages:
+        r0, r1 = int(stage[0]), int(stage[1])
+        o = int(np.searchsorted(first, r0, side="right")) - 1
+        r = r0
+        while r < r1:
+            while first[o + 1] <= r:
+                o += 1
+            e = min(r1, int(first[o + 1]))
+            draw.draw(int(Ms[o]), n_pts, e - r, out=out[r:e])
+            r = e
+        yield stage
+    draw.commit()
+
+
+def _check_grasp_many(datas, grasp_poses_list, ids, n_pts):
+    """predict_batch_many's checks, before any draw: per object (masked xyz (M,3) f64, masked normals, poses (B,4,4)
+    f64, ids (B,n_pts) int32 or None), or None for an object with no candidates (predict_batch returns [] for it
+    without looking at its data).  ValueError for anything predict_batch would fail on, and for ids outside the
+    object's masked cloud."""
+    datas, grasp_poses_list = list(datas), list(grasp_poses_list)
+    if len(grasp_poses_list) != len(datas):
+        raise ValueError(f"predict_batch_many: {len(grasp_poses_list)} pose lists for {len(datas)} objects")
+    if ids is not None and len(ids) != len(datas):
+        raise ValueError(f"predict_batch_many: {len(ids)} id arrays for {len(datas)} objects")
+    out = []
+    for o, (data, grasps) in enumerate(zip(datas, grasp_poses_list)):
+        B = len(grasps)
+        if B == 0:
+            out.append(None)
+            continue
+        poses = np.asarray(grasps, dtype=np.float64)
+        if poses.size != B * 16:
+            raise ValueError(f"predict_batch_many: object {o} has {B} poses of {poses.size // B} values, not 4x4")
+        if not hasattr(data, "keys") or "cloud_xyz" not in data or "cloud_normal" not in data:
+            raise ValueError(f"predict_batch_many: object {o} is not a dict with 'cloud_xyz' and 'cloud_normal'")
+        xyz = np.asarray(data["cloud_xyz"], dtype=np.float64)
+        nrm = np.asarray(data["cloud_normal"], dtype=np.float64)
+        if xyz.ndim != 2 or xyz.shape[1] != 3 or nrm.shape != xyz.shape:
+            raise ValueError(f"predict_batch_many: object {o} has cloud_xyz {xyz.shape} and cloud_normal {nrm.shape}; "
+                             f"both must be (M,3)")
+        valid_mask = xyz[:, 2] >= 0.1                                   # dataset_grasp.py:64
+        xyz, nrm = np.ascontiguousarray(xyz[valid_mask]), np.ascontiguousarray(nrm[valid_mask])
+        if xyz.shape[0] == 0:
+            raise ValueError("'a' cannot be empty unless no samples are taken")   # predict_batch's np.random.choice
+        sub = None
+        if ids is not None:
+            sub = np.asarray(ids[o])
+            if sub.shape != (B, n_pts):
+                raise ValueError(f"predict_batch_many: ids[{o}] has shape {sub.shape}, not ({B}, {n_pts})")
+            if sub.min() < 0 or sub.max() >= xyz.shape[0]:
+                raise ValueError(f"predict_batch_many: ids[{o}] indexes outside the {xyz.shape[0]} points with "
+                                 f"z >= 0.1")
+            sub = sub.astype(np.int32)
+        out.append((xyz, nrm, poses.reshape(B, 4, 4), sub))
+    return out
+
+
 class GraspPredicter:
     """predicter.py:39-94."""
 
@@ -286,6 +385,126 @@ class GraspPredicter:
         if len(grasp_poses) == 0:
             return []
         return result_list(self.score(data, grasp_poses, ids=ids, subsample=subsample).cpu().numpy())
+
+    def score_many(self, datas, grasp_poses_list, ids=None, subsample=None):
+        """``score`` for several objects, each with its own cloud and candidate list, in one pass: (probs (sum B_o,
+        n_out) float32 CUDA tensor, offsets (O+1,) int64), object o's rows probs[offsets[o]:offsets[o+1]] equal bit for
+        bit to ``score(datas[o], grasp_poses_list[o], ids[o], subsample)`` in a loop over the objects that skips those
+        with no candidates (as predict_batch does), from the same numpy state, which it leaves where the loop would.
+
+        ``datas`` are numpy dicts, not modified; ``ids`` (optional) a list of per-object (B_o, n_pts) subsets.  The
+        random numbers are the loop's:
+          "host"   -- one walk of numpy's global generator over all objects' subsets, in object order, drawn on a
+                      worker thread stage by stage (about ``chunk`` candidates) while the GPU scores the previous stage;
+          "device" -- one np.random.randint seed per object with candidates, and one cg_draw_ids_many_dev launch.
+        The FC layers run on the loop's launches (graspq_fc_groups): host mode ``chunk`` candidates per launch, device
+        and given-ids modes the object's whole list, cut at GRASPQ_CHUNK_B.  The whole list is checked before anything
+        is drawn: on a ValueError numpy's generator is untouched.
+
+        On engines 2 and 3 the fp16-overflow flag belongs to the context: when it is set after the pass (or was set
+        before it, which the loop's first call would see), the objects are scored again one at a time from the ids on
+        the device, each on this predicter's engine and, where that object overflows, on engine 1, as the loop does."""
+        import torch
+        mode = subsample or self.subsample
+        assert mode in ("host", "device"), mode
+        n_pts = int(self.cfg["n_pts"])
+        objs = _check_grasp_many(datas, grasp_poses_list, ids, n_pts)
+        counts = [0 if ob is None else ob[2].shape[0] for ob in objs]
+        offsets = np.zeros(len(objs) + 1, np.int64)
+        offsets[1:] = np.cumsum(counts)
+        B_all = int(offsets[-1])
+        live = [o for o, ob in enumerate(objs) if ob is not None]
+        Ms = [0 if ob is None else ob[0].shape[0] for ob in objs]
+        bases = np.zeros(len(objs), np.int64)
+        bases[1:] = np.cumsum(Ms)[:-1]
+        if sum(Ms) >= 2 ** 31:
+            raise ValueError("predict_batch_many: 2^31 cloud points or more in all")
+        launch = self.chunk if (ids is None and mode == "host") else None
+        groups, spans = graspq_fc_groups(counts, launch)
+        net, dev, ctx = self.model, self.model.device, self.model.ctx
+        with torch.cuda.device(dev):
+            d_probs = torch.empty((B_all, net.n_out), dtype=torch.float32, device=dev)
+            if B_all == 0:
+                return d_probs, offsets
+            cat = lambda k: np.ascontiguousarray(np.concatenate([objs[o][k] for o in live]))
+            d_xyz, d_nrm, d_pose = (torch.from_numpy(cat(k)).to(dev) for k in (0, 1, 2))
+            d_mean = torch.from_numpy(np.ascontiguousarray(self.cfg["mean"].reshape(-1))).to(dev) if "mean" in self.cfg else None
+            d_std = torch.from_numpy(np.ascontiguousarray(self.cfg["std"].reshape(-1))).to(dev) if "std" in self.cfg else None
+
+            def forward(r0, r1, g0, g1, d_ids):
+                net.graspq_many_dev(d_xyz, d_nrm, d_pose[r0:r1], d_ids[r0:r1], groups[g0:g1], d_mean, d_std,
+                                    out=(d_probs[r0:r1], None))
+
+            whole = [(0, B_all, 0, len(groups))]
+            if ids is not None:
+                d_ids = torch.from_numpy(np.concatenate([objs[o][3] + np.int32(bases[o]) for o in live])).to(dev)
+                stages = iter(whole)
+            elif mode == "device":
+                seeds = [int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64)) for _ in live]
+                d_ids = net.draw_ids_many_dev([Ms[o] for o in live], n_pts, [counts[o] for o in live], seeds,
+                                              bases[live])
+                stages = iter(whole)
+            else:
+                h_ids = self._pinned_ids(B_all, n_pts)
+                d_ids = torch.empty((B_all, n_pts), dtype=torch.int32, device=dev)
+                row_base = torch.from_numpy(np.repeat(bases.astype(np.int32), counts)).to(dev)[:, None]
+                stages = self._host_stages(walk_grasp_many(Ms, counts, n_pts, host_draw_stages(groups, self.chunk),
+                                                           h_ids), h_ids, d_ids, row_base)
+            ctx_engine = ctx.get_engine()
+            ctx.set_engine(self.engine)         # the context (one per device) is shared: this predicter's engine, per call
+            try:
+                stale = self.engine >= 2 and ctx.fp16_overflow()
+                for r0, r1, g0, g1 in stages:
+                    forward(r0, r1, g0, g1, d_ids)
+                overflow = self.engine >= 2 and ctx.fp16_overflow()
+                for o in (live if overflow or stale else []):
+                    r0, r1, (g0, g1) = int(offsets[o]), int(offsets[o + 1]), spans[o]
+                    own = False
+                    if overflow:
+                        forward(r0, r1, g0, g1, d_ids)
+                        own = ctx.fp16_overflow()
+                    if own or (stale and o == live[0]):
+                        print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (wgmma bf16 "
+                              "hi/lo x3)")
+                        ctx.set_engine(1)
+                        forward(r0, r1, g0, g1, d_ids)
+                        ctx.set_engine(self.engine)
+            finally:
+                ctx.set_engine(ctx_engine)
+        return d_probs, offsets
+
+    def _host_stages(self, walk, h_ids, d_ids, row_base):
+        """Runs ``walk`` (walk_grasp_many) on a worker thread and yields its stages as they are drawn, each copied to
+        d_ids and rebased to the rows of the concatenated clouds (one add of row_base per stage)."""
+        import queue
+        import threading
+        q = queue.Queue()
+
+        def producer():
+            try:
+                for stage in walk:
+                    q.put(stage)
+                q.put(None)
+            except Exception as e:   # surfaces in the consumer
+                q.put(e)
+        t = threading.Thread(target=producer, daemon=True)
+        t.start()
+        while (item := q.get()) is not None:
+            if isinstance(item, Exception):
+                t.join()
+                raise item
+            r0, r1 = item[0], item[1]
+            d_ids[r0:r1].copy_(h_ids[r0:r1], non_blocking=True)
+            d_ids[r0:r1].add_(row_base[r0:r1])
+            yield item
+        t.join()
+
+    def predict_batch_many(self, datas, grasp_poses_list, ids=None, subsample=None):
+        """``[self.predict_batch(d, g) for d, g in zip(datas, grasp_poses_list)]`` (with ``ids[o]`` for object o), bit
+        for bit and with the same consumption of numpy's global generator: ``score_many`` and one copy to the host."""
+        probs, off = self.score_many(datas, grasp_poses_list, ids=ids, subsample=subsample)
+        host = probs.cpu().numpy()
+        return [result_list(host[off[o]:off[o + 1]]) if off[o + 1] > off[o] else [] for o in range(len(off) - 1)]
 
 
 def result_list(probs):

@@ -122,6 +122,26 @@ int cg_graspq_forward_dev(cg_net *net,
                           const double *mean, const double *std,
                           float *out_probs, int32_t *out_label);
 
+/* cg_graspq_forward_dev for the candidates of several objects in one call
+ * (GraspPredicter.score_many).  cloud_xyz, cloud_nrm: the objects' clouds
+ * concatenated, (M_total,3); poses (B_total,4,4); ids (B_total,N) already
+ * rebased to rows of the concatenation.  fc_groups (HOST, n_groups entries of
+ * 1 .. CG_GRASPQ_CHUNK_B rows, summing to B_total): consecutive row groups,
+ * each the candidates one cg_graspq_forward_dev launch covers; every group's
+ * FC layers take the kernel that call would take (the row count selects it),
+ * so row b of the result equals, bit for bit, the row of the call on its group
+ * alone.  The trunks run over whole groups in passes of at most
+ * CG_GRASPQ_CHUNK_B candidates; groups of at most 8 rows share one FC launch
+ * per layer.  out_probs (B_total,n_out), out_label (B_total,) or NULL.       */
+#define CG_GRASPQ_CHUNK_B 16384
+int cg_graspq_forward_many_dev(cg_net *net,
+                               const double *cloud_xyz, const double *cloud_nrm, int M_total,
+                               const double *poses, int B_total,
+                               const int32_t *ids, int N,
+                               const double *mean, const double *std,
+                               const int32_t *fc_groups /* host */, int n_groups,
+                               float *out_probs, int32_t *out_label);
+
 /* The per-candidate point-subset draw of GraspDataset.transform
  * (dataset_grasp.py:72-73: np.random.choice(np.arange(M), size=n_pts,
  * replace=(M < n_pts)) from the GLOBAL legacy numpy generator, once per
@@ -151,6 +171,16 @@ int cg_host_legacy_skip(uint32_t *key, int32_t *pos, int64_t M, int32_t n_pts, i
 int cg_host_rng_isa(int level);
 int cg_draw_ids_dev(cg_ctx *ctx, int M, int n_pts, int count, uint64_t seed,
                     int64_t first_candidate, int32_t *out_ids);
+/* cg_draw_ids_dev for n_obj objects in one launch.  Object o owns output rows
+ * row_offsets[o] .. row_offsets[o+1]-1 (row_offsets: n_obj+1 ascending int64,
+ * row_offsets[0] = 0, row_offsets[n_obj] = rows; an object may own none);
+ * its rows are cg_draw_ids_dev(M[o], n_pts, its row count, seed[o],
+ * first_candidate = 0) plus base[o] (the object's first row in a
+ * concatenation of the clouds).  M, seed, row_offsets, base: device arrays.
+ * out_ids: (rows, n_pts) int32 on device.                                    */
+int cg_draw_ids_many_dev(cg_ctx *ctx, int n_obj, const int32_t *M, const uint64_t *seed,
+                         const int64_t *row_offsets, const int32_t *base, int n_pts, int rows,
+                         int32_t *out_ids);
 
 /* PointNetCls / PointNetSeg forward on an already materialised input tensor
  * x : (B,N,6) float32 (device).  Replaces pointnet2.py:289-299 / :316-329.
