@@ -161,6 +161,8 @@ SIGNATURES = {
     "cg_meanshift_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_spconv_index_dev": (_i, [_vp, _D, _i, _D, _D, _D, _D], TORCH),
     "cg_spconv_down_dev": (_i, [_vp, _D, _D, _i, _H, _i, _D, _D, _D, _D, _D], TORCH),
+    "cg_spconv_index_many_dev": (_i, [_vp, _D, _i, _i, _H, _H, _D, _D, _D, _D, _D], TORCH),
+    "cg_spconv_down_many_dev": (_i, [_vp, _D, _D, _D, _i, _i, _H, _i, _D, _D, _D, _D, _D, _D], TORCH),
     "cg_spconv_conv_dev": (_i, [_vp, _D, _i, _D, _i, _D, _i, _D, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_pointgroup_voxel_mean_dev": (_i, [_vp, _D, _i, _i, _D, _D, _i, _D], TORCH),
     "cg_pointgroup_head_dev": (_i, [_vp, _D, _i, _D, _i, _D, _D, _D, _D, _D, _D, _D, _i, _D, _D], TORCH),

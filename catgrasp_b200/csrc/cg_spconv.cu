@@ -5,6 +5,13 @@
 // x << 42 | y << 21 | z and held in ascending key order: row-major over (x, y, z), z fastest.  The order of a level's
 // rows reaches no output of the network (every gather goes through a table), so key order is the contract.
 //
+// A batched level holds the sites of B > 1 frames, each on its own spatial shape S_b, with the frame above the
+// coordinates: key = b << 3w | x << 2w | y << w | z, where w is the smallest width with 2^w >= every S_b on every axis
+// and the frame field takes f = bit_length(B - 1) bits; f + 3w <= 63, else the batch is refused.  So a batched level is
+// its frames' one-frame levels one after another, frame b's rows starting at its row base (the sites of the frames
+// before it), and every table entry of frame b is the one-frame entry plus that base.  Neighbours are bounded by the
+// field, 2^w, so no coordinate carries into the next field.  With one frame the layout is the one above (f = 0,
+// w = 21), whatever the shape.
 // Every convolution is one gather table nbr[Vout][K] (input row or -1) and one weight array W[K][Cin][Cout]:
 //   out[r] = (sum_k W[k]^T act(in[nbr[r][k]]) + bias) + residual[r]
 // with act(v) = max(v * scale + shift, 0) per channel when a BN prologue is given, else v, and an absent (-1) row
@@ -20,7 +27,8 @@
 //
 // Table builds size every output from a row bound the caller gives, write the true count to a device word and never
 // synchronise, so a network forward needs no host round trip after the first level's count.  A coarse level's bound
-// is min(the finer level's rows, the cells of the coarse shape): every parent has a child and is a coarse cell.
+// is max(1, min(the finer level's rows, the cells of the coarse shapes summed over the frames)): every parent has a
+// child and is a coarse cell of its child's frame.
 #include <cub/cub.cuh>
 #include "cg_common.cuh"
 
@@ -34,26 +42,39 @@ constexpr int CT_R = 64;              // conv tile: output rows per CTA
 constexpr int CT_K = 32;              //            input channels per shared-memory stage
 constexpr int CT_THREADS = 256;       // 16 x 16 threads, 4 rows x NJ channels each (16 NJ channels per CTA)
 
-__host__ __device__ __forceinline__ uint64_t sp_key(int x, int y, int z) {
-  return ((uint64_t)x << (2 * SP_BITS)) | ((uint64_t)y << SP_BITS) | (uint64_t)z;
+// the key of site (x, y, z) of frame b in fields of w bits
+__host__ __device__ __forceinline__ uint64_t sp_key(int b, int x, int y, int z, int w) {
+  return ((uint64_t)b << (3 * w)) | ((uint64_t)x << (2 * w)) | ((uint64_t)y << w) | (uint64_t)z;
 }
-__device__ __forceinline__ int sp_coord(uint64_t key, int axis) {
-  return (int)((key >> (SP_BITS * (2 - axis))) & (SP_MAX - 1));
+__device__ __forceinline__ int sp_coord(uint64_t key, int axis, int w) {
+  return (int)((key >> (w * (2 - axis))) & ((1ull << w) - 1));
 }
 
 unsigned blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
-__global__ void point_key_kernel(const int32_t *__restrict__ coords, int N, uint64_t *__restrict__ key,
-                                 int32_t *__restrict__ val) {
+// each point's key; frame b's points are rows [off[b], off[b + 1]) of coords (off null: one frame)
+__global__ void point_key_kernel(const int32_t *__restrict__ coords, int N, const int32_t *__restrict__ off, int B,
+                                 int w, uint64_t *__restrict__ key, int32_t *__restrict__ val) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  key[i] = sp_key(coords[3 * (size_t)i], coords[3 * (size_t)i + 1], coords[3 * (size_t)i + 2]);
+  int b = 0;
+  if (off) {   // the last frame whose first row is <= i
+    int lo = 0, hi = B - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (off[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    b = lo;
+  }
+  key[i] = sp_key(b, coords[3 * (size_t)i], coords[3 * (size_t)i + 1], coords[3 * (size_t)i + 2], w);
   val[i] = i;
 }
 
-// parent key of every child row below *nvox whose parent lies inside the coarse shape (sx, sy, sz), else SP_NONE
-__global__ void parent_key_kernel(const int32_t *__restrict__ vox, const int32_t *__restrict__ nvox, int M, int sx,
-                                  int sy, int sz, uint64_t *__restrict__ key, int32_t *__restrict__ val) {
+// parent key of every child row below *nvox whose parent lies inside its frame's coarse shape cshape[3 b ..], else
+// SP_NONE; frame[v] is the child's frame (null: frame 0)
+__global__ void parent_key_kernel(const int32_t *__restrict__ vox, const int32_t *__restrict__ frame,
+                                  const int32_t *__restrict__ nvox, int M, const int32_t *__restrict__ cshape, int w,
+                                  uint64_t *__restrict__ key, int32_t *__restrict__ val) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= M) return;
   val[v] = v;
@@ -61,8 +82,10 @@ __global__ void parent_key_kernel(const int32_t *__restrict__ vox, const int32_t
     key[v] = SP_NONE;
     return;
   }
+  const int b = frame ? frame[v] : 0;
   const int px = vox[3 * (size_t)v] >> 1, py = vox[3 * (size_t)v + 1] >> 1, pz = vox[3 * (size_t)v + 2] >> 1;
-  key[v] = px < sx && py < sy && pz < sz ? sp_key(px, py, pz) : SP_NONE;
+  const int *cs = cshape + 3 * (size_t)b;
+  key[v] = px < cs[0] && py < cs[1] && pz < cs[2] ? sp_key(b, px, py, pz, w) : SP_NONE;
 }
 
 __global__ void head_kernel(const uint64_t *__restrict__ key, int M, int32_t *__restrict__ head) {
@@ -70,11 +93,12 @@ __global__ void head_kernel(const uint64_t *__restrict__ key, int M, int32_t *__
   if (j < M) head[j] = key[j] != SP_NONE && (j == 0 || key[j] != key[j - 1]) ? 1 : 0;
 }
 
-// sorted (key, row) pairs -> the level: its keys and sites in key order, its size, and each row's site (-1: none)
+// sorted (key, row) pairs -> the level: its keys, sites and frames (frame null: not written) in key order, its size,
+// and each row's site (-1: none)
 __global__ void emit_level_kernel(const uint64_t *__restrict__ key, const int32_t *__restrict__ row,
-                                  const int32_t *__restrict__ head, const int32_t *__restrict__ vid, int M,
-                                  uint64_t *__restrict__ vkey, int32_t *__restrict__ vox, int32_t *__restrict__ nvox,
-                                  int32_t *__restrict__ row_site) {
+                                  const int32_t *__restrict__ head, const int32_t *__restrict__ vid, int M, int w,
+                                  uint64_t *__restrict__ vkey, int32_t *__restrict__ vox, int32_t *__restrict__ frame,
+                                  int32_t *__restrict__ nvox, int32_t *__restrict__ row_site) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= M) return;
   if (j == M - 1) *nvox = vid[j] + head[j];
@@ -86,13 +110,14 @@ __global__ void emit_level_kernel(const uint64_t *__restrict__ key, const int32_
   row_site[row[j]] = v;
   if (head[j]) {
     vkey[v] = key[j];
-    for (int a = 0; a < 3; a++) vox[3 * (size_t)v + a] = sp_coord(key[j], a);
+    for (int a = 0; a < 3; a++) vox[3 * (size_t)v + a] = sp_coord(key[j], a, w);
+    if (frame) frame[v] = (int)(key[j] >> (3 * w));
   }
 }
 
-// nbr[v][k] for every (v, k) with v < M: the site at v + (kx-1, ky-1, kz-1) by binary search, -1 when absent or v is
-// past the level's size
-__global__ void nbr_kernel(const uint64_t *__restrict__ vkey, const int32_t *__restrict__ nvox, int M,
+// nbr[v][k] for every (v, k) with v < M: the site at v + (kx-1, ky-1, kz-1) of the same frame by binary search, -1 when
+// absent, outside the w-bit fields or v is past the level's size
+__global__ void nbr_kernel(const uint64_t *__restrict__ vkey, const int32_t *__restrict__ nvox, int M, int w,
                            int32_t *__restrict__ nbr) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= (int64_t)M * 27) return;
@@ -101,9 +126,11 @@ __global__ void nbr_kernel(const uint64_t *__restrict__ vkey, const int32_t *__r
   int found = -1;
   if (v < n) {
     const uint64_t key = vkey[v];
-    const int x = sp_coord(key, 0) + k / 9 - 1, y = sp_coord(key, 1) + k / 3 % 3 - 1, z = sp_coord(key, 2) + k % 3 - 1;
-    if (x >= 0 && y >= 0 && z >= 0 && x < SP_MAX && y < SP_MAX && z < SP_MAX) {
-      const uint64_t q = sp_key(x, y, z);
+    const int lim = 1 << w;
+    const int x = sp_coord(key, 0, w) + k / 9 - 1, y = sp_coord(key, 1, w) + k / 3 % 3 - 1,
+              z = sp_coord(key, 2, w) + k % 3 - 1;
+    if (x >= 0 && y >= 0 && z >= 0 && x < lim && y < lim && z < lim) {
+      const uint64_t q = sp_key((int)(key >> (3 * w)), x, y, z, w);
       int lo = 0, hi = n;
       while (lo < hi) {
         const int mid = (lo + hi) >> 1;
@@ -127,44 +154,122 @@ __global__ void pairs_kernel(const int32_t *__restrict__ vox, const int32_t *__r
   up[8 * (size_t)c + k] = p;
 }
 
-// sorted (key, row) pairs of M rows -> head flags, their scan, the level (at most Mout sites, the caller's bound) and
-// its neighbour table (Mout rows)
-int build_level(cg_ctx *ctx, const uint64_t *skey, const int32_t *srow, int M, int Mout, int32_t *head, int32_t *vid,
-                void *tmp, size_t tmp_bytes, uint64_t *vkey, int32_t *vox, int32_t *nvox, int32_t *row_site,
-                int32_t *nbr) {
+// sorted (key, row) pairs of M rows -> head flags, their scan, the level (at most Mout sites, the caller's bound; its
+// frames too when frame is given) and its neighbour table (Mout rows)
+int build_level(cg_ctx *ctx, const uint64_t *skey, const int32_t *srow, int M, int Mout, int w, int32_t *head,
+                int32_t *vid, void *tmp, size_t tmp_bytes, uint64_t *vkey, int32_t *vox, int32_t *frame,
+                int32_t *nvox, int32_t *row_site, int32_t *nbr) {
   cudaStream_t st = ctx->stream;
   head_kernel<<<blocks(M, 256), 256, 0, st>>>(skey, M, head);
   CG_LAUNCH_CHECK(ctx);
   size_t tb = tmp_bytes;
   CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp, tb, head, vid, M, st));
-  emit_level_kernel<<<blocks(M, 256), 256, 0, st>>>(skey, srow, head, vid, M, vkey, vox, nvox, row_site);
+  emit_level_kernel<<<blocks(M, 256), 256, 0, st>>>(skey, srow, head, vid, M, w, vkey, vox, frame, nvox, row_site);
   CG_LAUNCH_CHECK(ctx);
-  nbr_kernel<<<blocks((int64_t)Mout * 27, 256), 256, 0, st>>>(vkey, nvox, Mout, nbr);
+  nbr_kernel<<<blocks((int64_t)Mout * 27, 256), 256, 0, st>>>(vkey, nvox, Mout, w, nbr);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
 }
 
-// scratch of one level build over M rows
-struct LevelWs {
-  uint64_t *kA, *kB, *vkey;
-  int32_t *rA, *rB, *head, *vid;
-  void *tmp;
-  size_t tmp_bytes;
-};
+int bit_length(int v) {
+  int n = 0;
+  while (v >> n) n++;
+  return n;
+}
 
-int carve_level(cg_ctx *ctx, int M, LevelWs &w) {
+// The one table build behind cg_spconv_{index,down}_dev and their _many forms, for B frames on the host shapes
+// (3 per frame; null for a one-frame index, which needs no shape).  Checks its arguments before any launch.
+//   index (coords given): the M points coords, frame b's at rows [off[b], off[b + 1]) (off: host, null for one
+//     frame) -> the level of their sites in out_rows = M rows, out_p2v = each point's site
+//   down (vox given): the M rows of a level with *nvox sites, site v of frame frame[v] (null: one frame) -> the level
+//     of their parents in out_rows rows, out_down (out_rows,8) and out_up (M,8)
+// out_frame (null: not written) takes each site's frame.
+int spconv_tables(cg_ctx *ctx, const std::string &who, int B, const int32_t *shapes, const int32_t *off,
+                  const int32_t *coords, const int32_t *vox, const int32_t *frame, const int32_t *nvox, int M,
+                  int out_rows, int32_t *out_vox, int32_t *out_nvox, int32_t *out_frame, int32_t *out_nbr,
+                  int32_t *out_p2v, int32_t *out_down, int32_t *out_up) {
+  const bool down = vox != nullptr;
+  CG_REQUIRE(ctx, B >= 1, who + ": B must be >= 1");
+  // the key layout (file comment): one frame keeps f = 0, w = 21
+  int f = 0, w = SP_BITS, smax = 1;
+  if (shapes) {
+    for (int i = 0; i < 3 * B; i++) {
+      CG_REQUIRE(ctx, shapes[i] >= 1 && shapes[i] <= SP_MAX, who + ": shape must be in [1, 2^21] per axis");
+      smax = std::max(smax, shapes[i]);
+    }
+  }
+  if (B > 1) {
+    f = bit_length(B - 1);
+    w = bit_length(smax - 1);
+    CG_REQUIRE(ctx, f + 3 * w <= 63,
+               who + ": " + std::to_string(B) + " frames need " + std::to_string(f) + " frame bits and a largest "
+               "shape of " + std::to_string(smax) + " needs " + std::to_string(w) + " bits per axis; the key holds "
+               "f + 3 w <= 63");
+  }
+  std::vector<int32_t> cs;
+  if (down) {
+    // get_conv_output_size for k2 s2 p0, per frame; a parent has at least one child and is a cell of its frame
+    int64_t cells = 0;
+    cs.resize(3 * (size_t)B);
+    for (int b = 0; b < B; b++) {
+      int64_t n = 1;
+      for (int a = 0; a < 3; a++) {
+        const int S = shapes[3 * b + a];
+        cs[3 * b + a] = S >= 2 ? (S - 2) / 2 + 1 : 0;
+        n *= cs[3 * b + a];
+      }
+      cells += n;
+    }
+    CG_REQUIRE(ctx, out_rows >= std::max<int64_t>(1, std::min<int64_t>(M, cells)),
+               who + ": out_rows must be at least min(M, coarse cells) and >= 1");
+    CG_REQUIRE(ctx, out_rows <= (1 << 30) / 27, who + ": out_rows must be <= 2^30 / 27");
+  } else if (off) {
+    CG_REQUIRE(ctx, off[0] == 0 && off[B] == M, who + ": the frame offsets must run from 0 to N");
+    for (int b = 0; b < B; b++) CG_REQUIRE(ctx, off[b] <= off[b + 1], who + ": the frame offsets must not decrease");
+  }
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
   size_t sort_tmp = 0, scan_tmp = 0;
   CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (uint64_t *)nullptr, (uint64_t *)nullptr,
-                                               (int32_t *)nullptr, (int32_t *)nullptr, M, 0, 64, ctx->stream));
-  CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int32_t *)nullptr, (int32_t *)nullptr, M, ctx->stream));
-  w.tmp_bytes = std::max(sort_tmp, scan_tmp);
-  const size_t Mz = (size_t)M;
-  return cg_ws_carve(ctx, [&](cg_arena &ar) {
-    w.kA = ar.take<uint64_t>(Mz); w.kB = ar.take<uint64_t>(Mz); w.vkey = ar.take<uint64_t>(Mz);
-    w.rA = ar.take<int32_t>(Mz); w.rB = ar.take<int32_t>(Mz);
-    w.head = ar.take<int32_t>(Mz); w.vid = ar.take<int32_t>(Mz);
-    w.tmp = ar.take<char>(w.tmp_bytes);
+                                               (int32_t *)nullptr, (int32_t *)nullptr, M, 0, 64, st));
+  CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int32_t *)nullptr, (int32_t *)nullptr, M, st));
+  const size_t tmp_bytes = std::max(sort_tmp, scan_tmp), Mz = (size_t)M;
+  const size_t n_off = !down && off ? (size_t)B + 1 : 0;
+  uint64_t *kA, *kB, *vkey;
+  int32_t *rA, *rB, *head, *vid, *d_off, *d_cs;
+  void *tmp;
+  int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
+    kA = ar.take<uint64_t>(Mz); kB = ar.take<uint64_t>(Mz); vkey = ar.take<uint64_t>(Mz);
+    rA = ar.take<int32_t>(Mz); rB = ar.take<int32_t>(Mz);
+    head = ar.take<int32_t>(Mz); vid = ar.take<int32_t>(Mz);
+    tmp = ar.take<char>(tmp_bytes);
+    d_off = ar.take<int32_t>(n_off); d_cs = ar.take<int32_t>(cs.size());
   });
+  if (rc != CG_OK) return rc;
+  // the frame tables, from pageable memory: staged at once, no synchronisation
+  if (n_off) CG_CUDA(ctx, cudaMemcpyAsync(d_off, off, sizeof(int32_t) * n_off, cudaMemcpyHostToDevice, st));
+  if (down) CG_CUDA(ctx, cudaMemcpyAsync(d_cs, cs.data(), sizeof(int32_t) * cs.size(), cudaMemcpyHostToDevice, st));
+  size_t tb = tmp_bytes;
+  if (!down) {
+    point_key_kernel<<<blocks(M, 256), 256, 0, st>>>(coords, M, n_off ? d_off : nullptr, B, w, kA, rA);
+    CG_LAUNCH_CHECK(ctx);
+    CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp, tb, kA, kB, rA, rB, M, 0, f + 3 * w, st));
+    return build_level(ctx, kB, rB, M, M, w, head, vid, tmp, tmp_bytes, vkey, out_vox, out_frame, out_nvox, out_p2v,
+                       out_nbr);
+  }
+  parent_key_kernel<<<blocks(M, 256), 256, 0, st>>>(vox, frame, nvox, M, d_cs, w, kA, rA);
+  CG_LAUNCH_CHECK(ctx);
+  // all 64 bits: a dropped child's SP_NONE sorts after every parent key
+  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp, tb, kA, kB, rA, rB, M, 0, 64, st));
+  // rA is free after the sort: it takes each child's parent row (-1: dropped, or a row past *nvox)
+  rc = build_level(ctx, kB, rB, M, out_rows, w, head, vid, tmp, tmp_bytes, vkey, out_vox, out_frame, out_nvox, rA,
+                   out_nbr);
+  if (rc != CG_OK) return rc;
+  CG_CUDA(ctx, cudaMemsetAsync(out_down, 0xff, sizeof(int32_t) * 8 * (size_t)out_rows, st));
+  CG_CUDA(ctx, cudaMemsetAsync(out_up, 0xff, sizeof(int32_t) * 8 * Mz, st));
+  pairs_kernel<<<blocks(M, 256), 256, 0, st>>>(vox, rA, M, out_down, out_up);
+  CG_LAUNCH_CHECK(ctx);
+  return CG_OK;
 }
 
 // one output tile of CT_R rows x 16 NJ channels (NJ = 1, 2 or 4, picked from Cout so a narrow layer does not run
@@ -328,17 +433,21 @@ extern "C" int cg_spconv_index_dev(cg_ctx *ctx, const int32_t *coords, int N, in
   CG_REQUIRE(ctx, N >= 1, "spconv_index: N must be >= 1");
   CG_REQUIRE(ctx, N <= (1 << 30) / 27, "spconv_index: at most 2^30 / 27 points (the neighbour table's int32 index)");
   CG_REQUIRE(ctx, coords && out_vox && out_nvox && out_p2v && out_nbr, "spconv_index: null argument");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  LevelWs w;
-  const int rc = carve_level(ctx, N, w);
-  if (rc != CG_OK) return rc;
-  cudaStream_t st = ctx->stream;
-  point_key_kernel<<<blocks(N, 256), 256, 0, st>>>(coords, N, w.kA, w.rA);
-  CG_LAUNCH_CHECK(ctx);
-  size_t tb = w.tmp_bytes;
-  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.kA, w.kB, w.rA, w.rB, N, 0, 3 * SP_BITS, st));
-  return build_level(ctx, w.kB, w.rB, N, N, w.head, w.vid, w.tmp, w.tmp_bytes, w.vkey, out_vox, out_nvox, out_p2v,
-                     out_nbr);
+  return spconv_tables(ctx, "spconv_index", 1, nullptr, nullptr, coords, nullptr, nullptr, nullptr, N, N, out_vox,
+                       out_nvox, nullptr, out_nbr, out_p2v, nullptr, nullptr);
+}
+
+extern "C" int cg_spconv_index_many_dev(cg_ctx *ctx, const int32_t *coords, int N, int B, const int32_t *offsets,
+                                        const int32_t *shapes, int32_t *out_vox, int32_t *out_nvox,
+                                        int32_t *out_frame, int32_t *out_p2v, int32_t *out_nbr) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, N >= 1, "spconv_index_many: N must be >= 1");
+  CG_REQUIRE(ctx, N <= (1 << 30) / 27,
+             "spconv_index_many: at most 2^30 / 27 points (the neighbour table's int32 index)");
+  CG_REQUIRE(ctx, coords && offsets && shapes && out_vox && out_nvox && out_frame && out_p2v && out_nbr,
+             "spconv_index_many: null argument");
+  return spconv_tables(ctx, "spconv_index_many", B, shapes, offsets, coords, nullptr, nullptr, nullptr, N, N, out_vox,
+                       out_nvox, out_frame, out_nbr, out_p2v, nullptr, nullptr);
 }
 
 extern "C" int cg_spconv_down_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *nvox, int M, const int32_t *shape,
@@ -348,35 +457,20 @@ extern "C" int cg_spconv_down_dev(cg_ctx *ctx, const int32_t *vox, const int32_t
   CG_REQUIRE(ctx, M >= 1 && M <= (1 << 30) / 27, "spconv_down: M must be in [1, 2^30 / 27]");
   CG_REQUIRE(ctx, vox && nvox && shape && out_vox && out_nvox && out_nbr && out_down && out_up,
              "spconv_down: null argument");
-  int cs[3];
-  int64_t cells = 1;
-  for (int a = 0; a < 3; a++) {
-    CG_REQUIRE(ctx, shape[a] >= 1 && shape[a] <= SP_MAX, "spconv_down: shape must be in [1, 2^21] per axis");
-    cs[a] = shape[a] >= 2 ? (shape[a] - 2) / 2 + 1 : 0;   // get_conv_output_size for k2 s2 p0
-    cells *= cs[a];
-  }
-  // a parent has at least one child and is a cell of the coarse shape
-  CG_REQUIRE(ctx, out_rows >= std::max<int64_t>(1, std::min<int64_t>(M, cells)),
-             "spconv_down: out_rows must be at least min(M, coarse cells) and >= 1");
-  CG_REQUIRE(ctx, out_rows <= (1 << 30) / 27, "spconv_down: out_rows must be <= 2^30 / 27");
-  CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  LevelWs w;
-  int rc = carve_level(ctx, M, w);
-  if (rc != CG_OK) return rc;
-  cudaStream_t st = ctx->stream;
-  parent_key_kernel<<<blocks(M, 256), 256, 0, st>>>(vox, nvox, M, cs[0], cs[1], cs[2], w.kA, w.rA);
-  CG_LAUNCH_CHECK(ctx);
-  size_t tb = w.tmp_bytes;
-  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.kA, w.kB, w.rA, w.rB, M, 0, 64, st));
-  // rA is free after the sort: it takes each child's parent row (-1: dropped, or a row past *nvox)
-  rc = build_level(ctx, w.kB, w.rB, M, out_rows, w.head, w.vid, w.tmp, w.tmp_bytes, w.vkey, out_vox, out_nvox, w.rA,
-                   out_nbr);
-  if (rc != CG_OK) return rc;
-  CG_CUDA(ctx, cudaMemsetAsync(out_down, 0xff, sizeof(int32_t) * 8 * (size_t)out_rows, st));
-  CG_CUDA(ctx, cudaMemsetAsync(out_up, 0xff, sizeof(int32_t) * 8 * (size_t)M, st));
-  pairs_kernel<<<blocks(M, 256), 256, 0, st>>>(vox, w.rA, M, out_down, out_up);
-  CG_LAUNCH_CHECK(ctx);
-  return CG_OK;
+  return spconv_tables(ctx, "spconv_down", 1, shape, nullptr, nullptr, vox, nullptr, nvox, M, out_rows, out_vox,
+                       out_nvox, nullptr, out_nbr, nullptr, out_down, out_up);
+}
+
+extern "C" int cg_spconv_down_many_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *frame, const int32_t *nvox,
+                                       int M, int B, const int32_t *shapes, int out_rows, int32_t *out_vox,
+                                       int32_t *out_nvox, int32_t *out_frame, int32_t *out_nbr, int32_t *out_down,
+                                       int32_t *out_up) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, M >= 1 && M <= (1 << 30) / 27, "spconv_down_many: M must be in [1, 2^30 / 27]");
+  CG_REQUIRE(ctx, vox && frame && nvox && shapes && out_vox && out_nvox && out_frame && out_nbr && out_down && out_up,
+             "spconv_down_many: null argument");
+  return spconv_tables(ctx, "spconv_down_many", B, shapes, nullptr, nullptr, vox, frame, nvox, M, out_rows, out_vox,
+                       out_nvox, out_frame, out_nbr, nullptr, out_down, out_up);
 }
 
 extern "C" int cg_spconv_conv_dev(cg_ctx *ctx, const float *in, int Cin, const int32_t *nbr, int K,

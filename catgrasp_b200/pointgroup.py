@@ -5,7 +5,8 @@ head (PointGroup/model/pointgroup/pointgroup.py, ``PointGroup.forward`` up to ``
 features to the per-point offsets (N,3) float32.  The level pyramid is built once (``spconv.index``, then six
 ``spconv.down``); after ``index`` nothing synchronises: every layer runs through ``cg_spconv_conv_dev`` on tables the
 forward built itself, so the gather-table check of the public ``spconv.conv`` (one synchronisation per call) is not
-needed.  The score / proposal branch never runs at inference (``epoch = prepare_epochs - 1``) and is not built.
+needed.  A batched level (``spconv.index_many``, several frames) runs through the same calls, and each frame's offsets
+equal its one-frame forward's bit for bit.  The score / proposal branch never runs at inference (``epoch = prepare_epochs - 1``) and is not built.
 
 Wiring, per level with C channels (UBlock):
   blocks: block_reps ResidualBlocks  x + SubM3(BN2 ReLU . SubM3(BN1 ReLU x))      (SubM k1 with bias on x when the

@@ -979,8 +979,8 @@ class PointGroupPredictor:
                 raise NotImplementedError(f"PointGroupPredictor: {key} = {c.get(key)!r}; only the shipped {key} = "
                                           f"{want!r} is implemented")
         if self.n_slice_per_side != 1:
-            raise NotImplementedError("PointGroupPredictor: n_slice_per_side must be 1 (the site tables hold one "
-                                      "batch)")
+            raise NotImplementedError("PointGroupPredictor: n_slice_per_side must be 1 (only whole frames are "
+                                      "batched)")
         if int(c["block_reps"]) not in (1, 2):
             raise NotImplementedError(f"PointGroupPredictor: block_reps = {c['block_reps']}; only 1 and 2 build")
 
@@ -1040,6 +1040,56 @@ class PointGroupPredictor:
             labels_all, xyz_shifted = labels_all.cpu().numpy(), xyz_shifted.cpu().numpy()
         self.xyz_shifted = xyz_shifted
         return labels_all
+
+    def predict_many(self, datas):
+        """predict for a list of frames: ``[self.predict(d) for d in datas]`` bit for bit, numpy labels for numpy input
+        and CUDA tensors for CUDA input, with self.xyz_shifted left as the loop leaves it (the last frame's).
+
+        The front (device_front) runs per frame, so each frame keeps its own spatial shape.  The network then runs
+        once over all frames: one batched spconv.index_many (its one synchronisation) and pyramid, one voxel mean, one
+        U-Net forward and one offset head, with no synchronisation after the index.  The offsets are split by frame
+        and pointgroup_labels runs per frame.
+
+        The whole list is checked first: ValueError for an empty list, mixed numpy / CUDA frames, or a frame whose
+        'cloud_xyz' and 'cloud_normal' are not both (M,3) with M >= 1; a frame without one of them gets predict's
+        KeyError.  A rejected call does no device work and leaves self.xyz_shifted untouched."""
+        import torch
+        from . import spconv
+        from .segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
+        datas = list(datas)
+        cuda_in = self._check_many(datas)
+        fronts = [self.device_front(d) for d in datas]
+        level, p2v = spconv.index_many([f[1] for f in fronts], [f[3] for f in fronts])
+        off = self.model.offsets(level, p2v, torch.cat([f[2] for f in fronts]))
+        out, bw, start = [], MEANSHIFT_BANDWIDTH[self.class_name], 0
+        for data, (xo, locs, _, _) in zip(datas, fronts):
+            labels_all, xyz_shifted = pointgroup_labels(xo, off[start:start + len(locs)], data["cloud_xyz"], bw)
+            start += len(locs)
+            if not cuda_in:
+                labels_all, xyz_shifted = labels_all.cpu().numpy(), xyz_shifted.cpu().numpy()
+            out.append(labels_all)
+        self.xyz_shifted = xyz_shifted
+        return out
+
+    @staticmethod
+    def _check_many(datas):
+        """predict_many's checks, before any device work: whether the frames are CUDA tensors."""
+        import torch
+        if not datas:
+            raise ValueError("predict_many: no frames")
+        kinds = set()
+        for b, d in enumerate(datas):
+            xyz, nrm = d["cloud_xyz"], d["cloud_normal"]                  # predict's KeyError for a missing array
+            for a in (xyz, nrm):
+                kinds.add("cuda" if isinstance(a, torch.Tensor) and a.is_cuda else
+                          "numpy" if isinstance(a, np.ndarray) else type(a).__name__)
+            if len(kinds) > 1 or not kinds <= {"cuda", "numpy"}:
+                raise ValueError(f"predict_many: the frames must be all numpy arrays or all CUDA tensors, got "
+                                 f"{sorted(kinds)}")
+            if len(xyz.shape) != 2 or xyz.shape[1] != 3 or xyz.shape[0] == 0 or tuple(nrm.shape) != tuple(xyz.shape):
+                raise ValueError(f"predict_many: frame {b} has cloud_xyz {tuple(xyz.shape)} and cloud_normal "
+                                 f"{tuple(nrm.shape)}; both must be (M,3) with M >= 1")
+        return kinds == {"cuda"}
 
 
 def _float_dtype(a):

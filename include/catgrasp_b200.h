@@ -549,6 +549,28 @@ int  cg_spconv_index_dev(cg_ctx *ctx, const int32_t *coords, int N, int32_t *out
 int  cg_spconv_down_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *nvox, int M, const int32_t *shape /* host */,
                         int out_rows, int32_t *out_vox, int32_t *out_nvox, int32_t *out_nbr, int32_t *out_down,
                         int32_t *out_up);
+/* Batched levels: the sites of B frames, each on its own spatial shape, in one level.  Key layout: a site (x, y, z)
+ * of frame b is the key b << 3w | x << 2w | y << w | z, and a level holds its sites in ascending key order, so frame
+ * by frame and, within a frame, in the (x, y, z) order above.  Width rule: w is the smallest width with 2^w >= every
+ * frame's shape on every axis, the frame field takes f = bit_length(B - 1) bits, and f + 3w must be <= 63, else
+ * CG_EINVAL with a message (a key is never wrapped); B = 1 keeps the one-frame layout (f = 0, w = 21).  Neighbours
+ * and parents stay inside their frame's fields.  Frame b's rows are [base_b, base_b + n_b), base_b the sites of the
+ * frames before it, and its sites, count n_b and every table entry equal the one-frame call's on frame b alone, plus
+ * base_b (-1 stays -1).
+ * cg_spconv_index_many_dev: coords (N,3) the frames' points concatenated, frame b's at rows
+ * [offsets[b], offsets[b + 1]) (host, B + 1, from 0 to N), each in [0, shapes[3 b + axis]) (not checked); shapes
+ * (host, B x 3) each in [1, 2^21].  Outputs as cg_spconv_index_dev's, and out_frame (N capacity) = each site's frame;
+ * out_p2v names the batched rows.                                                                                 */
+int  cg_spconv_index_many_dev(cg_ctx *ctx, const int32_t *coords, int N, int B, const int32_t *offsets /* host */,
+                              const int32_t *shapes /* host */, int32_t *out_vox, int32_t *out_nvox,
+                              int32_t *out_frame, int32_t *out_p2v, int32_t *out_nbr);
+/* cg_spconv_down_dev on a batched level: vox (M,3) and frame (M) its sites and their frames, shapes (host, B x 3) the
+ * frames' spatial shapes.  Each child is dropped against its own frame's coarse shape (S_b - 2) / 2 + 1.  Row bound:
+ * out_rows >= max(1, min(M, the coarse shapes' cell counts summed over the frames)), else CG_EINVAL; it is a bound
+ * only, the true count goes to out_nvox.  out_frame (out_rows capacity) = each parent's frame.                     */
+int  cg_spconv_down_many_dev(cg_ctx *ctx, const int32_t *vox, const int32_t *frame, const int32_t *nvox, int M, int B,
+                             const int32_t *shapes /* host */, int out_rows, int32_t *out_vox, int32_t *out_nvox,
+                             int32_t *out_frame, int32_t *out_nbr, int32_t *out_down, int32_t *out_up);
 /* out (M,Cout) rows r < *nout: (sum over k, then input channel, of W[k][ci][co] * act(in[nbr[r][k]][ci]) + bias[co])
  * + residual[r][co], one fp32 FMA chain per output, so two runs are bitwise equal.  in (rows,Cin); nbr (M,K), or NULL
  * with K = 1 for the 1x1 convolution (row r reads row r); W (K,Cin,Cout) as spconv stores (k..., Cin, Cout).  act(v) =
