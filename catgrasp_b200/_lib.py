@@ -152,13 +152,18 @@ SIGNATURES = {
     "cg_grasp_affordance_dev": (_i, [_vp, _D, _i, _D, _D, _D, _i, _H, _H, _i, _d, _D, _D], TORCH),
     "cg_depth2xyz_dev": (_i, [_vp, _D, _i, _i, _i, _H, _D], TORCH),
     "cg_cloud_index_create": (_i, [_vp, _D, _i, _d, _H], TORCH),
+    "cg_cloud_index_create_many": (_i, [_vp, _D, _H, _i, _d, _H], TORCH),
     "cg_cloud_index_destroy": (None, [_vp], None),
     "cg_cloud_index_info": (_i, [_vp, _H, _H, _H, _H], None),
+    "cg_cloud_index_sets": (_i, [_vp, _H, _H], None),
+    "cg_cloud_index_tables_dev": (_i, [_vp, _D, _D, _D, _D], TORCH),
     "cg_voxel_down_sample_dev": (_i, [_vp, _D, _D, _D], TORCH),
     "cg_cloud_nearest_dev": (_i, [_vp, _D, _i, _d, _D, _D], TORCH),
+    "cg_cloud_nearest_many_dev": (_i, [_vp, _D, _H, _i, _d, _D, _D], TORCH),
     "cg_cloud_radius_mask_dev": (_i, [_vp, _D, _i, _d, _i, _D], TORCH),
     "cg_cloud_normals_dev": (_i, [_vp, _d, _i, _H, _D, _D, _D], TORCH),
     "cg_meanshift_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
+    "cg_meanshift_many_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_spconv_index_dev": (_i, [_vp, _D, _i, _D, _D, _D, _D], TORCH),
     "cg_spconv_down_dev": (_i, [_vp, _D, _D, _i, _H, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_spconv_index_many_dev": (_i, [_vp, _D, _i, _i, _H, _H, _D, _D, _D, _D, _D], TORCH),

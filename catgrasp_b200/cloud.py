@@ -15,22 +15,48 @@ import torch
 from . import _lib
 
 
+def _offsets(off, n, what):
+    """``off`` as an int32 numpy array of S + 1 >= 2 ascending offsets from 0 to n; ValueError otherwise."""
+    o = np.asarray(off, dtype=np.int64).reshape(-1)
+    if len(o) < 2 or o[0] != 0 or o[-1] != n or (np.diff(o) < 0).any():
+        raise ValueError(f"{what}: need S + 1 >= 2 ascending offsets from 0 to {n}, got {o.tolist()}")
+    return o.astype(np.int32)
+
+
 class CloudIndex:
     """Points binned into cells of size ``cell`` (origin min_bound - cell/2) and sorted by (cell, index); built once
-    and shared by every query on the same cloud and cell size.  Holds its own copy of the points."""
+    and shared by every query on the same cloud and cell size.  Holds its own copy of the points.
 
-    def __init__(self, pts, cell, device=None):
+    With ``set_offsets`` (S + 1 ints from 0 to the point count) the points are S sets laid end to end, set s the rows
+    [set_offsets[s], set_offsets[s + 1]), each binned as a one-set index over it alone would bin it (its own origin);
+    ``cell_offsets`` then gives each set's cells, ``voxel_means`` comes out set-major and ``nearest_many`` searches
+    each query's own set.  A set with no points raises ValueError; a batch whose cell keys need more than 63 bits
+    raises CgError.  ``nearest``, ``within`` and ``normals`` need a one-set index."""
+
+    def __init__(self, pts, cell, device=None, set_offsets=None):
         self.ctx, p = _lib.inputs(pts, dtype=torch.float64, ctx=None if device is None else _lib.Context.get(device))
         p = p.reshape(-1, 3)
         self.device = self.ctx.device
         if p.shape[0] == 0:
             raise ValueError("CloudIndex needs at least one point")
         h = C.c_void_p()
-        self.ctx.call("cg_cloud_index_create", self.ctx.h, p, p.shape[0], float(cell), C.byref(h))
+        if set_offsets is None:
+            self.ctx.call("cg_cloud_index_create", self.ctx.h, p, p.shape[0], float(cell), C.byref(h))
+        else:
+            off = _offsets(set_offsets, p.shape[0], "CloudIndex")
+            if (np.diff(off) < 1).any():
+                raise ValueError(f"CloudIndex: every set needs at least one point, got offsets {off.tolist()}")
+            self.ctx.call("cg_cloud_index_create_many", self.ctx.h, p, off, len(off) - 1, float(cell), C.byref(h))
         self.h = h
-        n, u = C.c_int(), C.c_int()
+        n, u, S = C.c_int(), C.c_int(), C.c_int()
         self.ctx.call("cg_cloud_index_info", h, C.byref(n), C.byref(u), None, None)
         self.n_points, self.n_cells = n.value, u.value
+        self.ctx.call("cg_cloud_index_sets", h, C.byref(S), None)
+        self.n_sets = S.value
+        coff = np.zeros(self.n_sets + 1, np.int32)
+        self.ctx.call("cg_cloud_index_sets", h, None, coff)
+        self.set_offsets = np.array([0, self.n_points]) if set_offsets is None else off.astype(np.int64)
+        self.cell_offsets = coff.astype(np.int64)     # set s's cells (and voxel means): [cell_offsets[s], [s + 1])
 
     def __del__(self):
         h = getattr(self, "h", None)
@@ -57,6 +83,18 @@ class CloudIndex:
         idx = self._empty(q.shape[0], dtype=torch.int32)
         dist = self._empty(q.shape[0])
         self.ctx.call("cg_cloud_nearest_dev", self.h, q, q.shape[0], float(max_dist), idx, dist)
+        return dist, idx
+
+    def nearest_many(self, query, query_offsets, max_dist):
+        """nearest per set: the queries [query_offsets[s], query_offsets[s + 1]) search set s only.  (dists (Q,)
+        float64, indices (Q,) int32 into the whole index, -1 / inf where set s has no point within max_dist)."""
+        q = self._query(query)
+        off = _offsets(query_offsets, q.shape[0], "CloudIndex.nearest_many")
+        if len(off) != self.n_sets + 1:
+            raise ValueError(f"CloudIndex.nearest_many: {len(off) - 1} query ranges for {self.n_sets} sets")
+        idx = self._empty(q.shape[0], dtype=torch.int32)
+        dist = self._empty(q.shape[0])
+        self.ctx.call("cg_cloud_nearest_many_dev", self.h, q, off, q.shape[0], float(max_dist), idx, dist)
         return dist, idx
 
     def within(self, query, r, compare_sqrt):

@@ -10,6 +10,14 @@
 // Nothing depends on atomic arrival order: the results are a function of the inputs alone.  The index structure and
 // its query helpers are in cg_cloud_index.cuh, shared with cg_meanshift.cu.
 //
+// A many-set index (cg_cloud_index_create_many) holds S point sets laid end to end, each with what a one-set index
+// over it alone has: its own bounds, so its own origin (its min_bound - cell/2), its own largest cells and the 2^21
+// cell limit per axis.  Every set shares `cell`.  A key is s << 3b | x << 2b | y << b | z: b is the smallest width that
+// holds every set's largest cell, and the set field takes bit_length(S - 1) bits; a batch whose key needs more than
+// 63 bits is refused.  So the sorted points, the cell table and the voxel means are set-major, and set s's block is its
+// one-set index shifted by its first point (perm, start) and carrying its prefix (keys).  S = 1 is today's layout.  A
+// query of set s searches set s's cells only (IndexView::in_set); the build synchronises twice whatever S is.
+//
 // Decisions are float64 with the reference's operation order and no FMA contraction:
 //   d2 = (dx*dx + dy*dy) + dz*dz     scipy's sqeuclidean_distance_double (cKDTree.query, query_ball_point)
 // and a cell range is widened by 1e-6 cells on each side, far more than the rounding of (q - origin +- R) / cell for
@@ -25,10 +33,14 @@ namespace {
 
 constexpr int BT = 256;
 
-// per block: min xyz, max xyz, and 1.0 when a coordinate is not finite
-__global__ void __launch_bounds__(BT) bounds_kernel(const double *__restrict__ pts, int P, double *__restrict__ part) {
+// per block: min xyz, max xyz, and 1.0 when a coordinate is not finite.  Blocks [s * nbs, (s + 1) * nbs) cover set s,
+// the points [off[s], off[s + 1]) (off null: one set, the P points)
+__global__ void __launch_bounds__(BT) bounds_kernel(const double *__restrict__ pts, int P, const int32_t *__restrict__ off,
+                                                    int nbs, double *__restrict__ part) {
   double v[7] = {INFINITY, INFINITY, INFINITY, -INFINITY, -INFINITY, -INFINITY, 0.0};
-  for (int i = blockIdx.x * BT + threadIdx.x; i < P; i += gridDim.x * BT) {
+  const int s = off ? blockIdx.x / nbs : 0, c = blockIdx.x - s * nbs;
+  const int lo = off ? off[s] : 0, hi = off ? off[s + 1] : P;
+  for (int i = lo + c * BT + threadIdx.x; i < hi; i += nbs * BT) {
     for (int a = 0; a < 3; a++) {
       const double x = pts[3 * (size_t)i + a];
       if (!isfinite(x)) v[6] = 1.0;
@@ -54,19 +66,29 @@ __global__ void __launch_bounds__(BT) bounds_kernel(const double *__restrict__ p
   }
 }
 
+// block s: set s's bounds from its nb partials
 __global__ void __launch_bounds__(BT) bounds_final_kernel(const double *__restrict__ part, int nb, double *__restrict__ out) {
   if (threadIdx.x >= 7) return;
   const int a = threadIdx.x;
-  double x = part[a];
-  for (int b = 1; b < nb; b++) x = (a < 3) ? fmin(x, part[(size_t)b * 7 + a]) : fmax(x, part[(size_t)b * 7 + a]);
-  out[a] = x;
+  const double *p = part + (size_t)blockIdx.x * nb * 7;
+  double x = p[a];
+  for (int b = 1; b < nb; b++) x = (a < 3) ? fmin(x, p[(size_t)b * 7 + a]) : fmax(x, p[(size_t)b * 7 + a]);
+  out[(size_t)blockIdx.x * 7 + a] = x;
 }
 
+// sets null: one set with origin (ox, oy, oz); else point i's set from off, with that set's origin and prefix
 __global__ void key_kernel(const double *__restrict__ pts, int P, double ox, double oy, double oz, double cell, int bits,
+                           const CloudSet *__restrict__ sets, const int32_t *__restrict__ off, int S,
                            uint64_t *__restrict__ keys, int32_t *__restrict__ vals) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= P) return;
-  keys[i] = cell_key(pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2], ox, oy, oz, cell, bits);
+  uint64_t prefix = 0;
+  if (sets) {
+    const int s = set_of(off, S, i);
+    ox = sets[s].o[0]; oy = sets[s].o[1]; oz = sets[s].o[2];
+    prefix = (uint64_t)s << (3 * bits);
+  }
+  keys[i] = prefix | cell_key(pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2], ox, oy, oz, cell, bits);
   vals[i] = i;
 }
 
@@ -75,21 +97,25 @@ __global__ void head_flag_kernel(const uint64_t *__restrict__ keys, int P, int32
   if (j < P) flag[j] = (j == 0 || keys[j] != keys[j - 1]) ? 1 : 0;
 }
 
-// cell table and the points in key order; cid = exclusive scan of the head flags
+// cell table and the points in key order; cid = exclusive scan of the head flags.  coff (S+1): each set's first cell
+// (set = key >> sh; every set has a point, so a cell), coff[S] = U
 __global__ void table_kernel(const uint64_t *__restrict__ keys, const int32_t *__restrict__ perm, const int32_t *__restrict__ cid,
-                             const double *__restrict__ pts, int P, uint64_t *__restrict__ ukey, int32_t *__restrict__ start,
-                             double *__restrict__ spts, int *__restrict__ U) {
+                             const double *__restrict__ pts, int P, int sh, uint64_t *__restrict__ ukey,
+                             int32_t *__restrict__ start, double *__restrict__ spts, int *__restrict__ U,
+                             int32_t *__restrict__ coff) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= P) return;
   const bool head = j == 0 || keys[j] != keys[j - 1];
   if (head) {
     ukey[cid[j]] = keys[j];
     start[cid[j]] = j;
+    if (j == 0 || (keys[j] >> sh) != (keys[j - 1] >> sh)) coff[keys[j] >> sh] = cid[j];
   }
   if (j == P - 1) {                       // cells = heads before the last point, plus the last point if it is one
     const int u = cid[j] + (head ? 1 : 0);
     start[u] = P;
     *U = u;
+    coff[(keys[j] >> sh) + 1] = u;
   }
   const size_t o = 3 * (size_t)perm[j];
   spts[3 * (size_t)j] = pts[o];
@@ -136,10 +162,13 @@ __global__ void voxel_kernel(IndexView V, const double *__restrict__ nrm, double
 
 // ---- nearest point within a bound (cKDTree.query) ----------------------------------------------------------------
 
-__global__ void nearest_kernel(IndexView V, const double *__restrict__ q, int Q, double max_dist, int32_t *__restrict__ out_idx,
-                               double *__restrict__ out_dist) {
+// qoff null: every query searches the whole (one-set) index; else the queries [qoff[s], qoff[s + 1]) search set s
+// only, and the answer is the point's index in the whole index (set s's first point plus its index in the set)
+__global__ void nearest_kernel(IndexView V0, const int32_t *__restrict__ qoff, const double *__restrict__ q, int Q,
+                               double max_dist, int32_t *__restrict__ out_idx, double *__restrict__ out_dist) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= Q) return;
+  const IndexView V = qoff ? V0.in_set(set_of(qoff, V0.S, i)) : V0;
   const double qx = q[3 * (size_t)i], qy = q[3 * (size_t)i + 1], qz = q[3 * (size_t)i + 2];
   double best = INFINITY;
   int bi = 0x7fffffff;
@@ -413,78 +442,167 @@ extern "C" int cg_depth2xyz_dev(cg_ctx *ctx, const void *depth, int depth_is_f64
   return CG_OK;
 }
 
-extern "C" int cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, double cell, cg_cloud_index **out) {
-  if (!ctx) return CG_EINVAL;
+namespace {
+
+int bit_length(int v) {
+  int n = 0;
+  while (v >> n) n++;
+  return n;
+}
+
+// The one build behind cg_cloud_index_create (off null: one set of P points) and cg_cloud_index_create_many (S sets,
+// set s the points [off[s], off[s + 1]) of pts, off on the host).  Synchronises twice: the bounds, then the cells.
+int cloud_index_build(cg_ctx *ctx, const double *pts, int P, const int32_t *off, int S, double cell, cg_cloud_index **out) {
+  const bool many = off != nullptr;
   CG_REQUIRE(ctx, pts && out && P > 0, "cloud_index: null argument or no points");
   CG_REQUIRE(ctx, cell > 0.0 && std::isfinite(cell), "cloud_index: cell size must be positive and finite");
+  if (many) {
+    CG_REQUIRE(ctx, off[0] == 0 && off[S] == P, "cloud_index: the set offsets must run from 0 to the point count");
+    for (int s = 0; s < S; s++) CG_REQUIRE(ctx, off[s] < off[s + 1], "cloud_index: every set needs at least one point");
+  }
   *out = nullptr;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const int nb = (int)std::min<int64_t>(blocks(P, BT), 2 * (int64_t)ctx->num_sms);
-  // workspace: bounds partials | keys in/out | vals | head flags | scanned ids | U | CUB temp
+  const int nbs = std::max(1, nb / S);   // bounds blocks per set; one set keeps nb
+  const size_t Sz = (size_t)S;
+  // workspace: bounds partials | keys in/out | vals | head flags | scanned ids | U and the cell offsets | set offsets
+  // (many sets) | CUB temp
   size_t sort_tmp = 0, scan_tmp = 0;
   CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (uint64_t *)nullptr, (uint64_t *)nullptr, (int32_t *)nullptr,
                                                (int32_t *)nullptr, P, 0, 3 * MAX_AXIS_BITS, ctx->stream));
   CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int32_t *)nullptr, (int32_t *)nullptr, P, ctx->stream));
   const size_t tmp = std::max(sort_tmp, scan_tmp);
-  double *part; uint64_t *kin, *kout; int32_t *vin, *flag, *cid, *dU; void *dtmp;
+  double *part; uint64_t *kin, *kout; int32_t *vin, *flag, *cid, *dU, *doff; void *dtmp;
   int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
-    part = ar.take<double>(7 * (size_t)nb + 7);
+    part = ar.take<double>(7 * ((size_t)nbs * Sz + Sz));
     kin = ar.take<uint64_t>(P); kout = ar.take<uint64_t>(P);
     vin = ar.take<int32_t>(P); flag = ar.take<int32_t>(P); cid = ar.take<int32_t>(P);
-    dU = ar.take<int32_t>(1);
+    dU = ar.take<int32_t>(Sz + 2);
+    doff = ar.take<int32_t>(many ? Sz + 1 : 0);
     dtmp = ar.take<char>(tmp);
   });
   if (rc != CG_OK) return rc;
-  double *bnd = part + 7 * (size_t)nb;
+  double *bnd = part + 7 * (size_t)nbs * Sz;
+  // the set offsets, from pageable memory: staged at once, no synchronisation
+  if (many) CG_CUDA(ctx, cudaMemcpyAsync(doff, off, sizeof(int32_t) * (Sz + 1), cudaMemcpyHostToDevice, ctx->stream));
 
-  bounds_kernel<<<nb, BT, 0, ctx->stream>>>(pts, P, part);
+  bounds_kernel<<<nbs * S, BT, 0, ctx->stream>>>(pts, P, many ? doff : nullptr, nbs, part);
   CG_LAUNCH_CHECK(ctx);
-  bounds_final_kernel<<<1, BT, 0, ctx->stream>>>(part, nb, bnd);
+  bounds_final_kernel<<<S, BT, 0, ctx->stream>>>(part, nbs, bnd);
   CG_LAUNCH_CHECK(ctx);
-  double hb[7];
-  CG_CUDA(ctx, cudaMemcpyAsync(hb, bnd, sizeof(hb), cudaMemcpyDeviceToHost, ctx->stream));
+  std::vector<double> hb(7 * Sz);
+  CG_CUDA(ctx, cudaMemcpyAsync(hb.data(), bnd, sizeof(double) * hb.size(), cudaMemcpyDeviceToHost, ctx->stream));
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  CG_REQUIRE(ctx, hb[6] == 0.0, "cloud_index: a coordinate is NaN or infinite");
 
   cg_cloud_index ix;   // goes to the heap only when every step below has succeeded
   ix.ctx = ctx;
   ix.P = P;
   ix.cell = cell;
+  ix.S = S;
+  ix.sets.resize(Sz);
+  ix.set_hi.resize(3 * Sz);
   int64_t maxc = 0;
+  for (int s = 0; s < S; s++) {
+    const double *h = &hb[7 * (size_t)s];
+    CG_REQUIRE(ctx, h[6] == 0.0, "cloud_index: a coordinate is NaN or infinite");
+    for (int a = 0; a < 3; a++) {
+      const double o = h[a] - cell * 0.5;                               // open3d: min_bound - voxel_size * 0.5
+      const double top = floor((h[3 + a] - o) / cell);                  // the largest point's cell (floor is monotone)
+      CG_REQUIRE(ctx, top < (double)(1 << MAX_AXIS_BITS),
+                 "cloud_index: the cloud spans 2^21 or more cells on an axis; use a larger cell");
+      ix.sets[s].o[a] = o;
+      ix.sets[s].mc[a] = (int64_t)top;
+      ix.set_hi[3 * (size_t)s + a] = h[3 + a];
+      maxc = std::max(maxc, ix.sets[s].mc[a]);
+    }
+  }
   for (int a = 0; a < 3; a++) {
-    ix.origin[a] = hb[a] - cell * 0.5;                               // open3d: min_bound - voxel_size * 0.5
-    ix.hi[a] = hb[3 + a];
-    const double top = floor((hb[3 + a] - ix.origin[a]) / cell);     // the largest point's cell (floor is monotone)
-    CG_REQUIRE(ctx, top < (double)(1 << MAX_AXIS_BITS),
-               "cloud_index: the cloud spans 2^21 or more cells on an axis; use a larger cell");
-    ix.maxc[a] = (int64_t)top;
-    maxc = std::max(maxc, ix.maxc[a]);
+    ix.origin[a] = ix.sets[0].o[a];
+    ix.hi[a] = ix.set_hi[a];
+    ix.maxc[a] = ix.sets[0].mc[a];
   }
   int bits = 1;
   while ((int64_t(1) << bits) <= maxc) bits++;
   ix.bits = bits;
+  const int set_bits = bit_length(S - 1), key_bits = set_bits + 3 * bits;
+  CG_REQUIRE(ctx, key_bits <= 63,
+             "cloud_index: " + std::to_string(S) + " sets need " + std::to_string(set_bits) + " set bits and the "
+             "largest set spans " + std::to_string(maxc + 1) + " cells, " + std::to_string(bits) + " bits per axis; "
+             "the key holds set bits + 3 * bits <= 63");
+  ix.poff = many ? std::vector<int32_t>(off, off + S + 1) : std::vector<int32_t>{0, P};
+  // the set table and the set offsets (many sets) live behind the sorted points, in one allocation
+  const size_t pts_bytes = sizeof(double) * 3 * (size_t)P;
+  const size_t set_bytes = many ? sizeof(CloudSet) * Sz + sizeof(int32_t) * (Sz + 1) : 0;
   DevBuf spts, perm, ukey, start;
-  if ((rc = dev_alloc(ctx, spts, sizeof(double) * 3 * (size_t)P))) return rc;
+  if ((rc = dev_alloc(ctx, spts, pts_bytes + set_bytes))) return rc;
   if ((rc = dev_alloc(ctx, perm, sizeof(int32_t) * (size_t)P))) return rc;
   if ((rc = dev_alloc(ctx, ukey, sizeof(uint64_t) * (size_t)P))) return rc;
   if ((rc = dev_alloc(ctx, start, sizeof(int32_t) * ((size_t)P + 1)))) return rc;
   ix.spts = static_cast<double *>(spts.p); ix.perm = static_cast<int32_t *>(perm.p);
   ix.ukey = static_cast<uint64_t *>(ukey.p); ix.start = static_cast<int32_t *>(start.p);
+  if (many) {
+    CloudSet *d_sets = reinterpret_cast<CloudSet *>(static_cast<char *>(spts.p) + pts_bytes);
+    int32_t *d_poff = reinterpret_cast<int32_t *>(d_sets + S);
+    CG_CUDA(ctx, cudaMemcpyAsync(d_sets, ix.sets.data(), sizeof(CloudSet) * Sz, cudaMemcpyHostToDevice, ctx->stream));
+    CG_CUDA(ctx, cudaMemcpyAsync(d_poff, off, sizeof(int32_t) * (Sz + 1), cudaMemcpyHostToDevice, ctx->stream));
+    ix.d_sets = d_sets;
+    ix.d_poff = d_poff;
+  }
 
-  key_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(pts, P, ix.origin[0], ix.origin[1], ix.origin[2], cell, bits, kin, vin);
+  key_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(pts, P, ix.origin[0], ix.origin[1], ix.origin[2], cell, bits,
+                                                      ix.d_sets, many ? doff : nullptr, S, kin, vin);
   CG_LAUNCH_CHECK(ctx);
   size_t tb = tmp;
-  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(dtmp, tb, kin, kout, vin, ix.perm, P, 0, 3 * bits, ctx->stream));
+  CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(dtmp, tb, kin, kout, vin, ix.perm, P, 0, key_bits, ctx->stream));
   head_flag_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, P, flag);
   CG_LAUNCH_CHECK(ctx);
   tb = tmp;
   CG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(dtmp, tb, flag, cid, P, ctx->stream));
-  table_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, ix.perm, cid, pts, P, ix.ukey, ix.start, ix.spts, dU);
+  table_kernel<<<blocks(P, 256), 256, 0, ctx->stream>>>(kout, ix.perm, cid, pts, P, 3 * bits, ix.ukey, ix.start, ix.spts,
+                                                        dU, dU + 1);
   CG_LAUNCH_CHECK(ctx);
-  CG_CUDA(ctx, cudaMemcpyAsync(&ix.U, dU, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  std::vector<int32_t> hu(Sz + 2);
+  CG_CUDA(ctx, cudaMemcpyAsync(hu.data(), dU, sizeof(int32_t) * hu.size(), cudaMemcpyDeviceToHost, ctx->stream));
   CG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  ix.U = hu[0];
+  ix.coff.assign(hu.begin() + 1, hu.end());
   spts.release(); perm.release(); ukey.release(); start.release();   // owned by the index now
-  *out = new cg_cloud_index(ix);
+  *out = new cg_cloud_index(std::move(ix));
+  return CG_OK;
+}
+
+}  // namespace
+
+extern "C" int cg_cloud_index_create(cg_ctx *ctx, const double *pts, int P, double cell, cg_cloud_index **out) {
+  if (!ctx) return CG_EINVAL;
+  return cloud_index_build(ctx, pts, P, nullptr, 1, cell, out);
+}
+
+extern "C" int cg_cloud_index_create_many(cg_ctx *ctx, const double *pts, const int32_t *set_offsets, int S, double cell,
+                                          cg_cloud_index **out) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, set_offsets && S >= 1, "cloud_index_many: null set offsets or S < 1");
+  return cloud_index_build(ctx, pts, set_offsets[S], set_offsets, S, cell, out);
+}
+
+extern "C" int cg_cloud_index_sets(const cg_cloud_index *ix, int *out_sets, int32_t *out_cell_offsets) {
+  if (!ix) return CG_EINVAL;
+  if (out_sets) *out_sets = ix->S;
+  if (out_cell_offsets) std::copy(ix->coff.begin(), ix->coff.end(), out_cell_offsets);
+  return CG_OK;
+}
+
+extern "C" int cg_cloud_index_tables_dev(const cg_cloud_index *ix, double *out_pts, int32_t *out_perm,
+                                         uint64_t *out_keys, int32_t *out_start) {
+  if (!ix) return CG_EINVAL;
+  cg_ctx *ctx = ix->ctx;
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t P = (size_t)ix->P, U = (size_t)ix->U;
+  if (out_pts) CG_CUDA(ctx, cudaMemcpyAsync(out_pts, ix->spts, sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (out_perm) CG_CUDA(ctx, cudaMemcpyAsync(out_perm, ix->perm, sizeof(int32_t) * P, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (out_keys) CG_CUDA(ctx, cudaMemcpyAsync(out_keys, ix->ukey, sizeof(uint64_t) * U, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (out_start)
+    CG_CUDA(ctx, cudaMemcpyAsync(out_start, ix->start, sizeof(int32_t) * (U + 1), cudaMemcpyDeviceToDevice, ctx->stream));
   return CG_OK;
 }
 
@@ -523,11 +641,39 @@ extern "C" int cg_cloud_nearest_dev(const cg_cloud_index *ix, const double *quer
                                     double *out_dist) {
   if (!ix) return CG_EINVAL;
   cg_ctx *ctx = ix->ctx;
+  CG_REQUIRE(ctx, ix->S == 1, "cloud_nearest: the index holds several sets; use cg_cloud_nearest_many_dev");
   CG_REQUIRE(ctx, Q >= 0 && (Q == 0 || (query && out_idx && out_dist)), "cloud_nearest: bad arguments");   // empty: NULL allowed
   CG_REQUIRE(ctx, max_dist >= 0.0 && std::isfinite(max_dist), "cloud_nearest: max_dist must be finite and >= 0");
   if (Q == 0) return CG_OK;
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
-  nearest_kernel<<<blocks(Q, 128), 128, 0, ctx->stream>>>(view_of(ix), query, Q, max_dist, out_idx, out_dist);
+  nearest_kernel<<<blocks(Q, 128), 128, 0, ctx->stream>>>(view_of(ix), nullptr, query, Q, max_dist, out_idx, out_dist);
+  CG_LAUNCH_CHECK(ctx);
+  return CG_OK;
+}
+
+extern "C" int cg_cloud_nearest_many_dev(const cg_cloud_index *ix, const double *query, const int32_t *query_offsets, int Q,
+                                         double max_dist, int32_t *out_idx, double *out_dist) {
+  if (!ix) return CG_EINVAL;
+  cg_ctx *ctx = ix->ctx;
+  const int S = ix->S;
+  CG_REQUIRE(ctx, query_offsets, "cloud_nearest_many: null query offsets");
+  CG_REQUIRE(ctx, Q >= 0 && (Q == 0 || (query && out_idx && out_dist)), "cloud_nearest_many: bad arguments");
+  CG_REQUIRE(ctx, query_offsets[0] == 0 && query_offsets[S] == Q,
+             "cloud_nearest_many: the query offsets must run from 0 to Q, one range per set");
+  for (int s = 0; s < S; s++)
+    CG_REQUIRE(ctx, query_offsets[s] <= query_offsets[s + 1], "cloud_nearest_many: the query offsets must not decrease");
+  CG_REQUIRE(ctx, max_dist >= 0.0 && std::isfinite(max_dist), "cloud_nearest_many: max_dist must be finite and >= 0");
+  if (Q == 0) return CG_OK;
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  int32_t *qoff = nullptr;
+  if (S > 1) {
+    const int rc = cg_ws_carve(ctx, [&](cg_arena &ar) { qoff = ar.take<int32_t>((size_t)S + 1); });
+    if (rc != CG_OK) return rc;
+    // from pageable memory: staged at once, no synchronisation
+    CG_CUDA(ctx, cudaMemcpyAsync(qoff, query_offsets, sizeof(int32_t) * ((size_t)S + 1), cudaMemcpyHostToDevice,
+                                 ctx->stream));
+  }
+  nearest_kernel<<<blocks(Q, 128), 128, 0, ctx->stream>>>(view_of(ix), qoff, query, Q, max_dist, out_idx, out_dist);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
 }
@@ -536,6 +682,7 @@ extern "C" int cg_cloud_radius_mask_dev(const cg_cloud_index *ix, const double *
                                         uint8_t *out_mask) {
   if (!ix) return CG_EINVAL;
   cg_ctx *ctx = ix->ctx;
+  CG_REQUIRE(ctx, ix->S == 1, "cloud_radius_mask: the index holds several sets, and the queries carry none");
   CG_REQUIRE(ctx, Q >= 0 && (Q == 0 || (query && out_mask)), "cloud_radius_mask: bad arguments");   // empty: NULL allowed
   CG_REQUIRE(ctx, r >= 0.0 && std::isfinite(r), "cloud_radius_mask: r must be finite and >= 0");
   if (Q == 0) return CG_OK;
@@ -549,6 +696,7 @@ extern "C" int cg_cloud_normals_dev(const cg_cloud_index *ix, double radius, int
                                     double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count) {
   if (!ix) return CG_EINVAL;
   cg_ctx *ctx = ix->ctx;
+  CG_REQUIRE(ctx, ix->S == 1, "cloud_normals: the index holds several sets; normals are per one-set index");
   CG_REQUIRE(ctx, view_point && out_normals, "cloud_normals: null argument");
   CG_REQUIRE(ctx, radius >= 0.0 && std::isfinite(radius), "cloud_normals: radius must be finite and >= 0");
   CG_REQUIRE(ctx, max_nn >= 1 && max_nn <= CG_CLOUD_MAX_NN, "cloud_normals: 1 <= max_nn <= CG_CLOUD_MAX_NN");

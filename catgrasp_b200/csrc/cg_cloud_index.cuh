@@ -2,7 +2,14 @@
 // every source that searches a cloud (cg_cloud.cu, cg_meanshift.cu, cg_ransac.cu).  See cg_cloud.cu for the index's layout.
 #pragma once
 #include <cmath>
+#include <vector>
 #include "cg_common.cuh"
+
+// one set of a many-set index: its origin, its largest occupied cell per axis
+struct CloudSet {
+  double o[3];
+  int64_t mc[3];
+};
 
 struct cg_cloud_index {
   cg_ctx *ctx = nullptr;
@@ -16,6 +23,15 @@ struct cg_cloud_index {
   int32_t *perm = nullptr;     // (P) original index of each sorted point
   uint64_t *ukey = nullptr;    // (U) ascending unique keys
   int32_t *start = nullptr;    // (U+1) first sorted point of each cell; start[U] = P
+  // the sets (cg_cloud_index_create_many; one set otherwise): set s holds points [poff[s], poff[s+1]) in the caller's
+  // order and in key order, and cells [coff[s], coff[s+1]); its keys carry the prefix s << 3 bits.  origin, hi and
+  // maxc above are set 0's.  The device copies exist only when S > 1.
+  int S = 1;
+  std::vector<int32_t> poff, coff;          // host, S+1 each
+  std::vector<double> set_hi;               // host, (S,3): each set's max_bound
+  std::vector<CloudSet> sets;               // host, S
+  const CloudSet *d_sets = nullptr;         // device (S), inside the spts allocation
+  const int32_t *d_poff = nullptr;          // device (S+1), inside the spts allocation
 };
 
 namespace {
@@ -31,11 +47,35 @@ struct IndexView {
   int U, bits;
   double cell, ox, oy, oz;
   int64_t mx, my, mz;
+  uint64_t prefix;         // the set field of every key this view searches (0 for a one-set index)
+  const CloudSet *sets;    // a many-set index's table (S > 1), else null
+  const int32_t *poff;     // (S+1) its point offsets, else null
+  int S;
+
+  // the view of set s alone: its origin, its cell range and its key prefix, so a query sees only set s's cells
+  __device__ __forceinline__ IndexView in_set(int s) const {
+    IndexView v = *this;
+    const CloudSet &r = sets[s];
+    v.ox = r.o[0]; v.oy = r.o[1]; v.oz = r.o[2];
+    v.mx = r.mc[0]; v.my = r.mc[1]; v.mz = r.mc[2];
+    v.prefix = (uint64_t)s << (3 * bits);
+    return v;
+  }
 };
 
 inline IndexView view_of(const cg_cloud_index *ix) {
   return IndexView{ix->spts, ix->perm, ix->ukey, ix->start, ix->U, ix->bits, ix->cell, ix->origin[0], ix->origin[1],
-                   ix->origin[2], ix->maxc[0], ix->maxc[1], ix->maxc[2]};
+                   ix->origin[2], ix->maxc[0], ix->maxc[1], ix->maxc[2], 0ull, ix->d_sets, ix->d_poff, ix->S};
+}
+
+// the s with off[s] <= i < off[s + 1] (off ascending, every range non-empty, 0 <= i < off[S])
+__device__ __forceinline__ int set_of(const int32_t *off, int S, int i) {
+  int lo = 0, hi = S;
+  while (hi - lo > 1) {
+    const int m = (lo + hi) >> 1;
+    if (off[m] <= i) lo = m; else hi = m;
+  }
+  return lo;
 }
 
 __device__ __forceinline__ double dist2(double ax, double ay, double az, double bx, double by, double bz) {
@@ -84,18 +124,27 @@ __device__ __forceinline__ int upper_bound(const uint64_t *a, int lo, int hi, ui
   return lo;
 }
 
-// The cell range of a query: per (x, y) column, the contiguous run [s, e) of sorted points in cells z_lo..z_hi.
+// The cell range of a query: per (x, y) column, the contiguous run [s, e) of sorted points in cells z_lo..z_hi.  The
+// range is clamped to the view's largest cells, below 2^bits, so a column's keys never carry into the next set's.
 struct Columns {
   int64_t x0, x1, y0, y1, z0, z1;
   bool any;
-  __device__ Columns(const IndexView &V, double qx, double qy, double qz, double R) {
+  __device__ __forceinline__ Columns(const IndexView &V, double qx, double qy, double qz, double R) {
     any = axis_range(qx, V.ox, R, V.cell, V.mx, x0, x1) && axis_range(qy, V.oy, R, V.cell, V.my, y0, y1) &&
           axis_range(qz, V.oz, R, V.cell, V.mz, z0, z1);
   }
+  // as above, with the origin and cell range of `r` when it is not null (a set's row the caller keeps in shared memory,
+  // read axis by axis where it is used, so a long-lived query holds no registers for it)
+  __device__ __forceinline__ Columns(const IndexView &V, const volatile CloudSet *r, double qx, double qy, double qz,
+                                     double R) {
+    any = axis_range(qx, r ? r->o[0] : V.ox, R, V.cell, r ? r->mc[0] : V.mx, x0, x1) &&
+          axis_range(qy, r ? r->o[1] : V.oy, R, V.cell, r ? r->mc[1] : V.my, y0, y1) &&
+          axis_range(qz, r ? r->o[2] : V.oz, R, V.cell, r ? r->mc[2] : V.mz, z0, z1);
+  }
   // the occupied cells [a, b) of column (cx, cy), as positions in the cell table
   __device__ __forceinline__ void cells(const IndexView &V, int64_t cx, int64_t cy, int &a, int &b) const {
-    a = lower_bound(V.ukey, 0, V.U, pack(cx, cy, z0, V.bits));
-    b = upper_bound(V.ukey, a, V.U, pack(cx, cy, z1, V.bits));
+    a = lower_bound(V.ukey, 0, V.U, V.prefix | pack(cx, cy, z0, V.bits));
+    b = upper_bound(V.ukey, a, V.U, V.prefix | pack(cx, cy, z1, V.bits));
   }
   __device__ __forceinline__ void run(const IndexView &V, int64_t cx, int64_t cy, int &s, int &e) const {
     int a, b;

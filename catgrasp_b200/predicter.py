@@ -1017,6 +1017,64 @@ class PointGroupPredictor:
         feats = torch.cat([no.to(torch.float32), xo.to(torch.float32)], 1)
         return xo.to(torch.float32), locs, feats, shape
 
+    def device_front_many(self, datas):
+        """device_front for several frames in one pass: (xyz_original_all (N,3) float32, locs (N,3) int64, feats
+        (N,6) float32) CUDA tensors with the frames laid end to end, the B spatial shapes, and the row offsets (B + 1)
+        numpy, frame b at rows [offsets[b], offsets[b + 1]).  Frame b's rows, shape and offsets equal device_front of
+        frame b alone, bit for bit.  One keep-mask nonzero for all frames, one 0.5 mm index, one snap index, one snap
+        check and one read of every frame's shape: the synchronisations do not grow with the number of frames."""
+        import torch
+        from .cloud import CloudIndex
+        from . import _lib
+        self._check_structure()
+        datas = list(datas)
+        dev = self.model.ctx.device
+        xs, ns = [], []
+        for d in datas:
+            _, xyz, nrm = _lib.inputs(d["cloud_xyz"], d["cloud_normal"], ctx=self.model.ctx,
+                                      dtype=tuple(_float_dtype(a) for a in (d["cloud_xyz"], d["cloud_normal"])))
+            xs.append(xyz)
+            ns.append(nrm)
+        B = len(xs)
+        masks = [slice_keep_mask(x) for x in xs]
+        counts = torch.stack([m.sum() for m in masks]).cpu().numpy()                  # one synchronisation
+        keep = torch.nonzero_static(torch.cat(masks), size=int(counts.sum())).reshape(-1)
+        xdt = xs[0].dtype if len({x.dtype for x in xs}) == 1 else torch.float64      # float32 widens exactly
+        ndt = ns[0].dtype if len({n.dtype for n in ns}) == 1 else torch.float64
+        xo = torch.cat([x.to(xdt) for x in xs])[keep]
+        no = torch.cat([n.to(ndt) for n in ns])[keep]
+        ds = float(self.cfg["downsample_size"])
+        index = CloudIndex(xo, ds, dev, set_offsets=np.cumsum(np.r_[0, counts]))
+        down, _ = index.voxel_means()
+        row_off = index.cell_offsets
+        snap = ds * np.sqrt(3.0) * (1 + 1e-9)                 # as device_front
+        _, ids = CloudIndex(xo, snap, dev, set_offsets=index.set_offsets).nearest_many(down, row_off, snap)
+        del index
+        if bool((ids < 0).any()):
+            raise _lib.CgError("PointGroupPredictor: a voxel mean has no point within its voxel's diagonal")
+        ids = ids.to(torch.int64)
+        xo, no = xo[ids], no[ids]
+        # the sites per frame in the frame's own dtype: trunc(fl(fl(x * scale) - the frame's min))
+        fid = torch.repeat_interleave(torch.arange(B, device=xo.device), torch.from_numpy(np.diff(row_off)).to(xo.device))
+        rows = list(zip(row_off[:-1].tolist(), row_off[1:].tolist()))
+        scale = self.cfg_pg["scale"]
+
+        def sites(x):
+            s = x * scale
+            lo = torch.stack([s[a:e].amin(0) for a, e in rows])       # per frame, no synchronisation
+            return (s - lo[fid]).to(torch.int64)                         # truncation, as torch's .long() on the host
+        dts = [x.dtype for x in xs]
+        if len(set(dts)) == 1:
+            locs = sites(xo)
+        else:
+            f32 = torch.tensor([t == torch.float32 for t in dts], device=xo.device)[fid]
+            locs = torch.where(f32[:, None], sites(xo.to(torch.float32)), sites(xo.to(torch.float64)))
+        hi = (torch.stack([locs[a:e].amax(0) for a, e in rows]) + 1).cpu().numpy()       # one read of every shape
+        fs = int(self.cfg_pg["full_scale"][0])
+        shapes = [tuple(int(v) for v in np.maximum(h, fs)) for h in hi]
+        feats = torch.cat([no.to(torch.float32), xo.to(torch.float32)], 1)
+        return xo.to(torch.float32), locs, feats, shapes, row_off
+
     def host_front(self, data):
         """device_front with numpy results: (xyz_original_all (N,3) float32, locs (N,3) int64, feats (N,6) float32,
         spatial_shape (3 ints))."""
@@ -1045,30 +1103,33 @@ class PointGroupPredictor:
         """predict for a list of frames: ``[self.predict(d) for d in datas]`` bit for bit, numpy labels for numpy input
         and CUDA tensors for CUDA input, with self.xyz_shifted left as the loop leaves it (the last frame's).
 
-        The front (device_front) runs per frame, so each frame keeps its own spatial shape.  The network then runs
-        once over all frames: one batched spconv.index_many (its one synchronisation) and pyramid, one voxel mean, one
-        U-Net forward and one offset head, with no synchronisation after the index.  The offsets are split by frame
-        and pointgroup_labels runs per frame.
+        The front runs once over all frames (device_front_many), and each frame keeps its own spatial shape.  The
+        network then runs once over all frames: one batched spconv.index_many (its one synchronisation) and pyramid,
+        one voxel mean, one U-Net forward and one offset head, with no synchronisation after the index.  The
+        clustering runs once over all frames too (segment.pointgroup_labels_many's device form), so the index builds
+        and synchronisations of the whole call do not grow with the number of frames.
 
         The whole list is checked first: ValueError for an empty list, mixed numpy / CUDA frames, or a frame whose
         'cloud_xyz' and 'cloud_normal' are not both (M,3) with M >= 1; a frame without one of them gets predict's
         KeyError.  A rejected call does no device work and leaves self.xyz_shifted untouched."""
         import torch
-        from . import spconv
-        from .segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
+        from . import _lib, spconv
+        from .segment import MEANSHIFT_BANDWIDTH, _pointgroup_labels_cat
         datas = list(datas)
         cuda_in = self._check_many(datas)
-        fronts = [self.device_front(d) for d in datas]
-        level, p2v = spconv.index_many([f[1] for f in fronts], [f[3] for f in fronts])
-        off = self.model.offsets(level, p2v, torch.cat([f[2] for f in fronts]))
-        out, bw, start = [], MEANSHIFT_BANDWIDTH[self.class_name], 0
-        for data, (xo, locs, _, _) in zip(datas, fronts):
-            labels_all, xyz_shifted = pointgroup_labels(xo, off[start:start + len(locs)], data["cloud_xyz"], bw)
-            start += len(locs)
-            if not cuda_in:
-                labels_all, xyz_shifted = labels_all.cpu().numpy(), xyz_shifted.cpu().numpy()
-            out.append(labels_all)
-        self.xyz_shifted = xyz_shifted
+        xo, locs, feats, shapes, row_off = self.device_front_many(datas)
+        level, p2v = spconv.index_many(locs, shapes, row_off)
+        off = self.model.offsets(level, p2v, feats)
+        _, *clouds = _lib.inputs(*[d["cloud_xyz"] for d in datas], ctx=self.model.ctx, dtype=torch.float64)
+        cloud_off = np.cumsum([0] + [len(c) for c in clouds])
+        labels, shifted, sh_off = _pointgroup_labels_cat(xo, off, row_off, torch.cat(clouds), cloud_off,
+                                                         MEANSHIFT_BANDWIDTH[self.class_name])
+        if not cuda_in:
+            labels = labels.cpu().numpy()
+        out = [labels[cloud_off[b]:cloud_off[b + 1]] for b in range(len(datas))]
+        out = out if not cuda_in else [o.contiguous() for o in out]
+        xyz_shifted = shifted[sh_off[-2]:sh_off[-1]].contiguous()
+        self.xyz_shifted = xyz_shifted if cuda_in else xyz_shifted.cpu().numpy()
         return out
 
     @staticmethod

@@ -57,6 +57,63 @@ def _nearest(ref, query, reach):
     return idx.to(torch.int64)
 
 
+def _nearest_many(ref, ref_off, query, query_off, reach):
+    """_nearest per set (ref, query: float64 device tensors, set s the rows [off[s], off[s + 1]) of each, every ref
+    set non-empty): the index into ref of each query's nearest point of its own set, ties to the smaller index.  One
+    index build for the whole batch, and at most one more, shared by every set, for the queries with nothing within
+    `reach`; its bound, the diagonal of the box around every set's points and those queries, covers each set's own."""
+    _, idx = CloudIndex(ref, _query_cell(ref, reach), ref.device.index, set_offsets=ref_off).nearest_many(
+        query, query_off, reach)
+    miss = torch.nonzero(idx < 0).reshape(-1)
+    if miss.numel():
+        q = query[miss]
+        miss_off = np.searchsorted(miss.cpu().numpy(), np.asarray(query_off), side="left")
+        span = torch.maximum(ref.amax(0), q.amax(0)) - torch.minimum(ref.amin(0), q.amin(0))
+        bound = float(torch.linalg.norm(span)) * (1 + 1e-9)
+        _, far = CloudIndex(ref, _query_cell(ref, bound), ref.device.index, set_offsets=ref_off).nearest_many(
+            q, miss_off, bound)
+        if bool((far < 0).any()):
+            raise _lib.CgError("nearest: a query found no point within the joint bounding box's diagonal")
+        idx[miss] = far
+    return idx.to(torch.int64)
+
+
+def _set_ids(off, device):
+    """(N,) int64 device tensor: the set of each row, for offsets off (S + 1 host ints)."""
+    off = np.asarray(off, dtype=np.int64)
+    return torch.repeat_interleave(torch.arange(len(off) - 1, device=device),
+                                   torch.from_numpy(np.diff(off)).to(device))
+
+
+def _fit_many(x, off, bw, max_iter):
+    """MeanShift per set on the device: x (N,3) float32 / float64 CUDA, set s the rows [off[s], off[s + 1]).  Returns
+    (centres set-major, centre offsets (S + 1) numpy, labels (N,) int64 per set, n_iter (S,) numpy, seed centres,
+    seed counts (N,) int64, seed iterations (N,) int64).  Synchronises once after the clustering, once more in the
+    labelling (twice when a point has no centre within LABEL_REACH bandwidths)."""
+    ctx = _lib.Context.get(x.device.index)
+    f64 = x.dtype == torch.float64
+    off = np.asarray(off, dtype=np.int64)
+    S = len(off) - 1
+    index = CloudIndex(x, bw, x.device.index, set_offsets=off)
+    P = x.shape[0]
+    seed_c = torch.empty_like(x)
+    seed_n = torch.empty((P,), dtype=torch.int32, device=x.device)
+    seed_it = torch.empty_like(seed_n)
+    cen = torch.empty_like(x)
+    coff = torch.empty((S + 1,), dtype=torch.int32, device=x.device)
+    ctx.call("cg_meanshift_many_dev", index.h, x, int(f64), float(bw), int(max_iter), seed_c, seed_n, seed_it, cen,
+             coff)
+    n_iter = torch.stack([seed_it[a:b].amax() for a, b in zip(off[:-1].tolist(), off[1:].tolist())])
+    host = torch.cat([coff, n_iter]).cpu().numpy().astype(np.int64)                  # one synchronisation
+    coff_h, n_iter = host[:S + 1], host[S + 1:]
+    if (np.diff(coff_h) < 1).any():
+        raise ValueError("CloudIndex needs at least one point")                        # as fit: a set with no centre
+    centres = cen[:int(coff_h[-1])].contiguous()
+    labels = _nearest_many(centres.to(torch.float64), coff_h, x.to(torch.float64), off, LABEL_REACH * bw)
+    labels = labels - torch.from_numpy(coff_h[:-1]).to(x.device)[_set_ids(off, x.device)]
+    return centres, coff_h, labels, n_iter, seed_c, seed_n.to(torch.int64), seed_it.to(torch.int64)
+
+
 class MeanShift:
     """sklearn.cluster.MeanShift for the arguments the reference passes: every point seeds an ascent (seeds=None,
     bin_seeding=False) and every point is labelled (cluster_all=True).  n_jobs is accepted and ignored.
@@ -113,6 +170,35 @@ class MeanShift:
     def fit_predict(self, X, y=None):
         return self.fit(X).labels_
 
+    def fit_many(self, Xs):
+        """fit for several point sets in one pass: a list of fitted MeanShift instances, the s-th equal to
+        ``MeanShift(bandwidth, max_iter=...).fit(Xs[s])`` bit for bit.  The sets are numpy arrays or CUDA tensors
+        (not mixed) of one dtype, each of at most 2^21 points; results come back as fit returns them."""
+        self._check_params()
+        Xs = [_as_points(X) for X in list(Xs)]
+        if not Xs:
+            raise ValueError("MeanShift.fit_many: no point sets")
+        kinds = {getattr(X, "is_cuda", False) for X in Xs}
+        dtypes = {str(X.dtype).split(".")[-1] for X in Xs}
+        if len(kinds) > 1 or len(dtypes) > 1:
+            raise ValueError(f"MeanShift.fit_many: the sets must share one kind and dtype, got {sorted(dtypes)}")
+        f64 = dtypes == {"float64"}
+        ctx, *xs = _lib.inputs(*Xs, dtype=torch.float64 if f64 else torch.float32)
+        off = np.cumsum([0] + [len(x) for x in xs])
+        centres, coff, labels, n_iter, seed_c, seed_n, seed_it = _fit_many(torch.cat(xs), off, float(self.bandwidth),
+                                                                           self.max_iter)
+        out = []
+        for s, X in enumerate(Xs):
+            a, b, c, d = off[s], off[s + 1], coff[s], coff[s + 1]
+            m = MeanShift(bandwidth=self.bandwidth, cluster_all=self.cluster_all, n_jobs=self.n_jobs,
+                          seeds=self.seeds, bin_seeding=self.bin_seeding, max_iter=self.max_iter)
+            m.n_iter_ = int(n_iter[s])
+            (m.cluster_centers_, m.labels_, m.seed_centers_, m.seed_counts_, m.seed_iters_) = _lib.returned(
+                X, centres[c:d].contiguous(), labels[a:b].contiguous(), seed_c[a:b].contiguous(),
+                seed_n[a:b].contiguous(), seed_it[a:b].contiguous())
+            out.append(m)
+        return out
+
 
 def pointgroup_labels(xyz_original_all, pt_offsets, cloud_xyz, bandwidth):
     """predicter.py:308-338 after the network: the 2 mm voxel down-sampling of the network's points, each voxel mean
@@ -138,3 +224,52 @@ def pointgroup_labels(xyz_original_all, pt_offsets, cloud_xyz, bandwidth):
     labels = MeanShift(bandwidth=bandwidth).fit_predict(xyz_shifted)                      # :332
     nearest = _nearest(xyz_down.to(torch.float64), cloud, LABEL_REACH * DOWNSAMPLE)
     return _lib.returned(xyz_original_all, labels[nearest], xyz_shifted)                 # :334-336
+
+
+def _pointgroup_labels_cat(xo, off, xo_off, cloud, cloud_off, bandwidth):
+    """pointgroup_labels over several frames laid end to end, on the device: xo / off (N,3) float32 with frame b at
+    rows [xo_off[b], xo_off[b + 1]), cloud (M,3) float64 with frame b at [cloud_off[b], cloud_off[b + 1]).  Returns
+    (labels_all (M,) int64, xyz_shifted (U,3) float32, its frame offsets (B + 1) numpy).  One 2 mm index, one snap
+    index and one snap check for all frames."""
+    ds = CloudIndex(xo, DOWNSAMPLE, xo.device.index, set_offsets=xo_off)                  # :308-310
+    down, _ = ds.voxel_means()
+    down_off = ds.cell_offsets
+    del ds
+    snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)                                          # :311-313
+    _, ids = CloudIndex(xo, snap, xo.device.index, set_offsets=xo_off).nearest_many(down, down_off, snap)
+    if bool((ids < 0).any()):
+        raise _lib.CgError("pointgroup_labels: a voxel mean has no point within its voxel's diagonal")
+    ids = ids.to(torch.int64)
+    xyz_down = xo[ids]
+    xyz_shifted = xyz_down + off[ids]                                                    # :314, float32
+    if not bool(torch.isfinite(xyz_shifted).all() & torch.isfinite(cloud).all()):        # as _as_points, at once
+        raise ValueError("Input X contains NaN or infinity")
+    ms = MeanShift(bandwidth=bandwidth)
+    ms._check_params()
+    labels = _fit_many(xyz_shifted, down_off, float(ms.bandwidth), ms.max_iter)[2]            # :332
+    nearest = _nearest_many(xyz_down.to(torch.float64), down_off, cloud, cloud_off, LABEL_REACH * DOWNSAMPLE)
+    return labels[nearest], xyz_shifted, down_off                                         # :334-336
+
+
+def pointgroup_labels_many(xyz_original_alls, pt_offsetss, cloud_xyzs, bandwidth):
+    """pointgroup_labels for several frames in one pass: a list of (labels_all, xyz_shifted), the b-th equal to
+    ``pointgroup_labels(xyz_original_alls[b], pt_offsetss[b], cloud_xyzs[b], bandwidth)`` bit for bit.  The frames
+    are numpy arrays or CUDA tensors (not mixed); results come back as pointgroup_labels returns them.  The number
+    of index builds and synchronisations does not grow with the number of frames."""
+    xos, offs, clouds = list(xyz_original_alls), list(pt_offsetss), list(cloud_xyzs)
+    if not xos or len(offs) != len(xos) or len(clouds) != len(xos):
+        raise ValueError("pointgroup_labels_many: need one offsets array and one cloud per frame, and a frame")
+    if len({getattr(a, "is_cuda", False) for a in xos + offs + clouds}) > 1:
+        raise ValueError("pointgroup_labels_many: the frames must be all numpy arrays or all CUDA tensors")
+    xos, offs, clouds = [_as_points(a) for a in xos], [_as_points(a) for a in offs], [_as_points(a) for a in clouds]
+    for b, (xo, off) in enumerate(zip(xos, offs)):
+        if off.shape[0] != xo.shape[0]:
+            raise ValueError(f"pointgroup_labels_many: frame {b}'s pt_offsets must have one row per point")
+    ctx, *t = _lib.inputs(*xos, *offs, *clouds, dtype=(torch.float32,) * (2 * len(xos)) + (torch.float64,) * len(xos))
+    B = len(xos)
+    xo_off = np.cumsum([0] + [len(a) for a in xos])
+    cloud_off = np.cumsum([0] + [len(a) for a in clouds])
+    labels, shifted, sh_off = _pointgroup_labels_cat(torch.cat(t[:B]), torch.cat(t[B:2 * B]), xo_off,
+                                                     torch.cat(t[2 * B:]), cloud_off, bandwidth)
+    return [_lib.returned(xos[b], labels[cloud_off[b]:cloud_off[b + 1]].contiguous(),
+                          shifted[sh_off[b]:sh_off[b + 1]].contiguous()) for b in range(B)]

@@ -490,9 +490,28 @@ int cg_depth2xyz_dev(cg_ctx *ctx, const void *depth, int depth_is_f64, int H, in
  * afterwards.  Synchronises the context's stream twice (the bounds, then the cell count).  Fails with CG_EINVAL on a
  * non-finite coordinate or when the cloud spans 2^21 or more cells on an axis.                                     */
 int  cg_cloud_index_create(cg_ctx *ctx, const double *pts /* device */, int P, double cell, cg_cloud_index **out);
+/* An index over S point sets laid end to end in pts: set s is the points [set_offsets[s], set_offsets[s+1]) (host,
+ * S+1, from 0).  Every set shares `cell` and keeps what cg_cloud_index_create over it alone has: its own origin
+ * (its min_bound - cell/2), its own cells and the 2^21-cell limit per axis.  A key is s << 3b | x << 2b | y << b | z,
+ * b the smallest width that holds every set's largest cell, the set field bit_length(S - 1) bits.  So the voxel means
+ * (cg_voxel_down_sample_dev) come out set-major, set s's block equal to its one-set output.  CG_EINVAL for an empty
+ * set, before any launch, and for a batch whose key needs more than 63 bits, after the bounds pass and before any
+ * allocation or further launch.  S = 1 is cg_cloud_index_create.  Synchronises twice whatever S is.  The one-set
+ * queries (nearest, radius mask, normals, meanshift) refuse an index with S > 1: their queries carry no set.       */
+int  cg_cloud_index_create_many(cg_ctx *ctx, const double *pts /* device */, const int32_t *set_offsets /* host */,
+                                int S, double cell, cg_cloud_index **out);
 void cg_cloud_index_destroy(cg_cloud_index *index);
-/* P, number of occupied cells (= the voxel count of cg_voxel_down_sample_dev), cell size, origin[3]; any may be NULL */
+/* P, number of occupied cells (= the voxel count of cg_voxel_down_sample_dev), cell size, origin[3] (set 0's); any may
+ * be NULL */
 int  cg_cloud_index_info(const cg_cloud_index *index, int *out_points, int *out_cells, double *out_cell, double *out_origin);
+/* the number of sets S and, unless NULL, out_cell_offsets (host, S+1): set s's occupied cells are
+ * [out_cell_offsets[s], out_cell_offsets[s+1]) of the cell table and of the voxel means */
+int  cg_cloud_index_sets(const cg_cloud_index *index, int *out_sets, int32_t *out_cell_offsets /* host */);
+/* device copies of the index's tables, each NULL to skip: out_pts (P,3) the points in key order, out_perm (P) each
+ * one's index in pts, out_keys (U) the ascending cell keys, out_start (U+1) each cell's first sorted point.  Does not
+ * synchronise. */
+int  cg_cloud_index_tables_dev(const cg_cloud_index *index, double *out_pts, int32_t *out_perm, uint64_t *out_keys,
+                               int32_t *out_start);
 /* open3d VoxelDownSample with voxel_size = the index's cell: one output per occupied cell, in ascending (ix, iy, iz)
  * order; mean = members summed in ascending point index, divided by the count; normals (P,3) or NULL: the summed
  * normal divided by its norm (a zero sum stays zero).  out_pts / out_normals hold cg_cloud_index_info's cell count. */
@@ -502,6 +521,10 @@ int  cg_voxel_down_sample_dev(const cg_cloud_index *index, const double *normals
  * cg_cloud_radius_mask_dev, Q = 0 is a no-op whose pointers may be NULL (an empty torch tensor has no storage).    */
 int  cg_cloud_nearest_dev(const cg_cloud_index *index, const double *query, int Q, double max_dist, int32_t *out_idx,
                           double *out_dist);
+/* cg_cloud_nearest_dev per set: the queries [query_offsets[s], query_offsets[s+1]) (host, S+1, from 0 to Q; a range
+ * may be empty) search set s only.  out_idx is the one-set answer plus set s's first point; -1 / +inf stay.         */
+int  cg_cloud_nearest_many_dev(const cg_cloud_index *index, const double *query, const int32_t *query_offsets /* host */,
+                               int Q, double max_dist, int32_t *out_idx, double *out_dist);
 /* out_mask[i] = 1 when some indexed point has d2 <= r*r (compare_sqrt = 0, query_ball_point's test) or
  * sqrt(d2) <= r (compare_sqrt = 1, the `dists <= R` test on cKDTree.query's distances), else 0.                   */
 int  cg_cloud_radius_mask_dev(const cg_cloud_index *index, const double *query, int Q, double r, int compare_sqrt,
@@ -529,6 +552,13 @@ int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn
 int  cg_meanshift_dev(const cg_cloud_index *index, const void *X, int x_is_f64, double bandwidth, int max_iter,
                       void *out_seed_centres, int32_t *out_seed_counts, int32_t *out_seed_iters, void *out_centres,
                       int32_t *out_n_centres);
+/* cg_meanshift_dev per set over a cg_cloud_index_create_many index (cell = bandwidth) of X, sets laid end to end:
+ * set s's seeds, centres and counts equal cg_meanshift_dev on set s alone, bit for bit (its own origin and fixed-point
+ * scale, its own collapse, order and suppression).  The 2^21-point limit is per set.  out_centres come out set-major;
+ * out_centre_offsets (device, S+1): set s's centres are [off[s], off[s+1]).  Never synchronises.                  */
+int  cg_meanshift_many_dev(const cg_cloud_index *index, const void *X, int x_is_f64, double bandwidth, int max_iter,
+                           void *out_seed_centres, int32_t *out_seed_counts, int32_t *out_seed_iters, void *out_centres,
+                           int32_t *out_centre_offsets);
 
 /* ---- sparse 3-D convolution (spconv 1.x semantics; cg_spconv.cu) ----
  * The layer types of PointGroup's U-Net (PointGroup/model/pointgroup/pointgroup.py): SubMConv3d k3 and k1,
