@@ -107,6 +107,7 @@ SIGNATURES = {
     "cg_ctx_fp16_overflow": (_i, [_vp, _H], None),
     "cg_ctx_profile": (_i, [_vp, _i], None),
     "cg_ctx_profile_read": (_i, [_vp, _H, _H], None),
+    "cg_ctx_fill_workspaces": (_i, [_vp, _i], None),
     "cg_net_create": (_i, [_vp, _i, _i, _H, _sz, _H], OWN),
     "cg_net_destroy": (None, [_vp], None),
     "cg_net_blob_floats": (_sz, [_i, _i], None),
@@ -294,6 +295,11 @@ class Context:
         ms, n = C.c_double(), C.c_int64()
         self.check(self.lib.cg_ctx_profile_read(self.h, C.byref(ms), C.byref(n)))
         return ms.value, n.value
+
+    def fill_workspaces(self, byte):
+        """Set every byte of the context's workspaces to ``byte`` on its current stream -- a test hook: the next call
+        starts on memory it must write before it reads."""
+        self.check(self.lib.cg_ctx_fill_workspaces(self.h, int(byte)))
 
     def launch_count(self):
         return int(self.lib.cg_ctx_launch_count(self.h))

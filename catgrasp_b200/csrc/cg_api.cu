@@ -136,6 +136,14 @@ static int grow(cg_ctx *ctx, void **p, size_t *cur, size_t bytes) {
 int cg_ws_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->ws, &ctx->ws_bytes, bytes); }
 int cg_io_reserve(cg_ctx *ctx, size_t bytes) { return grow(ctx, &ctx->io, &ctx->io_bytes, bytes); }
 
+extern "C" int cg_ctx_fill_workspaces(cg_ctx *ctx, int byte) {
+  if (!ctx) return CG_EINVAL;
+  CG_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (ctx->ws) CG_CUDA(ctx, cudaMemsetAsync(ctx->ws, byte, ctx->ws_bytes, ctx->stream));
+  if (ctx->io) CG_CUDA(ctx, cudaMemsetAsync(ctx->io, byte, ctx->io_bytes, ctx->stream));
+  return CG_OK;
+}
+
 // CG_TRACE diagnostics: durations between consecutive post-launch events on the context's stream, grouped by call site
 void cg_trace_mark(cg_ctx *ctx, const char *where) {
   cudaEvent_t e;

@@ -78,6 +78,11 @@ int         cg_ctx_fp16_overflow(cg_ctx *ctx, int *out);
  * returns the summed duration and the launch count, then clears the list.   */
 int         cg_ctx_profile(cg_ctx *ctx, int enable);
 int         cg_ctx_profile_read(cg_ctx *ctx, double *ms_total, int64_t *launches);
+/* Set every byte of the context's reserved workspaces (the ws and io arenas
+ * its calls carve scratch and staged I/O from) to `byte` -- a test hook, so a
+ * call that reads memory it did not write shows up.  Enqueued on the context
+ * stream, no synchronisation; never grows an arena, skips one not yet made.  */
+int         cg_ctx_fill_workspaces(cg_ctx *ctx, int byte);
 
 /* ---- networks ----------------------------------------------------------
  * Replaces: pointnet2.py:275-299 (PointNetCls), :302-329 (PointNetSeg),
