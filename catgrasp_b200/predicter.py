@@ -145,13 +145,16 @@ def host_draw_stages(groups, chunk):
     return stages
 
 
-def walk_grasp_many(Ms, counts, n_pts, stages, out):
+def walk_grasp_many(Ms, counts, n_pts, stages, out, skip=(0, 0)):
     """The host-mode draws of a loop of GraspPredicter.predict_batch calls in ONE walk of numpy's global generator
     (cg_host_legacy_choice): object o's counts[o] subsets of n_pts points out of Ms[o] (replace = Ms[o] < n_pts), in
     object order, into the rows of ``out`` (sum(counts), n_pts) int32.  A generator: it draws stage by stage (row
     ranges from host_draw_stages, cut anywhere) and yields each stage as it is drawn; the generator's state is put
-    back once, after the last stage."""
+    back once, after the last stage.  ``skip`` = (before, after): for one object whose rows are a window of its
+    candidate list, the candidates walked over without drawing ahead of the window and after it."""
     draw = _LegacyDraw()
+    if skip[0]:
+        draw.skip(int(Ms[0]), n_pts, skip[0])
     first = np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64))])
     for stage in stages:
         r0, r1 = int(stage[0]), int(stage[1])
@@ -164,6 +167,8 @@ def walk_grasp_many(Ms, counts, n_pts, stages, out):
             draw.draw(int(Ms[o]), n_pts, e - r, out=out[r:e])
             r = e
         yield stage
+    if skip[1]:
+        draw.skip(int(Ms[-1]), n_pts, skip[1])
     draw.commit()
 
 
@@ -265,57 +270,9 @@ class GraspPredicter:
             self._pin = torch.empty((need + need // 4,), dtype=torch.int32).pin_memory()
         return self._pin[:need].view(B, n_pts)
 
-    def _given_ids(self, ids, lo, hi):
-        """Caller-given subsets: numpy's global generator is not touched.  Yields (first row, device ids) launches."""
-        import torch
-        if hi > lo:
-            yield 0, torch.from_numpy(np.ascontiguousarray(np.asarray(ids)[lo:hi], dtype=np.int32)).to(self.model.device)
-
-    def _device_draw(self, M, lo, hi):
-        """The counter-based draw on the GPU (cg_draw_ids_dev): consumes ONE value of numpy's global generator, the
-        seed, whatever the shard; a candidate's subset depends on the seed and its place in the whole list only."""
-        seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
-        if hi > lo:
-            yield 0, self.model.draw_ids_dev(M, int(self.cfg["n_pts"]), hi - lo, seed=seed, first_candidate=lo)
-
-    def _host_draw(self, M, lo, hi, B_all):
-        """The reference's draw: walks numpy's global generator over the WHOLE list in C (skip the ``lo`` candidates
-        before the shard, draw the shard, skip the ``B_all - hi`` after it) and puts the advanced state back.  The
-        worker thread draws chunk k+1 into the pinned buffer while the GPU scores chunk k."""
-        import queue
-        import threading
-        import torch
-        B, n_pts = hi - lo, int(self.cfg["n_pts"])
-        h_ids = self._pinned_ids(B, n_pts)
-        d_ids = torch.empty((B, n_pts), dtype=torch.int32, device=self.model.device)
-        draw = _LegacyDraw()
-        q = queue.Queue()
-
-        def producer():
-            try:
-                draw.skip(M, n_pts, lo)
-                for c0 in range(0, B, self.chunk):
-                    c1 = min(B, c0 + self.chunk)
-                    draw.draw(M, n_pts, c1 - c0, out=h_ids[c0:c1])
-                    q.put((c0, c1))
-                draw.skip(M, n_pts, B_all - hi)
-                q.put(None)
-            except Exception as e:   # surfaces in the consumer
-                q.put(e)
-        t = threading.Thread(target=producer, daemon=True)
-        t.start()
-        while (item := q.get()) is not None:
-            if isinstance(item, Exception):
-                raise item
-            c0, c1 = item
-            d_ids[c0:c1].copy_(h_ids[c0:c1], non_blocking=True)
-            yield c0, d_ids[c0:c1]
-        t.join()
-        draw.commit()
-
     def score(self, data, grasp_poses, ids=None, subsample=None, shard=None):
         """The probabilities of candidates ``shard=(lo, hi)`` of the list (default: all of it) as a (hi-lo, n_out)
-        float32 CUDA tensor.
+        float32 CUDA tensor: ``score_many`` with one object, whose rows are that window of its list.
 
         ``data`` is not modified (the reference deep-copies it, :72).  ``ids`` (B,n_pts) overrides the draw.
         ``subsample`` (default ``self.subsample``):
@@ -323,61 +280,16 @@ class GraspPredicter:
                       with the same consumption of the global numpy generator; drawn in C in chunks on a worker thread
                       while the GPU scores the previous chunk;
           "device" -- a statistically equivalent counter-based draw on the GPU (cg_draw_ids_dev); consumes ONE value
-                      of the global numpy generator (the seed) instead of one shuffle per candidate.  Not the
-                      reference's numbers: use it when throughput matters more than replaying a reference run.
+                      of the global numpy generator (the seed) instead of one shuffle per candidate, and a candidate's
+                      subset depends on the seed and its place in the whole list only.  Not the reference's numbers:
+                      use it when throughput matters more than replaying a reference run.
         The random stream is consumed for the WHOLE list whatever the shard, so every rank of a sharded call stays on
         the reference's stream (catgrasp_b200.dist.sharded_predict_batch).
         """
-        import torch
         B_all = len(grasp_poses)
         lo, hi = (0, B_all) if shard is None else (int(shard[0]), int(shard[1]))
         assert 0 <= lo <= hi <= B_all
-        mode = subsample or self.subsample
-        assert mode in ("host", "device"), mode
-        xyz = np.asarray(data["cloud_xyz"], dtype=np.float64)
-        nrm = np.asarray(data["cloud_normal"], dtype=np.float64)
-        valid_mask = xyz[:, 2] >= 0.1                                   # dataset_grasp.py:64
-        xyz = np.ascontiguousarray(xyz[valid_mask].reshape(-1, 3))
-        nrm = np.ascontiguousarray(nrm[valid_mask].reshape(-1, 3))
-        M = xyz.shape[0]
-        poses = np.ascontiguousarray(np.asarray(grasp_poses, dtype=np.float64).reshape(B_all, 4, 4)[lo:hi])
-        net, dev, ctx = self.model, self.model.device, self.model.ctx
-        with torch.cuda.device(dev):
-            d_xyz, d_nrm = torch.from_numpy(xyz).to(dev), torch.from_numpy(nrm).to(dev)
-            d_pose = torch.from_numpy(poses).to(dev)
-            d_mean = torch.from_numpy(np.ascontiguousarray(self.cfg["mean"].reshape(-1))).to(dev) if "mean" in self.cfg else None
-            d_std = torch.from_numpy(np.ascontiguousarray(self.cfg["std"].reshape(-1))).to(dev) if "std" in self.cfg else None
-            d_probs = torch.empty((hi - lo, net.n_out), dtype=torch.float32, device=dev)
-            d_label = torch.empty((hi - lo,), dtype=torch.int32, device=dev)
-
-            def forward(c0, d_ids):
-                c1 = c0 + d_ids.shape[0]
-                net.graspq_dev(d_xyz, d_nrm, d_pose[c0:c1], d_ids, d_mean, d_std, out=(d_probs[c0:c1], d_label[c0:c1]))
-
-            if ids is not None:
-                launches = self._given_ids(ids, lo, hi)
-            elif mode == "device":
-                launches = self._device_draw(M, lo, hi)
-            else:
-                launches = self._host_draw(M, lo, hi, B_all)
-            ctx_engine = ctx.get_engine()
-            ctx.set_engine(self.engine)         # the context (one per device) is shared: this predicter's engine, per call
-            try:
-                done = []
-                for c0, d_ids in launches:
-                    forward(c0, d_ids)
-                    done.append((c0, d_ids))
-                if self.engine >= 2 and ctx.fp16_overflow():
-                    # the fast engines clamp the 128->1024 layer's inputs to the fp16 range: redo on the near-fp32
-                    # engine from the ids already on the device, launch for launch (a launch's batch size selects the
-                    # FC kernel, so the same cuts give the bits of a call made on engine 1)
-                    print("GraspPredicter: activation beyond the fp16 range, re-running on engine 1 (wgmma bf16 hi/lo x3)")
-                    ctx.set_engine(1)
-                    for c0, d_ids in done:
-                        forward(c0, d_ids)
-            finally:
-                ctx.set_engine(ctx_engine)
-        return d_probs
+        return self._score([data], [grasp_poses], None if ids is None else [ids], subsample, window=(lo, hi))[0]
 
     def predict_batch(self, data, grasp_poses, ids=None, subsample=None):
         """predicter.py:67-94.  Returns list of [label np.int64, confidence np.float32, probs (n_out,) f32]: ``score``
@@ -404,16 +316,25 @@ class GraspPredicter:
         On engines 2 and 3 the fp16-overflow flag belongs to the context: when it is set after the pass (or was set
         before it, which the loop's first call would see), the objects are scored again one at a time from the ids on
         the device, each on this predicter's engine and, where that object overflows, on engine 1, as the loop does."""
+        return self._score(datas, grasp_poses_list, ids, subsample)
+
+    def _score(self, datas, grasp_poses_list, ids, subsample, window=None):
+        """score_many; with ``window`` = (lo, hi), the rows [lo, hi) of its one object's candidate list (score)."""
         import torch
         mode = subsample or self.subsample
         assert mode in ("host", "device"), mode
         n_pts = int(self.cfg["n_pts"])
         objs = _check_grasp_many(datas, grasp_poses_list, ids, n_pts)
+        live = [o for o, ob in enumerate(objs) if ob is not None]
+        lo, skip = 0, (0, 0)
+        if window is not None and live:
+            (lo, hi), (xyz, nrm, poses, sub) = window, objs[0]
+            skip = (lo, poses.shape[0] - hi)          # host mode walks the candidates around the window
+            objs[0] = (xyz, nrm, poses[lo:hi], None if sub is None else sub[lo:hi])
         counts = [0 if ob is None else ob[2].shape[0] for ob in objs]
         offsets = np.zeros(len(objs) + 1, np.int64)
         offsets[1:] = np.cumsum(counts)
         B_all = int(offsets[-1])
-        live = [o for o, ob in enumerate(objs) if ob is not None]
         Ms = [0 if ob is None else ob[0].shape[0] for ob in objs]
         bases = np.zeros(len(objs), np.int64)
         bases[1:] = np.cumsum(Ms)[:-1]
@@ -421,10 +342,14 @@ class GraspPredicter:
             raise ValueError("predict_batch_many: 2^31 cloud points or more in all")
         launch = self.chunk if (ids is None and mode == "host") else None
         groups, spans = graspq_fc_groups(counts, launch)
+        seeds = [int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64)) for _ in live] \
+            if ids is None and mode == "device" else None
         net, dev, ctx = self.model, self.model.device, self.model.ctx
         with torch.cuda.device(dev):
             d_probs = torch.empty((B_all, net.n_out), dtype=torch.float32, device=dev)
             if B_all == 0:
+                if live and ids is None and mode == "host":      # an empty window still walks its whole list
+                    list(walk_grasp_many(Ms, counts, n_pts, [], None, skip))
                 return d_probs, offsets
             cat = lambda k: np.ascontiguousarray(np.concatenate([objs[o][k] for o in live]))
             d_xyz, d_nrm, d_pose = (torch.from_numpy(cat(k)).to(dev) for k in (0, 1, 2))
@@ -435,32 +360,35 @@ class GraspPredicter:
                 net.graspq_many_dev(d_xyz, d_nrm, d_pose[r0:r1], d_ids[r0:r1], groups[g0:g1], d_mean, d_std,
                                     out=(d_probs[r0:r1], None))
 
-            whole = [(0, B_all, 0, len(groups))]
+            stages = [(0, B_all, 0, len(groups))]
             if ids is not None:
                 d_ids = torch.from_numpy(np.concatenate([objs[o][3] + np.int32(bases[o]) for o in live])).to(dev)
-                stages = iter(whole)
+            elif mode == "device" and window is not None:
+                # cg_draw_ids_many_dev numbers an object's candidates from 0: a window starts at candidate lo
+                d_ids = net.draw_ids_dev(Ms[0], n_pts, B_all, seeds[0], first_candidate=lo)
             elif mode == "device":
-                seeds = [int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64)) for _ in live]
                 d_ids = net.draw_ids_many_dev([Ms[o] for o in live], n_pts, [counts[o] for o in live], seeds,
                                               bases[live])
-                stages = iter(whole)
             else:
                 h_ids = self._pinned_ids(B_all, n_pts)
                 d_ids = torch.empty((B_all, n_pts), dtype=torch.int32, device=dev)
                 row_base = torch.from_numpy(np.repeat(bases.astype(np.int32), counts)).to(dev)[:, None]
                 stages = self._host_stages(walk_grasp_many(Ms, counts, n_pts, host_draw_stages(groups, self.chunk),
-                                                           h_ids), h_ids, d_ids, row_base)
+                                                           h_ids, skip), h_ids, d_ids, row_base)
             ctx_engine = ctx.get_engine()
             ctx.set_engine(self.engine)         # the context (one per device) is shared: this predicter's engine, per call
             try:
-                stale = self.engine >= 2 and ctx.fp16_overflow()
+                # with one object the flag after the pass is its own, whoever set it; with several, a flag left by
+                # earlier work is read first, as the loop's first call would see it
+                several = len(live) > 1
+                stale = several and self.engine >= 2 and ctx.fp16_overflow()
                 for r0, r1, g0, g1 in stages:
                     forward(r0, r1, g0, g1, d_ids)
                 overflow = self.engine >= 2 and ctx.fp16_overflow()
                 for o in (live if overflow or stale else []):
                     r0, r1, (g0, g1) = int(offsets[o]), int(offsets[o + 1]), spans[o]
-                    own = False
-                    if overflow:
+                    own = overflow and not several
+                    if overflow and several:
                         forward(r0, r1, g0, g1, d_ids)
                         own = ctx.fp16_overflow()
                     if own or (stale and o == live[0]):
@@ -589,18 +517,16 @@ class NunocsPredicter:
         return coords, conf_z
 
     def predict(self, data, ids=None):
-        """predicter.py:135-203: (nocs_cloud, transform) or (None, None); numpy for numpy input, CUDA tensors for
-        CUDA input.  Sets data_transformed, confidence_z, pred_bins and, with a pose, best_ratio and nocs_pose.
-        ``ids`` (n_pts,) overrides the cloud subset; ``self.subsample`` picks the random numbers ("host" / "device")."""
-        assert self.subsample in ("host", "device"), self.subsample
-        self._kd_resolution()
-        if self.subsample == "device":
-            return self._predict_device(data, ids)
-        if getattr(data["cloud_xyz"], "is_cuda", False):
-            data = {k: (v.cpu().numpy() if hasattr(v, "is_cuda") else v) for k, v in data.items()}
-            nocs, tf = self._predict_host(data, ids)
-            return (None, None) if tf is None else self._on(self.model.device, nocs, tf)
-        return self._predict_host(data, ids)
+        """predicter.py:135-203: ``predict_many([data], [ids])[0]``, (nocs_cloud, transform) or (None, None); numpy for
+        numpy input, CUDA tensors for CUDA input.  Sets data_transformed, confidence_z, pred_bins and, with a pose,
+        best_ratio and nocs_pose.  ``ids`` (n_pts,) overrides the cloud subset; ``self.subsample`` picks the random
+        numbers ("host" / "device").  In host mode on numpy input it writes zero 'cloud_nocs' and 'cloud_rgb' arrays
+        into ``data``, as the reference's predict does through predict_nocs."""
+        out = self.predict_many([data], None if ids is None else [ids])[0]
+        if self.subsample == "host" and not getattr(data["cloud_xyz"], "is_cuda", False):
+            data["cloud_nocs"] = np.zeros(data["cloud_xyz"].shape)
+            data["cloud_rgb"] = np.zeros(data["cloud_xyz"].shape)
+        return out
 
     def _on(self, dev, *arrays):
         import torch
@@ -616,31 +542,6 @@ class NunocsPredicter:
         return ransac9d_pose(source, target, ids, self.THRESHOLDS, max_scale=self.max_scale, min_scale=self.min_scale,
                              max_dimensions=self.MAX_DIMENSIONS, ratio_threshold=self.ERR_THRES,
                              kdtree_eval_resolution=self._kd_resolution())
-
-    def _predict_host(self, data, ids):
-        """The reference's numbers: the transform's subset from np.random.choice, then both thresholds' subsets in
-        one C draw that continues numpy's stream where the reference's two loops would (aligning.py:91-97), one
-        fused launch on them, and predict's post-processing in numpy on the two winners' T (predicter.py:152-172)."""
-        nocs_cloud, _ = self.predict_nocs(data, ids=ids)
-        ori_cloud = self.data_transformed["cloud_xyz_original"]
-        symmetry_tf = np.eye(4)
-        source = np.ascontiguousarray((symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3], dtype=np.float64)
-        target = np.ascontiguousarray(ori_cloud, dtype=np.float64)
-        N, H = len(source), int(self.ransac_max_iter)
-        if N < 4:
-            raise ValueError("Cannot take a larger sample than population when 'replace=False'")   # as np.random.choice
-        draw = _LegacyDraw()
-        hyp = draw.draw(N, 4, len(self.THRESHOLDS) * H)
-        draw.commit()
-        dev = self.model.device
-        res = self._ransac(*self._on(dev, source, target, hyp))
-        best_ratio, best_transform = self._choose_host(res["record"].cpu().numpy(), source, target)
-        if best_transform is None:
-            return None, None
-        self.best_ratio = best_ratio
-        self.nocs_pose = best_transform.copy()
-        nocs_cloud = (symmetry_tf @ to_homo(nocs_cloud).T).T[:, :3]
-        return nocs_cloud, best_transform
 
     def _choose_host(self, record, source, target):
         """predict's choice between the thresholds in numpy (predicter.py:152-172) from a pose search's host record:
@@ -669,60 +570,16 @@ class NunocsPredicter:
         the same ids, 'input' equals transform()'s bit for bit.  Returns a dict of CUDA tensors ('cloud_xyz',
         'cloud_normal', 'cloud_xyz_original', 'keep_ids', 'input').  With CUDA input the masked point count is read
         on the host (one synchronisation): it sizes the draw."""
-        import torch
-        from . import _lib
-        n_pts = int(self.cfg["n_pts"])
-        ctx, xyz, nrm = _lib.inputs(data["cloud_xyz"], data["cloud_normal"], dtype=torch.float64, ctx=self.model.ctx)
-        if getattr(data["cloud_xyz"], "is_cuda", False):
-            keep_ids = torch.nonzero(data["cloud_xyz"][:, 2] >= 0.1).reshape(-1).to(xyz.device)   # in the input's dtype
-        else:
-            keep_ids = torch.from_numpy(np.nonzero(np.asarray(data["cloud_xyz"])[:, 2] >= 0.1)[0]).to(xyz.device)
-        if ids is None:
-            sub = self.model.draw_ids_dev(keep_ids.numel(), n_pts, 1, seed, first_candidate=0)[0].long()
-        else:
-            sub = torch.as_tensor(np.asarray(ids) if not hasattr(ids, "is_cuda") else ids).to(xyz.device).long()
-        keep_ids = keep_ids[sub]
-        x0, nr = xyz[keep_ids], nrm[keep_ids]
-        mn = x0.amin(0)
-        scale = (x0.amax(0) - mn).max()
-        xn = (x0 - mn) / (scale + 1e-15)
-        inp = torch.cat([xn, nr], 1)
-        if "mean" in self.cfg:
-            mean, std = self._on(xyz.device, self.cfg["mean"].reshape(1, -1), self.cfg["std"].reshape(1, -1))
-            inp = (inp - mean) / (std + 1e-15)
-        return {"cloud_xyz": xn, "cloud_normal": nr, "cloud_xyz_original": x0, "keep_ids": keep_ids, "input": inp}
-
-    def _predict_device(self, data, ids):
-        """Device mode: consumes ONE value of numpy's global generator (the seed, np.random.randint as
-        GraspPredicter's device draw does).  Candidate 0 of cg_draw_ids_dev(seed) is the cloud subset, candidates
-        1 .. H the first threshold's subsets and H+1 .. 2H the second's; the forward, the RANSAC and predict's
-        choice between thresholds run on the device.  The host waits for the masked point count with CUDA input,
-        and for the record (whether there is a pose, best_ratio) and, with numpy input, the copy of the results."""
-        import torch
-        from .aligning import read_record
-        seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
-        cuda_in = getattr(data["cloud_xyz"], "is_cuda", False)
-        H, n_thr = int(self.ransac_max_iter), len(self.THRESHOLDS)
-        dt = self.device_transform(data, ids=ids, seed=seed)
-        coords, conf_z, bins = self.model.nunocs_dev(dt["input"].to(torch.float32), int(self.cfg["ce_loss_bins"]))
-        source = coords.to(torch.float64)
-        hyp = self.model.draw_ids_dev(source.shape[0], 4, n_thr * H, seed, first_candidate=1)
-        res = self._ransac(source, dt["cloud_xyz_original"], hyp)
-        found = read_record(res["record"].cpu().numpy(), n_thr)
-        host = (lambda t: t.cpu().numpy()) if not cuda_in else (lambda t: t)
-        self.data_transformed = {k: host(v) for k, v in dt.items()}
-        self.confidence_z, self.pred_bins = host(conf_z), host(bins)
-        if found["chosen"] < 0:
-            return None, None
-        self.best_ratio = float(found["best_ratio"])
-        pose = host(res["pose"].clone())
-        self.nocs_pose = pose.copy() if not cuda_in else pose.clone()
-        return host(source), pose
+        mask = data["cloud_xyz"][:, 2] >= 0.1
+        count = int(mask.sum()) if getattr(mask, "is_cuda", False) else int(np.count_nonzero(mask))
+        dt = self._device_transform_many([data], [ids], [seed], [count])
+        return {k: v[0] for k, v in dt.items()}
 
     def predict_many(self, datas, ids=None):
-        """predict for a list of objects: ``[self.predict(d) for d in datas]`` (with ``ids[b]`` for object b), bit for
-        bit, from the same state of numpy's global generator, which it leaves where the loop would; the attributes
-        data_transformed, confidence_z, pred_bins, best_ratio and nocs_pose are left as the loop leaves them.
+        """predict for a list of objects: each object's result as predict gives it for that object alone (with
+        ``ids[b]`` for object b), bit for bit, from the same state of numpy's global generator, which it leaves where a
+        loop of predict calls would; the attributes data_transformed, confidence_z, pred_bins, best_ratio and
+        nocs_pose are left as that loop leaves them.
         ``datas`` are all numpy or all CUDA-tensor dicts with 'cloud_xyz' and 'cloud_normal' (M_b,3); they are not
         modified.  ``ids`` (optional) is a list of B subsets of n_pts indices into the masked cloud, or None entries.
         Returns one (nocs_cloud, pose) per object, (None, None) for an object with no pose.
@@ -986,42 +843,19 @@ class PointGroupPredictor:
 
     def device_front(self, data):
         """predicter.py:234-300 with n_slice_per_side = 1, on the device for numpy or CUDA input: (xyz_original_all
-        (N,3) float32, locs (N,3) int64, feats (N,6) float32) CUDA tensors and spatial_shape (3 ints).  Every step is
-        in the input's dtype as the reference computes it: the keep mask, the 0.5 mm voxel means snapped to their
-        nearest point, and the sites trunc(fl(fl(x * scale) - min)), the scale first and each operation rounded on
-        its own."""
-        import torch
-        from .cloud import CloudIndex
-        from . import _lib
-        self._check_structure()
-        dev = self.model.ctx.device
-        ctx, xyz, nrm = _lib.inputs(data["cloud_xyz"], data["cloud_normal"], ctx=self.model.ctx,
-                                    dtype=tuple(_float_dtype(a) for a in (data["cloud_xyz"], data["cloud_normal"])))
-        keep = torch.nonzero(slice_keep_mask(xyz)).reshape(-1)
-        xo, no = xyz[keep], nrm[keep]
-        ds = float(self.cfg["downsample_size"])
-        down, _ = CloudIndex(xo, ds, dev).voxel_means()
-        # the snap (cKDTree.query): a voxel mean and its members share a voxel, so the nearest member is within the
-        # diagonal, widened by 1e-9 relative against rounding at a voxel face
-        snap = ds * np.sqrt(3.0) * (1 + 1e-9)
-        _, ids = CloudIndex(xo, snap, dev).nearest(down, snap)
-        if bool((ids < 0).any()):
-            raise _lib.CgError("PointGroupPredictor: a voxel mean has no point within its voxel's diagonal")
-        ids = ids.to(torch.int64)
-        xo, no = xo[ids], no[ids]
-        s = xo * self.cfg_pg["scale"]
-        s = s - s.amin(0)
-        locs = s.to(torch.int64)                                         # truncation, as torch's .long() on the host
-        hi = (locs.amax(0) + 1).cpu().numpy()
-        shape = tuple(int(v) for v in np.maximum(hi, int(self.cfg_pg["full_scale"][0])))
-        feats = torch.cat([no.to(torch.float32), xo.to(torch.float32)], 1)
-        return xo.to(torch.float32), locs, feats, shape
+        (N,3) float32, locs (N,3) int64, feats (N,6) float32) CUDA tensors and spatial_shape (3 ints), as
+        device_front_many gives them for one frame."""
+        xo, locs, feats, shapes, _ = self.device_front_many([data])
+        return xo, locs, feats, shapes[0]
 
     def device_front_many(self, datas):
-        """device_front for several frames in one pass: (xyz_original_all (N,3) float32, locs (N,3) int64, feats
-        (N,6) float32) CUDA tensors with the frames laid end to end, the B spatial shapes, and the row offsets (B + 1)
-        numpy, frame b at rows [offsets[b], offsets[b + 1]).  Frame b's rows, shape and offsets equal device_front of
-        frame b alone, bit for bit.  One keep-mask nonzero for all frames, one 0.5 mm index, one snap index, one snap
+        """predicter.py:234-300 with n_slice_per_side = 1 for several frames in one pass, on the device for numpy or
+        CUDA input: (xyz_original_all (N,3) float32, locs (N,3) int64, feats (N,6) float32) CUDA tensors with the
+        frames laid end to end, the B spatial shapes, and the row offsets (B + 1) numpy, frame b at rows [offsets[b],
+        offsets[b + 1]).  Every step is in the frame's dtype as the reference computes it: the keep mask, the 0.5 mm
+        voxel means snapped to their nearest point, and the sites trunc(fl(fl(x * scale) - min)), the scale first and
+        each operation rounded on its own.  Each frame keeps its own minimum and spatial shape, so its rows do not
+        depend on the other frames.  One keep-mask nonzero for all frames, one 0.5 mm index, one snap index, one snap
         check and one read of every frame's shape: the synchronisations do not grow with the number of frames."""
         import torch
         from .cloud import CloudIndex
@@ -1047,7 +881,9 @@ class PointGroupPredictor:
         index = CloudIndex(xo, ds, dev, set_offsets=np.cumsum(np.r_[0, counts]))
         down, _ = index.voxel_means()
         row_off = index.cell_offsets
-        snap = ds * np.sqrt(3.0) * (1 + 1e-9)                 # as device_front
+        # the snap (cKDTree.query): a voxel mean and its members share a voxel, so the nearest member is within the
+        # diagonal, widened by 1e-9 relative against rounding at a voxel face
+        snap = ds * np.sqrt(3.0) * (1 + 1e-9)
         _, ids = CloudIndex(xo, snap, dev, set_offsets=index.set_offsets).nearest_many(down, row_off, snap)
         del index
         if bool((ids < 0).any()):
@@ -1090,18 +926,12 @@ class PointGroupPredictor:
 
     def predict(self, data):
         """predicter.py:232-338: labels_all (M,) int64, one per point of data['cloud_xyz'], and self.xyz_shifted; numpy
-        for numpy input, CUDA tensors for CUDA input."""
-        from .segment import MEANSHIFT_BANDWIDTH, pointgroup_labels
-        xo, off = self.offsets(data)
-        labels_all, xyz_shifted = pointgroup_labels(xo, off, data["cloud_xyz"], MEANSHIFT_BANDWIDTH[self.class_name])
-        if not getattr(data["cloud_xyz"], "is_cuda", False):
-            labels_all, xyz_shifted = labels_all.cpu().numpy(), xyz_shifted.cpu().numpy()
-        self.xyz_shifted = xyz_shifted
-        return labels_all
+        for numpy input, CUDA tensors for CUDA input.  ``predict_many([data])[0]``."""
+        return self.predict_many([data])[0]
 
     def predict_many(self, datas):
-        """predict for a list of frames: ``[self.predict(d) for d in datas]`` bit for bit, numpy labels for numpy input
-        and CUDA tensors for CUDA input, with self.xyz_shifted left as the loop leaves it (the last frame's).
+        """predict for a list of frames: each frame's labels as predict gives them for it alone, bit for bit, numpy
+        labels for numpy input and CUDA tensors for CUDA input, with self.xyz_shifted the last frame's.
 
         The front runs once over all frames (device_front_many), and each frame keeps its own spatial shape.  The
         network then runs once over all frames: one batched spconv.index_many (its one synchronisation) and pyramid,

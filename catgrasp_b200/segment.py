@@ -40,28 +40,12 @@ def _as_points(X):
     return X
 
 
-def _nearest(ref, query, reach):
-    """Index of the nearest ref point for every query (ref, query: float64 device tensors): first within `reach`,
-    then, for the queries with nothing that close, within the diagonal of the joint bounding box, so none goes
-    unanswered.  Either way the answer is the global nearest point with ties to the smaller index."""
-    _, idx = CloudIndex(ref, _query_cell(ref, reach), ref.device.index).nearest(query, reach)
-    miss = torch.nonzero(idx < 0).reshape(-1)
-    if miss.numel():
-        q = query[miss]
-        span = torch.maximum(ref.amax(0), q.amax(0)) - torch.minimum(ref.amin(0), q.amin(0))
-        bound = float(torch.linalg.norm(span)) * (1 + 1e-9)
-        _, far = CloudIndex(ref, _query_cell(ref, bound), ref.device.index).nearest(q, bound)
-        if bool((far < 0).any()):
-            raise _lib.CgError("nearest: a query found no point within the joint bounding box's diagonal")
-        idx[miss] = far
-    return idx.to(torch.int64)
-
-
 def _nearest_many(ref, ref_off, query, query_off, reach):
-    """_nearest per set (ref, query: float64 device tensors, set s the rows [off[s], off[s + 1]) of each, every ref
-    set non-empty): the index into ref of each query's nearest point of its own set, ties to the smaller index.  One
-    index build for the whole batch, and at most one more, shared by every set, for the queries with nothing within
-    `reach`; its bound, the diagonal of the box around every set's points and those queries, covers each set's own."""
+    """Index of the nearest ref point for every query, per set (ref, query: float64 device tensors, set s the rows
+    [off[s], off[s + 1]) of each, every ref set non-empty): the index into ref of each query's nearest point of its own
+    set, ties to the smaller index.  First within `reach`, then, for the queries with nothing that close, within the
+    diagonal of the box around every set's points and those queries, which covers each set's own, so none goes
+    unanswered.  One index build for the whole batch, and at most one more, shared by every set, for those queries."""
     _, idx = CloudIndex(ref, _query_cell(ref, reach), ref.device.index, set_offsets=ref_off).nearest_many(
         query, query_off, reach)
     miss = torch.nonzero(idx < 0).reshape(-1)
@@ -120,7 +104,7 @@ class MeanShift:
 
     fit(X) sets cluster_centers_ (K,3) in X's dtype, labels_ (N,) int64 and n_iter_, and also the per-seed results
     seed_centers_ (N,3), seed_counts_ (N,) (points within bandwidth of the final centre, 0 when none) and
-    seed_iters_ (N,).  X holds at most 2^21 points."""
+    seed_iters_ (N,); it is fit_many with one set.  X holds at most 2^21 points."""
 
     def __init__(self, bandwidth=None, cluster_all=True, n_jobs=None, seeds=None, bin_seeding=False, max_iter=300):
         self.bandwidth = bandwidth
@@ -147,33 +131,16 @@ class MeanShift:
             raise ValueError(f"MeanShift: max_iter must be an integer >= 0, got {it!r}")
 
     def fit(self, X, y=None):
-        self._check_params()
-        X = _as_points(X)
-        f64 = X.dtype in (torch.float64, np.float64)
-        ctx, x = _lib.inputs(X, dtype=torch.float64 if f64 else torch.float32)
-        bw = float(self.bandwidth)
-        index = CloudIndex(x, bw)
-        P = x.shape[0]
-        seed_c = torch.empty_like(x)
-        seed_n = torch.empty((P,), dtype=torch.int32, device=x.device)
-        seed_it = torch.empty_like(seed_n)
-        cen = torch.empty_like(x)
-        nc = torch.empty((1,), dtype=torch.int32, device=x.device)
-        ctx.call("cg_meanshift_dev", index.h, x, int(f64), bw, int(self.max_iter), seed_c, seed_n, seed_it, cen, nc)
-        centres = cen[:int(nc.item())].contiguous()
-        labels = _nearest(centres.to(torch.float64), x.to(torch.float64), LABEL_REACH * bw)
-        self.n_iter_ = int(seed_it.max().item())
-        (self.cluster_centers_, self.labels_, self.seed_centers_, self.seed_counts_,
-         self.seed_iters_) = _lib.returned(X, centres, labels, seed_c, seed_n.to(torch.int64), seed_it.to(torch.int64))
+        vars(self).update(vars(self.fit_many([X])[0]))
         return self
 
     def fit_predict(self, X, y=None):
         return self.fit(X).labels_
 
     def fit_many(self, Xs):
-        """fit for several point sets in one pass: a list of fitted MeanShift instances, the s-th equal to
-        ``MeanShift(bandwidth, max_iter=...).fit(Xs[s])`` bit for bit.  The sets are numpy arrays or CUDA tensors
-        (not mixed) of one dtype, each of at most 2^21 points; results come back as fit returns them."""
+        """fit for several point sets in one pass: a list of fitted MeanShift instances, the s-th as fit leaves it
+        for Xs[s] alone, bit for bit.  The sets are numpy arrays or CUDA tensors (not mixed) of one dtype, each of at
+        most 2^21 points; each set's results come back in its own kind and dtype."""
         self._check_params()
         Xs = [_as_points(X) for X in list(Xs)]
         if not Xs:
@@ -204,26 +171,8 @@ def pointgroup_labels(xyz_original_all, pt_offsets, cloud_xyz, bandwidth):
     """predicter.py:308-338 after the network: the 2 mm voxel down-sampling of the network's points, each voxel mean
     snapped to its nearest point, those points moved by their offsets (float32), clustered by MeanShift, and every
     point of cloud_xyz labelled with its nearest snapped point's cluster.  Returns (labels_all (M,) int64,
-    xyz_shifted (U,3) float32)."""
-    xo = _as_points(xyz_original_all)
-    off = _as_points(pt_offsets)
-    cloud = _as_points(cloud_xyz)
-    if off.shape[0] != xo.shape[0]:
-        raise ValueError("pt_offsets must have one row per point of xyz_original_all")
-    _, xo_d, off, cloud = _lib.inputs(xo, off, cloud, dtype=(torch.float32, torch.float32, torch.float64))
-    down, _ = CloudIndex(xo_d, DOWNSAMPLE).voxel_means()                                # :308-310
-    # :311-313 snap: a voxel mean and its members share a voxel, so the nearest member is within the diagonal; the
-    # bound is widened by 1e-9 relative so rounding at a voxel face cannot exclude it
-    snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)
-    _, ids = CloudIndex(xo_d, snap).nearest(down, snap)
-    if bool((ids < 0).any()):
-        raise _lib.CgError("pointgroup_labels: a voxel mean has no point within its voxel's diagonal")
-    ids = ids.to(torch.int64)
-    xyz_down = xo_d[ids]
-    xyz_shifted = xyz_down + off[ids]                                                    # :314, float32
-    labels = MeanShift(bandwidth=bandwidth).fit_predict(xyz_shifted)                      # :332
-    nearest = _nearest(xyz_down.to(torch.float64), cloud, LABEL_REACH * DOWNSAMPLE)
-    return _lib.returned(xyz_original_all, labels[nearest], xyz_shifted)                 # :334-336
+    xyz_shifted (U,3) float32): pointgroup_labels_many with one frame."""
+    return pointgroup_labels_many([xyz_original_all], [pt_offsets], [cloud_xyz], bandwidth)[0]
 
 
 def _pointgroup_labels_cat(xo, off, xo_off, cloud, cloud_off, bandwidth):
@@ -235,7 +184,9 @@ def _pointgroup_labels_cat(xo, off, xo_off, cloud, cloud_off, bandwidth):
     down, _ = ds.voxel_means()
     down_off = ds.cell_offsets
     del ds
-    snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)                                          # :311-313
+    # :311-313 snap: a voxel mean and its members share a voxel, so the nearest member is within the diagonal; the
+    # bound is widened by 1e-9 relative so rounding at a voxel face cannot exclude it
+    snap = DOWNSAMPLE * np.sqrt(3.0) * (1 + 1e-9)
     _, ids = CloudIndex(xo, snap, xo.device.index, set_offsets=xo_off).nearest_many(down, down_off, snap)
     if bool((ids < 0).any()):
         raise _lib.CgError("pointgroup_labels: a voxel mean has no point within its voxel's diagonal")
@@ -252,15 +203,13 @@ def _pointgroup_labels_cat(xo, off, xo_off, cloud, cloud_off, bandwidth):
 
 
 def pointgroup_labels_many(xyz_original_alls, pt_offsetss, cloud_xyzs, bandwidth):
-    """pointgroup_labels for several frames in one pass: a list of (labels_all, xyz_shifted), the b-th equal to
-    ``pointgroup_labels(xyz_original_alls[b], pt_offsetss[b], cloud_xyzs[b], bandwidth)`` bit for bit.  The frames
-    are numpy arrays or CUDA tensors (not mixed); results come back as pointgroup_labels returns them.  The number
-    of index builds and synchronisations does not grow with the number of frames."""
+    """pointgroup_labels for several frames in one pass: a list of (labels_all, xyz_shifted), the b-th as
+    pointgroup_labels gives it for frame b alone, bit for bit.  The arrays are numpy arrays or CUDA tensors; frame b's
+    results are CUDA tensors where xyz_original_alls[b] is one, else numpy.  The number of index builds and
+    synchronisations does not grow with the number of frames."""
     xos, offs, clouds = list(xyz_original_alls), list(pt_offsetss), list(cloud_xyzs)
     if not xos or len(offs) != len(xos) or len(clouds) != len(xos):
         raise ValueError("pointgroup_labels_many: need one offsets array and one cloud per frame, and a frame")
-    if len({getattr(a, "is_cuda", False) for a in xos + offs + clouds}) > 1:
-        raise ValueError("pointgroup_labels_many: the frames must be all numpy arrays or all CUDA tensors")
     xos, offs, clouds = [_as_points(a) for a in xos], [_as_points(a) for a in offs], [_as_points(a) for a in clouds]
     for b, (xo, off) in enumerate(zip(xos, offs)):
         if off.shape[0] != xo.shape[0]:

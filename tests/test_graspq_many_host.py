@@ -3,9 +3,10 @@
 - walk_grasp_many (the host-mode subsets of several objects in one walk of numpy's generator) equals a loop of
   draw_subsample_ids_numpy, id for id and in the generator's state afterwards: objects with M < n_pts, M == n_pts and
   M > n_pts, objects with no candidates, and stages cut at every chunk edge (1023 / 1024 / 1025).
-- graspq_fc_groups reproduces the launch cuts of the loop: GraspPredicter.score's own launches, recorded on a stand-in
-  network, cut at GRASPQ_CHUNK_B as cg_graspq_forward_dev cuts them.
-- A rejected list leaves numpy's generator untouched, in both subsample modes and with given ids.
+- graspq_fc_groups gives the launch cuts of a loop of one-object calls: ``chunk`` candidates per launch in host mode,
+  the whole list in device and given-ids modes, each launch cut at GRASPQ_CHUNK_B as cg_graspq_forward_dev cuts it.
+- A rejected list, or a rejected one-object score call, leaves numpy's generator untouched, in both subsample modes
+  and with given ids.
 - The Python constants match the header's, and the codegen of the two kernels the batched path extends.
 """
 import contextlib
@@ -70,29 +71,9 @@ def test_stages_pack_whole_groups():
     assert host_draw_stages([], 1024) == []
 
 
-class _Ctx:
-    def get_engine(self):
-        return 3
-
-    def set_engine(self, e):
-        pass
-
-    def fp16_overflow(self):
-        return False
-
-
 class _Net:
-    """Records the candidate count of every graspq_dev launch GraspPredicter.score makes."""
-    device, n_out, ctx = torch.device("cpu"), 2, _Ctx()
-
-    def __init__(self):
-        self.launches = []
-
-    def graspq_dev(self, xyz, nrm, poses, ids, mean, std, out):
-        self.launches.append(int(ids.shape[0]))
-
-    def draw_ids_dev(self, M, n_pts, count, seed, first_candidate=0):
-        return torch.zeros((count, n_pts), dtype=torch.int32)
+    """A stand-in network: the calls below return before any launch."""
+    device, n_out, ctx = torch.device("cpu"), 2, None
 
 
 def _predicter(n_pts=8, chunk=1024, subsample="host", net=None):
@@ -111,33 +92,38 @@ def _obj(M, seed, z=0.7):
     return {"cloud_xyz": xyz, "cloud_normal": rng.normal(size=(M, 3))}
 
 
+BIG = 2 * GRASPQ_CHUNK_B + 5
+# per (mode, chunk), the FC row groups of the counts that are not one group of themselves
+CUTS = {("host", 1024): {1025: [1024, 1], BIG: [1024] * 32 + [5]},
+        ("host", 3): {7: [3, 3, 1], 8: [3, 3, 2], 9: [3, 3, 3], 63: [3] * 21, 64: [3] * 21 + [1], 65: [3] * 21 + [2],
+                      1023: [3] * 341, 1024: [3] * 341 + [1], 1025: [3] * 341 + [2], BIG: [3] * 10924 + [1]},
+        ("host", 20000): {BIG: [GRASPQ_CHUNK_B, 20000 - GRASPQ_CHUNK_B, BIG - 20000]},
+        ("device", 1024): {BIG: [GRASPQ_CHUNK_B, GRASPQ_CHUNK_B, 5]},
+        ("given", 1024): {BIG: [GRASPQ_CHUNK_B, GRASPQ_CHUNK_B, 5]}}
+
+
 @pytest.mark.parametrize("mode, chunk", [("host", 1024), ("host", 3), ("host", 20000), ("device", 1024),
                                          ("given", 1024)])
-def test_groups_are_the_loops_launch_cuts(monkeypatch, mode, chunk):
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    counts = [0, 1, 7, 8, 9, 63, 64, 65, 1023, 1024, 1025, 2 * GRASPQ_CHUNK_B + 5]
-    launch = chunk if mode == "host" else None
-    groups, spans = graspq_fc_groups(counts, launch)
-    net = _Net()
-    p = _predicter(chunk=chunk, subsample="device" if mode == "device" else "host", net=net)
+def test_fc_groups_follow_the_launch_rule(mode, chunk):
+    """A one-object call launches ``chunk`` candidates at a time in host mode and its whole list in device and
+    given-ids modes, and cg_graspq_forward_dev runs each launch in passes of at most GRASPQ_CHUNK_B candidates."""
+    counts = [0, 1, 7, 8, 9, 63, 64, 65, 1023, 1024, 1025, BIG]
+    groups, spans = graspq_fc_groups(counts, chunk if mode == "host" else None)
     for o, B in enumerate(counts):
-        if B == 0:
-            continue
-        net.launches = []
-        data, poses = _obj(20, o), np.tile(np.eye(4), (B, 1, 1))
-        ids = np.zeros((B, 8), np.int32) if mode == "given" else None
-        p.score(data, poses, ids=ids)
-        # cg_graspq_forward_dev runs each launch in passes of at most GRASPQ_CHUNK_B candidates
-        want = [min(GRASPQ_CHUNK_B, L - k) for L in net.launches for k in range(0, L, GRASPQ_CHUNK_B)]
+        want = CUTS[mode, chunk].get(B, [B] if B else [])
         assert list(groups[spans[o, 0]:spans[o, 1]]) == want, (o, B)
     assert spans[0, 0] == spans[0, 1] and groups.sum() == sum(counts)
 
 
-def _rejects(p, datas, grasps, match, **kw):
+def _rejects(p, datas, grasps, match, ids=None, one=False):
+    """predict_batch_many(datas, grasps) raises, or with ``one`` score on the one object, and draws nothing."""
     np.random.seed(11)
     before = _state()
     with pytest.raises(ValueError, match=match):
-        p.predict_batch_many(datas, grasps, **kw)
+        if one:
+            p.score(datas[0], grasps[0], ids=None if ids is None else ids[0])
+        else:
+            p.predict_batch_many(datas, grasps, ids=ids)
     assert _same(before, _state())
 
 
@@ -155,6 +141,9 @@ def test_rejected_list_leaves_the_generator_untouched(mode):
     _rejects(p, [good, good], [g2, g2], "has shape", ids=[np.zeros((2, 8), np.int32), np.zeros((2, 7), np.int32)])
     _rejects(p, [good, good], [g2, g2], "indexes outside",
              ids=[np.zeros((2, 8), np.int32), np.full((2, 8), 30, np.int32)])
+    _rejects(p, [far], [g2], "cannot be empty unless no samples are taken", one=True)
+    _rejects(p, [good], [g2], "has shape", ids=[np.zeros((2, 7), np.int32)], one=True)
+    _rejects(p, [good], [g2], "indexes outside", ids=[np.full((2, 8), 30, np.int32)], one=True)
 
 
 def test_objects_without_candidates_are_not_checked(monkeypatch):

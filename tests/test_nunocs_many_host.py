@@ -1,7 +1,7 @@
 """CPU: NunocsPredicter.predict_many's host logic, which needs no device.
 
 - The whole list is checked before any random number is drawn: every rejected call leaves numpy's generator as it
-  was, including when the failing object comes after valid ones.
+  was, including when the failing object comes after valid ones, and so does a rejected one-object predict.
 - draw_nunocs_many (the host-mode draws of B objects in one walk of numpy's generator) equals the loop's draws, word for
   word: per object draw_subsample_ids' np.random.choice, then a _LegacyDraw of 2H RANSAC 4-subsets, and the same state
   afterwards.
@@ -41,11 +41,15 @@ def _same(a, b):
     return a[0] == b[0] and np.array_equal(a[1], b[1]) and a[2:] == b[2:]
 
 
-def _rejects(p, datas, match, **kw):
+def _rejects(p, datas, match, ids=None, one=False):
+    """predict_many(datas) raises, or with ``one`` predict on the one object, and draws nothing."""
     np.random.seed(11)
     before = _state()
     with pytest.raises(ValueError, match=match):
-        p.predict_many(datas, **kw)
+        if one:
+            p.predict(datas[0], ids=None if ids is None else ids[0])
+        else:
+            p.predict_many(datas, ids=ids)
     assert _same(before, _state())
 
 
@@ -55,6 +59,7 @@ def test_empty_masked_cloud_is_rejected_before_any_draw(mode):
     far = _obj(50, 2, z=0.05)                      # every point below z = 0.1: predict's np.random.choice raises
     _rejects(p, [_obj(100, 1), _obj(30, 3), far], "cannot be empty unless no samples are taken")
     _rejects(p, [far], "cannot be empty")
+    _rejects(p, [far], "cannot be empty", one=True)
 
 
 def test_malformed_and_mixed_inputs_are_rejected_before_any_draw():
@@ -71,6 +76,8 @@ def test_malformed_and_mixed_inputs_are_rejected_before_any_draw():
     _rejects(p, [good], "ids\\[0\\] has shape", ids=[np.arange(10)])
     _rejects(p, [good, good], "indexes outside", ids=[None, np.arange(64) + 40])
     _rejects(p, [good, good], "indexes outside", ids=[np.arange(64) - 1, None])
+    _rejects(p, [good], "ids\\[0\\] has shape", ids=[np.arange(10)], one=True)
+    _rejects(p, [good], "indexes outside", ids=[np.arange(64) + 40], one=True)
 
 
 def test_bad_kdtree_resolution_is_rejected_before_any_draw():
@@ -82,6 +89,7 @@ def test_bad_kdtree_resolution_is_rejected_before_any_draw():
 
 def test_too_few_points_per_object_is_rejected_before_any_draw():
     _rejects(_predicter(n_pts=3), [_obj(100, 1)], "larger sample than population")
+    _rejects(_predicter(n_pts=3), [_obj(100, 1)], "larger sample than population", one=True)
 
 
 def test_empty_list_draws_nothing():

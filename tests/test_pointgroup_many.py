@@ -266,6 +266,8 @@ def test_predict_many_rejections(predictor):
     with pytest.raises(KeyError) as err:
         predictor.predict_many([good, no_normal])
     assert err.value.args == loop_err.value.args
+    with pytest.raises(ValueError, match="M >= 1"):
+        predictor.predict({"cloud_xyz": good["cloud_xyz"][:0], "cloud_normal": good["cloud_normal"][:0]})
     assert ctx.launch_count() == 0 and predictor.xyz_shifted is marker
 
 
