@@ -22,7 +22,8 @@
 // the same as moving the line by (eps, eps^2) in (y, z): a closed mesh is crossed an even number of times on every
 // line.  A crossing at x_c counts for every node with x_i > x_c; a line with an odd total means the mesh is open and
 // the build fails.  Snapping moves the geometry by at most res * 2^-17, so the sign is exact for nodes farther than that
-// from the surface.
+// from the surface.  Parity is not the winding number: where closed parts overlap, a line crosses two surfaces and the
+// overlap comes out positive (outside), as SDFGen's odd-crossing rule gives it.  That is the contract, not a bug to fix.
 #include <math.h>
 #include <algorithm>
 #include "cg_common.cuh"

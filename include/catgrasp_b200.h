@@ -256,8 +256,10 @@ int cg_sdf_lookup_dev(cg_sdf *sdf, const float *grid_coords, int P, int mode,
  * Node (i,j,k) lies at origin + (i,j,k) * resolution (float64 from the float32
  * values).  Each value is the exact distance from the node to the nearest
  * triangle, computed in float64 and rounded once to float32, negative inside
- * (ray parity along x).  Errors (CG_EINVAL, no handle created): nv or nf <= 0,
- * an index out of range, a non-finite vertex, resolution <= 0 or not finite,
+ * (ray parity along x: where closed parts overlap, the overlap is positive,
+ * as with SDFGen's odd crossing count).  Errors (CG_EINVAL, no handle
+ * created): nv or nf <= 0, an index out of range, a non-finite vertex,
+ * resolution <= 0 or not finite,
  * padding < 0, more than 2048 nodes along an axis, a mesh that is not closed.
  * CG_ENOMEM when the device is out of memory.                              */
 int cg_sdf_from_mesh(cg_ctx *ctx, const double *vertices, int nv, const int32_t *faces, int nf,

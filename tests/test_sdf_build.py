@@ -1,11 +1,15 @@
-"""The mesh -> signed-distance grid builder (csrc/cg_sdf_build.cu, Sdf3D.from_mesh) and its float64 oracle
-(oracle/sdf_mesh_ref.c: brute-force distance, sign by winding number).
+"""The mesh -> signed-distance grid builder (csrc/cg_sdf_build.cu, Sdf3D.from_mesh) and its oracles
+(oracle/sdf_mesh_ref.c: brute-force float64 distance, sign by winding number; oracle/sdf_parity_exact.py: the exact
+ray parity of the builder's contract).
 
-CPU tests pin the oracle: against the analytic box-union SDF of the gripper proxy, a numpy restatement, half-space tests
-on convex hulls and an analytic inside test of a hex nut with a bore.  GPU tests compare the builder with the oracle
-node by node (|delta| <= 1 float32 ulp, equal signs wherever |d| >= res * 2^-12, exact geometry, bitwise repeatable),
-check that bad input is refused, and run the collision filter on built grids."""
+CPU tests pin the distance oracle: against the analytic box-union SDF of the gripper proxy, a numpy restatement,
+half-space tests on convex hulls and an analytic inside test of a hex nut with a bore.  GPU tests compare the builder
+with the oracles node by node (magnitudes equal to float32(|d_ref|) bit for bit, signs equal to the exact parity
+wherever |d| > res * 2^-16 and to the winding number wherever |d| >= res * 2^-12, exact geometry, bitwise repeatable),
+check that bad input is refused, and run the collision filter on built grids.  tests/test_sdf_build_edges.py takes
+the builder to its grid, brick, tile and lattice edges."""
 import ctypes as C
+from fractions import Fraction
 
 import numpy as np
 import pytest
@@ -13,8 +17,10 @@ import pytest
 from catgrasp_b200.synthetic import (_box_mesh, _box_sdf, hex_nut_mesh_inside, make_filter_case, make_gripper_proxy,
                                      make_hex_nut_mesh, tessellated_box_mesh)
 from oracle.sdf_mesh_ref import grid_geometry, node_positions, sdf_mesh_ref
+from oracle.sdf_parity_exact import parity_lines
 
-SIGN_TOL = 2.0 ** -12          # signs are compared where |d_ref| >= res * 2^-12
+SIGN_TOL = 2.0 ** -12          # winding-number signs are compared where |d_ref| >= res * 2^-12
+PARITY_TOL = 2.0 ** -16        # parity signs where |d_ref| > res * 2^-16: twice the snap bound of the builder
 
 
 def _proxy_boxes(name):
@@ -186,8 +192,8 @@ def _gpu_case(name):
     if name in ("proxy_open", "proxy_enclosed"):
         d = g[name.split("_")[1]]
         return d["V"], d["F"], 0.001, 5, None
-    if name == "proxy_pad0":
-        return g["open"]["V"], g["open"]["F"], 0.001, 0, None
+    if name in ("proxy_pad0", "proxy_pad1"):
+        return g["open"]["V"], g["open"]["F"], 0.001, int(name[-1]), None
     if name == "proxy_tess200k":
         V, F = _tessellated_proxy("open", 75)
         return V, F, 0.001, 5, (1500, 50)
@@ -209,29 +215,56 @@ def _gpu_case(name):
     raise KeyError(name)
 
 
-GPU_CASES = ["proxy_open", "proxy_enclosed", "proxy_pad0", "proxy_tess200k", "hex_nut", "hull0", "hull1", "thin_shell",
-             "dyadic", "degenerate_pair"]
+GPU_CASES = ["proxy_open", "proxy_enclosed", "proxy_pad0", "proxy_pad1", "proxy_tess200k", "hex_nut", "hull0", "hull1",
+             "thin_shell", "dyadic", "degenerate_pair"]
 
 
-def _check_nodes(built, V, F, res, idx):
-    origin = built.origin_
+def on_lattice(V, origin, res):
+    """True when every vertex coordinate is origin + an integer multiple of res * 2^-16 exactly (small meshes only):
+    the builder's snap then moves nothing, so its sign is the exact parity at every node, on the surface too."""
+    V = np.asarray(V, np.float64)
+    if V.size > 3000:
+        return False
+    step = Fraction(float(res)) / 2 ** 16
+    return all(((Fraction(float(v)) - Fraction(float(o))) / step).denominator == 1 for col, o in zip(V.T, origin)
+               for v in col)
+
+
+def check_nodes(built, V, F, idx, winding=True):
+    """Compare the built grid with the oracles at the nodes idx (n, 3): |value| equal to float32(|d_ref|) bit for bit,
+    the sign equal to the exact ray parity wherever |d_ref| > res * 2^-16 (at every node, zeros included, when the
+    mesh lies on the snap lattice), and (``winding``: closed non-overlapping meshes, where the two rules coincide) to
+    the winding number wherever |d_ref| >= res * 2^-12.
+    Returns (nodes checked, signs decided by parity, magnitude mismatches, inside nodes)."""
+    origin, res = built.origin_, built.resolution_
     sd, _ = sdf_mesh_ref(V, F, node_positions(origin, res, idx))
-    ref = sd.astype(np.float32)
     got = built.data_[idx[:, 0], idx[:, 1], idx[:, 2]]
     assert np.all(np.isfinite(got))
-    mag_err = np.abs(np.abs(got).astype(np.float64) - np.abs(ref).astype(np.float64))
-    ulp = np.spacing(np.abs(ref)).astype(np.float64)
-    bad = mag_err > ulp
-    assert not bad.any(), (idx[bad][:5], got[bad][:5], sd[bad][:5])
-    decided = np.abs(sd) >= res * SIGN_TOL
-    wrong = decided & (np.signbit(got) != (sd < 0))
-    assert not wrong.any(), (idx[wrong][:5], got[wrong][:5], sd[wrong][:5])
-    return int(decided.sum()), int((sd < 0).sum())
+    mag = np.abs(got).view(np.uint32) != np.abs(sd).astype(np.float32).view(np.uint32)
+    assert not mag.any(), (int(mag.sum()), idx[mag][:5], got[mag][:5], sd[mag][:5])
+    lines, inv = np.unique(idx[:, 1:], axis=0, return_inverse=True)
+    inside, open_, _ = parity_lines(V, F, origin, res, built.dims_, lines)
+    assert not open_.any()
+    par = inside[inv.reshape(-1), idx[:, 0]]
+    decided = (np.abs(sd) > res * PARITY_TOL) | on_lattice(V, origin, res)
+    wrong = decided & (np.signbit(got) != par)
+    assert not wrong.any(), (int(wrong.sum()), idx[wrong][:5], got[wrong][:5], sd[wrong][:5])
+    if winding:
+        wdec = np.abs(sd) >= res * SIGN_TOL
+        wrong = wdec & (np.signbit(got) != (sd < 0))
+        assert not wrong.any(), (idx[wrong][:5], got[wrong][:5], sd[wrong][:5])
+    return idx.shape[0], int(decided.sum()), int(mag.sum()), int((decided & par).sum())
+
+
+def report(capsys, name, stats):
+    n, dec, mis, ins = stats
+    with capsys.disabled():
+        print(f"\n  {name}: {n} nodes checked, {dec} signs decided ({ins} inside), {mis} magnitude mismatches")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", GPU_CASES)
-def test_builder_matches_oracle(name):
+def test_builder_matches_oracle(name, capsys):
     _cuda()
     from catgrasp_b200.sdf import Sdf3D
     V, F, res, pad, sample = _gpu_case(name)
@@ -248,8 +281,9 @@ def test_builder_matches_oracle(name):
         jj, kk = np.meshgrid(np.arange(dims[1]), np.arange(dims[2]), indexing="ij")
         slab = np.stack([np.full(jj.size, i_slab), jj.reshape(-1), kk.reshape(-1)], 1)
         idx = np.concatenate([rand, slab])
-    n_dec, n_in = _check_nodes(built, V, F, float(res32), idx)
-    assert n_in > 0 and n_dec > idx.shape[0] // 2
+    stats = check_nodes(built, V, F, idx)
+    report(capsys, name, stats)
+    assert stats[3] > 0 and stats[1] > idx.shape[0] // 2
     again = Sdf3D.from_mesh(V, F, res, pad)
     assert np.array_equal(again.data_.view(np.uint32), built.data_.view(np.uint32))
 
