@@ -163,6 +163,7 @@ SIGNATURES = {
     "cg_cloud_nearest_many_dev": (_i, [_vp, _D, _H, _i, _d, _D, _D], TORCH),
     "cg_cloud_radius_mask_dev": (_i, [_vp, _D, _i, _d, _i, _D], TORCH),
     "cg_cloud_normals_dev": (_i, [_vp, _d, _i, _H, _D, _D, _D], TORCH),
+    "cg_cloud_normals_many_dev": (_i, [_vp, _d, _i, _H, _D, _D, _D], TORCH),
     "cg_meanshift_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_meanshift_many_dev": (_i, [_vp, _D, _i, _d, _i, _D, _D, _D, _D, _D], TORCH),
     "cg_spconv_index_dev": (_i, [_vp, _D, _i, _D, _D, _D, _D], TORCH),
@@ -173,6 +174,7 @@ SIGNATURES = {
     "cg_pointgroup_voxel_mean_dev": (_i, [_vp, _D, _i, _i, _D, _D, _i, _D], TORCH),
     "cg_pointgroup_head_dev": (_i, [_vp, _D, _i, _D, _i, _D, _D, _D, _D, _D, _D, _D, _i, _D, _D], TORCH),
     "cg_segment_table_dev": (_i, [_vp, _D, _i, _D, _i, _i, _i, _D, _D, _D, _D, _D, _D, _D, _D, _D], TORCH),
+    "cg_segment_table_many_dev": (_i, [_vp, _D, _i, _D, _i, _i, _H, _H, _D, _D, _D, _D, _D, _D, _D, _D, _D], TORCH),
     "cg_rank_grasps_dev": (_i, [_vp, _D, _i, _i, _i, _D, _D, _D, _D], TORCH),
     "cg_square_distance_dev": (_i, [_vp, _D, _D, _i, _i, _i, _D], TORCH),
     "cg_index_points_dev": (_i, [_vp, _D, _D, _i, _i, _i, _i, _D], TORCH),

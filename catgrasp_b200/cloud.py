@@ -29,9 +29,9 @@ class CloudIndex:
 
     With ``set_offsets`` (S + 1 ints from 0 to the point count) the points are S sets laid end to end, set s the rows
     [set_offsets[s], set_offsets[s + 1]), each binned as a one-set index over it alone would bin it (its own origin);
-    ``cell_offsets`` then gives each set's cells, ``voxel_means`` comes out set-major and ``nearest_many`` searches
-    each query's own set.  A set with no points raises ValueError; a batch whose cell keys need more than 63 bits
-    raises CgError.  ``nearest``, ``within`` and ``normals`` need a one-set index."""
+    ``cell_offsets`` then gives each set's cells, ``voxel_means`` comes out set-major, and ``nearest_many`` and
+    ``normals_many`` search each point's own set.  A set with no points raises ValueError; a batch whose cell keys need
+    more than 63 bits raises CgError.  ``nearest``, ``within`` and ``normals`` need a one-set index."""
 
     def __init__(self, pts, cell, device=None, set_offsets=None):
         self.ctx, p = _lib.inputs(pts, dtype=torch.float64, ctx=None if device is None else _lib.Context.get(device))
@@ -114,6 +114,17 @@ class CloudIndex:
         self.ctx.call("cg_cloud_normals_dev", self.h, float(radius), int(max_nn), vp, out, nbr, cnt)
         return (out, nbr, cnt) if neighbours else out
 
+    def normals_many(self, radius, max_nn, view_port=(0.0, 0.0, 0.0), neighbours=False):
+        """normals per set, one view point for all: set s's rows are what ``normals`` gives on a one-set index of
+        set s alone, bit for bit, whatever either index's cell; neighbour ids index the whole index (set s's first
+        point added, -1 padding kept)."""
+        out = self._empty(self.n_points, 3)
+        nbr = self._empty(self.n_points, max_nn, dtype=torch.int32) if neighbours else None
+        cnt = self._empty(self.n_points, dtype=torch.int32) if neighbours else None
+        vp = np.ascontiguousarray(view_port, dtype=np.float64).reshape(3)
+        self.ctx.call("cg_cloud_normals_many_dev", self.h, float(radius), int(max_nn), vp, out, nbr, cnt)
+        return (out, nbr, cnt) if neighbours else out
+
 
 def _query_cell(pts, r):
     """Cell size for an index queried at radius r: r itself, but no finer than 1/2^20 of the cloud's largest extent
@@ -126,12 +137,31 @@ def _query_cell(pts, r):
     return max(float(r), span / 2.0 ** 20, 1e-12)
 
 
-def depth2xyzmap(depth, K):
+def _query_cell_many(p, off, r):
+    """The largest of the non-empty sets' _query_cell: every set of ``p`` (N,3), rows [off[s], off[s + 1]), then spans
+    fewer than 2^21 cells per axis.  One read of the spans on a CUDA tensor, whatever the number of sets."""
+    rows = [(a, b) for a, b in zip(off[:-1], off[1:]) if b > a]
+    if isinstance(p, torch.Tensor):
+        span = float(torch.stack([(p[a:b].amax(0) - p[a:b].amin(0)).max() for a, b in rows]).max())
+    else:
+        span = max(float((p[a:b].max(0) - p[a:b].min(0)).max()) for a, b in rows)
+    return max(float(r), span / 2.0 ** 20, 1e-12)
+
+
+def depth2xyzmap(depth, K, out=None):
     """Utils.py:239-251 (called at run_grasp_simulation.py:198): (H,W) depth, float32 or float64 -> (H,W,3) float32
-    camera-frame points; pixels with depth < 0.1 are (0,0,0)."""
+    camera-frame points; pixels with depth < 0.1 are (0,0,0).  ``out``: a contiguous float32 CUDA tensor of H*W*3
+    elements on the depth's device to write the points into (a frame's slice of a buffer shared by several frames),
+    returned as it is."""
     d = depth if isinstance(depth, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(depth))
     ctx, d = _lib.inputs(d, dtype=d.dtype if d.dtype in (torch.float32, torch.float64) else torch.float64)
     H, W = d.shape[:2]
+    if out is not None:
+        if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == H * W * 3):
+            raise ValueError(f"depth2xyzmap: out must be a contiguous float32 CUDA tensor of {H * W * 3} elements")
+        ctx.call("cg_depth2xyz_dev", ctx.h, d, int(d.dtype == torch.float64), H, W,
+                 np.ascontiguousarray(K, dtype=np.float64).reshape(9), out)
+        return out
     out = torch.empty((H, W, 3), dtype=torch.float32, device=d.device)
     ctx.call("cg_depth2xyz_dev", ctx.h, d, int(d.dtype == torch.float64), H, W,
              np.ascontiguousarray(K, dtype=np.float64).reshape(9), out)
@@ -180,6 +210,21 @@ def estimate_normals(pts, radius, max_nn, view_port=(0.0, 0.0, 0.0)):
         z = np.zeros((0, 3))
         return torch.from_numpy(z).to(pts.device) if getattr(pts, "is_cuda", False) else z
     return _lib.returned(pts, CloudIndex(pts, _query_cell(pts, radius)).normals(radius, max_nn, view_port))
+
+
+def estimate_normals_many(pts, set_offsets, radius, max_nn, view_port=(0.0, 0.0, 0.0)):
+    """estimate_normals per set, in one index build: ``pts`` (N,3) holds S sets laid end to end, set s the rows
+    [set_offsets[s], set_offsets[s + 1]) (S + 1 ascending offsets from 0 to N; a set may be empty).  Returns (N,3)
+    float64, set s's rows equal to estimate_normals on set s alone, bit for bit.  Synchronises three times whatever S
+    is (the cell size, the index build's two).  One view point serves every set."""
+    off = _offsets(set_offsets, pts.shape[0], "estimate_normals_many").astype(np.int64)
+    if pts.shape[0] == 0:
+        z = np.zeros((0, 3))
+        return torch.from_numpy(z).to(pts.device) if getattr(pts, "is_cuda", False) else z
+    kept = np.concatenate([[0], np.cumsum(np.diff(off)[np.diff(off) > 0])])    # empty sets have no rows to index
+    p = pts.reshape(-1, 3)
+    cell = _query_cell_many(p, off, radius)
+    return _lib.returned(pts, CloudIndex(p, cell, set_offsets=kept).normals_many(radius, max_nn, view_port))
 
 
 def prepare_object(ob_pts, ob_normals, scene_pts, gripper_diameter, octo_resolution=0.001, K=None):

@@ -16,7 +16,8 @@
 // holds every set's largest cell, and the set field takes bit_length(S - 1) bits; a batch whose key needs more than
 // 63 bits is refused.  So the sorted points, the cell table and the voxel means are set-major, and set s's block is its
 // one-set index shifted by its first point (perm, start) and carrying its prefix (keys).  S = 1 is today's layout.  A
-// query of set s searches set s's cells only (IndexView::in_set); the build synchronises twice whatever S is.
+// query of set s searches set s's cells only (IndexView::in_set); the build synchronises twice whatever S is.  The
+// many-set queries are nearest (queries carry a set table) and normals (each sorted point finds its set from poff).
 //
 // Decisions are float64 with the reference's operation order and no FMA contraction:
 //   d2 = (dx*dx + dy*dy) + dz*dz     scipy's sqeuclidean_distance_double (cKDTree.query, query_ball_point)
@@ -313,13 +314,19 @@ __device__ void smallest_eigvec(double a[3][3], double out[3]) {
   for (int k = 0; k < 3; k++) out[k] = m == 0 ? v[k][0] : (m == 1 ? v[k][1] : v[k][2]);
 }
 
-__global__ void __launch_bounds__(NW * 32) normals_kernel(IndexView V, int P, double r, double r2, int max_nn, double vx,
-                                                          double vy, double vz, double *__restrict__ out_n,
-                                                          int32_t *__restrict__ out_nbr, int32_t *__restrict__ out_cnt) {
+// A many-set index (V0.S > 1): sorted point j belongs to the set whose point range holds j (the sorted points are
+// set-major) and searches that set's cells only, so its neighbours, counts and normal are those of a one-set index over
+// the set alone; ids stay indices into the whole index.  The minimum of one CTA per SM keeps ptxas from trading the
+// set's view for a stack frame and spills.
+__global__ void __launch_bounds__(NW * 32, 1) normals_kernel(IndexView V0, int P, double r, double r2, int max_nn,
+                                                             double vx, double vy, double vz, double *__restrict__ out_n,
+                                                             int32_t *__restrict__ out_nbr, int32_t *__restrict__ out_cnt) {
   __shared__ NbrBuf bufs[NW];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   NbrBuf &B = bufs[w];
   for (int j = blockIdx.x * NW + w; j < P; j += gridDim.x * NW) {
+    IndexView V = V0;
+    if (V0.S > 1) V = V0.in_set(set_of(V0.poff, V0.S, j));
     const double qx = V.spts[3 * (size_t)j], qy = V.spts[3 * (size_t)j + 1], qz = V.spts[3 * (size_t)j + 2];
     const Columns C(V, qx, qy, qz, r);
     int n = 0;
@@ -692,14 +699,15 @@ extern "C" int cg_cloud_radius_mask_dev(const cg_cloud_index *ix, const double *
   return CG_OK;
 }
 
-extern "C" int cg_cloud_normals_dev(const cg_cloud_index *ix, double radius, int max_nn, const double *view_point,
-                                    double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count) {
-  if (!ix) return CG_EINVAL;
+namespace {
+
+// the one launch behind cg_cloud_normals_dev and cg_cloud_normals_many_dev; a many-set index's sets are in its view
+int cloud_normals(const cg_cloud_index *ix, const char *what, double radius, int max_nn, const double *view_point,
+                  double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count) {
   cg_ctx *ctx = ix->ctx;
-  CG_REQUIRE(ctx, ix->S == 1, "cloud_normals: the index holds several sets; normals are per one-set index");
-  CG_REQUIRE(ctx, view_point && out_normals, "cloud_normals: null argument");
-  CG_REQUIRE(ctx, radius >= 0.0 && std::isfinite(radius), "cloud_normals: radius must be finite and >= 0");
-  CG_REQUIRE(ctx, max_nn >= 1 && max_nn <= CG_CLOUD_MAX_NN, "cloud_normals: 1 <= max_nn <= CG_CLOUD_MAX_NN");
+  CG_REQUIRE(ctx, view_point && out_normals, std::string(what) + ": null argument");
+  CG_REQUIRE(ctx, radius >= 0.0 && std::isfinite(radius), std::string(what) + ": radius must be finite and >= 0");
+  CG_REQUIRE(ctx, max_nn >= 1 && max_nn <= CG_CLOUD_MAX_NN, std::string(what) + ": 1 <= max_nn <= CG_CLOUD_MAX_NN");
   static_assert(CG_CLOUD_MAX_NN <= NRM_CAP - 32, "compaction must free room");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   const int grid = (int)std::min<int64_t>(blocks(ix->P, NW), 16 * (int64_t)ctx->num_sms);
@@ -707,4 +715,19 @@ extern "C" int cg_cloud_normals_dev(const cg_cloud_index *ix, double radius, int
                                                     view_point[1], view_point[2], out_normals, out_nbr, out_nbr_count);
   CG_LAUNCH_CHECK(ctx);
   return CG_OK;
+}
+
+}  // namespace
+
+extern "C" int cg_cloud_normals_dev(const cg_cloud_index *ix, double radius, int max_nn, const double *view_point,
+                                    double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count) {
+  if (!ix) return CG_EINVAL;
+  CG_REQUIRE(ix->ctx, ix->S == 1, "cloud_normals: the index holds several sets; use cg_cloud_normals_many_dev");
+  return cloud_normals(ix, "cloud_normals", radius, max_nn, view_point, out_normals, out_nbr, out_nbr_count);
+}
+
+extern "C" int cg_cloud_normals_many_dev(const cg_cloud_index *ix, double radius, int max_nn, const double *view_point,
+                                         double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count) {
+  if (!ix) return CG_EINVAL;
+  return cloud_normals(ix, "cloud_normals_many", radius, max_nn, view_point, out_normals, out_nbr, out_nbr_count);
 }

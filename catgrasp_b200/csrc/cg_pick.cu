@@ -11,6 +11,13 @@
 // reversed(sorted(items, key=count)) gives them.  The kept points are grouped by one stable radix sort of (rank in
 // that order, point index), so each segment's indices come out ascending, as `scene_seg == seg_id` selects them.
 //
+// Several frames (cg_segment_table_many_dev) run as one table of L = sum L_b labels: frame b's labels are the rows
+// [loff[b], loff[b+1]) and its points [poff[b], poff[b+1]).  A kernel finds a point's or a row's frame by a binary
+// search of those offsets (null for one frame) and shifts frame-local labels to rows and back.  The label sort is
+// segmented by frame; the point sort key is frame b's offset slot (loff[b] + b) plus the rank, so frame b's points
+// stay in its own range [poff[b], poff[b+1]); the offsets are one scan by frame over L + B slots, each frame's first
+// slot 0.  Every output block is what the one-frame table of that frame gives, bit for bit.
+//
 // Ranking.  p_G = (pred * arange(C)).sum() / denom, denom = len(cfg_grasp['classes']) - 1, with numpy's pairwise
 // summation order (8 <= C <= 128: eight accumulators over the first C - C % 8 terms, combined
 // ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the rest in sequence; C < 8: left to right).  The products are exact in float64.  The permutation is Python's stable
@@ -34,6 +41,16 @@ __device__ __forceinline__ double ord_val(uint64_t k) {
   return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
 }
 
+// the b with off[b] <= i < off[b + 1] (off ascending from 0, ranges may be empty, 0 <= i < off[B])
+__device__ __forceinline__ int frame_of(const int32_t *__restrict__ off, int B, int64_t i) {
+  int lo = 0, hi = B;
+  while (hi - lo > 1) {
+    const int m = (lo + hi) >> 1;
+    if (off[m] <= i) lo = m; else hi = m;
+  }
+  return lo;
+}
+
 __device__ __forceinline__ int64_t load_label(const void *labels, int is_i64, int64_t i) {
   return is_i64 ? static_cast<const int64_t *>(labels)[i] : (int64_t) static_cast<const int32_t *>(labels)[i];
 }
@@ -52,10 +69,13 @@ __global__ void seg_init_kernel(int L, int32_t *__restrict__ count, uint64_t *__
   }
 }
 
-// count, min and max per label; labels outside [0, L) are skipped.  SMEM: per-CTA privatised tables (L <= ST_SMEM_L)
+// count, min and max per label; labels outside [0, L) are skipped.  SMEM: per-CTA privatised tables (L <= ST_SMEM_L).
+// Several frames (poff non-null): point i's frame-local label l is row loff[b] + l, skipped outside [0, L_b)
 template <bool SMEM>
 __global__ void __launch_bounds__(ST_THREADS) seg_stats_kernel(const void *__restrict__ labels, int lab_i64,
                                                                const void *__restrict__ x, int x_f64, int M, int L,
+                                                               const int32_t *__restrict__ poff,
+                                                               const int32_t *__restrict__ loff, int B,
                                                                int32_t *__restrict__ count,
                                                                uint64_t *__restrict__ kmin,
                                                                uint64_t *__restrict__ kmax) {
@@ -74,8 +94,14 @@ __global__ void __launch_bounds__(ST_THREADS) seg_stats_kernel(const void *__res
   int32_t *cnt = SMEM ? s_cnt : count;
   uint64_t *mn = SMEM ? s_min : kmin, *mx = SMEM ? s_max : kmax;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t l = load_label(labels, lab_i64, i);
-    if (l < 0 || l >= L) continue;
+    int64_t l = load_label(labels, lab_i64, i);
+    if (poff) {
+      const int b = frame_of(poff, B, i);
+      if (l < 0 || l >= loff[b + 1] - loff[b]) continue;
+      l += loff[b];
+    } else if (l < 0 || l >= L) {
+      continue;
+    }
     atomicAdd(&cnt[l], 1);
     for (int a = 0; a < 3; a++) {
       const unsigned long long k = ord_key(load_x(x, x_f64, 3 * i + a));
@@ -134,43 +160,58 @@ __global__ void seg_decide_kernel(int L, int x_f64, const int32_t *__restrict__ 
   sort_key[l] = inlier ? ((uint64_t)n << 32) | (uint32_t)l : 0ull;   // kept keys are > 0: n >= 500
 }
 
-// the sorted keys -> the kept labels in order, their rank per label, and the kept count
+// the sorted keys -> the kept labels in order (frame-local), their rank per row, the kept count per frame, and the
+// offset slots: frame b's slot loff[b] + b is 0 and slot loff[b] + b + 1 + k the k-th kept segment's count (0 past
+// the kept ones).  Several frames (loff non-null): each slot's frame also goes to slot_frame, the scan's key
 __global__ void seg_order_kernel(int L, const uint64_t *__restrict__ sorted_key, const uint8_t *__restrict__ inlier,
-                                 int32_t *__restrict__ order, int32_t *__restrict__ rank,
-                                 int32_t *__restrict__ n_kept, int32_t *__restrict__ seg_len) {
+                                 const int32_t *__restrict__ loff, int B, int32_t *__restrict__ order,
+                                 int32_t *__restrict__ rank, int32_t *__restrict__ n_kept, int32_t *__restrict__ seg_len,
+                                 int32_t *__restrict__ slot_frame) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= L) return;
+  const int b = loff ? frame_of(loff, B, k) : 0;
+  const int base = loff ? loff[b] : 0, Lb = loff ? loff[b + 1] - base : L, kk = k - base;
+  int32_t *len = seg_len + base + b;
   const uint64_t key = sorted_key[k];
   if (key) {
     const int l = (int)(uint32_t)key;
-    order[k] = l;
-    rank[l] = k;
-    seg_len[k] = (int32_t)(key >> 32);
-    if (k + 1 == L || sorted_key[k + 1] == 0ull) *n_kept = k + 1;
+    order[k] = l - base;
+    rank[l] = kk;
+    len[kk + 1] = (int32_t)(key >> 32);
+    if (kk + 1 == Lb || sorted_key[k + 1] == 0ull) n_kept[b] = kk + 1;
   } else {
     order[k] = -1;
-    seg_len[k] = 0;
-    if (k == 0) *n_kept = 0;
+    len[kk + 1] = 0;
+    if (kk == 0) n_kept[b] = 0;
+  }
+  if (kk == 0) len[0] = 0;
+  if (slot_frame) {
+    slot_frame[base + b + kk + 1] = b;
+    if (kk == 0) slot_frame[base + b] = b;
   }
   if (!inlier[k]) rank[k] = -1;
 }
 
 // scene_seg with outliers set to -1 (:240), and the compaction key of every point: its segment's rank, or L past the
-// last segment
+// last segment.  Several frames (poff non-null): the rank plus frame b's offset slot loff[b] + b, L_b past its last
+// segment, and the point's index within its frame
 __global__ void seg_points_kernel(const void *__restrict__ labels, int lab_i64, int M, int L,
+                                  const int32_t *__restrict__ poff, const int32_t *__restrict__ loff, int B,
                                   const int32_t *__restrict__ rank, void *__restrict__ out_labels,
                                   uint32_t *__restrict__ pkey, int32_t *__restrict__ pval) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M) return;
+  const int b = poff ? frame_of(poff, B, i) : 0;
+  const int base = poff ? loff[b] : 0, Lb = poff ? loff[b + 1] - base : L;
   const int64_t l = load_label(labels, lab_i64, i);
-  const int r = (l >= 0 && l < L) ? rank[l] : -1;
+  const int r = (l >= 0 && l < Lb) ? rank[base + l] : -1;
   const int64_t out = r >= 0 ? l : -1;
   if (lab_i64)
     static_cast<int64_t *>(out_labels)[i] = out;
   else
     static_cast<int32_t *>(out_labels)[i] = (int32_t)out;
-  pkey[i] = r >= 0 ? (uint32_t)r : (uint32_t)L;
-  pval[i] = i;
+  pkey[i] = (uint32_t)(base + b) + (r >= 0 ? (uint32_t)r : (uint32_t)Lb);
+  pval[i] = poff ? i - poff[b] : i;
 }
 
 // numpy's pairwise_sum (loops_utils.h) for n <= 128 terms
@@ -211,69 +252,132 @@ __global__ void rank_score_kernel(const float *__restrict__ probs, int G, int C,
 
 }  // namespace
 
-extern "C" int cg_segment_table_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64,
-                                    int M, int L, void *out_labels, int32_t *out_count, double *out_min,
-                                    double *out_max, uint8_t *out_inlier, int32_t *out_order, int32_t *out_n_kept,
-                                    int32_t *out_offsets, int32_t *out_index) {
-  if (!ctx) return CG_EINVAL;
-  CG_REQUIRE(ctx, M >= 0 && L >= 1 && L < (1 << 30), "segment_table: M must be >= 0 and L in [1, 2^30)");
+namespace {
+
+// The one table behind cg_segment_table_dev (B = 1, poff = {0, M}, loff = {0, L}) and cg_segment_table_many_dev.
+// poff and loff are host arrays of B + 1; the frame tables reach the device only when B > 1.
+int segment_table(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64, int B,
+                  const int32_t *poff, const int32_t *loff, void *out_labels, int32_t *out_count, double *out_min,
+                  double *out_max, uint8_t *out_inlier, int32_t *out_order, int32_t *out_n_kept, int32_t *out_offsets,
+                  int32_t *out_index) {
+  const int M = poff[B], L = loff[B];
+  const bool many = B > 1;
   CG_REQUIRE(ctx, out_count && out_min && out_max && out_inlier && out_order && out_n_kept && out_offsets,
              "segment_table: null argument");
   CG_REQUIRE(ctx, M == 0 || (labels && x && out_labels && out_index), "segment_table: null argument");
   CG_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t Lz = (size_t)L, Mz = (size_t)M;
+  const size_t Lz = (size_t)L, Mz = (size_t)M, Bz = (size_t)B, slots = Lz + Bz;
   size_t tmp_l = 0, tmp_m = 0, tmp_s = 0;
   int lbits = 1;
-  while ((1ll << lbits) <= L) lbits++;   // point keys are ranks in [0, L]
-  CG_CUDA(ctx, cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_l, (uint64_t *)nullptr, (uint64_t *)nullptr, L,
-                                                        0, 64, st));
+  while ((1ll << lbits) <= (int64_t)(L + B - 1)) lbits++;   // point keys are offset slots in [0, L + B)
+  if (many)
+    CG_CUDA(ctx, cub::DeviceSegmentedRadixSort::SortKeysDescending(nullptr, tmp_l, (uint64_t *)nullptr, (uint64_t *)nullptr,
+                                                                   L, B, (int32_t *)nullptr, (int32_t *)nullptr, 0, 64, st));
+  else
+    CG_CUDA(ctx, cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_l, (uint64_t *)nullptr, (uint64_t *)nullptr, L,
+                                                          0, 64, st));
   if (M > 0)
     CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, tmp_m, (uint32_t *)nullptr, (uint32_t *)nullptr,
                                                  (int32_t *)nullptr, (int32_t *)nullptr, M, 0, lbits, st));
-  CG_CUDA(ctx, cub::DeviceScan::InclusiveSum(nullptr, tmp_s, (int32_t *)nullptr, (int32_t *)nullptr, L, st));
+  if (many)
+    CG_CUDA(ctx, cub::DeviceScan::InclusiveSumByKey(nullptr, tmp_s, (int32_t *)nullptr, (int32_t *)nullptr,
+                                                    (int32_t *)nullptr, (int)slots, ::cuda::std::equal_to<>(), st));
+  else
+    CG_CUDA(ctx, cub::DeviceScan::InclusiveSum(nullptr, tmp_s, (int32_t *)nullptr, (int32_t *)nullptr, (int)slots, st));
   const size_t tmp_bytes = std::max(tmp_l, std::max(tmp_m, tmp_s));
-  int32_t *cnt, *rank, *seg_len, *pval;
+  int32_t *cnt, *rank, *seg_len, *slot_frame, *pval, *dpoff, *dloff;
   uint64_t *kmin, *kmax, *key, *key_sorted;
   uint32_t *pkey, *pkey_sorted;
   void *tmp;
   const int rc = cg_ws_carve(ctx, [&](cg_arena &ar) {
-    cnt = ar.take<int32_t>(Lz); rank = ar.take<int32_t>(Lz); seg_len = ar.take<int32_t>(Lz);
+    cnt = ar.take<int32_t>(Lz); rank = ar.take<int32_t>(Lz); seg_len = ar.take<int32_t>(slots);
+    slot_frame = ar.take<int32_t>(many ? slots : 0);
+    dpoff = ar.take<int32_t>(many ? Bz + 1 : 0); dloff = ar.take<int32_t>(many ? Bz + 1 : 0);
     kmin = ar.take<uint64_t>(3 * Lz); kmax = ar.take<uint64_t>(3 * Lz);
     key = ar.take<uint64_t>(Lz); key_sorted = ar.take<uint64_t>(Lz);
     pkey = ar.take<uint32_t>(Mz); pkey_sorted = ar.take<uint32_t>(Mz); pval = ar.take<int32_t>(Mz);
     tmp = ar.take<char>(tmp_bytes);
   });
   if (rc != CG_OK) return rc;
+  if (many) {   // from pageable memory: staged at once, no synchronisation
+    CG_CUDA(ctx, cudaMemcpyAsync(dpoff, poff, sizeof(int32_t) * (Bz + 1), cudaMemcpyHostToDevice, st));
+    CG_CUDA(ctx, cudaMemcpyAsync(dloff, loff, sizeof(int32_t) * (Bz + 1), cudaMemcpyHostToDevice, st));
+  } else {
+    dpoff = dloff = slot_frame = nullptr;
+  }
   seg_init_kernel<<<blocks(L, 256), 256, 0, st>>>(L, cnt, kmin, kmax);
   CG_LAUNCH_CHECK(ctx);
   if (M > 0) {
     const unsigned g = std::min<unsigned>(blocks(M, ST_THREADS), 4u * (unsigned)ctx->num_sms);
     if (L <= ST_SMEM_L)
-      seg_stats_kernel<true><<<g, ST_THREADS, 0, st>>>(labels, labels_is_i64, x, x_is_f64, M, L, cnt, kmin, kmax);
+      seg_stats_kernel<true><<<g, ST_THREADS, 0, st>>>(labels, labels_is_i64, x, x_is_f64, M, L, dpoff, dloff, B, cnt,
+                                                       kmin, kmax);
     else
-      seg_stats_kernel<false><<<g, ST_THREADS, 0, st>>>(labels, labels_is_i64, x, x_is_f64, M, L, cnt, kmin, kmax);
+      seg_stats_kernel<false><<<g, ST_THREADS, 0, st>>>(labels, labels_is_i64, x, x_is_f64, M, L, dpoff, dloff, B, cnt,
+                                                        kmin, kmax);
     CG_LAUNCH_CHECK(ctx);
   }
   seg_decide_kernel<<<blocks(L, 256), 256, 0, st>>>(L, x_is_f64, cnt, kmin, kmax, out_min, out_max, out_count,
                                                     out_inlier, key);
   CG_LAUNCH_CHECK(ctx);
   size_t tb = tmp_bytes;
-  CG_CUDA(ctx, cub::DeviceRadixSort::SortKeysDescending(tmp, tb, key, key_sorted, L, 0, 64, st));
-  seg_order_kernel<<<blocks(L, 256), 256, 0, st>>>(L, key_sorted, out_inlier, out_order, rank, out_n_kept, seg_len);
+  if (many)
+    CG_CUDA(ctx, cub::DeviceSegmentedRadixSort::SortKeysDescending(tmp, tb, key, key_sorted, L, B, dloff, dloff + 1, 0,
+                                                                   64, st));
+  else
+    CG_CUDA(ctx, cub::DeviceRadixSort::SortKeysDescending(tmp, tb, key, key_sorted, L, 0, 64, st));
+  seg_order_kernel<<<blocks(L, 256), 256, 0, st>>>(L, key_sorted, out_inlier, dloff, B, out_order, rank, out_n_kept,
+                                                   seg_len, slot_frame);
   CG_LAUNCH_CHECK(ctx);
-  // offsets[0] = 0, offsets[k + 1] = offsets[k] + the k-th kept segment's count (0 past the kept ones)
-  CG_CUDA(ctx, cudaMemsetAsync(out_offsets, 0, sizeof(int32_t), st));
+  // offsets: each frame's slots scanned on their own, its first slot 0
   tb = tmp_bytes;
-  CG_CUDA(ctx, cub::DeviceScan::InclusiveSum(tmp, tb, seg_len, out_offsets + 1, L, st));
+  if (many)
+    CG_CUDA(ctx, cub::DeviceScan::InclusiveSumByKey(tmp, tb, slot_frame, seg_len, out_offsets, (int)slots,
+                                                    ::cuda::std::equal_to<>(), st));
+  else
+    CG_CUDA(ctx, cub::DeviceScan::InclusiveSum(tmp, tb, seg_len, out_offsets, (int)slots, st));
   if (M > 0) {
-    seg_points_kernel<<<blocks(M, 256), 256, 0, st>>>(labels, labels_is_i64, M, L, rank, out_labels, pkey, pval);
+    seg_points_kernel<<<blocks(M, 256), 256, 0, st>>>(labels, labels_is_i64, M, L, dpoff, dloff, B, rank, out_labels,
+                                                      pkey, pval);
     CG_LAUNCH_CHECK(ctx);
     // stable: within a segment the point indices stay ascending
     tb = tmp_bytes;
     CG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp, tb, pkey, pkey_sorted, pval, out_index, M, 0, lbits, st));
   }
   return CG_OK;
+}
+
+}  // namespace
+
+extern "C" int cg_segment_table_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64,
+                                    int M, int L, void *out_labels, int32_t *out_count, double *out_min,
+                                    double *out_max, uint8_t *out_inlier, int32_t *out_order, int32_t *out_n_kept,
+                                    int32_t *out_offsets, int32_t *out_index) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, M >= 0 && L >= 1 && L < (1 << 30), "segment_table: M must be >= 0 and L in [1, 2^30)");
+  const int32_t poff[2] = {0, M}, loff[2] = {0, L};
+  return segment_table(ctx, labels, labels_is_i64, x, x_is_f64, 1, poff, loff, out_labels, out_count, out_min, out_max,
+                       out_inlier, out_order, out_n_kept, out_offsets, out_index);
+}
+
+extern "C" int cg_segment_table_many_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64,
+                                         int B, const int32_t *point_offsets, const int32_t *label_offsets,
+                                         void *out_labels, int32_t *out_count, double *out_min, double *out_max,
+                                         uint8_t *out_inlier, int32_t *out_order, int32_t *out_n_kept,
+                                         int32_t *out_offsets, int32_t *out_index) {
+  if (!ctx) return CG_EINVAL;
+  CG_REQUIRE(ctx, B >= 1 && point_offsets && label_offsets, "segment_table_many: B >= 1 and both offset tables");
+  CG_REQUIRE(ctx, point_offsets[0] == 0 && label_offsets[0] == 0, "segment_table_many: the offsets must start at 0");
+  int64_t L = 0;
+  for (int b = 0; b < B; b++) {
+    CG_REQUIRE(ctx, point_offsets[b] <= point_offsets[b + 1], "segment_table_many: the point offsets must not decrease");
+    CG_REQUIRE(ctx, label_offsets[b] < label_offsets[b + 1], "segment_table_many: every frame needs L_b >= 1 labels");
+    L = label_offsets[b + 1];
+  }
+  CG_REQUIRE(ctx, L + B < (1 << 30), "segment_table_many: the frames' labels plus B must be below 2^30");
+  return segment_table(ctx, labels, labels_is_i64, x, x_is_f64, B, point_offsets, label_offsets, out_labels, out_count,
+                       out_min, out_max, out_inlier, out_order, out_n_kept, out_offsets, out_index);
 }
 
 extern "C" int cg_rank_grasps_dev(cg_ctx *ctx, const float *probs, int G, int C, int denom, const double *p_T_given_G,

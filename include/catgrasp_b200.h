@@ -504,7 +504,8 @@ int  cg_cloud_index_create(cg_ctx *ctx, const double *pts /* device */, int P, d
  * (cg_voxel_down_sample_dev) come out set-major, set s's block equal to its one-set output.  CG_EINVAL for an empty
  * set, before any launch, and for a batch whose key needs more than 63 bits, after the bounds pass and before any
  * allocation or further launch.  S = 1 is cg_cloud_index_create.  Synchronises twice whatever S is.  The one-set
- * queries (nearest, radius mask, normals, meanshift) refuse an index with S > 1: their queries carry no set.       */
+ * queries (nearest, radius mask, normals, meanshift) refuse an index with S > 1: their queries carry no set; the
+ * _many entries (nearest, normals, meanshift) search each query's own set.                                        */
 int  cg_cloud_index_create_many(cg_ctx *ctx, const double *pts /* device */, const int32_t *set_offsets /* host */,
                                 int S, double cell, cg_cloud_index **out);
 void cg_cloud_index_destroy(cg_cloud_index *index);
@@ -544,6 +545,12 @@ int  cg_cloud_radius_mask_dev(const cg_cloud_index *index, const double *query, 
  * int32 (neighbours in order, -1 padded) and out_nbr_count (P) may be NULL.                                      */
 int  cg_cloud_normals_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point /* host */,
                           double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count);
+/* cg_cloud_normals_dev per set over a cg_cloud_index_create_many index: set s's rows equal cg_cloud_normals_dev on a
+ * one-set index of set s alone, bit for bit (normals and counts; neighbour ids plus set s's first point, -1 stays),
+ * whatever cell either index was built with: membership is d2 <= radius*radius and the kept neighbours are the
+ * max_nn smallest (d2, index) keys.  One view_point serves every set.  S = 1 gives cg_cloud_normals_dev's result.   */
+int  cg_cloud_normals_many_dev(const cg_cloud_index *index, double radius, int max_nn, const double *view_point /* host */,
+                               double *out_normals, int32_t *out_nbr, int32_t *out_nbr_count);
 
 /* ---- mean-shift clustering ---- */
 /* sklearn MeanShift(bandwidth, seeds=None, bin_seeding=False, cluster_all=True) up to its labels (predicter.py:332).
@@ -649,6 +656,18 @@ int  cg_pointgroup_head_dev(cg_ctx *ctx, const float *in, int m, const int32_t *
 int  cg_segment_table_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64, int M, int L,
                           void *out_labels, int32_t *out_count, double *out_min, double *out_max, uint8_t *out_inlier,
                           int32_t *out_order, int32_t *out_n_kept, int32_t *out_offsets, int32_t *out_index);
+/* cg_segment_table_many_dev: the tables of B frames laid end to end, each block bit for bit what cg_segment_table_dev
+ * gives on that frame alone.  Frame b's points are rows [point_offsets[b], point_offsets[b+1]) of labels and x (host,
+ * B+1, from 0, not decreasing: M_b = 0 is allowed) with frame-local labels in [0, L_b); its labels are the rows
+ * [label_offsets[b], label_offsets[b+1]) (host, B+1, from 0, every L_b >= 1, sum L_b + B < 2^30).  Outputs, frame b's
+ * block of each: out_labels (M) and out_index (M) at frame b's point rows, frame-local labels and point indices;
+ * out_count, out_inlier, out_order (L) and out_min / out_max (L,3) at its label rows; out_n_kept (B) at b;
+ * out_offsets (L+B) at [label_offsets[b] + b, label_offsets[b+1] + b + 1).  B = 1 is cg_segment_table_dev.         */
+int  cg_segment_table_many_dev(cg_ctx *ctx, const void *labels, int labels_is_i64, const void *x, int x_is_f64, int B,
+                               const int32_t *point_offsets /* host */, const int32_t *label_offsets /* host */,
+                               void *out_labels, int32_t *out_count, double *out_min, double *out_max,
+                               uint8_t *out_inlier, int32_t *out_order, int32_t *out_n_kept, int32_t *out_offsets,
+                               int32_t *out_index);
 /* cg_rank_grasps_dev: run_grasp_simulation.py:311-328.  probs (G,C) float32, p_T_given_G (G) float64 ->
  * out_p_G (G) = (pred * arange(C)).sum() / denom bit for bit with numpy (float64 products, numpy's pairwise summation
  * order), denom = len(cfg_grasp['classes']) - 1 (:313; the shipped grasp-Q net has C = 10 outputs for 11 class edges,
